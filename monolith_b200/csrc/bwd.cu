@@ -11,10 +11,11 @@
 //   3 sort    : stable LSD radix sort of (slot, position), 11 bits per pass (2 passes for 2 M occurrences):
 //               the occurrences of a FID become one contiguous run in position order
 //   4 runs    : run heads -> ordered run list (start, first position, resolved row)
-//   5 reduce + update : seg_reduce_kernel streams the sorted occurrences in 32-occurrence pieces; runs of <= 64
-//               occurrences are summed in occurrence order (the CPU reference's order: bit-exact) and the optimizer is
-//               applied from registers; hot FIDs are cut into run-aligned 32-occurrence blocks combined by a fixed
-//               32-ary tree (deterministic, pairwise-accurate)
+//   5 reduce  : seg_reduce_kernel streams the sorted occurrences in 32-occurrence pieces; runs of <= 64
+//               occurrences are summed in occurrence order (the CPU reference's order: bit-exact) and stored per run;
+//               hot FIDs are cut into run-aligned 32-occurrence blocks combined by a fixed 128-ary tree
+//               (deterministic, pairwise-accurate)
+//   6 apply   : runs_apply_kernel streams the per-run sums and applies the optimizer, one row per run
 #include <algorithm>
 #include <cstring>
 
@@ -306,30 +307,18 @@ runs_write_kernel(const uint2* __restrict__ sorted, int64_t n, int nblk, const u
   }
 }
 
-struct SortWs {
-  uint32_t* k0;                 // input keys (position = index)
-  uint2 *a, *b;                 // ping-pong item buffers [M]
-  uint32_t* cnt;                // [nblk_radix][2048]
-  uint32_t* dtot;               // [passes][2048]
-  uint32_t* blk_runs;           // [nblk_runs]
-  uint32_t* run_start;          // [M + 1]
-  uint32_t* run_first_pos;      // [M]
-  uint32_t* piece_run_base;     // [ceil(M / 32)]
-  uint32_t* n_runs;             // device counter
-  uint32_t* run_of_sorted = nullptr;  // optional [M]: run index of every sorted element
-  const Entry* claim_set = nullptr;   // optional: the claim set (keys are its slots) holding resolved rows ...
-  uint32_t* rowidx = nullptr;         // ... gathered per run into rowidx[j]
-  static int radix_blocks(int64_t M) { return (int)((M + kRadixTile - 1) / kRadixTile); }
-  static int run_blocks(int64_t M) { return (int)((M + kRunTile - 1) / kRunTile); }
-  static int passes(int bits) { return std::max(1, (bits + kRadixBits - 1) / kRadixBits); }
-};
+static int radix_blocks(int64_t M) { return (int)((M + kRadixTile - 1) / kRadixTile); }
+static int run_blocks(int64_t M) { return (int)((M + kRunTile - 1) / kRunTile); }
+static int sort_passes(int bits) { return std::max(1, (bits + kRadixBits - 1) / kRadixBits); }
 
-// stable LSD radix sort of (key >> pre_shift, position) over `bits` key bits, then the ordered run list (one run
-// per distinct key).  Everything stays on the stream; counts stay on the device.
-static const uint2* sort_and_runs(const SortWs& w, int64_t M, int bits, int pre_shift, cudaStream_t s) {
-  const int passes = SortWs::passes(bits);
-  const int nb = SortWs::radix_blocks(M);
-  const void* in = w.k0;
+// stable LSD radix sort of (keys[i] >> pre_shift, i) over `bits` key bits, then the ordered run list (one run per
+// distinct key; claim_set != null: the keys are its slots and each run's resolved row is gathered into w.rowidx).
+// Everything stays on the stream; counts stay on the device.
+static const uint2* sort_and_runs(const SortWs& w, const uint32_t* keys, int64_t M, int bits, int pre_shift,
+                                  const Entry* claim_set, cudaStream_t s) {
+  const int passes = sort_passes(bits);
+  const int nb = radix_blocks(M);
+  const void* in = keys;
   uint2* out = w.a;
   for (int p = 0; p < passes; ++p) {
     uint32_t* dt = w.dtot + kRadixBins * p;
@@ -354,13 +343,13 @@ static const uint2* sort_and_runs(const SortWs& w, int64_t M, int bits, int pre_
     out = (out == w.a) ? w.b : w.a;
   }
   const uint2* sorted = static_cast<const uint2*>(in);
-  const int nr = SortWs::run_blocks(M);
+  const int nr = run_blocks(M);
   runs_count_kernel<<<resident_grid(runs_count_kernel, nr, 1), kThreads, 0, s>>>(sorted, M, nr, w.blk_runs);
   MONO_CHECK_LAUNCH();
   runs_scan_kernel<<<1, 1024, 0, s>>>(w.blk_runs, nr, w.n_runs, w.run_start, M);
   MONO_CHECK_LAUNCH();
   runs_write_kernel<<<resident_grid(runs_write_kernel, nr, 1), kThreads, 0, s>>>(
-      sorted, M, nr, w.blk_runs, w.run_start, w.run_first_pos, w.piece_run_base, w.run_of_sorted, w.claim_set, w.rowidx);
+      sorted, M, nr, w.blk_runs, w.run_start, w.run_first_pos, w.piece_run_base, w.run_of_sorted, claim_set, w.rowidx);
   MONO_CHECK_LAUNCH();
   return sorted;
 }
@@ -394,7 +383,7 @@ struct BwdArgs {
   int64_t grad_stride;
   int grad_col;
   const float* lr;              // device, slice learning rates of the table
-  float* ugrad;                 // [runs][D] summed gradient of every run (= unique FID), run order (MODE_STORE)
+  float* ugrad;                 // [runs][D] summed gradient of every run (= unique FID), run order
   float* scratch;               // alias of ugrad for the generic (multi-segment) apply path
 };
 
@@ -537,11 +526,8 @@ __device__ __forceinline__ float* run_dst(float* ugrad, int n_parts, const int64
 // batch (half of the occurrences) are plain 32-row units like everything else — no run-length classes, no
 // work lists, no atomics, no device-side scheduling.
 //
-// Where results go:
-//   SHORT unit  MODE_APPLY: the optimizer is applied right here from registers (row index of the run parked by
-//               the claim kernel; w / optimizer-state rows prefetched together with the gradient rows): the
-//               per-unique gradient buffer is never written.  MODE_STORE: summed row -> run_dst (local ugrad,
-//               or the owner's peer window for the sharded backward).
+// Where results go (the optimizer is applied afterwards, by runs_apply_kernel):
+//   SHORT unit  -> run_dst: the run's row of the local ugrad, or of the owner's peer window for the sharded backward.
 //   LONG block  -> part[slot], slot = 2 * piece + (block 0 ? 1 : 0): at most one block of the run that covers the
 //               piece start and at most one long-run head can START in a 32-occurrence piece, and block k + i of a
 //               run starts exactly i pieces after block k.  The tree levels and the final pass therefore find
@@ -604,8 +590,6 @@ __device__ __forceinline__ void load_items(const uint2* __restrict__ src, int64_
   }
 }
 
-enum { MODE_STORE = 0, MODE_APPLY = 1 };
-
 // positions of the 4 consecutive elements e .. e+3 (e a multiple of 4, < 32) of a chunk held EPL-per-lane
 template <int G>
 __device__ __forceinline__ void fetch4(const uint32_t (&v)[32 / G], int e, uint32_t (&out)[4]) {
@@ -628,7 +612,7 @@ __device__ __forceinline__ void fetch4(const uint32_t (&v)[32 / G], int e, uint3
   }
 }
 
-// The reduction kernel (MODE_STORE): unit sums go to run_dst (short runs) / part (long-run blocks).
+// The reduction kernel: unit sums go to run_dst (short runs) / part (long-run blocks).
 // Memory-level parallelism is what bounds it (a dependent random HBM round trip costs microseconds under load, so
 // ~100 KB must be in flight per SM): the gradient rows of a group's stream are requested kStage = 16 at a time with cp.async
 // (LDGSTS) into shared memory — every lane copies ITS 16-byte column slice of each row into a private slot, so nothing
@@ -882,8 +866,8 @@ tree_level_kernel(float* __restrict__ part, const SegMeta* __restrict__ meta, in
 }
 
 // Long runs, last step: the head slot of a long run combines what the tree left (blocks 0, top, 2 * top, ... — at most
-// 32 of them, in order) and applies the optimizer (MODE_APPLY) or stores the row (MODE_STORE).
-template <int G, int MODE, int OPT>
+// 32 of them, in order) and stores the run's summed row to run_dst.
+template <int G>
 __global__ void __launch_bounds__(kThreads)
 long_finish_kernel(SegArgs sa, uint32_t top, const PeerOut po) {
   __shared__ int64_t s_start[kMaxPeers + 1];
@@ -913,15 +897,7 @@ long_finish_kernel(SegArgs sa, uint32_t top, const PeerOut po) {
       for (int u = 0; u < 16; ++u)
         if ((uint64_t)k0 + (uint64_t)u * top < m.nblk) add4(acc, stage[u][threadIdx.x]);
     }
-    const uint32_t j = m.run;
-    if (MODE == MODE_APPLY) {
-      const uint32_t ri = a.rowidx[j];
-      if (ri == kEmptyRow) continue;
-      const RowPre pre = bwd_prefetch<G, OPT>(a, ri, c);
-      bwd_apply<G, OPT>(a, j, ri, acc, c, pre);
-    } else {
-      if (c < D) *reinterpret_cast<float4*>(run_dst(a.ugrad, po.n, s_start, s_base, j, D) + c) = acc;
-    }
+    if (c < D) *reinterpret_cast<float4*>(run_dst(a.ugrad, po.n, s_start, s_base, m.run, D) + c) = acc;
   }
 }
 
@@ -1110,18 +1086,87 @@ claim_miss_kernel(const TableDev* __restrict__ t, Entry* set, const uint32_t* __
 // ==========================================================================================
 // host side
 // ==========================================================================================
-static const PeerOut no_peer = {};  // n == 0: MODE_STORE writes the local ugrad buffer
+static const PeerOut no_peer = {};  // n == 0: the reduce writes the local ugrad buffer
 
-struct ReduceScratch {  // sizes of the reduction scratch for M occurrences of dim D
-  int64_t n_pieces;
-  size_t part_bytes, meta_bytes, prb_bytes;
-  ReduceScratch(int64_t M, int D) {
-    n_pieces = (M + kPiece - 1) / kPiece;
-    part_bytes = sizeof(float) * 2 * (size_t)n_pieces * D;
-    meta_bytes = sizeof(SegMeta) * 2 * (size_t)n_pieces;
-    prb_bytes = 4 * (size_t)n_pieces;
+// Optional parts of the pipeline scratch (scratch_plan)
+enum : unsigned { kPartK0 = 1, kPartRowIdx = 2, kPartMiss = 4, kPartOcc = 8, kPartRunOfSorted = 16, kPartUGrad = 32 };
+
+// Layout of the pipeline scratch for M occurrences of dim D sorted on `bits` key bits: one 256-byte aligned region
+// per part, the optional ones only when `parts` asks for them.  base == nullptr only sizes it (.bytes).
+static BwdScratch scratch_plan(int64_t M, int D, int bits, unsigned parts, char* base) {
+  size_t off = 0;
+  auto take = [&](size_t bytes, unsigned part = 0) -> void* {
+    if (part && !(parts & part)) return nullptr;
+    const uintptr_t p = reinterpret_cast<uintptr_t>(base) + off;
+    off = (off + bytes + 255) & ~(size_t)255;
+    return reinterpret_cast<void*>(p);
+  };
+  const size_t m4 = 4 * (size_t)M;
+  BwdScratch w;
+  w.n_pieces = (M + kPiece - 1) / kPiece;
+  w.k0 = (uint32_t*)take(m4, kPartK0);
+  w.sort.a = (uint2*)take(8 * (size_t)M);
+  w.sort.b = (uint2*)take(8 * (size_t)M);
+  w.sort.cnt = (uint32_t*)take(4 * (size_t)kRadixBins * radix_blocks(M));
+  w.ctr = (uint32_t*)take(kCtrBytes);
+  w.sort.dtot = (uint32_t*)take(4 * (size_t)kRadixBins * sort_passes(bits));  // right behind the counters
+  w.sort.n_runs = w.ctr + kCtrRuns;
+  w.sort.blk_runs = (uint32_t*)take(4 * (size_t)run_blocks(M));
+  w.sort.run_start = (uint32_t*)take(m4 + 4);
+  w.sort.run_first_pos = (uint32_t*)take(m4);
+  w.sort.rowidx = (uint32_t*)take(m4, kPartRowIdx);
+  w.miss = (uint32_t*)take(m4, kPartMiss);
+  w.sort.run_of_sorted = (uint32_t*)take(m4, kPartRunOfSorted);
+  w.occ = (uint32_t*)take(m4, kPartOcc);
+  w.sort.piece_run_base = (uint32_t*)take(4 * (size_t)w.n_pieces);
+  w.part = (float*)take(sizeof(float) * 2 * (size_t)w.n_pieces * D);
+  w.meta = (SegMeta*)take(sizeof(SegMeta) * 2 * (size_t)w.n_pieces);
+  w.ugrad = (float*)take(sizeof(float) * (size_t)M * D, kPartUGrad);
+  w.sorted = nullptr;
+  w.bytes = off;
+  return w;
+}
+
+// The reduce reads and writes gradient rows as 16-byte vectors, one per lane of a group of at most 32 lanes.
+static void check_grad_rows(const char* who, int D, const float* pooled_grad = nullptr, int64_t grad_stride = 0,
+                            int grad_col = 0, const float* out_rows = nullptr) {
+  if ((D & 3) || D > 128) throw ArgError(std::string(who) + " needs dim % 4 == 0 and dim <= 128");
+  if ((grad_stride & 3) || (grad_col & 3) || (reinterpret_cast<uintptr_t>(pooled_grad) & 15) ||
+      (reinterpret_cast<uintptr_t>(out_rows) & 15))
+    throw ArgError(std::string(who) + " needs 16-byte aligned rows");
+}
+
+// Arguments of a reduce over the plan's sorted list: the gradient rows of pooled_grad (row_offsets != null: CSR
+// rows, occurrence -> row mapped into w.occ first), per-run sums to ugrad (or the peer windows of the launch).
+static SegArgs seg_args(const BwdScratch& w, int64_t M, int D, const float* pooled_grad, int64_t grad_stride,
+                        int grad_col, const int32_t* row_offsets, int64_t n_rows, int pooling, float* ugrad,
+                        cudaStream_t s) {
+  SegArgs sa;
+  std::memset(&sa, 0, sizeof(sa));
+  BwdArgs& a = sa.b;
+  a.td.dim = D;
+  a.sorted = w.sorted;
+  a.n = M;
+  a.n_runs = w.sort.n_runs;
+  a.run_start = w.sort.run_start;
+  a.run_first_pos = w.sort.run_first_pos;
+  a.row_offsets = row_offsets;
+  a.pooling = pooling;
+  a.pooled_grad = pooled_grad;
+  a.grad_stride = grad_stride;
+  a.grad_col = grad_col;
+  a.ugrad = ugrad;
+  sa.piece_run_base = w.sort.piece_run_base;
+  sa.part = w.part;
+  sa.meta = w.meta;
+  sa.n_pieces = w.n_pieces;
+  if (row_offsets) {
+    occ_row_kernel<<<resident_grid(occ_row_kernel, n_rows, kThreads), kThreads, 0, s>>>(row_offsets, n_rows, w.occ);
+    MONO_CHECK_LAUNCH();
+    a.occ_row = w.occ;
   }
-};
+  return sa;
+}
 
 constexpr size_t kStageBytes = sizeof(float4) * kStage * kThreads;
 template <int GL, int VPL, bool PLAIN, bool AHEAD>
@@ -1145,7 +1190,7 @@ static void launch_seg(const SegArgs& sa, const PeerOut& po, cudaStream_t s) {
 }
 
 // per-run gradient sums -> run_dst (a.ugrad, or the owners' peer windows)
-static void launch_reduce(const SegArgs& sa, int G, int /*unused*/, const PeerOut& po, cudaStream_t s) {
+static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, cudaStream_t s) {
   const int64_t np = sa.n_pieces;
   if (np <= 0) return;
   int levels = 0;
@@ -1157,13 +1202,13 @@ static void launch_reduce(const SegArgs& sa, int G, int /*unused*/, const PeerOu
   const int D = sa.b.td.dim;
   const bool plain = sa.b.occ_row == nullptr && !(sa.b.pooling == MONO_POOL_MEAN && sa.b.row_offsets != nullptr);
   const bool two = knob(KNOB_SEG_VPL) == 2;
-#define SEG_GO(GG, MODE, OO)                                                                                        \
+#define SEG_G(GG)                                                                                                   \
   do {                                                                                                              \
     static bool attr_set = false;                                                                                   \
     if (!attr_set) {                                                                                                \
       MONO_CUDA(cudaFuncSetAttribute(tree_level_kernel<GG>, cudaFuncAttributeMaxDynamicSharedMemorySize,            \
                                      (int)kStageBytes));                                                            \
-      MONO_CUDA(cudaFuncSetAttribute(long_finish_kernel<GG, MODE, OO>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+      MONO_CUDA(cudaFuncSetAttribute(long_finish_kernel<GG>, cudaFuncAttributeMaxDynamicSharedMemorySize,           \
                                      (int)kStageBytes));                                                            \
       attr_set = true;                                                                                              \
     }                                                                                                               \
@@ -1180,12 +1225,10 @@ static void launch_reduce(const SegArgs& sa, int G, int /*unused*/, const PeerOu
                               kThreads, kStageBytes, s>>>(sa.part, sa.meta, 2 * np, stride, D);                     \
       MONO_CHECK_LAUNCH();                                                                                          \
     }                                                                                                               \
-    long_finish_kernel<GG, MODE, OO>                                                                                \
-        <<<resident_grid(long_finish_kernel<GG, MODE, OO>, np, kThreads / GG, kThreads, kStageBytes), kThreads,     \
-           kStageBytes, s>>>(sa, (uint32_t)top, po);                                                                \
+    long_finish_kernel<GG><<<resident_grid(long_finish_kernel<GG>, np, kThreads / GG, kThreads, kStageBytes),      \
+                             kThreads, kStageBytes, s>>>(sa, (uint32_t)top, po);                                    \
     MONO_CHECK_LAUNCH();                                                                                            \
   } while (0)
-#define SEG_G(GG) SEG_GO(GG, MODE_STORE, 0)
   switch (G) {
     case 4: SEG_G(4); break;
     case 8: SEG_G(8); break;
@@ -1193,7 +1236,6 @@ static void launch_reduce(const SegArgs& sa, int G, int /*unused*/, const PeerOu
     default: SEG_G(32); break;
   }
 #undef SEG_G
-#undef SEG_GO
 }
 
 static int bits_for(uint64_t cap) {
@@ -1212,9 +1254,7 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
   if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN) throw ArgError("pool_backward: SUM or MEAN");
   HostTable& ht = mt->tables[k];
   const int D = ht.dim;
-  if ((D & 3) || D > 128) throw ArgError("pool_backward needs dim % 4 == 0 and dim <= 128");
-  if ((grad_stride & 3) || (grad_col & 3) || (reinterpret_cast<uintptr_t>(pooled_grad) & 15))
-    throw ArgError("pool_backward needs 16-byte aligned gradient rows");
+  check_grad_rows("pool_backward", D, pooled_grad, grad_stride, grad_col);
   const int64_t M = n_fids;
   ensure_capacity(mt, k, (uint64_t)M, s);
   upload_tables(mt, s);
@@ -1229,96 +1269,48 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
   // the register-resident apply exists for the four vectorised optimizers; anything else: store + generic apply_row
   const int opt_sel = (ht.segs.size() == 1 && ht.segs[0].opt_type <= MONO_OPT_ADAM) ? ht.segs[0].opt_type : -1;
 
-  // ---- scratch layout ----
-  uint32_t cap = 1024;
-  while ((uint64_t)cap < 2 * (uint64_t)M) cap <<= 1;
+  // ---- scratch ----
+  const uint32_t cap = claim_set_slots(M);
   const int bits = bits_for(cap);
-  const int passes = SortWs::passes(bits);
-  const ReduceScratch rs(M, D);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-  const size_t o_k0 = take(4 * (size_t)M), o_a = take(8 * (size_t)M), o_b = take(8 * (size_t)M);
-  const size_t o_cnt = take(4 * (size_t)kRadixBins * SortWs::radix_blocks(M));
-  const size_t o_ctr = take(4096 + 4 * (size_t)kRadixBins * passes);  // counters + digit totals per pass
-  const size_t o_brun = take(4 * (size_t)SortWs::run_blocks(M));
-  const size_t o_rs = take(4 * ((size_t)M + 1)), o_rfp = take(4 * (size_t)M), o_ridx = take(4 * (size_t)M);
-  const size_t o_miss = take(4 * (size_t)M);
-  const size_t o_occ = take(row_offsets ? 4 * (size_t)M : 0);
-  const size_t o_prb = take(rs.prb_bytes), o_part = take(rs.part_bytes), o_meta = take(rs.meta_bytes);
-  const size_t o_ug = take(sizeof(float) * (size_t)M * D);
-  char* ws = (char*)mt->ws_a.get(off, s);
+  const unsigned parts = kPartK0 | kPartRowIdx | kPartMiss | (row_offsets ? kPartOcc : 0u) | kPartUGrad;
+  BwdScratch w = scratch_plan(M, D, bits, parts, nullptr);
+  w = scratch_plan(M, D, bits, parts, (char*)mt->ws_a.get(w.bytes, s));
   uint32_t epoch = 0;
   Entry* set = (Entry*)mt->claim_set.get(sizeof(Entry) * (size_t)cap, s, &epoch);
-  uint32_t* ctr = (uint32_t*)(ws + o_ctr);  // [0] n_runs [8] miss_ctr [512..] owner counts (unused here)
-  MONO_CUDA(cudaMemsetAsync(ctr, 0, 4096, s));
+  MONO_CUDA(cudaMemsetAsync(w.ctr, 0, kCtrBytes, s));
 
   // 1 claim: k0[i] = set slot of occurrence i; the winner of a slot resolves its FID in the table (row parked in
   //   the set entry, expiry timestamp bumped) or queues it as absent
-  uint32_t* k0 = (uint32_t*)(ws + o_k0);
+  uint32_t* miss_ctr = w.ctr + kCtrMisses;
   ClaimResolve cr;
   cr.t = mt->d_tables + k;
   cr.update_ts = (uint32_t)update_time;
-  cr.miss_ctr = ctr + 8;
-  cr.miss_slots = (uint32_t*)(ws + o_miss);
+  cr.miss_ctr = miss_ctr;
+  cr.miss_slots = w.miss;
   if (knob(KNOB_CLAIM_DUAL))
     fid_claim_kernel<true, true><<<resident_grid(fid_claim_kernel<true, true>, M, kThreads), kThreads, 0, s>>>(
-        fids_dev, M, set, cap, 1, epoch, k0, ctr + 512, cr, knob(KNOB_CLAIM_PF));
+        fids_dev, M, set, cap, 1, epoch, w.k0, w.ctr + kCtrOwners, cr, knob(KNOB_CLAIM_PF));
   else
     fid_claim_kernel<true><<<resident_grid(fid_claim_kernel<true>, M, kThreads), kThreads, 0, s>>>(
-        fids_dev, M, set, cap, 1, epoch, k0, ctr + 512, cr, knob(KNOB_CLAIM_PF));
+        fids_dev, M, set, cap, 1, epoch, w.k0, w.ctr + kCtrOwners, cr, knob(KNOB_CLAIM_PF));
   MONO_CHECK_LAUNCH();
   // 2 absent FIDs: allocate a row + lock-free insert (few in steady state; the count stays on the device)
   claim_miss_kernel<<<resident_grid(claim_miss_kernel, std::min<int64_t>(M, (int64_t)device_sms() * 2 * kThreads), kThreads), kThreads, 0, s>>>(
-      mt->d_tables + k, set, ctr + 8, cr.miss_slots, (uint32_t)update_time);
+      mt->d_tables + k, set, miss_ctr, w.miss, (uint32_t)update_time);
   MONO_CHECK_LAUNCH();
-  launch_upsert_finalize(mt, cb, ctr + 8, (uint32_t)update_time, s);
+  launch_upsert_finalize(mt, cb, miss_ctr, (uint32_t)update_time, s);
   // 3 stable LSD radix sort of (slot, position)  +  4 ordered run list (with each run's resolved row)
-  SortWs sw;
-  sw.k0 = k0;
-  sw.a = (uint2*)(ws + o_a);
-  sw.b = (uint2*)(ws + o_b);
-  sw.cnt = (uint32_t*)(ws + o_cnt);
-  sw.dtot = (uint32_t*)(ws + o_ctr + 4096);
-  sw.blk_runs = (uint32_t*)(ws + o_brun);
-  sw.run_start = (uint32_t*)(ws + o_rs);
-  sw.run_first_pos = (uint32_t*)(ws + o_rfp);
-  sw.piece_run_base = (uint32_t*)(ws + o_prb);
-  sw.n_runs = ctr;
-  sw.claim_set = set;
-  sw.rowidx = (uint32_t*)(ws + o_ridx);
-  const uint2* sorted = sort_and_runs(sw, M, bits, 0, s);
-  // 5 reduce + update
-  SegArgs sa;
+  w.sorted = sort_and_runs(w.sort, w.k0, M, bits, 0, set, s);
+  // 5 reduce
+  SegArgs sa = seg_args(w, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, w.ugrad, s);
   BwdArgs& a = sa.b;
   a.td = ht.dev;  // descriptor is current: ensure_capacity / upload_tables ran above
   a.t = mt->d_tables + k;
   a.fids = fids_dev;
-  a.sorted = sorted;
-  a.n = M;
-  a.n_runs = ctr;
-  a.run_start = sw.run_start;
-  a.run_first_pos = sw.run_first_pos;
-  a.rowidx = sw.rowidx;
-  a.occ_row = nullptr;
-  a.row_offsets = row_offsets;
-  a.pooling = pooling;
-  a.pooled_grad = pooled_grad;
-  a.grad_stride = grad_stride;
-  a.grad_col = grad_col;
+  a.rowidx = w.sort.rowidx;
   a.lr = cb.lr;
-  a.ugrad = (float*)(ws + o_ug);
   a.scratch = a.ugrad;
-  sa.piece_run_base = sw.piece_run_base;
-  sa.part = (float*)(ws + o_part);
-  sa.meta = (SegMeta*)(ws + o_meta);
-  sa.n_pieces = rs.n_pieces;
-  if (row_offsets) {
-    uint32_t* occ = (uint32_t*)(ws + o_occ);
-    occ_row_kernel<<<resident_grid(occ_row_kernel, n_rows, kThreads), kThreads, 0, s>>>(row_offsets, n_rows, occ);
-    MONO_CHECK_LAUNCH();
-    a.occ_row = occ;
-  }
-  launch_reduce(sa, G, -1, no_peer, s);
+  launch_reduce(sa, G, no_peer, s);
   // 6 apply: one streaming pass over the runs — row index, summed gradient, w / optimizer state of every distinct FID
   const int pf = knob(KNOB_APPLY_PF);
 #define BWD2(GG, OO)                                                                                             \
@@ -1357,73 +1349,26 @@ void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, c
   if (M <= 0) return;
   if (M >= ((int64_t)1 << 31) || total_floats >= ((int64_t)1 << 31)) throw ArgError("scatter_rows: sizes exceed 2^31");
   if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN) throw ArgError("scatter_rows: SUM or MEAN");
-  if ((dim & 3) || dim > 128) throw ArgError("scatter_rows needs dim % 4 == 0 and dim <= 128");
-  if ((grad_stride & 3) || (grad_col & 3) || (reinterpret_cast<uintptr_t>(pooled_grad) & 15) ||
-      (reinterpret_cast<uintptr_t>(out_rows) & 15))
-    throw ArgError("scatter_rows needs 16-byte aligned rows");
+  check_grad_rows("scatter_rows", dim, pooled_grad, grad_stride, grad_col, out_rows);
   const int D = dim;
   // offsets are multiples of 4 floats (16-byte aligned rows; every dim in the fused buffer is a multiple
   // of 4): drop the two zero bits from the sort key
   const int shift = 2;
   int bits = 1;
   while (((int64_t)1 << bits) < ((total_floats >> shift) + 1)) ++bits;
-  const int passes = SortWs::passes(bits);
-  const ReduceScratch rs(M, D);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-  const size_t o_a = take(8 * (size_t)M), o_b = take(8 * (size_t)M);
-  const size_t o_cnt = take(4 * (size_t)kRadixBins * SortWs::radix_blocks(M));
-  const size_t o_ctr = take(4096 + 4 * (size_t)kRadixBins * passes);
-  const size_t o_brun = take(4 * (size_t)SortWs::run_blocks(M));
-  const size_t o_rs = take(4 * ((size_t)M + 1)), o_rfp = take(4 * (size_t)M);
-  const size_t o_occ = take(row_offsets ? 4 * (size_t)M : 0);
-  const size_t o_prb = take(rs.prb_bytes), o_part = take(rs.part_bytes), o_meta = take(rs.meta_bytes);
-  const size_t o_ug = take(sizeof(float) * (size_t)M * D);
+  const unsigned parts = (row_offsets ? kPartOcc : 0u) | kPartUGrad;
+  BwdScratch w = scratch_plan(M, D, bits, parts, nullptr);
   char* ws = nullptr;
-  MONO_CUDA(cudaMallocAsync((void**)&ws, off, s));
-  uint32_t* ctr = (uint32_t*)(ws + o_ctr);
-  MONO_CUDA(cudaMemsetAsync(ctr, 0, 4096, s));
-  SortWs sw;
-  sw.k0 = reinterpret_cast<uint32_t*>(const_cast<int32_t*>(offs_dev));  // read-only: the first pass copies the keys out
-  sw.a = (uint2*)(ws + o_a);
-  sw.b = (uint2*)(ws + o_b);
-  sw.cnt = (uint32_t*)(ws + o_cnt);
-  sw.dtot = (uint32_t*)(ws + o_ctr + 4096);
-  sw.blk_runs = (uint32_t*)(ws + o_brun);
-  sw.run_start = (uint32_t*)(ws + o_rs);
-  sw.run_first_pos = (uint32_t*)(ws + o_rfp);
-  sw.piece_run_base = (uint32_t*)(ws + o_prb);
-  sw.n_runs = ctr;
-  const uint2* sorted = sort_and_runs(sw, M, bits, shift, s);
-  SegArgs sa;
-  std::memset(&sa, 0, sizeof(sa));
-  BwdArgs& a = sa.b;
-  a.td.dim = D;
-  a.sorted = sorted;
-  a.n = M;
-  a.n_runs = ctr;
-  a.run_start = sw.run_start;
-  a.run_first_pos = sw.run_first_pos;
-  a.row_offsets = row_offsets;
-  a.pooling = pooling;
-  a.pooled_grad = pooled_grad;
-  a.grad_stride = grad_stride;
-  a.grad_col = grad_col;
-  a.ugrad = (float*)(ws + o_ug);
-  sa.piece_run_base = sw.piece_run_base;
-  sa.part = (float*)(ws + o_part);
-  sa.meta = (SegMeta*)(ws + o_meta);
-  sa.n_pieces = rs.n_pieces;
-  if (row_offsets) {
-    uint32_t* occ = (uint32_t*)(ws + o_occ);
-    occ_row_kernel<<<resident_grid(occ_row_kernel, n_rows, kThreads), kThreads, 0, s>>>(row_offsets, n_rows, occ);
-    MONO_CHECK_LAUNCH();
-    a.occ_row = occ;
-  }
+  MONO_CUDA(cudaMallocAsync((void**)&ws, w.bytes, s));
+  w = scratch_plan(M, D, bits, parts, ws);
+  MONO_CUDA(cudaMemsetAsync(w.ctr, 0, kCtrBytes, s));
+  // the offsets are the sort keys (read-only: the first pass copies them out)
+  w.sorted = sort_and_runs(w.sort, reinterpret_cast<const uint32_t*>(offs_dev), M, bits, shift, nullptr, s);
+  const SegArgs sa = seg_args(w, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, w.ugrad, s);
   const int G = pick_group(D);
-  launch_reduce(sa, G, -1, no_peer, s);
+  launch_reduce(sa, G, no_peer, s);
 #define EMIT(GG)                                                                                              \
-  runs_emit_kernel<GG><<<resident_grid(runs_emit_kernel<GG>, M, kThreads / GG), kThreads, 0, s>>>(a, shift, out_rows); \
+  runs_emit_kernel<GG><<<resident_grid(runs_emit_kernel<GG>, M, kThreads / GG), kThreads, 0, s>>>(sa.b, shift, out_rows); \
   MONO_CHECK_LAUNCH()
   switch (G) {
     case 4: EMIT(4); break;
@@ -1461,16 +1406,36 @@ group_emit_kernel(const int64_t* __restrict__ fids, const uint2* __restrict__ so
   for (int64_t j = t0; j < nr; j += stride) uniq_out[j] = fids[run_first_pos[j]];
 }
 
+mono_grouping* grouping_create(int device) {
+  auto g = new mono_grouping();
+  g->device = device;
+  return g;
+}
+
+void grouping_destroy(mono_grouping* g) {
+  if (!g) return;
+  cudaSetDevice(g->device);
+  cudaDeviceSynchronize();
+  g->ws.release();
+  g->claim_set.release();
+  if (g->h_counts) cudaFreeHost(g->h_counts);
+  if (g->ev_claimed) cudaEventDestroy(g->ev_claimed);
+  if (g->ev_copied) cudaEventDestroy(g->ev_copied);
+  if (g->side) cudaStreamDestroy(g->side);
+  delete g;
+}
+
 void grouping_build(mono_grouping* g, const int64_t* fids_dev, int64_t M, int N, int dim,
                     int64_t* uniq_out, int32_t* occ_offset_out, int32_t* shard_counts_host,
                     int64_t* n_unique_host, cudaStream_t s) {
   MONO_CUDA(cudaSetDevice(g->device));
   if (N <= 0 || N > 256) throw ArgError("grouping: num_shards must be in [1, 256]");
   if (M < 0 || M >= ((int64_t)1 << 29)) throw ArgError("grouping: bad occurrence count");
-  if ((dim & 3) || dim <= 0 || dim > 128) throw ArgError("grouping needs dim % 4 == 0 and dim <= 128");
+  if (dim <= 0) throw ArgError("grouping: dim must be positive");
+  check_grad_rows("grouping", dim);
   g->M = M;
   g->dim = dim;
-  g->sorted = nullptr;
+  g->plan = BwdScratch{};
   if (M == 0) {
     if (!shard_counts_host) throw ArgError("grouping: the device-driven step needs a non-empty batch");
     for (int n = 0; n < N; ++n) shard_counts_host[n] = 0;
@@ -1483,8 +1448,7 @@ void grouping_build(mono_grouping* g, const int64_t* fids_dev, int64_t M, int N,
     MONO_CUDA(cudaEventCreateWithFlags(&g->ev_claimed, cudaEventDisableTiming));
     MONO_CUDA(cudaEventCreateWithFlags(&g->ev_copied, cudaEventDisableTiming));
   }
-  uint64_t cap0 = 1024;
-  while (cap0 < 2 * (uint64_t)M) cap0 <<= 1;
+  const uint64_t cap0 = claim_set_slots(M);
   for (int attempt = 0; attempt < 2; ++attempt) {
     // attempt 0: the regions share 2M slots (load <= 0.5 for hash-balanced owners);
     // attempt 1 (a region overflowed: heavily skewed owners): every region can hold all M FIDs.
@@ -1492,41 +1456,17 @@ void grouping_build(mono_grouping* g, const int64_t* fids_dev, int64_t M, int N,
     if (cap > ((uint64_t)1 << 31)) throw ArgError("grouping: FID owners too skewed for this batch size");
     const uint32_t R = (uint32_t)(cap / (uint64_t)N);
     const int bits = bits_for(cap);
-    const int passes = SortWs::passes(bits);
-    const ReduceScratch rs(M, dim);
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-    const size_t o_k0 = take(4 * (size_t)M), o_a = take(8 * (size_t)M), o_b = take(8 * (size_t)M);
-    const size_t o_cnt = take(4 * (size_t)kRadixBins * SortWs::radix_blocks(M));
-    const size_t o_ctr = take(4096 + 4 * (size_t)kRadixBins * passes + 4 * 260);
-    const size_t o_brun = take(4 * (size_t)SortWs::run_blocks(M));
-    const size_t o_rs = take(4 * ((size_t)M + 1)), o_rfp = take(4 * (size_t)M), o_ros = take(4 * (size_t)M);
-    const size_t o_prb = take(rs.prb_bytes);
-    // reduce() scratch
-    const size_t o_occ = take(4 * (size_t)M), o_part = take(rs.part_bytes), o_meta = take(rs.meta_bytes);
-    char* ws = (char*)g->ws.get(off, s);
+    const unsigned parts = kPartK0 | kPartRunOfSorted | kPartOcc;  // occ: reduce()'s CSR map
+    BwdScratch w = scratch_plan(M, dim, bits, parts, nullptr);
+    w = scratch_plan(M, dim, bits, parts, (char*)g->ws.get(w.bytes, s));
     uint32_t epoch = 0;
     Entry* set = (Entry*)g->claim_set.get(sizeof(Entry) * (size_t)cap, s, &epoch);
-    uint32_t* ctr = (uint32_t*)(ws + o_ctr);
-    uint32_t* owner_cnt = (uint32_t*)(ws + o_ctr + 4096 + 4 * (size_t)kRadixBins * passes);
-    MONO_CUDA(cudaMemsetAsync(ctr, 0, 4096, s));
-    MONO_CUDA(cudaMemsetAsync(owner_cnt, 0, 4 * 260, s));
-    SortWs sw;
-    sw.k0 = (uint32_t*)(ws + o_k0);
-    sw.a = (uint2*)(ws + o_a);
-    sw.b = (uint2*)(ws + o_b);
-    sw.cnt = (uint32_t*)(ws + o_cnt);
-    sw.dtot = (uint32_t*)(ws + o_ctr + 4096);
-    sw.blk_runs = (uint32_t*)(ws + o_brun);
-    sw.run_start = (uint32_t*)(ws + o_rs);
-    sw.run_first_pos = (uint32_t*)(ws + o_rfp);
-    sw.piece_run_base = (uint32_t*)(ws + o_prb);
-    sw.n_runs = ctr;
-    sw.run_of_sorted = (uint32_t*)(ws + o_ros);
+    uint32_t* owner_cnt = w.ctr + kCtrOwners;
+    MONO_CUDA(cudaMemsetAsync(w.ctr, 0, kCtrBytes, s));
     ClaimResolve cr0;
     std::memset(&cr0, 0, sizeof(cr0));
     fid_claim_kernel<false><<<resident_grid(fid_claim_kernel<false>, M, kThreads), kThreads, 0, s>>>(
-        fids_dev, M, set, R, N, epoch, sw.k0, owner_cnt, cr0, knob(KNOB_CLAIM_PF));
+        fids_dev, M, set, R, N, epoch, w.k0, owner_cnt, cr0, knob(KNOB_CLAIM_PF));
     MONO_CHECK_LAUNCH();
     // counts -> host on the side stream, while the sort below keeps the GPU busy.  Device-driven callers
     // (shard_counts_host == nullptr: xstep.cu) never read them on the host: nothing waits, the per-owner counts stay
@@ -1538,11 +1478,10 @@ void grouping_build(mono_grouping* g, const int64_t* fids_dev, int64_t M, int N,
       MONO_CUDA(cudaMemcpyAsync(g->h_counts, owner_cnt, 4 * 257, cudaMemcpyDeviceToHost, g->side));
       MONO_CUDA(cudaEventRecord(g->ev_copied, g->side));
     }
-    const uint2* sorted = sort_and_runs(sw, M, bits, 0, s);
+    w.sorted = sort_and_runs(w.sort, w.k0, M, bits, 0, nullptr, s);
     group_emit_kernel<<<resident_grid(group_emit_kernel, M, kThreads), kThreads, 0, s>>>(
-        fids_dev, sorted, sw.run_of_sorted, sw.run_first_pos, ctr, M, dim, occ_offset_out, uniq_out);
+        fids_dev, w.sorted, w.sort.run_of_sorted, w.sort.run_first_pos, w.sort.n_runs, M, dim, occ_offset_out, uniq_out);
     MONO_CHECK_LAUNCH();
-    g->owner_cnt = owner_cnt;
     if (host_counts) {
       MONO_CUDA(cudaEventSynchronize(g->ev_copied));
       if (g->h_counts[256] != 0) continue;  // region overflow: redo with full-size regions
@@ -1553,14 +1492,7 @@ void grouping_build(mono_grouping* g, const int64_t* fids_dev, int64_t M, int N,
       }
       if (n_unique_host) *n_unique_host = total;
     }
-    g->sorted = sorted;
-    g->run_start = sw.run_start;
-    g->run_first_pos = sw.run_first_pos;
-    g->piece_run_base = sw.piece_run_base;
-    g->ctr = ctr;
-    g->occ = (uint32_t*)(ws + o_occ);
-    g->part = (float*)(ws + o_part);
-    g->meta = ws + o_meta;
+    g->plan = w;
     return;
   }
   throw ArgError("grouping: scratch set overflow (internal)");
@@ -1573,37 +1505,13 @@ static void grouping_reduce_impl(mono_grouping* g, const float* pooled_grad, int
   const int64_t M = g->M;
   const int D = g->dim;
   if (M <= 0) return;
-  if (!g->sorted) throw ArgError("grouping_reduce before grouping_build");
+  if (!g->plan.sorted) throw ArgError("grouping_reduce before grouping_build");
   if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN) throw ArgError("grouping_reduce: SUM or MEAN");
-  if ((grad_stride & 3) || (grad_col & 3) || (reinterpret_cast<uintptr_t>(pooled_grad) & 15) ||
-      (po.n == 0 && (reinterpret_cast<uintptr_t>(out_rows) & 15)))
-    throw ArgError("grouping_reduce needs 16-byte aligned rows");
-  const ReduceScratch rs(M, D);
-  SegArgs sa;
-  std::memset(&sa, 0, sizeof(sa));
-  BwdArgs& a = sa.b;
-  a.td.dim = D;
-  a.sorted = g->sorted;
-  a.n = M;
-  a.n_runs = g->ctr;
-  a.run_start = g->run_start;
-  a.run_first_pos = g->run_first_pos;
-  a.row_offsets = row_offsets;
-  a.pooling = pooling;
-  a.pooled_grad = pooled_grad;
-  a.grad_stride = grad_stride;
-  a.grad_col = grad_col;
-  a.ugrad = out_rows;  // runs are already in the bucketed order: the sums are written in place
-  sa.piece_run_base = g->piece_run_base;
-  sa.part = g->part;
-  sa.meta = static_cast<SegMeta*>(g->meta);
-  sa.n_pieces = rs.n_pieces;
-  if (row_offsets) {
-    occ_row_kernel<<<resident_grid(occ_row_kernel, n_rows, kThreads), kThreads, 0, s>>>(row_offsets, n_rows, g->occ);
-    MONO_CHECK_LAUNCH();
-    a.occ_row = g->occ;
-  }
-  launch_reduce(sa, pick_group(D), -1, po, s);
+  check_grad_rows("grouping_reduce", D, pooled_grad, grad_stride, grad_col, po.n == 0 ? out_rows : nullptr);
+  // runs are already in the bucketed order: the sums are written in place
+  const SegArgs sa = seg_args(g->plan, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling,
+                              out_rows, s);
+  launch_reduce(sa, pick_group(D), po, s);
 }
 
 // out_rows[u] = summed gradient of the u-th distinct FID of the bucketed list (ref: ScatterGrad)

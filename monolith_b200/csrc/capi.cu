@@ -512,23 +512,12 @@ int mono_grouping_create(int32_t device, mono_grouping_t** out) {
   return guarded([&] {
     require(out != nullptr, "grouping_create: null out");
     MONO_CUDA(cudaSetDevice(device));
-    auto g = new mono_grouping();
-    g->device = device;
-    *out = g;
+    *out = grouping_create(device);
   });
 }
 
 int mono_grouping_destroy(mono_grouping_t* g) {
-  if (!g) return MONO_OK;
-  cudaSetDevice(g->device);
-  cudaDeviceSynchronize();
-  g->ws.release();
-  g->claim_set.release();
-  if (g->h_counts) cudaFreeHost(g->h_counts);
-  if (g->ev_claimed) cudaEventDestroy(g->ev_claimed);
-  if (g->ev_copied) cudaEventDestroy(g->ev_copied);
-  if (g->side) cudaStreamDestroy(g->side);
-  delete g;
+  grouping_destroy(g);
   return MONO_OK;
 }
 

@@ -147,6 +147,14 @@ struct ClaimSet {
   }
 };
 
+// Slots of a claim set for n keys (n <= 2^30): the smallest power of two >= max(1024, 2n), so the set is at most
+// half full.
+inline uint32_t claim_set_slots(int64_t n) {
+  uint32_t cap = 1024;
+  while ((uint64_t)cap < 2 * (uint64_t)n) cap <<= 1;
+  return cap;
+}
+
 // Ring of pinned host blocks mirrored by device blocks: small per-call descriptors (segments,
 // learning rates) are written to a pinned block and copied H2D on the call's stream.
 struct StageRing {
@@ -183,6 +191,43 @@ struct HostTable {
   cudaEvent_t snap_ev = nullptr;
 };
 
+// ---- scratch of the backward's claim -> sort -> run list -> reduce pipeline (bwd.cu scratch_plan) ----
+// Counters block at the head of the scratch (one memset clears it every call), word offsets:
+constexpr int kCtrRuns = 0;       // runs of the sorted list (= distinct keys)
+constexpr int kCtrMisses = 8;     // FIDs the claim found absent from the table
+constexpr int kCtrOwners = 512;   // distinct FIDs per owner [256], then the claim set's region-overflow flag
+constexpr size_t kCtrBytes = 4096;
+
+struct SortWs {                 // the sort's and the run list's regions
+  uint2 *a, *b;                 // ping-pong item buffers [M]
+  uint32_t* cnt;                // [radix blocks][2048]
+  uint32_t* dtot;               // [passes][2048]
+  uint32_t* blk_runs;           // [run blocks]
+  uint32_t* run_start;          // [M + 1]
+  uint32_t* run_first_pos;      // [M]
+  uint32_t* piece_run_base;     // [ceil(M / 32)]
+  uint32_t* n_runs;             // device counter
+  uint32_t* run_of_sorted;      // optional [M]: run index of every sorted element
+  uint32_t* rowidx;             // optional [M]: each run's resolved row, gathered from the claim set
+};
+
+struct SegMeta;  // bwd.cu
+
+// Typed views into one scratch buffer; the optional parts a caller did not ask for are null.
+struct BwdScratch {
+  size_t bytes;
+  uint32_t* ctr;                // counters block (kCtr*)
+  uint32_t* k0;                 // optional [M]: claim keys (the claim-set slot of every occurrence)
+  uint32_t* miss;               // optional [M]: slots of the FIDs the claim found absent
+  uint32_t* occ;                // optional [M]: occurrence -> pooled row (CSR gradient source)
+  SortWs sort;
+  float* part;                  // [2 * n_pieces][D] long-run block sums
+  SegMeta* meta;                // [2 * n_pieces]
+  float* ugrad;                 // optional [M][D]: summed gradient of every run
+  int64_t n_pieces;
+  const uint2* sorted;          // the sorted {key, position} list, once the sort has run
+};
+
 }  // namespace mono
 
 struct mono_mtable {
@@ -213,23 +258,14 @@ struct mono_mtable {
   bool lookup_must_confirm(cudaStream_t s) const { return confirm_always || (any_insert && insert_stream != s); }
 };
 
-// one reusable grouping of a batch (see ops.cu "Owner grouping")
+// one reusable grouping of a batch (see bwd.cu "Owner grouping")
 struct mono_grouping {
   int device = 0;
   mono::DevBuf ws;
   mono::ClaimSet claim_set;
   int64_t M = 0;
   int dim = 0;
-  // views into ws valid after build()
-  const uint2* sorted = nullptr;        // {set slot, position} sorted by slot, stable
-  uint32_t* run_start = nullptr;
-  uint32_t* run_first_pos = nullptr;
-  uint32_t* piece_run_base = nullptr;
-  uint32_t* ctr = nullptr;
-  uint32_t* occ = nullptr;              // scratch of reduce(): occurrence -> pooled row
-  float* part = nullptr;                // long-run block sums
-  void* meta = nullptr;                 // SegMeta[2 * pieces]
-  uint32_t* owner_cnt = nullptr;        // device: distinct FIDs per owner [N], [256] = region-overflow flag
+  mono::BwdScratch plan{};       // views into ws, valid after build() (plan.sorted != nullptr)
   uint32_t* h_counts = nullptr;  // pinned: per-owner distinct counts [256] + overflow flag
   cudaStream_t side = nullptr;   // carries the early counts copy while the sort runs on the caller's stream
   cudaEvent_t ev_claimed = nullptr, ev_copied = nullptr;
@@ -350,6 +386,8 @@ void grouping_reduce_push(mono_grouping* g, const float* pooled_grad, int64_t gr
                           const int32_t* row_offsets, int64_t n_rows, int pooling, const PeerOut& po,
                           cudaStream_t s);
 
+mono_grouping* grouping_create(int device);
+void grouping_destroy(mono_grouping* g);  // synchronises the device first
 void grouping_build(mono_grouping* g, const int64_t* fids_dev, int64_t M, int N, int dim,
                     int64_t* uniq_out, int32_t* occ_offset_out, int32_t* shard_counts_host,
                     int64_t* n_unique_host, cudaStream_t s);

@@ -1213,8 +1213,7 @@ void run_upsert(mono_mtable* mt, UpsertOp op, const CallSeg* h_segs, int nsegs,
     // Sequential semantics for duplicates (ref: per-id loops in BatchOptimize / AssignAdd):
     // round r applies the r-th occurrence of every key; within a round keys are unique.
     if (n_total > ((int64_t)1 << 30)) throw ArgError("more than 2^30 non-unique ids in one call");
-    uint32_t cap = 1024;
-    while ((uint64_t)cap < 2 * (uint64_t)n_total) cap <<= 1;  // <= 2^31: n_total <= 2^30 checked above
+    const uint32_t cap = claim_set_slots(n_total);  // <= 2^31: n_total <= 2^30 checked above
     SetEntry* set = (SetEntry*)mt->ws_a.get(sizeof(SetEntry) * (size_t)cap, s);
     uint32_t* slot_of = (uint32_t*)mt->ws_b.get(sizeof(uint32_t) * (size_t)n_total, s);
     uint32_t* lists = (uint32_t*)mt->ws_c.get(sizeof(uint32_t) * (size_t)n_total * 3 + 64, s);
@@ -1335,8 +1334,7 @@ void run_upsert_groups(mono_mtable* mt, const CallSeg* h_segs, int nsegs, const 
   const int G = pick_group(max_dim_of(mt, h_segs, nsegs));
 
   if (n_total > ((int64_t)1 << 30)) throw ArgError("more than 2^30 ids in one grouped optimize call");
-  uint32_t cap = 1024;
-  while ((uint64_t)cap < 2 * (uint64_t)n_total) cap <<= 1;
+  const uint32_t cap = claim_set_slots(n_total);
   // scratch: [ctr 64 B | miss_list | rowidx | leaders | followers | fol_leader | slot_of] u32[n_total] each
   char* ws = (char*)mt->ws_miss.get(64 + 6 * sizeof(uint32_t) * (size_t)n_total, s);
   uint32_t* ctr = reinterpret_cast<uint32_t*>(ws);  // [0] misses [1] leaders [2] followers

@@ -346,8 +346,7 @@ mono_xstep* xstep_create(mono_mtable* mt, int k, mono_peer* win, int64_t cap_pai
   x->me = win->rank;
   x->D = D;
   for (int q = 0; q < 2; ++q) {
-    x->grouping[q] = new mono_grouping();
-    x->grouping[q]->device = mt->device;
+    x->grouping[q] = grouping_create(mt->device);
     MONO_CUDA(cudaEventCreateWithFlags(&x->ev_prep[q], cudaEventDisableTiming));
     MONO_CUDA(cudaEventCreateWithFlags(&x->ev_bwd[q], cudaEventDisableTiming));
   }
@@ -379,15 +378,7 @@ void xstep_destroy(mono_xstep* x) {
     x->offs[q].release();
     if (x->ev_prep[q]) cudaEventDestroy(x->ev_prep[q]);
     if (x->ev_bwd[q]) cudaEventDestroy(x->ev_bwd[q]);
-    mono_grouping* g = x->grouping[q];
-    if (!g) continue;
-    g->ws.release();
-    g->claim_set.release();
-    if (g->h_counts) cudaFreeHost(g->h_counts);
-    if (g->ev_claimed) cudaEventDestroy(g->ev_claimed);
-    if (g->ev_copied) cudaEventDestroy(g->ev_copied);
-    if (g->side) cudaStreamDestroy(g->side);
-    delete g;
+    grouping_destroy(x->grouping[q]);
   }
   delete x;
 }
@@ -416,7 +407,7 @@ void xstep_forward(mono_xstep* x, const int64_t* fids_dev, int64_t M, const int3
     grouping_build(g, fids_dev, M, x->N, x->D, uniq, offs, nullptr, nullptr, s);
   }
   x->prep_seq = 0;
-  const uint32_t* owner_cnt = g->owner_cnt;
+  const uint32_t* owner_cnt = g->plan.ctr + kCtrOwners;
   xput_ids_kernel<<<resident_grid(xput_ids_kernel, M, kThreads), kThreads, 0, s>>>(uniq, owner_cnt, w, par);
   MONO_CHECK_LAUNCH();
   xsignal_kernel<<<1, 32, 0, s>>>(w, kPhaseIds, seq, owner_cnt);
@@ -470,7 +461,7 @@ void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride
   for (int r = 0; r < x->N; ++r)
     po.base[r] = x->win->base[r] + kPeerFlagBytes + w.off_grads + (int64_t)x->me * x->C * x->D * 4;
   mono_grouping* g = x->grouping[par];
-  po.cnt_dev = g->owner_cnt;
+  po.cnt_dev = g->plan.ctr + kCtrOwners;
   grouping_reduce_push(g, pooled_grad, grad_stride, grad_col, row_offsets, x->last_rows, pooling, po, s);
   xsignal_kernel<<<1, 32, 0, s>>>(w, kPhaseGrads, seq, nullptr);
   MONO_CHECK_LAUNCH();
@@ -488,8 +479,7 @@ void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride
   sg.table = x->k;
   sg.lr_off = 0;
   CallBlob cb = stage_call(mt, &sg, 1, lr_host, ht.slices, s);
-  uint32_t cap = 1024;
-  while ((uint64_t)cap < 2 * (uint64_t)cap_total) cap <<= 1;
+  const uint32_t cap = claim_set_slots(cap_total);
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
   const size_t o_ctr = take(256), o_ridx = take(4 * (size_t)cap_total), o_miss = take(4 * (size_t)cap_total);
