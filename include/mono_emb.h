@@ -183,8 +183,9 @@ int mono_mtable_lookup_pool(mono_mtable_t* t, int32_t k, const int64_t* fids_dev
  *   MonolithMultiHashTableOptimize (ref: RT/ops/multi_hash_table_update_op.cc:47-100)
  * for the occurrences fids_dev[row_offsets[r]:row_offsets[r+1]] of pooled row r (row_offsets NULL:
  * one FID per row).  Every distinct FID receives ONE optimizer step with the sum (SUM) or the sum
- * of g/n (MEAN) of its occurrences' pooled-row gradients, accumulated in occurrence order without
- * float atomics (run-to-run bit-stable); absent FIDs are inserted (upsert) exactly like optimize.
+ * of g/n (MEAN) of its occurrences' pooled-row gradients, summed without float atomics (run-to-run
+ * bit-stable) in the order described at mono_scatter_grad_rows; absent FIDs are inserted (upsert)
+ * exactly like optimize.
  * Needs dim(k) % 4 == 0, dim(k) <= 128 and 16-byte aligned gradient rows.  No host sync. */
 int mono_mtable_pool_backward(mono_mtable_t* t, int32_t k, const int64_t* fids_dev, int64_t n_fids,
                               const int32_t* row_offsets_dev, int64_t n_rows, int32_t pooling,
@@ -307,7 +308,8 @@ int mono_dedup(int32_t device, const int64_t* ids_dev, int64_t n, int64_t* uniqu
  *                          post-all-to-all row buffer  (== fused_emb_offset of the reference op)
  * and on the host (SYNC): shard_counts_host[num_shards], n_unique_host.
  * reduce(): with the grouping built last, out_rows_dev[u*dim : +dim] = sum (SUM) / sum of g/n (MEAN)
- * of the pooled-row gradients of FID u's occurrences, in occurrence order, without float atomics. */
+ * of the pooled-row gradients of FID u's occurrences, without float atomics, in the order described
+ * at mono_scatter_grad_rows. */
 typedef struct mono_grouping mono_grouping_t;
 int mono_grouping_create(int32_t device, mono_grouping_t** out);
 int mono_grouping_destroy(mono_grouping_t* g);
@@ -336,8 +338,12 @@ int mono_gather_pool_grad(int32_t device, const float* pooled_grad_dev, int64_t 
 
 /* Deterministic variant of mono_gather_pool_grad (no float atomics): occurrences are radix-sorted
  * by destination offset and each destination row is written once with the sum of its occurrences'
- * pooled-row gradients in occurrence order (run-to-run bit-stable; the reference GPU kernel uses
- * atomicAdd, map_id_to_embedding.cu.cc:75-118).  emb_offset_dev[m] is the float offset of
+ * pooled-row gradients (run-to-run bit-stable; the reference GPU kernel uses atomicAdd,
+ * map_id_to_embedding.cu.cc:75-118).  Summation order: a row with at most 64 occurrences is summed
+ * sequentially in occurrence order (the CPU reference's order); a longer run is summed in 32-occurrence
+ * blocks aligned to its first occurrence, and the blocks are combined by a fixed tree whose shape
+ * depends on the run length, the row width (dim picks the lane group) and the call's occurrence count
+ * (which picks the tree depth: none up to 16 384 occurrences, one level up to 2^21, two above).  emb_offset_dev[m] is the float offset of
  * occurrence m's row inside grad_fused_dev (multiples of dim; total_floats = buffer length).
  * Destination rows that no occurrence refers to are left untouched.  dim % 4 == 0, dim <= 128. */
 int mono_scatter_grad_rows(int32_t device, const float* pooled_grad_dev, int64_t grad_stride,

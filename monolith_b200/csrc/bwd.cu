@@ -13,8 +13,9 @@
 //   4 runs    : run heads -> ordered run list (start, first position, resolved row)
 //   5 reduce  : seg_reduce_kernel streams the sorted occurrences in 32-occurrence pieces; runs of <= 64
 //               occurrences are summed in occurrence order (the CPU reference's order: bit-exact) and stored per run;
-//               hot FIDs are cut into run-aligned 32-occurrence blocks combined by a fixed 128-ary tree
-//               (deterministic, pairwise-accurate)
+//               hot FIDs are cut into run-aligned 32-occurrence blocks, combined by 0-2 levels of 128-member tree
+//               nodes (the depth follows the call's occurrence count) and a final in-order pass (deterministic,
+//               pairwise-accurate; tests/reduce_order.py restates the order)
 //   6 apply   : runs_apply_kernel streams the per-run sums and applies the optimizer, one row per run
 #include <algorithm>
 #include <cstring>
@@ -517,9 +518,12 @@ __device__ __forceinline__ float* run_dst(float* ugrad, int n_parts, const int64
 //   * a SHORT run (<= kShortRun occurrences of one FID) is one unit, summed sequentially in occurrence
 //     order = the CPU reference's order (bit-exact);
 //   * a LONG run (> kShortRun) is cut into 32-occurrence BLOCKS aligned to the START OF THE RUN; each block is
-//     one unit, summed sequentially; block sums are then combined by a fixed 32-ary tree over the block index
-//     (tree_level_kernel), so the association depends on the run length only: run-to-run bit-stable whatever
-//     scratch-set slot the FID got, and pairwise-accurate (checked against fp64 in tests/test_gpu_parity.py).
+//     one unit, summed sequentially; block sums are then combined over the block index by tree levels of
+//     kTreeFan-member nodes (tree_level_kernel; as many levels as keep the final pass at <= kFinishMax terms for the
+//     call's piece count) and the in-order final pass (long_finish_kernel).  The association depends on the run
+//     length, on G (the node's lane-group split) and on the call's tree depth, nothing else: run-to-run bit-stable
+//     whatever scratch-set slot the FID got, and pairwise-accurate (tests/reduce_order.py restates it;
+//     tests/test_gpu_reduce_order.py checks it bit for bit).
 // A group owns the units that START inside its piece and follows its last unit past the end of the piece (at most
 // 63 occurrences); occurrences in front of the first unit start belong to the previous group's last unit.  Every
 // group therefore streams 32 + <64 gradient rows whatever the run-length distribution is: hot FIDs of a Zipf
@@ -799,9 +803,9 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
 
 // One level of the fixed tree over the block index of the long runs: the slot of block k, k a multiple of
 // kTreeFan * stride, receives (in place) the sum of the slots of blocks k, k + stride, ..., k + (kTreeFan - 1) * stride.
-// A WARP owns a node: its 32 / G lane groups each sum a contiguous quarter (kTreeFan * G / 32 members, in block
-// order, 16 requests in flight per lane), then the group sums are added in group order through shuffles — the
-// association is a function of (run length, row width) only, so results are run-to-run bit-stable.  (One lane group
+// A WARP owns a node: its 32 / G lane groups each sum a contiguous share (kTreeFan * G / 32 members, in block
+// order, from 0, 16 requests in flight per lane), then the group sums are added in group order through shuffles —
+// the association is a function of (run length, row width, tree depth) only, so results are run-to-run bit-stable.  (One lane group
 // per node means 8 dependent stages of 16 loads: the hottest FIDs' chains become the kernel.)
 template <int G>
 __global__ void __launch_bounds__(kThreads)
@@ -866,7 +870,7 @@ tree_level_kernel(float* __restrict__ part, const SegMeta* __restrict__ meta, in
 }
 
 // Long runs, last step: the head slot of a long run combines what the tree left (blocks 0, top, 2 * top, ... — at most
-// 32 of them, in order) and stores the run's summed row to run_dst.
+// kFinishMax of them, in order) and stores the run's summed row to run_dst.
 template <int G>
 __global__ void __launch_bounds__(kThreads)
 long_finish_kernel(SegArgs sa, uint32_t top, const PeerOut po) {
@@ -1340,8 +1344,8 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
 // Deterministic replacement of the float-atomic scatter of pooled-row gradients
 // (ref: FusedGatherGradKernel, map_id_to_embedding.cu.cc:75-118; ScatterGrad,
 // fused_embedding_to_layout.h:286-347): out_rows[offs[m] : +dim] = sum over the occurrences m with that
-// offset of pooled_grad[row(m)] (or /n for MEAN), summed in occurrence order.  Rows of out_rows that
-// no occurrence points at are left untouched.
+// offset of pooled_grad[row(m)] (or /n for MEAN), in the reduce's order (occurrence order for <= 64
+// occurrences).  Rows of out_rows that no occurrence points at are left untouched.
 void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, const int32_t* row_offsets,
                       int64_t n_rows, int pooling, const float* pooled_grad, int64_t grad_stride,
                       int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s) {

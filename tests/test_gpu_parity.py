@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from tests import orc
+from tests import reduce_order as ro
 from tests.helpers import sgd_table, table
 
 pytestmark = pytest.mark.gpu
@@ -414,7 +415,8 @@ def test_gather_pool_fwd_bwd(dim, dev):
 
 @pytest.mark.parametrize("dim", [4, 16, 32, 128])
 def test_scatter_grad_rows_deterministic(dim, dev):
-  """Sort-based scatter == oracle ScatterGrad (sequential order) bit for bit on short runs, 2e-3 on hot rows."""
+  """Sort-based scatter == oracle ScatterGrad (sequential order) bit for bit on short runs; the hot row (thousands of
+  occurrences, block + tree order) bit for bit equal to tests/reduce_order.py."""
   from monolith_b200 import distribution_ops as dops
   rng = np.random.default_rng(dim * 3)
   U, R = 3000, 40000
@@ -433,7 +435,8 @@ def test_scatter_grad_rows_deterministic(dim, dev):
     cold = np.ones(U, bool)
     cold[7] = False
     np.testing.assert_array_equal(got[cold], want[cold])
-    np.testing.assert_allclose(got[7], want[7], rtol=2e-3, atol=2e-3)
+    _, model, _ = ro.call_sums(ro.occurrence_rows(pg, n, offs, pooling), u_of, ro.pick_group(dim))
+    np.testing.assert_array_equal(got.view(np.uint32), model.view(np.uint32))
     again = dops.scatter_grad_rows(T(pg, dev), T(eo, dev), dim, torch.zeros(U * dim, device=dev), T(offs, dev), pooling)
     np.testing.assert_array_equal(again.cpu().numpy().reshape(U, dim), got)  # bit-stable run to run
 
@@ -458,8 +461,10 @@ def test_owner_grouping_build_reduce(N, dev):
   want = orc.gather_pool_grad(pg, o, D, u.size * D).reshape(-1, D)        # oracle ScatterGrad in the same layout
   cnt = np.bincount(o // D, minlength=u.size)
   cold = cnt <= 64
+  assert (~cold).sum() >= 20
   np.testing.assert_array_equal(out[cold], want[cold])
-  np.testing.assert_allclose(out[~cold], want[~cold], rtol=2e-3, atol=2e-3)
+  _, model, _ = ro.call_sums(pg, o // D, ro.pick_group(D))                 # hot FIDs: block + tree order
+  np.testing.assert_array_equal(out.view(np.uint32), model.view(np.uint32))
   out2 = g.reduce(T(pg, dev), torch.empty(u.size * D, device=dev)).cpu().numpy().reshape(-1, D)
   np.testing.assert_array_equal(out, out2)
 
@@ -851,22 +856,16 @@ def test_pool_backward_vs_oracle(case, n, dev):
     gpu.pool_backward("t", T(fids, dev), T(pg, dev), None, "sum", req_time=10 + step)
     u, inv = orc.dedup(fids)
     ug = orc.gather_pool_grad(pg, inv * D, D, u.size * D).reshape(-1, D)
-    cpu.apply_gradients({"t": (u, ug)}, req_time=10 + step)
+    # FIDs that occur <= kShortRun (64) times are summed in the reference order (the oracle's ScatterGrad); the ~40
+    # hot FIDs (up to 60 K occurrences) in run-aligned blocks combined by the tree: the oracle gets those sums
+    _, model, cnt = ro.call_sums(pg, inv, ro.pick_group(D))
+    short = cnt <= ro.SHORT_RUN
+    np.testing.assert_array_equal(model[short].view(np.uint32), ug[short].view(np.uint32))
+    cpu.apply_gradients({"t": (u, model)}, req_time=10 + step)
   keys = cpu.keys("t")
   assert gpu.size("t") == keys.size
-  got, want = gpu_lookup(gpu, {"t": keys}, dev)["t"], cpu.lookup({"t": keys})["t"]
-  # FIDs that occur <= kShortRun (64) times per batch are summed in the reference order; the ~40 hot
-  # FIDs (up to 60 K occurrences) are summed piecewise, i.e. in a different association than the
-  # sequential CPU sum: fp32 reassociation error of a 60 K-term sum (the reference GPU path's float
-  # atomics have the same property, in random order).
-  hot = np.isin(keys, (np.int64(7) << 48) | np.arange(0, 40, dtype=np.int64))
-  np.testing.assert_allclose(got[~hot], want[~hot], rtol=2e-5, atol=1e-6)
-  np.testing.assert_allclose(got[hot], want[hot], rtol=2e-3, atol=2e-3)
-  # rows whose FID occurs at most kShortRun times are summed in the reference order: bit-exact
-  cnt = dict(zip(*np.unique(fids, return_counts=True)))
-  rare = np.array([k for k in keys if cnt.get(k, 0) <= 8][:2000], np.int64)
-  if n == 3000 and case[0] in ("adagrad32", "sgd8"):
-    np.testing.assert_array_equal(gpu_lookup(gpu, {"t": rare}, dev)["t"], cpu.lookup({"t": rare})["t"])
+  got = gpu.lookup_entry("t", T(keys, dev))["raw"].cpu().numpy()
+  np.testing.assert_array_equal(got.view(np.uint32), cpu.lookup_entry("t", keys).view(np.uint32))
   e = gpu.lookup_entry("t", T(keys[:100], dev))
   assert bool((e["last_update_ts_sec"] >= 10).all())
 
@@ -886,9 +885,15 @@ def test_pool_backward_csr_mean_and_determinism(dev):
     t.pool_backward("t", T(fids, dev), T(pg, dev), T(offs, dev), "mean", req_time=3)
   u, inv = orc.dedup(fids)
   ug = orc.gather_pool_grad(pg, inv * D, D, u.size * D, offs, "mean").reshape(-1, D)
-  cpu.apply_gradients({"t": (u, ug)}, req_time=3)
+  # hot FIDs (long MEAN runs: the divisor path past the piece end) summed in the model's block + tree order
+  _, model, cnt = ro.call_sums(ro.occurrence_rows(pg, fids.size, offs, "mean"), inv, ro.pick_group(D))
+  assert (cnt > ro.SHORT_RUN).sum() >= 5
+  np.testing.assert_array_equal(model[cnt <= ro.SHORT_RUN].view(np.uint32), ug[cnt <= ro.SHORT_RUN].view(np.uint32))
+  cpu.apply_gradients({"t": (u, model)}, req_time=3)
   got = gpu_lookup(gpu, {"t": u}, dev)["t"]
-  np.testing.assert_allclose(got, cpu.lookup({"t": u})["t"], rtol=2e-5, atol=1e-6)
+  np.testing.assert_array_equal(got.view(np.uint32), cpu.lookup({"t": u})["t"].view(np.uint32))
+  np.testing.assert_array_equal(gpu.lookup_entry("t", T(u, dev))["raw"].cpu().numpy().view(np.uint32),
+                                cpu.lookup_entry("t", u).view(np.uint32))
   np.testing.assert_array_equal(got, gpu_lookup(gpu2, {"t": u}, dev)["t"])  # run-to-run bit-stable
 
 
@@ -945,10 +950,11 @@ def test_sharding_sparse_fids_device_negative_fids_and_random(dev):
 # hot FIDs: which of the two fp32 sums is closer to the exact one?
 # ------------------------------------------------------------------------------------------------
 def test_hot_fid_gradient_sum_is_closer_to_fp64_than_the_sequential_cpu_sum(dev):
-  """A FID with 60 000 occurrences: the GPU reduces its gradient rows piecewise (1024-row pieces summed in order, pieces
-  combined in order), the CPU reference sums them sequentially in fp32.  Against the exact (fp64) sum the GPU result is
-  within 1e-5 of the sum's scale and at least as accurate as the sequential fp32 sum.  SGD with lr 1 on a zero-initialised
-  row makes the row equal to minus the summed gradient, so the sum itself is observable."""
+  """A FID with 60 000 occurrences: the GPU sums its gradient rows in run-aligned 32-row blocks, combines the blocks in
+  128-member tree nodes (one level for this call size) and adds the nodes in order (tests/reduce_order.py); the CPU
+  reference sums them sequentially in fp32.  Against the exact (fp64) sum the GPU result is within 1e-5 of the sum's
+  scale and at least as accurate as the sequential fp32 sum.  SGD with lr 1 on a zero-initialised row makes the row
+  equal to minus the summed gradient, so the sum itself is observable."""
   D, n = 32, 60000
   rng = np.random.default_rng(123)
   gpu, cpu = pair({"t": table([(D, "sgd", {})], [1.0])}, dev)
@@ -967,6 +973,8 @@ def test_hot_fid_gradient_sum_is_closer_to_fp64_than_the_sequential_cpu_sum(dev)
   assert err_gpu <= 1e-5 * np.abs(exact).max(), (err_gpu, np.abs(exact).max())
   assert err_gpu <= 5e-7 * scale
   assert err_gpu <= err_seq + 1e-12, (err_gpu, err_seq)
+  _, model, _ = ro.call_sums(pg, inv, ro.pick_group(D))
+  np.testing.assert_array_equal(got.astype(np.float32).view(np.uint32), model.view(np.uint32))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1160,9 +1168,9 @@ def test_sharded_direct_step_world1_vs_oracle(mode, dev):
 # ------------------------------------------------------------------------------------------------
 def test_bench_shape_step_vs_oracle(dev):
   """One full sparse step at the benchmark's batch shape (C2: 1 048 576 samples x 2 slots, Zipf(1.05) ranks, dim 32,
-  Adagrad) over a 1 M-key vocabulary: pooled rows bit for bit; after the fused backward every entry whose FID occurs
-  <= 64 times bit for bit (reference summation order), the hot FIDs within 1e-5 of the row's scale (tree vs sequential
-  fp32 sums; see the fp64 test above)."""
+  Adagrad) over a 1 M-key vocabulary: pooled rows bit for bit; after the fused backward every entry bit for bit, with
+  the oracle fed the gradient sums of tests/reduce_order.py (the reference order for FIDs that occur <= 64 times, run-
+  aligned blocks and one tree level for the hot ones)."""
   import bench
   D = 32
   from monolith_b200 import entry
@@ -1182,18 +1190,14 @@ def test_bench_shape_step_vs_oracle(dev):
   pg = rng.standard_normal((M, D)).astype(np.float32)
   gpu.pool_backward("t", T(fids, dev), T(pg, dev), None, "sum", req_time=7)
   u, inv = orc.dedup(fids)
-  ug = orc.gather_pool_grad(pg, inv * D, D, u.size * D).reshape(-1, D)
+  _, ug, cnt = ro.call_sums(pg, inv, ro.pick_group(D))
   cpu.apply_gradients({"t": (u, ug)}, req_time=7)
   assert gpu.size("t") == cpu.size("t") == vocab.size
   got = gpu.lookup_entry("t", T(vocab, dev))["raw"].cpu().numpy()
   want = cpu.lookup_entry("t", vocab)
-  cnt = np.bincount(np.searchsorted(vocab, fids), minlength=vocab.size)
   cold = cnt <= 64
-  assert cold.sum() > 0.95 * vocab.size and (~cold).sum() > 100
-  np.testing.assert_array_equal(got[cold].view(np.uint32), want[cold].view(np.uint32))
-  np.testing.assert_array_equal(got[~cold][:, -2:].view(np.uint32), want[~cold][:, -2:].view(np.uint32))
-  scale = np.abs(want[~cold][:, :-2]).max(axis=1, keepdims=True) + 1e-3
-  assert float((np.abs(got[~cold][:, :-2] - want[~cold][:, :-2]) / scale).max()) < 2e-3
+  assert cold.sum() > 0.95 * u.size and (~cold).sum() > 100
+  np.testing.assert_array_equal(got.view(np.uint32), want.view(np.uint32))
 
 
 def test_two_host_threads_share_one_handle(dev):
@@ -1341,8 +1345,9 @@ def test_streaming_insert_evict_50_steps_vs_oracle(dev):
   small enough to GROW under load (capacity 1024 against ~30 K keys), every step 5 % never-seen FIDs, a TTL eviction scan
   every 8 steps (one-day window, ref: CuckooEmbeddingHashTable::Evict via the bridge's eviction thread,
   embedding_hash_table_tf_bridge.cc:73-104).  After every eviction and at the end: membership, rows, optimizer state and
-  timestamps equal the oracle's — bit for bit for every FID that never had more than 64 occurrences in a step (freed rows
-  are reused, the bucket array is rehashed several times), within the tree-sum tolerance for the hot ones."""
+  timestamps equal the oracle's bit for bit (freed rows are reused, the bucket array is rehashed several times), with the
+  oracle fed the gradient sums of tests/reduce_order.py: hot FIDs (> 64 occurrences in a step) are summed in
+  run-aligned 32-row blocks, not sequentially."""
   from monolith_b200 import entry
   rng = np.random.default_rng(50)
   D, M = 8, 4200
@@ -1370,12 +1375,11 @@ def test_streaming_insert_evict_50_steps_vs_oracle(dev):
     u, inv = orc.dedup(ids)
     cnt = np.bincount(inv, minlength=u.size)
     hot_fids.update(u[cnt > 64].tolist())
-    cold = ~np.isin(ids, np.fromiter(hot_fids, np.int64, len(hot_fids)))
     pooled = gpu.lookup_pool("t", T(ids, dev), None, "sum").cpu().numpy()
-    np.testing.assert_array_equal(pooled[cold].view(np.uint32), cpu.lookup({"t": ids})["t"][cold].view(np.uint32))
+    np.testing.assert_array_equal(pooled.view(np.uint32), cpu.lookup({"t": ids})["t"].view(np.uint32))
     g = rng.standard_normal((M, D)).astype(np.float32)
     gpu.pool_backward("t", T(ids, dev), T(g, dev), None, "sum", req_time=now)
-    ug = orc.gather_pool_grad(g, inv * D, D, u.size * D).reshape(-1, D)
+    _, ug, _ = ro.call_sums(g, inv, ro.pick_group(D))
     cpu.apply_gradients({"t": (u, ug)}, req_time=now)
     if (step + 1) % 8 == 0:
       gpu.evict("t", now)
@@ -1389,6 +1393,4 @@ def test_streaming_insert_evict_50_steps_vs_oracle(dev):
   ec = cpu.lookup_entry("t", keys)
   hot = np.isin(keys, np.fromiter(hot_fids, np.int64, len(hot_fids)))
   assert 0 < hot.sum() < 200
-  np.testing.assert_array_equal(eg[~hot].view(np.uint32), ec[~hot].view(np.uint32))
-  np.testing.assert_allclose(eg[hot][:, :-2], ec[hot][:, :-2], rtol=2e-3, atol=2e-4)
-  np.testing.assert_array_equal(eg[hot][:, -2:].view(np.uint32), ec[hot][:, -2:].view(np.uint32))
+  np.testing.assert_array_equal(eg.view(np.uint32), ec.view(np.uint32))
