@@ -143,6 +143,9 @@ void launch_gather_pool(const float* fused_emb, const int32_t* emb_offset, const
                         int out_col, cudaStream_t s) {
   if (n_rows <= 0) return;
   if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN) throw ArgError("gather_pool: SUM or MEAN");
+  // One occurrence per output row: MEAN is x / 1, the identity, except that the division would replace a NaN's payload
+  // with the canonical NaN.  Pool as SUM (a copy), so every width keeps all 32 bits, as gather_rows_kernel does.
+  if (row_offsets == nullptr) pooling = MONO_POOL_SUM;
   const int G = pick_group(dim);
   if (row_offsets == nullptr && (dim & 3) == 0 && dim <= 4 * G && (out_stride & 3) == 0 && (out_col & 3) == 0 &&
       ((reinterpret_cast<uintptr_t>(fused_emb) | reinterpret_cast<uintptr_t>(out)) & 15) == 0) {

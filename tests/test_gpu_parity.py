@@ -266,7 +266,7 @@ def test_multi_table_multi_segment_parity(dev):
   got = gpu_lookup(gpu, vocab, dev)
   want = cpu.lookup(vocab)
   for k in vocab:
-    np.testing.assert_array_equal(got[k], want[k])
+    np.testing.assert_array_equal(got[k].view(np.uint32), want[k].view(np.uint32))
     eg = gpu.lookup_entry(k, T(vocab[k], dev))["raw"].cpu().numpy()
     np.testing.assert_array_equal(eg.view(np.uint32), cpu.lookup_entry(k, vocab[k]).view(np.uint32))
 
@@ -340,11 +340,12 @@ def test_lookup_pool_bit_exact(dim, pooling, dev):
   offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
   fids = rng.choice(np.concatenate([vocab, vocab[:200] + 1]), size=int(offs[-1]))
   got = gpu.lookup_pool("t", T(fids, dev), T(offs, dev), pooling).cpu().numpy()
-  np.testing.assert_array_equal(got, cpu.lookup_pool("t", fids, offs, pooling))
+  np.testing.assert_array_equal(got.view(np.uint32), cpu.lookup_pool("t", fids, offs, pooling).view(np.uint32))
   # one FID per row (no offsets), written into a wider buffer at a column offset
   out = torch.full((fids.size, dim + 8), -1.0, device=dev)
   gpu.lookup_pool("t", T(fids, dev), None, pooling, out=out, out_col=4)
-  np.testing.assert_array_equal(out[:, 4:4 + dim].cpu().numpy(), cpu.lookup_pool("t", fids, None, pooling))
+  np.testing.assert_array_equal(out[:, 4:4 + dim].cpu().numpy().view(np.uint32),
+                                cpu.lookup_pool("t", fids, None, pooling).view(np.uint32))
   assert bool((out[:, :4] == -1).all()) and bool((out[:, 4 + dim:] == -1).all())
 
 
@@ -679,7 +680,8 @@ def test_growth_from_tiny_capacity(dev):
     gpu.apply_gradients({"t": (T(chunk, dev), T(g, dev))}, req_time=5, ids_unique=True)
     cpu.apply_gradients({"t": (chunk, g)}, req_time=5)
   assert gpu.size("t") == allk.size == cpu.size("t")
-  np.testing.assert_array_equal(gpu_lookup(gpu, {"t": allk}, dev)["t"], cpu.lookup({"t": allk})["t"])
+  np.testing.assert_array_equal(gpu_lookup(gpu, {"t": allk}, dev)["t"].view(np.uint32),
+                                cpu.lookup({"t": allk})["t"].view(np.uint32))
   assert bool(gpu.contains("t", T(allk[:1000], dev)).all())
   assert not bool(gpu.contains("t", T(allk[:1000] ^ 1, dev)).any()) or True  # xor may collide with a real key
   keys = torch.cat([ids for ids, _ in gpu.export("t", chunk=1 << 16)]).cpu().numpy()
@@ -692,7 +694,7 @@ def test_special_keys(dev):
   v = np.arange(12, dtype=np.float32).reshape(6, 2)
   gpu.assign({"t": (T(ks, dev), T(v, dev))}, req_time=3)
   cpu.assign({"t": (ks, v)}, req_time=3)
-  np.testing.assert_array_equal(gpu_lookup(gpu, {"t": ks}, dev)["t"], v)
+  np.testing.assert_array_equal(gpu_lookup(gpu, {"t": ks}, dev)["t"].view(np.uint32), v.view(np.uint32))
   assert gpu.size("t") == 6 == cpu.size("t")
 
 
