@@ -94,20 +94,20 @@ def k_gather(d, csr, rows_ok=True):
 # ------------------------------------------------------------------------------------------------
 # running a case: profiled once (kernel names), then again (determinism)
 # ------------------------------------------------------------------------------------------------
-def _canon(name):
+def _canon(name, family=FAMILY):
   m = re.search(r"(\w+)(<[^()]*?>)?\(", name)
-  if not m or m.group(1) not in FAMILY:
+  if not m or m.group(1) not in family:
     return None
   return m.group(1) + (m.group(2) or "").replace(" ", "")
 
 
-def traced(fn):
-  """-> (fn(), names of the forward kernels torch.profiler recorded while it ran)."""
+def traced(fn, family=FAMILY):
+  """-> (fn(), names of the kernels of `family` (default: the forward's) torch.profiler recorded while it ran)."""
   torch.cuda.synchronize()
   with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
     out = fn()
     torch.cuda.synchronize()
-  return out, {c for c in (_canon(e.name) for e in prof.events()) if c}
+  return out, {c for c in (_canon(e.name, family) for e in prof.events()) if c}
 
 
 def _bytes(out):
@@ -115,8 +115,9 @@ def _bytes(out):
   return [np.ascontiguousarray(o).view(np.uint8) for o in outs]
 
 
-def run(fn, expect):
-  """fn() -> numpy array(s).  Asserts the forward kernels it launched are exactly `expect`.
+def run(fn, expect, family=FAMILY, seen=SEEN):
+  """fn() -> numpy array(s).  Asserts the kernels of `family` it launched are exactly `expect` and adds them to
+  `seen`.  fn is called several times, so a case that changes state builds it from scratch inside fn.
 
   torch.profiler now and then loses a whole batch of device records (a few traces in a thousand, two or three in
   a row; the traces after them are complete).  A lost record can only make a kernel MISSING from a trace, never add
@@ -124,10 +125,10 @@ def run(fn, expect):
   once, and a case that really launches less than `expect` fails after ten traces."""
   expect = {expect} if isinstance(expect, str) else set(expect)
   for _ in range(10):
-    out, names = traced(fn)
+    out, names = traced(fn, family)
     if not names < expect:
       break
-  SEEN.update(names)
+  seen.update(names)
   assert names == expect, f"ran {sorted(names)}, aimed at {sorted(expect)}"
   for a, b in zip(_bytes(out), _bytes(fn())):
     np.testing.assert_array_equal(a, b, err_msg="not bit-stable run to run")

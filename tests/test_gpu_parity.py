@@ -1108,59 +1108,51 @@ def test_hash_filter_paths_vs_oracle(dev):
 # ------------------------------------------------------------------------------------------------
 # device-driven sharded step (csrc/xstep.cu) with world = 1: the whole flag / header / window protocol against itself
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("mode", ["one_fid_per_row", "csr_mean"])
-def test_sharded_direct_step_world1_vs_oracle(mode, dev):
+SHARDED_OPTS = [("adagrad", {}), ("amsgrad", {"use_nesterov": True, "weight_decay_factor": 0.01})]
+
+
+@pytest.mark.parametrize("mode,opt", [(m, o) for o in SHARDED_OPTS for m in ("one_fid_per_row", "csr_mean")],
+                         ids=["one_fid_per_row", "csr_mean", "amsgrad-one_fid_per_row", "amsgrad-csr_mean"])
+def test_sharded_direct_step_world1_vs_oracle(mode, opt, dev):
+  """Adagrad (the owner's apply takes apply_row's float4 path) and AMSGrad (the generic path): the forward output and
+  every entry bit for bit, the hot FID included, with the oracle fed the sums of tests/reduce_order.py."""
   from monolith_b200 import MultiHashTable
   from monolith_b200.distributed_ps import ShardedStep
   D = 16
-  cfg = {"t": table([(D, "adagrad", {})], [0.1])}
+  cfg = {"t": table([(D, opt[0], opt[1])], [0.1 if opt[0] == "adagrad" else 0.01])}
   gpu, cpu = pair(cfg, dev)
   st = ShardedStep(gpu, "t", D, 1, 0, dev, exchange="direct")
   rng = np.random.default_rng(31)
-  hot = fid(5, 3)
   batches = []
   for step in range(5):
     n = 6000 + (500 * step if step < 3 else 1000)                # growing batches: the window is re-created once or twice
     ids = rng.integers(0, 900 + 50 * step, n)
-    ids[rng.random(n) < 0.25] = 3                                # hot FID: a > 64-occurrence run (tree-reduced)
+    ids[rng.random(n) < 0.25] = 3                                # hot FID: a > 64-occurrence run (block-reduced)
     fids = (np.int64(5) << 48) | ids.astype(np.int64)
     if mode == "csr_mean":
       lens = rng.integers(0, 5, n)
-      ro = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
-      ro = ro[ro <= n]
-      ro[-1] = n
-      R, pool = ro.size - 1, "mean"
+      offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+      offs = offs[offs <= n]
+      offs[-1] = n
+      R, pool = offs.size - 1, "mean"
     else:
-      ro, R, pool = None, n, "sum"
-    batches.append((fids, ro, R, pool, rng.standard_normal((R, D)).astype(np.float32), T(fids, dev)))
+      offs, R, pool = None, n, "sum"
+    batches.append((fids, offs, R, pool, rng.standard_normal((R, D)).astype(np.float32), T(fids, dev)))
   try:
-    for step, (fids, ro, R, pool, g, f_dev) in enumerate(batches):
+    for step, (fids, offs, R, pool, g, f_dev) in enumerate(batches):
       out = torch.empty(R, D, device=dev)
-      st.step(f_dev, T(g, dev), out, 20 + step, None if ro is None else T(ro, dev), pool)
+      st.step(f_dev, T(g, dev), out, 20 + step, None if offs is None else T(offs, dev), pool)
       if step + 1 < len(batches):
         st.prepare(batches[step + 1][5])                           # next batch's grouping on a side stream (same tensor object)
-      want = cpu.lookup_pool("t", fids, ro, pool)
-      got = out.cpu().numpy()
-      if ro is None:
-        cold = fids != hot
-        np.testing.assert_array_equal(got[cold].view(np.uint32), want[cold].view(np.uint32))
-        np.testing.assert_allclose(got[~cold], want[~cold], rtol=2e-3, atol=2e-3)
-      else:
-        np.testing.assert_allclose(got, want, rtol=2e-3, atol=2e-3)
-      u, inv = orc.dedup(fids)
-      ug = orc.gather_pool_grad(g, inv * D, D, u.size * D, ro, pool).reshape(-1, D)
+      want = cpu.lookup_pool("t", fids, offs, pool)
+      np.testing.assert_array_equal(out.cpu().numpy().view(np.uint32), want.view(np.uint32))
+      x = ro.occurrence_rows(g, fids.size, offs, pool)
+      u, ug, _ = ro.call_sums(x, fids, ro.pick_group(D))
       cpu.apply_gradients({"t": (u, ug)}, req_time=20 + step)
     keys = cpu.keys("t")
     assert gpu.size("t") == keys.size
     got = gpu.lookup_entry("t", T(keys, dev))["raw"].cpu().numpy()
-    want = cpu.lookup_entry("t", keys)
-    cold = keys != hot
-    if mode == "one_fid_per_row":
-      np.testing.assert_array_equal(got[cold].view(np.uint32), want[cold].view(np.uint32))
-    else:
-      np.testing.assert_allclose(got[cold][:, :-2], want[cold][:, :-2], rtol=2e-5, atol=1e-6)
-    np.testing.assert_allclose(got[~cold][:, :-2], want[~cold][:, :-2], rtol=2e-3, atol=2e-3)
-    np.testing.assert_array_equal(got[:, -2:].view(np.uint32), want[:, -2:].view(np.uint32))
+    np.testing.assert_array_equal(got.view(np.uint32), cpu.lookup_entry("t", keys).view(np.uint32))
   finally:
     st.close_direct()
 
