@@ -193,6 +193,55 @@ int mono_mtable_pool_backward(mono_mtable_t* t, int32_t k, const int64_t* fids_d
                               const float* learning_rate_host /*[slice_size(k)]*/,
                               int64_t update_time, int64_t global_step, void* stream);
 
+/* ---- fused forward and backward over many features and tables in one call ------------------
+ * A part is one feature's slice of a step: FIDs of table `table`, pooled by `pooling` into rows
+ * (row_offsets_dev as for mono_mtable_lookup_pool, NULL = one FID per row and then n_rows == n_fids);
+ * row r is rows_dev + r*stride + col: the forward's output row, the backward's row gradient.
+ *
+ * mono_mtable_lookup_pool_parts: every part's output is bit-identical to mono_mtable_lookup_pool on
+ * that part alone (any dim up to 512, CSR or one-FID rows, SUM or MEAN, any stride and column; parts
+ * may write disjoint columns of one tensor).  Kernel launches: one per distinct kernel instantiation
+ * among the parts (the kernel mono_mtable_lookup_pool would pick for each), not one per part.
+ * MONO_ERR_INVALID_ARGUMENT, before any device work: n_parts outside [0, MONO_MAX_POOL_PARTS], a bad
+ * table index, dim > 512, pooling other than SUM or MEAN, n_rows != n_fids without offsets.
+ *
+ * mono_mtable_pool_backward_parts: for every table named by some part, the occurrences
+ * of all its parts are ONE batch, taken in part order and then occurrence order, as the reference's
+ * per-table ScatterGrad sees them: each distinct FID of the table gets one upsert, one timestamp bump,
+ * one admission-filter count and one optimizer step with the sum of its terms (a term is the part's
+ * row gradient, divided by the row's n for a CSR MEAN part).  The sum is associated as for
+ * mono_mtable_pool_backward, with the tree depth set by the table's occurrence count in the call, so
+ * parts of one table with one pooling give exactly the bits of one mono_mtable_pool_backward over
+ * their concatenated FIDs, stacked gradient rows and rebased row offsets.  Tables do not interact.
+ * learning_rate_host has sum_k slice_size(k) floats for ALL tables, table order (as optimize).
+ * Kernel launches: 1 occurrence map + 1 claim + 1 miss + 1 finalize + 3 per radix pass + 3 run list,
+ * then per distinct table k of the call 3 + L(k) (reduce, L(k) tree levels, finish, apply), where
+ * passes = ceil(bits / 11) for bits = ceil(log2(sum_k claim slots(k))), claim slots(k) = the smallest
+ * power of two >= max(1024, 2 M(k)), L(k) = 0 for M(k) <= 16384 occurrences, 1 up to 2^21, else 2.
+ * MONO_ERR_INVALID_ARGUMENT, before any device work (no table changes): n_parts outside
+ * [0, MONO_MAX_POOL_PARTS], a bad table index, a part whose table breaks the pool_backward conditions
+ * (dim % 4 == 0, dim <= 128, 16-byte aligned gradient rows), pooling other than SUM or MEAN,
+ * n_rows != n_fids without offsets, or more than 2^30 occurrences in total.  No host sync. */
+#define MONO_MAX_POOL_PARTS 1024
+
+typedef struct mono_pool_part {
+  int32_t table;                    /* k, sorted-name index                                   */
+  const int64_t* fids_dev;
+  int64_t n_fids;
+  const int32_t* row_offsets_dev;   /* [n_rows+1] or NULL = one FID per row                   */
+  int64_t n_rows;
+  int32_t pooling;                  /* MONO_POOL_SUM | MONO_POOL_MEAN                          */
+  float* rows_dev;                  /* forward: output rows; backward: pooled-row gradients   */
+  int64_t stride;                   /* floats between rows                                    */
+  int32_t col;                      /* first column of the table's dim(k) floats in a row     */
+} mono_pool_part;
+
+int mono_mtable_lookup_pool_parts(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                  void* stream);
+int mono_mtable_pool_backward_parts(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                    const float* learning_rate_host /*[sum_k slice_size(k)]*/,
+                                    int64_t update_time, int64_t global_step, void* stream);
+
 /* ---- updates ----------------------------------------------------------------------------- */
 
 #define MONO_FLAG_IDS_UNIQUE 1u      /* caller guarantees ids unique per table within this call   */

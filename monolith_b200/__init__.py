@@ -7,6 +7,6 @@ C ABI of include/mono_emb.h, and a host-side mirror of the reference's Python in
 There is no CPU fallback: compute entry points raise when the CUDA library or a GPU is missing.
 """
 from . import entry  # noqa: F401
-from .multi_hash_table_ops import MultiHashTable  # noqa: F401
+from .multi_hash_table_ops import MultiHashTable, PoolPart  # noqa: F401
 
-__all__ = ["entry", "MultiHashTable"]
+__all__ = ["entry", "MultiHashTable", "PoolPart"]

@@ -29,6 +29,13 @@ class SliceTask(C.Structure):  # mono_slice_task
               ("out_row_stride", C.c_int32), ("out_col", C.c_int32), ("accumulate", C.c_int32)]
 
 
+class PoolPartC(C.Structure):  # mono_pool_part
+  _fields_ = [("table", C.c_int32), ("fids_dev", C.c_void_p), ("n_fids", C.c_int64),
+              ("row_offsets_dev", C.c_void_p), ("n_rows", C.c_int64), ("pooling", C.c_int32),
+              ("rows_dev", C.c_void_p), ("stride", C.c_int64), ("col", C.c_int32)]
+
+
+MAX_POOL_PARTS = 1024  # MONO_MAX_POOL_PARTS
 OPT_SGD, OPT_ADAGRAD, OPT_FTRL, OPT_ADAM = 0, 1, 2, 3
 OPT_MOMENTUM, OPT_RMSPROP, OPT_RMSPROPV2, OPT_ADADELTA, OPT_AMSGRAD = 4, 5, 6, 7, 8
 OPT_MOVING_AVERAGE, OPT_GROUP_ADAGRAD = 9, 10
@@ -71,6 +78,8 @@ SIGNATURES = {
     "mono_mtable_contains": (C.c_int, [_p, _i32, _p, _i64, _p, _p]),
     "mono_mtable_lookup_pool": (C.c_int, [_p, _i32, _p, _p, _i64, _i32, _p, _i64, _i32, _p]),
     "mono_mtable_pool_backward": (C.c_int, [_p, _i32, _p, _i64, _p, _i64, _i32, _p, _i64, _i32, _p, _i64, _i64, _p]),
+    "mono_mtable_lookup_pool_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p]),
+    "mono_mtable_pool_backward_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p]),
     "mono_mtable_optimize": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i64, _u32, _p]),
     "mono_mtable_fused_optimize": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i32, _u32, _p]),
     "mono_mtable_assign": (C.c_int, [_p, _p, _p, _p, _i64, _u32, _p]),

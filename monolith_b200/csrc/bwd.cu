@@ -383,6 +383,12 @@ struct BwdArgs {
   const float* pooled_grad;
   int64_t grad_stride;
   int grad_col;
+  // parts call (run_pool_backward_parts): one table's occurrences are the sorted range [lo, n); each occurrence's
+  // gradient row and MEAN divisor (0: none) come from the call's occurrence map, its run range from run_of_sorted
+  int64_t lo;
+  const float* const* occ_src;
+  const float* occ_div;
+  const uint32_t* run_of_sorted;
   const float* lr;              // device, slice learning rates of the table
   float* ugrad;                 // [runs][D] summed gradient of every run (= unique FID), run order
   float* scratch;               // alias of ugrad for the generic (multi-segment) apply path
@@ -395,6 +401,8 @@ struct GradSrc {
   int64_t stride;
   const uint32_t* occ_row;
   const int32_t* row_offsets;
+  const float* const* occ_src;  // parts call: gradient row (column included) of every occurrence
+  const float* occ_div;         // parts call: MEAN divisor of every occurrence, 0 = none
   bool mean;
 };
 __device__ __forceinline__ GradSrc make_grad_src(const BwdArgs& a, int c) {
@@ -403,7 +411,9 @@ __device__ __forceinline__ GradSrc make_grad_src(const BwdArgs& a, int c) {
   g.stride = a.grad_stride;
   g.occ_row = a.occ_row;
   g.row_offsets = a.row_offsets;
-  g.mean = a.pooling == MONO_POOL_MEAN && a.row_offsets != nullptr;
+  g.occ_src = a.occ_src;
+  g.occ_div = a.occ_div;
+  g.mean = a.pooling == MONO_POOL_MEAN && (a.row_offsets != nullptr || a.occ_div != nullptr);
   return g;
 }
 // gradient row of occurrence m, columns c..c+3
@@ -547,10 +557,11 @@ struct SegMeta {  // one per partial slot
 
 struct SegArgs {
   BwdArgs b;                        // gradient source, table, run list (run_start / rowidx / run_first_pos)
-  const uint32_t* piece_run_base;   // [ceil(M/32)]: number of run heads in front of piece p
+  const uint32_t* piece_run_base;   // [n_pieces]: number of run heads in front of piece p of the range
   float* part;                      // [2 * n_pieces][D]
   SegMeta* meta;                    // [2 * n_pieces]
-  int64_t n_pieces;
+  int64_t n_pieces;                 // pieces of the range [b.lo, b.n) of the sorted list
+  int64_t piece0;                   // the range's first piece in the sorted list (b.lo / 32)
 };
 
 template <int EPL>
@@ -654,7 +665,7 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
   for (int64_t p0 = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * RPI; p0 < sa.n_pieces; p0 += wstride) {
     const int64_t p = p0 + grp;
     if (p >= sa.n_pieces) continue;  // whole groups leave together: the shuffles below use the group mask only
-    const int64_t base = p * kPiece;
+    const int64_t base = (sa.piece0 + p) * kPiece;
     // ---- lane-parallel loads: the piece's sort keys and positions, the run index in front of the piece ----
     uint32_t pm0[EPL], sk[EPL];
     load_items<G>(a.sorted, base, M, sk, pm0);
@@ -666,7 +677,7 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
       load_items<G>(a.sorted, base + kPiece, M, skx, reinterpret_cast<uint32_t (&)[EPL]>(pm1));
       load_items<G>(a.sorted, base + 2 * kPiece, M, skx, reinterpret_cast<uint32_t (&)[EPL]>(pm2));
     }
-    const uint32_t j0 = sa.piece_run_base[p];
+    uint32_t j0 = sa.piece_run_base[p];
     uint32_t sk_prev = __shfl_up_sync(gmask, sk[EPL - 1], 1, G);
     if (gl == 0) sk_prev = base > 0 ? a.sorted[base - 1].x : ~sk[0];
     uint32_t hb = 0;
@@ -676,7 +687,14 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
       const uint32_t before = q == 0 ? sk_prev : sk[q - 1];
       if (i < M && (i == 0 || sk[q] != before)) hb |= 1u << q;
     }
-    const uint32_t H = __reduce_or_sync(gmask, hb << (gl * EPL));  // run heads inside the piece
+    uint32_t H = __reduce_or_sync(gmask, hb << (gl * EPL));  // run heads inside the piece
+    // a range that starts inside the piece (parts call): the heads in front of it are another table's runs
+    const bool lead_ok = base >= a.lo;
+    if (!lead_ok) {
+      const uint32_t foreign = (1u << (uint32_t)(a.lo - base)) - 1u;  // a.lo - base < 32: the range's first piece
+      j0 += __popc(H & foreign);
+      H &= ~foreign;
+    }
     const int nheads = __popc(H);
     const int nvalid = (int)min((int64_t)kPiece, M - base);
     // run boundaries around the piece (three independent loads)
@@ -688,7 +706,7 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
     uint32_t S = H;                                                  // unit starts
     int lead_o = -1;                                                 // start of the leading long-run block, if any
     uint32_t lead_k = 0, lead_nb = 0;
-    if (e_first > 0 && rs_0 - rs_prev > (uint32_t)kShortRun) {
+    if (lead_ok && e_first > 0 && rs_0 - rs_prev > (uint32_t)kShortRun) {
       const uint32_t into = (uint32_t)base - rs_prev;                // occurrences of that run in front of the piece
       const int o = (int)((kPiece - (into & (kPiece - 1))) & (kPiece - 1));
       if (o < e_first) {
@@ -740,7 +758,7 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
           const int e = eb + u;
           if (e >= e_begin && e < e_stop) {
             const uint32_t r = (!PLAIN && gs.occ_row) ? gs.occ_row[m[u]] : m[u];
-            const float* src = gs.base + (size_t)r * gs.stride;
+            const float* src = (!PLAIN && gs.occ_src) ? gs.occ_src[m[u]] + c : gs.base + (size_t)r * gs.stride;
 #pragma unroll
             for (int v = 0; v < VPL; ++v)
               if (in[v]) cp_async16(&stage[(b4 + u) * VPL + v][threadIdx.x], src + v * G * 4);
@@ -769,7 +787,7 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
             const uint32_t r = gs.occ_row ? gs.occ_row[m[u]] : m[u];
-            fn[u] = (float)(gs.row_offsets[r + 1] - gs.row_offsets[r]);
+            fn[u] = gs.occ_div ? gs.occ_div[m[u]] : (float)(gs.row_offsets[r + 1] - gs.row_offsets[r]);
           }
         }
 #pragma unroll
@@ -780,7 +798,7 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
           for (int v = 0; v < VPL; ++v) {
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
             if (in[v]) x = stage[(b4 + u) * VPL + v][threadIdx.x];
-            if (!PLAIN && gs.mean) {
+            if (!PLAIN && gs.mean && fn[u] != 0.f) {
               x.x = __fdiv_rn(x.x, fn[u]); x.y = __fdiv_rn(x.y, fn[u]); x.z = __fdiv_rn(x.z, fn[u]); x.w = __fdiv_rn(x.w, fn[u]);
             }
             if ((st4 >> u) & 1u) acc[v] = x; else add4(acc[v], x);
@@ -913,10 +931,14 @@ template <int G, int OPT>
 __global__ void __launch_bounds__(kThreads) runs_apply_kernel(BwdArgs a, int prefetch) {
   const int gl = Group<G>::gl();
   const int c = gl * 4;
-  const int64_t nr = *a.n_runs;
+  int64_t j_lo = 0, nr = *a.n_runs;
+  if (a.run_of_sorted) {  // parts call: the runs of the sorted range [lo, n)
+    j_lo = a.run_of_sorted[a.lo];
+    nr = (int64_t)a.run_of_sorted[a.n - 1] + 1;
+  }
   const int D = a.td.dim;
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
-  int64_t j = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
+  int64_t j = j_lo + (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
   uint32_t ri_next = j < nr ? a.rowidx[j] : kEmptyRow;
   for (; j < nr; j += gstride) {
     const uint32_t ri = ri_next;
@@ -965,11 +987,35 @@ __global__ void __launch_bounds__(kThreads) runs_emit_kernel(BwdArgs a, int shif
 // resolves the FID in the table right away — lane-level probe, expiry-timestamp bump
 // (ref: entry.SetTimestamp(update_time), cuckoo_embedding_hash_table.cc:243), row index parked in the set
 // entry; absent FIDs are queued (set slot) for claim_miss_kernel.  No separate resolve pass over the uniques.
+// One table of a parts call: its occurrences are [occ_begin, occ_end) of the table-major concatenation, its FIDs
+// are claimed in the set's slots [slot_base, slot_base + slots)
+struct CallTable {
+  int64_t occ_begin, occ_end;
+  uint32_t slot_base, slots;
+  int32_t table, pad;
+};
+// Linear scans over the call's tables: a multi-table merges slots of one config, so K is a handful (2-5 in Monolith
+// models) and the regions array stays in L1.
+__device__ __forceinline__ int call_table_of_occ(const CallTable* __restrict__ rg, int n, int64_t i) {
+  int r = 0;
+  while (r + 1 < n && i >= rg[r].occ_end) ++r;
+  return r;
+}
+__device__ __forceinline__ int call_table_of_slot(const CallTable* __restrict__ rg, int n, uint32_t slot) {
+  int r = 0;
+  while (r + 1 < n && slot >= rg[r + 1].slot_base) ++r;
+  return r;
+}
+
 struct ClaimResolve {
-  const TableDev* t;
-  uint32_t update_ts;
-  uint32_t* miss_ctr;
-  uint32_t* miss_slots;
+  const TableDev* t = nullptr;
+  uint32_t update_ts = 0;
+  uint32_t* miss_ctr = nullptr;
+  uint32_t* miss_slots = nullptr;
+  // parts call: occurrence i belongs to the call table whose [occ_begin, occ_end) holds it; it claims in that table's
+  // region of the set and resolves in tables[table]; null: one region per owner (key mod N), table t
+  const CallTable* regions = nullptr;
+  int n_regions = 0;
 };
 
 template <bool RESOLVE, bool DUAL = false>
@@ -997,7 +1043,7 @@ fid_claim_kernel(const int64_t* __restrict__ fids, int64_t n, Entry* set, uint32
     const int64_t key = key_next;
     if (i + stride < n) {
       key_next = __ldg(fids + i + stride);
-      if (prefetch) {
+      if (prefetch && !cr.regions) {
         const uint32_t o_n = N == 1 ? 0u : (uint32_t)((uint64_t)key_next % (uint64_t)N);
         prefetch_l2(set + o_n * R + __umulhi((uint32_t)(mix64((uint64_t)key_next) >> 24), R));
         if (RESOLVE) {
@@ -1008,7 +1054,14 @@ fid_claim_kernel(const int64_t* __restrict__ fids, int64_t n, Entry* set, uint32
       }
     }
     const uint32_t owner = N == 1 ? 0u : (uint32_t)((uint64_t)key % (uint64_t)N);
-    const uint32_t base = owner * R;
+    uint32_t base = owner * R;
+    const TableDev* tk = cr.t;
+    if (cr.regions) {
+      const CallTable& rg = cr.regions[call_table_of_occ(cr.regions, cr.n_regions, i)];
+      base = rg.slot_base;
+      R = rg.slots;
+      tk = cr.t + rg.table;
+    }
     uint32_t idx = __umulhi((uint32_t)(mix64((uint64_t)key) >> 24), R);
     uint32_t found = 0xFFFFFFFFu;
     bool won = false;
@@ -1044,7 +1097,7 @@ fid_claim_kernel(const int64_t* __restrict__ fids, int64_t n, Entry* set, uint32
       atomicAdd(&cnt[owner], 1u);
       if (RESOLVE) {
         Entry* slot = nullptr;
-        const uint32_t row = probe_lane_slot<DUAL>(cr.t, key, &slot);
+        const uint32_t row = probe_lane_slot<DUAL>(tk, key, &slot);
         if (row != kEmptyRow) {
           slot->ts = cr.update_ts;
           set[found].row = row;
@@ -1062,11 +1115,13 @@ fid_claim_kernel(const int64_t* __restrict__ fids, int64_t n, Entry* set, uint32
 // FIDs the claim found absent from the table (each exactly once): take a row (free list first, then the bump
 // allocator), publish {fid, row, ts} with the lock-free cuckoo insert and park row | fresh in the set entry.
 __global__ void __launch_bounds__(kThreads)
-claim_miss_kernel(const TableDev* __restrict__ t, Entry* set, const uint32_t* __restrict__ miss_ctr,
-                  const uint32_t* __restrict__ miss_slots, uint32_t update_ts) {
+claim_miss_kernel(const TableDev* __restrict__ tables, Entry* set, const uint32_t* __restrict__ miss_ctr,
+                  const uint32_t* __restrict__ miss_slots, uint32_t update_ts,
+                  const CallTable* __restrict__ regions /* parts call: the slot's table; null: tables[0] */, int n_regions) {
   const int64_t n = (int64_t)*miss_ctr;
   for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x) {
     const uint32_t sl = miss_slots[q];
+    const TableDev* t = regions ? tables + regions[call_table_of_slot(regions, n_regions, sl)].table : tables;
     // admission filter: the backward hands every distinct FID once per step (count 1), as the reference's
     // deduplicated optimize does; a FID below its slot's threshold gets no row (its run is skipped by the apply)
     if (should_be_filtered(t, ld_entry_cg(set + sl).key, 1u)) continue;
@@ -1093,7 +1148,10 @@ claim_miss_kernel(const TableDev* __restrict__ t, Entry* set, const uint32_t* __
 static const PeerOut no_peer = {};  // n == 0: the reduce writes the local ugrad buffer
 
 // Optional parts of the pipeline scratch (scratch_plan)
-enum : unsigned { kPartK0 = 1, kPartRowIdx = 2, kPartMiss = 4, kPartOcc = 8, kPartRunOfSorted = 16, kPartUGrad = 32 };
+enum : unsigned {
+  kPartK0 = 1, kPartRowIdx = 2, kPartMiss = 4, kPartOcc = 8, kPartRunOfSorted = 16, kPartUGrad = 32,
+  kPartOccMap = 64  // parts call: concatenated FIDs, gradient row and MEAN divisor of every occurrence
+};
 
 // Layout of the pipeline scratch for M occurrences of dim D sorted on `bits` key bits: one 256-byte aligned region
 // per part, the optional ones only when `parts` asks for them.  base == nullptr only sizes it (.bytes).
@@ -1126,6 +1184,9 @@ static BwdScratch scratch_plan(int64_t M, int D, int bits, unsigned parts, char*
   w.part = (float*)take(sizeof(float) * 2 * (size_t)w.n_pieces * D);
   w.meta = (SegMeta*)take(sizeof(SegMeta) * 2 * (size_t)w.n_pieces);
   w.ugrad = (float*)take(sizeof(float) * (size_t)M * D, kPartUGrad);
+  w.fids = (int64_t*)take(8 * (size_t)M, kPartOccMap);
+  w.occ_src = (const float**)take(sizeof(float*) * (size_t)M, kPartOccMap);
+  w.occ_div = (float*)take(m4, kPartOccMap);
   w.sorted = nullptr;
   w.bytes = off;
   return w;
@@ -1140,11 +1201,18 @@ static void check_grad_rows(const char* who, int D, const float* pooled_grad = n
     throw ArgError(std::string(who) + " needs 16-byte aligned rows");
 }
 
+// One table's share of a parts call: the sorted range [lo, hi) and whether any of its parts pools by MEAN
+struct SortedRange {
+  int64_t lo, hi;
+  bool mean;
+};
+
 // Arguments of a reduce over the plan's sorted list: the gradient rows of pooled_grad (row_offsets != null: CSR
 // rows, occurrence -> row mapped into w.occ first), per-run sums to ugrad (or the peer windows of the launch).
+// range != null (parts call): only the sorted range of one table, gradient rows from the plan's occurrence map.
 static SegArgs seg_args(const BwdScratch& w, int64_t M, int D, const float* pooled_grad, int64_t grad_stride,
                         int grad_col, const int32_t* row_offsets, int64_t n_rows, int pooling, float* ugrad,
-                        cudaStream_t s) {
+                        cudaStream_t s, const SortedRange* range = nullptr) {
   SegArgs sa;
   std::memset(&sa, 0, sizeof(sa));
   BwdArgs& a = sa.b;
@@ -1164,6 +1232,17 @@ static SegArgs seg_args(const BwdScratch& w, int64_t M, int D, const float* pool
   sa.part = w.part;
   sa.meta = w.meta;
   sa.n_pieces = w.n_pieces;
+  if (range) {
+    a.n = range->hi;
+    a.lo = range->lo;
+    a.pooling = range->mean ? MONO_POOL_MEAN : MONO_POOL_SUM;
+    a.occ_src = w.occ_src;
+    a.occ_div = w.occ_div;
+    a.run_of_sorted = w.sort.run_of_sorted;
+    sa.piece0 = range->lo / kPiece;
+    sa.n_pieces = (range->hi + kPiece - 1) / kPiece - sa.piece0;
+    sa.piece_run_base += sa.piece0;
+  }
   if (row_offsets) {
     occ_row_kernel<<<resident_grid(occ_row_kernel, n_rows, kThreads), kThreads, 0, s>>>(row_offsets, n_rows, w.occ);
     MONO_CHECK_LAUNCH();
@@ -1195,8 +1274,10 @@ static void launch_seg(const SegArgs& sa, const PeerOut& po, cudaStream_t s) {
 
 // per-run gradient sums -> run_dst (a.ugrad, or the owners' peer windows)
 static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, cudaStream_t s) {
-  const int64_t np = sa.n_pieces;
-  if (np <= 0) return;
+  const int64_t nr = sa.n_pieces;
+  if (nr <= 0) return;
+  // the tree depth follows the range's occurrence count (the whole list but for one table of a parts call)
+  const int64_t np = (sa.b.n - sa.b.lo + kPiece - 1) / kPiece;
   int levels = 0;
   uint64_t top = 1;
   while ((uint64_t)np > top * kFinishMax) {  // the final pass adds up to kFinishMax nodes per run, 16 loads in flight
@@ -1204,7 +1285,8 @@ static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, cudaStrea
     ++levels;
   }
   const int D = sa.b.td.dim;
-  const bool plain = sa.b.occ_row == nullptr && !(sa.b.pooling == MONO_POOL_MEAN && sa.b.row_offsets != nullptr);
+  const bool plain = sa.b.occ_row == nullptr && sa.b.occ_src == nullptr &&
+                     !(sa.b.pooling == MONO_POOL_MEAN && sa.b.row_offsets != nullptr);
   const bool two = knob(KNOB_SEG_VPL) == 2;
 #define SEG_G(GG)                                                                                                   \
   do {                                                                                                              \
@@ -1225,11 +1307,11 @@ static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, cudaStrea
     }                                                                                                               \
     uint32_t stride = 1;                                                                                            \
     for (int l = 0; l < levels; ++l, stride *= kTreeFan) {                                                          \
-      tree_level_kernel<GG><<<resident_grid(tree_level_kernel<GG>, 2 * np, kThreads, kThreads, kStageBytes),        \
-                              kThreads, kStageBytes, s>>>(sa.part, sa.meta, 2 * np, stride, D);                     \
+      tree_level_kernel<GG><<<resident_grid(tree_level_kernel<GG>, 2 * nr, kThreads, kThreads, kStageBytes),        \
+                              kThreads, kStageBytes, s>>>(sa.part, sa.meta, 2 * nr, stride, D);                     \
       MONO_CHECK_LAUNCH();                                                                                          \
     }                                                                                                               \
-    long_finish_kernel<GG><<<resident_grid(long_finish_kernel<GG>, np, kThreads / GG, kThreads, kStageBytes),      \
+    long_finish_kernel<GG><<<resident_grid(long_finish_kernel<GG>, nr, kThreads / GG, kThreads, kStageBytes),      \
                              kThreads, kStageBytes, s>>>(sa, (uint32_t)top, po);                                    \
     MONO_CHECK_LAUNCH();                                                                                            \
   } while (0)
@@ -1246,6 +1328,36 @@ static int bits_for(uint64_t cap) {
   int bits = 0;
   while (((uint64_t)1 << bits) < cap) ++bits;
   return bits;
+}
+
+// the register-resident apply exists for the four vectorised optimizers; anything else: store + generic apply_row
+static int apply_opt_sel(const HostTable& ht) {
+  const int opt_sel = (ht.segs.size() == 1 && ht.segs[0].opt_type <= MONO_OPT_ADAM) ? ht.segs[0].opt_type : -1;
+  return opt_sel;
+}
+
+// the optimizer step of every run of the reduce's range (M: its occurrence count, sizes the grid)
+static void launch_apply(const BwdArgs& a, int G, int opt_sel, int64_t M, cudaStream_t s) {
+  const int pf = knob(KNOB_APPLY_PF);
+#define BWD2(GG, OO)                                                                                             \
+  runs_apply_kernel<GG, OO><<<resident_grid(runs_apply_kernel<GG, OO>, M, kThreads / GG), kThreads, 0, s>>>(a, pf);  \
+  MONO_CHECK_LAUNCH()
+#define BWD(GG)                                                         \
+  switch (opt_sel) {                                                    \
+    case MONO_OPT_SGD: BWD2(GG, MONO_OPT_SGD); break;                   \
+    case MONO_OPT_ADAGRAD: BWD2(GG, MONO_OPT_ADAGRAD); break;           \
+    case MONO_OPT_FTRL: BWD2(GG, MONO_OPT_FTRL); break;                 \
+    case MONO_OPT_ADAM: BWD2(GG, MONO_OPT_ADAM); break;                 \
+    default: BWD2(GG, -1); break;                                       \
+  }
+  switch (G) {
+    case 4: BWD(4); break;
+    case 8: BWD(8); break;
+    case 16: BWD(16); break;
+    default: BWD(32); break;
+  }
+#undef BWD2
+#undef BWD
 }
 
 void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t n_fids,
@@ -1270,8 +1382,6 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
   sg.lr_off = 0;
   CallBlob cb = stage_call(mt, &sg, 1, lr_host, ht.slices, s);
   const int G = pick_group(D);
-  // the register-resident apply exists for the four vectorised optimizers; anything else: store + generic apply_row
-  const int opt_sel = (ht.segs.size() == 1 && ht.segs[0].opt_type <= MONO_OPT_ADAM) ? ht.segs[0].opt_type : -1;
 
   // ---- scratch ----
   const uint32_t cap = claim_set_slots(M);
@@ -1286,7 +1396,7 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
   // 1 claim: k0[i] = set slot of occurrence i; the winner of a slot resolves its FID in the table (row parked in
   //   the set entry, expiry timestamp bumped) or queues it as absent
   uint32_t* miss_ctr = w.ctr + kCtrMisses;
-  ClaimResolve cr;
+  ClaimResolve cr{};
   cr.t = mt->d_tables + k;
   cr.update_ts = (uint32_t)update_time;
   cr.miss_ctr = miss_ctr;
@@ -1300,7 +1410,7 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
   MONO_CHECK_LAUNCH();
   // 2 absent FIDs: allocate a row + lock-free insert (few in steady state; the count stays on the device)
   claim_miss_kernel<<<resident_grid(claim_miss_kernel, std::min<int64_t>(M, (int64_t)device_sms() * 2 * kThreads), kThreads), kThreads, 0, s>>>(
-      mt->d_tables + k, set, miss_ctr, w.miss, (uint32_t)update_time);
+      mt->d_tables + k, set, miss_ctr, w.miss, (uint32_t)update_time, nullptr, 0);
   MONO_CHECK_LAUNCH();
   launch_upsert_finalize(mt, cb, miss_ctr, (uint32_t)update_time, s);
   // 3 stable LSD radix sort of (slot, position)  +  4 ordered run list (with each run's resolved row)
@@ -1316,29 +1426,215 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
   a.scratch = a.ugrad;
   launch_reduce(sa, G, no_peer, s);
   // 6 apply: one streaming pass over the runs — row index, summed gradient, w / optimizer state of every distinct FID
-  const int pf = knob(KNOB_APPLY_PF);
-#define BWD2(GG, OO)                                                                                             \
-  runs_apply_kernel<GG, OO><<<resident_grid(runs_apply_kernel<GG, OO>, M, kThreads / GG), kThreads, 0, s>>>(a, pf);  \
-  MONO_CHECK_LAUNCH()
-#define BWD(GG)                                                         \
-  switch (opt_sel) {                                                    \
-    case MONO_OPT_SGD: BWD2(GG, MONO_OPT_SGD); break;                   \
-    case MONO_OPT_ADAGRAD: BWD2(GG, MONO_OPT_ADAGRAD); break;           \
-    case MONO_OPT_FTRL: BWD2(GG, MONO_OPT_FTRL); break;                 \
-    case MONO_OPT_ADAM: BWD2(GG, MONO_OPT_ADAM); break;                 \
-    default: BWD2(GG, -1); break;                                       \
-  }
-  switch (G) {
-    case 4: BWD(4); break;
-    case 8: BWD(8); break;
-    case 16: BWD(16); break;
-    default: BWD(32); break;
-  }
-#undef BWD2
-#undef BWD
+  launch_apply(a, G, apply_opt_sel(ht), M, s);
   ht.issued_total += (uint64_t)M;
   ht.max_update_ts = std::max<int64_t>(ht.max_update_ts, update_time);
   request_snapshot(mt, k, s);
+}
+
+// ---- fused backward over many parts (features) of several tables in one call ----
+// A part as the occurrence map kernel sees it (parts ordered table-major, part order inside a table)
+struct PartDev {
+  const int64_t* fids;
+  const int32_t* row_offsets;   // null: one FID per row
+  const float* rows;            // gradient rows, column included
+  int64_t stride;
+  int64_t occ_begin;            // first occurrence in the table-major concatenation
+  int64_t row_begin;            // first row in the concatenation of the parts' rows
+  int32_t mean, pad;            // CSR MEAN: terms divided by the row's n
+};
+
+// One thread per row of the concatenated parts: the row's occurrences get their FID, gradient row and MEAN divisor
+__global__ void __launch_bounds__(kThreads)
+parts_occ_kernel(const PartDev* __restrict__ parts, int n_parts, int64_t n_rows, int64_t* __restrict__ fids_out,
+                 const float** __restrict__ src_out, float* __restrict__ div_out) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_rows; r += (int64_t)gridDim.x * blockDim.x) {
+    int lo = 0, hi = n_parts - 1;  // the last part whose rows start at or before r
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (parts[mid].row_begin <= r) lo = mid;
+      else hi = mid - 1;
+    }
+    const PartDev& p = parts[lo];
+    const int64_t lr = r - p.row_begin;
+    int64_t b = lr, e = lr + 1;
+    if (p.row_offsets) {
+      b = p.row_offsets[lr];
+      e = p.row_offsets[lr + 1];
+    }
+    const float* src = p.rows + lr * p.stride;
+    const float dv = p.mean ? (float)(e - b) : 0.f;
+    for (int64_t m = b; m < e; ++m) {
+      fids_out[p.occ_begin + m] = p.fids[m];
+      src_out[p.occ_begin + m] = src;
+      div_out[p.occ_begin + m] = dv;
+    }
+  }
+}
+
+// The occurrences of all parts of one table are one batch (part order, then occurrence order): the claim set gets one
+// region per table, so one claim, one sort and one run list serve every table and leave each table's occurrences as
+// one contiguous sorted range; the reduce and the apply then run once per table over its range, with its row width,
+// optimizer and tree depth.  Everything is checked before the first device operation.
+void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, const float* lr_host,
+                             int64_t update_time, cudaStream_t s) {
+  const int K = (int)mt->tables.size();
+  if (n_parts < 0 || n_parts > MONO_MAX_POOL_PARTS) throw ArgError("pool_backward_parts: bad part count");
+  if ((n_parts > 0 && !parts) || !lr_host) throw ArgError("pool_backward_parts: null argument");
+  std::vector<int64_t> per_table(K, 0);
+  std::vector<char> mean(K, 0);
+  int64_t M = 0, n_rows = 0;
+  for (int i = 0; i < n_parts; ++i) {
+    const mono_pool_part& p = parts[i];
+    if (p.table < 0 || p.table >= K) throw ArgError("pool_backward_parts: bad table index");
+    if (p.pooling != MONO_POOL_SUM && p.pooling != MONO_POOL_MEAN) throw ArgError("pool_backward_parts: SUM or MEAN");
+    if (p.n_fids < 0 || p.n_rows < 0) throw ArgError("pool_backward_parts: negative count");
+    if (!p.row_offsets_dev && p.n_rows != p.n_fids)
+      throw ArgError("pool_backward_parts: n_rows must equal n_fids without offsets");
+    if (p.n_fids > 0 && (!p.fids_dev || !p.rows_dev)) throw ArgError("pool_backward_parts: null argument");
+    check_grad_rows("pool_backward_parts", mt->tables[p.table].dim, p.rows_dev, p.stride, p.col);
+    M += p.n_fids;
+    if (M > ((int64_t)1 << 30)) throw ArgError("pool_backward_parts: more than 2^30 occurrences in one call");
+    if (p.n_fids == 0) continue;
+    per_table[p.table] += p.n_fids;
+    n_rows += p.n_rows;
+    if (p.pooling == MONO_POOL_MEAN && p.row_offsets_dev) mean[p.table] = 1;
+  }
+  mt->note_insert(s);
+  if (M == 0) return;
+  // call tables in table order, each with its occurrence range, claim region and learning rates
+  std::vector<CallTable> ct;
+  std::vector<CallSeg> segs;
+  uint64_t cap = 0;
+  int64_t occ = 0;
+  int n_lr = 0, Dmax = 4;
+  for (int k = 0; k < K; ++k) {
+    const int lr_off = n_lr;
+    n_lr += mt->tables[k].slices;
+    if (!per_table[k]) continue;
+    CallTable c;
+    c.occ_begin = occ;
+    c.occ_end = occ + per_table[k];
+    c.slot_base = (uint32_t)cap;
+    c.slots = claim_set_slots(per_table[k]);
+    c.table = k;
+    c.pad = 0;
+    ct.push_back(c);
+    CallSeg sg;
+    sg.id_begin = c.occ_begin;
+    sg.id_end = c.occ_end;
+    sg.val_off = 0;
+    sg.table = k;
+    sg.lr_off = lr_off;
+    segs.push_back(sg);
+    cap += c.slots;
+    occ = c.occ_end;
+    Dmax = std::max(Dmax, mt->tables[k].dim);
+  }
+  if (cap > ((uint64_t)1 << 31)) throw ArgError("pool_backward_parts: claim set over 2^31 slots");
+  const size_t ct_off = (sizeof(PartDev) * (size_t)n_parts + 15) & ~(size_t)15;
+  if (ct_off + sizeof(CallTable) * ct.size() > StageRing::kBlockBytes)
+    throw ArgError("pool_backward_parts: too many parts and tables for one call descriptor");
+  // the parts, table-major
+  std::vector<PartDev> pd;
+  std::vector<int64_t> occ_at(K), row_at(K);
+  {
+    int64_t o = 0, r = 0;
+    for (int k = 0; k < K; ++k) {
+      occ_at[k] = o;
+      row_at[k] = r;
+      for (int i = 0; i < n_parts; ++i)
+        if (parts[i].table == k && parts[i].n_fids > 0) {
+          o += parts[i].n_fids;
+          r += parts[i].n_rows;
+        }
+    }
+  }
+  for (int k = 0; k < K; ++k)
+    for (int i = 0; i < n_parts; ++i) {
+      const mono_pool_part& p = parts[i];
+      if (p.table != k || p.n_fids == 0) continue;
+      PartDev d;
+      d.fids = p.fids_dev;
+      d.row_offsets = p.row_offsets_dev;
+      d.rows = p.rows_dev + p.col;
+      d.stride = p.stride;
+      d.occ_begin = occ_at[k];
+      d.row_begin = row_at[k];
+      d.mean = p.pooling == MONO_POOL_MEAN && p.row_offsets_dev ? 1 : 0;
+      d.pad = 0;
+      pd.push_back(d);
+      occ_at[k] += p.n_fids;
+      row_at[k] += p.n_rows;
+    }
+
+  for (const CallTable& c : ct) ensure_capacity(mt, c.table, (uint64_t)(c.occ_end - c.occ_begin), s);
+  upload_tables(mt, s);
+  CallBlob cb = stage_call(mt, segs.data(), (int)segs.size(), lr_host, n_lr, s);
+  const int rb = mt->ring.acquire();
+  std::memcpy(mt->ring.h(rb), pd.data(), sizeof(PartDev) * pd.size());
+  std::memcpy(mt->ring.h(rb) + ct_off, ct.data(), sizeof(CallTable) * ct.size());
+  mt->ring.commit(rb, ct_off + sizeof(CallTable) * ct.size(), s);
+  const PartDev* d_parts = reinterpret_cast<const PartDev*>(mt->ring.d(rb));
+  const CallTable* d_ct = reinterpret_cast<const CallTable*>(mt->ring.d(rb) + ct_off);
+  const int T = (int)ct.size();
+
+  // ---- scratch ----
+  const int bits = bits_for(cap);
+  const unsigned sparts = kPartK0 | kPartRowIdx | kPartMiss | kPartRunOfSorted | kPartUGrad | kPartOccMap;
+  BwdScratch w = scratch_plan(M, Dmax, bits, sparts, nullptr);
+  w = scratch_plan(M, Dmax, bits, sparts, (char*)mt->ws_a.get(w.bytes, s));
+  uint32_t epoch = 0;
+  Entry* set = (Entry*)mt->claim_set.get(sizeof(Entry) * (size_t)cap, s, &epoch);
+  MONO_CUDA(cudaMemsetAsync(w.ctr, 0, kCtrBytes, s));
+
+  // 0 occurrence map: FIDs, gradient row and MEAN divisor of every occurrence, table-major
+  parts_occ_kernel<<<resident_grid(parts_occ_kernel, n_rows, kThreads), kThreads, 0, s>>>(
+      d_parts, (int)pd.size(), n_rows, w.fids, w.occ_src, w.occ_div);
+  MONO_CHECK_LAUNCH();
+  // 1 claim in the occurrence's table region, resolve in that table  +  2 absent FIDs  (as run_pool_backward)
+  uint32_t* miss_ctr = w.ctr + kCtrMisses;
+  ClaimResolve cr{};
+  cr.t = mt->d_tables;
+  cr.update_ts = (uint32_t)update_time;
+  cr.miss_ctr = miss_ctr;
+  cr.miss_slots = w.miss;
+  cr.regions = d_ct;
+  cr.n_regions = T;
+  if (knob(KNOB_CLAIM_DUAL))
+    fid_claim_kernel<true, true><<<resident_grid(fid_claim_kernel<true, true>, M, kThreads), kThreads, 0, s>>>(
+        w.fids, M, set, (uint32_t)cap, 1, epoch, w.k0, w.ctr + kCtrOwners, cr, knob(KNOB_CLAIM_PF));
+  else
+    fid_claim_kernel<true><<<resident_grid(fid_claim_kernel<true>, M, kThreads), kThreads, 0, s>>>(
+        w.fids, M, set, (uint32_t)cap, 1, epoch, w.k0, w.ctr + kCtrOwners, cr, knob(KNOB_CLAIM_PF));
+  MONO_CHECK_LAUNCH();
+  claim_miss_kernel<<<resident_grid(claim_miss_kernel, std::min<int64_t>(M, (int64_t)device_sms() * 2 * kThreads), kThreads), kThreads, 0, s>>>(
+      mt->d_tables, set, miss_ctr, w.miss, (uint32_t)update_time, d_ct, T);
+  MONO_CHECK_LAUNCH();
+  launch_upsert_finalize(mt, cb, miss_ctr, (uint32_t)update_time, s);
+  // 3 sort + 4 run list, once: slots are table-major, so each table's runs are one contiguous range
+  w.sorted = sort_and_runs(w.sort, w.k0, M, bits, 0, set, s);
+  // 5 reduce + 6 apply, per table over its range
+  for (int q = 0; q < T; ++q) {
+    const int k = ct[q].table;
+    HostTable& ht = mt->tables[k];
+    const int64_t Mk = ct[q].occ_end - ct[q].occ_begin;
+    const SortedRange rg = {ct[q].occ_begin, ct[q].occ_end, mean[k] != 0};
+    SegArgs sa = seg_args(w, M, ht.dim, nullptr, 0, 0, nullptr, 0, MONO_POOL_SUM, w.ugrad, s, &rg);
+    BwdArgs& a = sa.b;
+    a.td = ht.dev;
+    a.t = mt->d_tables + k;
+    a.fids = w.fids;
+    a.rowidx = w.sort.rowidx;
+    a.lr = cb.lr + segs[q].lr_off;
+    a.scratch = a.ugrad;
+    const int G = pick_group(ht.dim);
+    launch_reduce(sa, G, no_peer, s);
+    launch_apply(a, G, apply_opt_sel(ht), Mk, s);
+    ht.issued_total += (uint64_t)Mk;
+    ht.max_update_ts = std::max<int64_t>(ht.max_update_ts, update_time);
+    request_snapshot(mt, k, s);
+  }
 }
 
 // Deterministic replacement of the float-atomic scatter of pooled-row gradients

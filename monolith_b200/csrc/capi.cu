@@ -316,6 +316,23 @@ int mono_mtable_pool_backward(mono_mtable_t* t, int32_t k, const int64_t* fids_d
   });
 }
 
+int mono_mtable_lookup_pool_parts(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                  void* stream) {
+  return guarded([&] {
+    HandleGuard hg_(t);
+    run_lookup_pool_parts(t, parts_host, n_parts, (cudaStream_t)stream);
+  });
+}
+
+int mono_mtable_pool_backward_parts(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                    const float* learning_rate_host, int64_t update_time,
+                                    int64_t /*global_step*/, void* stream) {
+  return guarded([&] {
+    HandleGuard hg_(t);
+    run_pool_backward_parts(t, parts_host, n_parts, learning_rate_host, update_time, (cudaStream_t)stream);
+  });
+}
+
 int mono_mtable_optimize(mono_mtable_t* t, const int64_t* ids_dev, const int64_t* id_split_host,
                          const float* grads_dev, const float* learning_rate_host,
                          int64_t update_time, int64_t /*global_step*/, uint32_t flags, void* stream) {

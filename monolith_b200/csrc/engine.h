@@ -224,6 +224,9 @@ struct BwdScratch {
   float* part;                  // [2 * n_pieces][D] long-run block sums
   SegMeta* meta;                // [2 * n_pieces]
   float* ugrad;                 // optional [M][D]: summed gradient of every run
+  int64_t* fids;                // optional [M]: a parts call's FIDs, table-major
+  const float** occ_src;        // optional [M]: its gradient row (column included) of every occurrence
+  float* occ_div;               // optional [M]: its MEAN divisor of every occurrence (0 = none)
   int64_t n_pieces;
   const uint2* sorted;          // the sorted {key, position} list, once the sort has run
 };
@@ -444,6 +447,10 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
                        const int32_t* row_offsets, int64_t n_rows, int pooling,
                        const float* pooled_grad, int64_t grad_stride, int grad_col,
                        const float* lr_host, int64_t update_time, cudaStream_t s);
+
+void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, cudaStream_t s);
+void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, const float* lr_host,
+                             int64_t update_time, cudaStream_t s);
 
 void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, const int32_t* row_offsets,
                       int64_t n_rows, int pooling, const float* pooled_grad, int64_t grad_stride,

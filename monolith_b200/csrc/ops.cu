@@ -47,11 +47,34 @@ __device__ __forceinline__ void store_vec(float* dst, int c, int D, const float4
 // SINGLE: the call has one segment (one table): table fields and the output base are warp-uniform
 // and hoisted, which keeps the kernel at ~40 registers => 6 resident blocks (48 warps) per SM.
 // CONFIRM: the call may run beside inserts of another stream (mono_mtable::lookup_must_confirm): misses are confirmed.
+// One part of a multi-feature forward (lookup_pool_parts): the one-table forward kernels take an optional array of
+// these and then serve part blockIdx.y, with exactly the arguments a single-part launch would have passed.
+struct FwdPart {
+  CallSeg seg;                  // lookup_kernel: the part's one segment
+  const TableDev* t;
+  const int64_t* fids;
+  const int32_t* row_offsets;
+  int64_t n_rows;
+  float* out;
+  int64_t out_stride;
+  int32_t out_col, pooling;
+};
+
 template <int G, bool SINGLE, bool DUAL = false, bool CONFIRM = true>
 __global__ void __launch_bounds__(kThreads, SINGLE && !DUAL ? 6 : 4)
 lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ segs, int nsegs,
               const int64_t* __restrict__ ids, int64_t n_total, float* __restrict__ out,
-              int64_t out_stride /* <= 0: rows packed at dim floats */, int out_col, int prefetch) {
+              int64_t out_stride /* <= 0: rows packed at dim floats */, int out_col, int prefetch,
+              const FwdPart* __restrict__ parts = nullptr) {
+  if (SINGLE && parts) {
+    const FwdPart& p = parts[blockIdx.y];
+    segs = &p.seg;
+    ids = p.fids;
+    n_total = p.n_rows;
+    out = p.out;
+    out_stride = p.out_stride;
+    out_col = p.out_col;
+  }
   constexpr int RPI = 32 / G;   // rows copied per iteration of a warp
   constexpr int ITERS = G;      // iterations to drain the 32 resolved rows
   constexpr int UNR = 4;        // row loads in flight per lane
@@ -254,7 +277,14 @@ __device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src_smem, uint32_t 
 template <int ROWB>  // bytes per row: dim * 4, a multiple of 16
 __global__ void __launch_bounds__(kThreads)
 lookup_tma_kernel(const TableDev* __restrict__ t0, const int64_t* __restrict__ ids, int64_t n_total,
-                  float* __restrict__ out) {
+                  float* __restrict__ out, const FwdPart* __restrict__ parts = nullptr) {
+  if (parts) {
+    const FwdPart& p = parts[blockIdx.y];
+    t0 = p.t;
+    ids = p.fids;
+    n_total = p.n_rows;
+    out = p.out;
+  }
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int NW = kThreads / 32;
   constexpr int TILEB = 32 * ROWB;
@@ -379,7 +409,19 @@ template <int G, int NV, int U>  // NV = 16-byte vectors per lane (dim <= 4*G*NV
 __global__ void __launch_bounds__(kThreads)
 lookup_pool_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ fids,
                    const int32_t* __restrict__ row_offsets, int64_t n_rows, int pooling,
-                   float* __restrict__ out, int64_t out_stride, int out_col) {
+                   float* __restrict__ out, int64_t out_stride, int out_col,
+                   const FwdPart* __restrict__ parts = nullptr) {
+  if (parts) {
+    const FwdPart& p = parts[blockIdx.y];
+    t = p.t;
+    fids = p.fids;
+    row_offsets = p.row_offsets;
+    n_rows = p.n_rows;
+    pooling = p.pooling;
+    out = p.out;
+    out_stride = p.out_stride;
+    out_col = p.out_col;
+  }
   constexpr int GPW = 32 / G;
   const int lane = threadIdx.x & 31, gl = Group<G>::gl();
   const int D = t->dim;
@@ -491,8 +533,20 @@ template <int G>
 __global__ void __launch_bounds__(kThreads, 2)
 lookup_pool_staged_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ fids,
                           const int32_t* __restrict__ row_offsets, int64_t n_rows, int pooling,
-                          float* __restrict__ out, int64_t out_stride, int out_col) {
+                          float* __restrict__ out, int64_t out_stride, int out_col,
+                          const FwdPart* __restrict__ parts = nullptr) {
   constexpr int U = 4;
+  if (parts) {
+    const FwdPart& p = parts[blockIdx.y];
+    t = p.t;
+    fids = p.fids;
+    row_offsets = p.row_offsets;
+    n_rows = p.n_rows;
+    pooling = p.pooling;
+    out = p.out;
+    out_stride = p.out_stride;
+    out_col = p.out_col;
+  }
   constexpr int GPW = 32 / G;
   constexpr int KPL = kStage / G > 0 ? kStage / G : 1;  // keys probed per lane and chunk
   extern __shared__ float4 stage_raw[];  // [kStage][kThreads]
@@ -911,9 +965,8 @@ static int max_dim_of(mono_mtable* mt, const CallSeg* h_segs, int nsegs) {
   return m;
 }
 
-// launcher: returns false when the TMA variant does not apply (the caller falls back to lookup_kernel)
-static bool try_lookup_tma(mono_mtable* mt, int k, const int64_t* ids_dev, int64_t n_total, float* out_dev,
-                           int64_t out_stride, int out_col, cudaStream_t s) {
+// whether the TMA variant serves a one-FID-per-row lookup of table k into out_dev
+static bool tma_applies(mono_mtable* mt, int k, const float* out_dev, int64_t out_stride, int out_col) {
   static const int env_mode = [] {  // MONO_LOOKUP_TMA=0/1 presets mono_set_option("lookup_tma")
     const char* e = std::getenv("MONO_LOOKUP_TMA");
     if (e) g_opt_lookup_tma.store(std::atoi(e) != 0);
@@ -929,7 +982,12 @@ static bool try_lookup_tma(mono_mtable* mt, int k, const int64_t* ids_dev, int64
   if ((D & 3) || (rowb != 128 && rowb != 256)) return false;
   if (out_col != 0 || (out_stride > 0 && out_stride != D) || (reinterpret_cast<uintptr_t>(out_dev) & 15)) return false;
   if (ht.dev.emb_stride != (uint32_t)D) return false;  // rows are 16-byte aligned and contiguous when dim % 4 == 0
-  const TableDev* t = mt->d_tables + k;
+  return true;
+}
+
+// TMA lookup of rows of `rowb` bytes; parts != null: one grid row (blockIdx.y) per part, n_total = the largest
+static void launch_tma(int rowb, const TableDev* t, const int64_t* ids_dev, int64_t n_total, float* out_dev,
+                       const FwdPart* parts, int n_parts, cudaStream_t s) {
   constexpr int NW = kThreads / 32;
 #define LT(RB)                                                                                         \
   do {                                                                                                 \
@@ -939,13 +997,20 @@ static bool try_lookup_tma(mono_mtable* mt, int k, const int64_t* ids_dev, int64
       MONO_CUDA(cudaFuncSetAttribute(lookup_tma_kernel<RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
       attr = true;                                                                                     \
     }                                                                                                  \
-    lookup_tma_kernel<RB><<<resident_grid(lookup_tma_kernel<RB>, (n_total + 31) / 32, NW, kThreads, smem), kThreads, smem, s>>>( \
-        t, ids_dev, n_total, out_dev);                                                                 \
+    lookup_tma_kernel<RB><<<dim3(resident_grid(lookup_tma_kernel<RB>, (n_total + 31) / 32, NW, kThreads, smem), n_parts), \
+                            kThreads, smem, s>>>(t, ids_dev, n_total, out_dev, parts);                 \
   } while (0)
   if (rowb == 128) LT(128);
   else LT(256);
 #undef LT
   MONO_CHECK_LAUNCH();
+}
+
+// launcher: returns false when the TMA variant does not apply (the caller falls back to lookup_kernel)
+static bool try_lookup_tma(mono_mtable* mt, int k, const int64_t* ids_dev, int64_t n_total, float* out_dev,
+                           int64_t out_stride, int out_col, cudaStream_t s) {
+  if (!tma_applies(mt, k, out_dev, out_stride, out_col)) return false;
+  launch_tma(mt->tables[k].dim * 4, mt->d_tables + k, ids_dev, n_total, out_dev, nullptr, 1, s);
   return true;
 }
 
@@ -955,16 +1020,16 @@ static void launch_lookup_staged(mono_mtable* mt, const CallSeg* d_segs, int nse
 #define L(GG)                                                                                      \
   if (nsegs == 1 && knob(KNOB_LOOKUP_DUAL))                                                        \
     lookup_kernel<GG, true, true><<<resident_grid(lookup_kernel<GG, true, true>, n_total, kThreads), kThreads, 0, s>>>( \
-        mt->d_tables, d_segs, nsegs, ids_dev, n_total, out_dev, out_stride, out_col, pf);          \
+        mt->d_tables, d_segs, nsegs, ids_dev, n_total, out_dev, out_stride, out_col, pf, nullptr);          \
   else if (nsegs == 1 && !mt->lookup_must_confirm(s))                                              \
     lookup_kernel<GG, true, false, false><<<resident_grid(lookup_kernel<GG, true, false, false>, n_total, kThreads), kThreads, 0, s>>>( \
-        mt->d_tables, d_segs, nsegs, ids_dev, n_total, out_dev, out_stride, out_col, pf);          \
+        mt->d_tables, d_segs, nsegs, ids_dev, n_total, out_dev, out_stride, out_col, pf, nullptr);          \
   else if (nsegs == 1)                                                                             \
     lookup_kernel<GG, true><<<resident_grid(lookup_kernel<GG, true>, n_total, kThreads), kThreads, 0, s>>>( \
-        mt->d_tables, d_segs, nsegs, ids_dev, n_total, out_dev, out_stride, out_col, pf);          \
+        mt->d_tables, d_segs, nsegs, ids_dev, n_total, out_dev, out_stride, out_col, pf, nullptr);          \
   else                                                                                             \
     lookup_kernel<GG, false><<<resident_grid(lookup_kernel<GG, false>, n_total, kThreads), kThreads, 0, s>>>( \
-        mt->d_tables, d_segs, nsegs, ids_dev, n_total, out_dev, out_stride, out_col, pf)
+        mt->d_tables, d_segs, nsegs, ids_dev, n_total, out_dev, out_stride, out_col, pf, nullptr)
   const int pf = knob(KNOB_LOOKUP_PF);
   switch (G) {
     case 4: L(4); break;
@@ -1026,33 +1091,67 @@ void launch_lookup_push(mono_mtable* mt, int k, const int64_t* ids_dev, int64_t 
   MONO_CHECK_LAUNCH();
 }
 
-void launch_lookup_pool(mono_mtable* mt, int k, const int64_t* fids_dev, const int32_t* row_offsets,
-                        int64_t n_rows, int pooling, float* out, int64_t out_stride, int out_col,
-                        cudaStream_t s) {
-  if (n_rows <= 0) return;
-  if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN)
-    throw ArgError("lookup_pool supports SUM and MEAN pooling");
-  upload_tables(mt, s);
+// The kernel that serves a lookup_pool of one table (lookup_pool_parts launches each distinct one once)
+struct PoolPlan {
+  enum Kind { kTma, kLookup, kStaged, kPool } kind;
+  int a, b, c;  // kTma: row bytes; kLookup: G, variant (0 dual, 1 no miss confirm, 2 confirm); kStaged: G; kPool: G, nv
+  bool operator==(const PoolPlan& o) const { return kind == o.kind && a == o.a && b == o.b && c == o.c; }
+};
+
+static PoolPlan plan_lookup_pool(mono_mtable* mt, const FwdPart& p, cudaStream_t s) {
+  const int k = p.seg.table;
   const int D = mt->tables[k].dim;
-  if (D > 512) throw ArgError("lookup_pool supports dim <= 512");
   const int G = pick_group(D);
   const int nv = (D + 4 * G - 1) / (4 * G);
-  if (row_offsets == nullptr) {
+  const int64_t n_rows = p.n_rows, out_stride = p.out_stride;
+  const int out_col = p.out_col;
+  const float* out = p.out;
+  if (p.row_offsets == nullptr) {
     // one FID per pooled row: SUM and MEAN are the identity (x / 1 == x): probe + gather only
-    if (try_lookup_tma(mt, k, fids_dev, n_rows, out, out_stride, out_col, s)) return;
-    CallSeg sg;
-    sg.id_begin = 0;
-    sg.id_end = n_rows;
-    sg.val_off = 0;
-    sg.table = k;
-    sg.lr_off = 0;
-    CallBlob cb = stage_call(mt, &sg, 1, nullptr, 0, s);
-    launch_lookup_staged(mt, cb.segs, 1, G, fids_dev, n_rows, out, out_stride, out_col, s);
+    if (tma_applies(mt, k, p.out, p.out_stride, p.out_col)) return {PoolPlan::kTma, D * 4, 0, 0};
+    return {PoolPlan::kLookup, G, knob(KNOB_LOOKUP_DUAL) ? 0 : !mt->lookup_must_confirm(s) ? 1 : 2, 0};
+  }
+  if ((D & 3) == 0 && D <= 128 && (out_stride & 3) == 0 && (out_col & 3) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 &&
+      n_rows < ((int64_t)1 << 31))
+    return {PoolPlan::kStaged, G, 0, 0};
+  return {PoolPlan::kPool, G, nv <= 2 ? nv : 4, 0};  // nv 3 and 4 share an instantiation
+}
+
+// a: the arguments of a single-table call (parts == null), or of any part of a parts launch whose kernels then serve
+// part blockIdx.y of `parts` (n_rows: the largest part, sizes the grid)
+static void launch_pool_plan(mono_mtable* mt, const PoolPlan& pl, const FwdPart& a, const FwdPart* parts,
+                             int n_parts, cudaStream_t s) {
+  const int64_t n_rows = a.n_rows;
+  if (pl.kind == PoolPlan::kTma) {
+    launch_tma(pl.a, a.t, a.fids, n_rows, a.out, parts, n_parts, s);
     return;
   }
-  const TableDev* t = mt->d_tables + k;
-  if ((D & 3) == 0 && D <= 128 && (out_stride & 3) == 0 && (out_col & 3) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 &&
-      n_rows < ((int64_t)1 << 31)) {
+  if (pl.kind == PoolPlan::kLookup) {
+    const CallSeg* d_seg = parts ? &parts[0].seg : stage_call(mt, &a.seg, 1, nullptr, 0, s).segs;
+    const int pf = knob(KNOB_LOOKUP_PF);
+#define L(GG)                                                                                                        \
+  if (pl.b == 0)                                                                                                     \
+    lookup_kernel<GG, true, true><<<dim3(resident_grid(lookup_kernel<GG, true, true>, n_rows, kThreads), n_parts),   \
+                                    kThreads, 0, s>>>(mt->d_tables, d_seg, 1, a.fids, n_rows, a.out, a.out_stride,   \
+                                                      a.out_col, pf, parts);                                         \
+  else if (pl.b == 1)                                                                                                \
+    lookup_kernel<GG, true, false, false><<<dim3(resident_grid(lookup_kernel<GG, true, false, false>, n_rows, kThreads), \
+                                                 n_parts), kThreads, 0, s>>>(mt->d_tables, d_seg, 1, a.fids, n_rows, \
+                                                                             a.out, a.out_stride, a.out_col, pf, parts); \
+  else                                                                                                               \
+    lookup_kernel<GG, true><<<dim3(resident_grid(lookup_kernel<GG, true>, n_rows, kThreads), n_parts), kThreads, 0,  \
+                              s>>>(mt->d_tables, d_seg, 1, a.fids, n_rows, a.out, a.out_stride, a.out_col, pf, parts)
+    switch (pl.a) {
+      case 4: L(4); break;
+      case 8: L(8); break;
+      case 16: L(16); break;
+      default: L(32); break;
+    }
+#undef L
+    MONO_CHECK_LAUNCH();
+    return;
+  }
+  if (pl.kind == PoolPlan::kStaged) {
     constexpr size_t kStageBytes = sizeof(float4) * kStage * kThreads;
 #define LPS(GG)                                                                                                   \
   do {                                                                                                            \
@@ -1062,11 +1161,11 @@ void launch_lookup_pool(mono_mtable* mt, int k, const int64_t* fids_dev, const i
                                      (int)kStageBytes));                                                          \
       attr_set = true;                                                                                            \
     }                                                                                                             \
-    lookup_pool_staged_kernel<GG><<<resident_grid(lookup_pool_staged_kernel<GG>, n_rows, (kThreads / GG) * 4,     \
-                                                  kThreads, kStageBytes), kThreads, kStageBytes, s>>>(            \
-        t, fids_dev, row_offsets, n_rows, pooling, out, out_stride, out_col);                                     \
+    lookup_pool_staged_kernel<GG><<<dim3(resident_grid(lookup_pool_staged_kernel<GG>, n_rows, (kThreads / GG) * 4, \
+                                                       kThreads, kStageBytes), n_parts), kThreads, kStageBytes, s>>>( \
+        a.t, a.fids, a.row_offsets, n_rows, a.pooling, a.out, a.out_stride, a.out_col, parts);                    \
   } while (0)
-    switch (G) {
+    switch (pl.a) {
       case 4: LPS(4); break;
       case 8: LPS(8); break;
       case 16: LPS(16); break;
@@ -1076,11 +1175,12 @@ void launch_lookup_pool(mono_mtable* mt, int k, const int64_t* fids_dev, const i
     MONO_CHECK_LAUNCH();
     return;
   }
+#define LP(GG, NV, UU)                                                                                           \
+  lookup_pool_kernel<GG, NV, UU>                                                                                 \
+      <<<dim3(resident_grid(lookup_pool_kernel<GG, NV, UU>, n_rows, (kThreads / GG) * UU), n_parts), kThreads, 0, s>>>( \
+          a.t, a.fids, a.row_offsets, n_rows, a.pooling, a.out, a.out_stride, a.out_col, parts)
   // U rows in flight per lane group: enough independent HBM round trips per warp to cover latency
-#define LP(GG, NV, UU)                                                                            \
-  lookup_pool_kernel<GG, NV, UU>                                                                   \
-      <<<resident_grid(lookup_pool_kernel<GG, NV, UU>, n_rows, (kThreads / GG) * UU), kThreads, 0, s>>>( \
-          t, fids_dev, row_offsets, n_rows, pooling, out, out_stride, out_col)
+  const int G = pl.a, nv = pl.b;
   if (G == 4) LP(4, 1, 4);
   else if (G == 8) LP(8, 1, 4);
   else if (G == 16) LP(16, 1, 4);
@@ -1089,6 +1189,91 @@ void launch_lookup_pool(mono_mtable* mt, int k, const int64_t* fids_dev, const i
   else LP(32, 4, 1);
 #undef LP
   MONO_CHECK_LAUNCH();
+}
+
+static FwdPart fwd_part(mono_mtable* mt, int k, const int64_t* fids_dev, const int32_t* row_offsets, int64_t n_rows,
+                        int pooling, float* out, int64_t out_stride, int out_col) {
+  FwdPart p;
+  p.seg.id_begin = 0;
+  p.seg.id_end = n_rows;
+  p.seg.val_off = 0;
+  p.seg.table = k;
+  p.seg.lr_off = 0;
+  p.t = mt->d_tables + k;
+  p.fids = fids_dev;
+  p.row_offsets = row_offsets;
+  p.n_rows = n_rows;
+  p.out = out;
+  p.out_stride = out_stride;
+  p.out_col = out_col;
+  p.pooling = pooling;
+  return p;
+}
+
+void launch_lookup_pool(mono_mtable* mt, int k, const int64_t* fids_dev, const int32_t* row_offsets,
+                        int64_t n_rows, int pooling, float* out, int64_t out_stride, int out_col,
+                        cudaStream_t s) {
+  if (n_rows <= 0) return;
+  if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN)
+    throw ArgError("lookup_pool supports SUM and MEAN pooling");
+  upload_tables(mt, s);
+  const int D = mt->tables[k].dim;
+  if (D > 512) throw ArgError("lookup_pool supports dim <= 512");
+  const FwdPart a = fwd_part(mt, k, fids_dev, row_offsets, n_rows, pooling, out, out_stride, out_col);
+  launch_pool_plan(mt, plan_lookup_pool(mt, a, s), a, nullptr, 1, s);
+}
+
+// Every part exactly as lookup_pool would serve it alone, but the parts that lookup_pool would serve with the same
+// kernel share one launch: one grid row per part, the parts' arguments in one staged array.
+void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, cudaStream_t s) {
+  const int K = (int)mt->tables.size();
+  if (n_parts < 0 || n_parts > MONO_MAX_POOL_PARTS) throw ArgError("lookup_pool_parts: bad part count");
+  if (n_parts > 0 && !parts) throw ArgError("lookup_pool_parts: null argument");
+  for (int i = 0; i < n_parts; ++i) {
+    const mono_pool_part& p = parts[i];
+    if (p.table < 0 || p.table >= K) throw ArgError("lookup_pool_parts: bad table index");
+    if (p.pooling != MONO_POOL_SUM && p.pooling != MONO_POOL_MEAN) throw ArgError("lookup_pool_parts: SUM or MEAN");
+    if (p.n_rows < 0 || p.n_fids < 0) throw ArgError("lookup_pool_parts: negative count");
+    if (!p.row_offsets_dev && p.n_rows != p.n_fids)
+      throw ArgError("lookup_pool_parts: n_rows must equal n_fids without offsets");
+    if (p.n_rows > 0 && (!p.rows_dev || (p.n_fids > 0 && !p.fids_dev))) throw ArgError("lookup_pool_parts: null argument");
+    if (mt->tables[p.table].dim > 512) throw ArgError("lookup_pool_parts supports dim <= 512");
+  }
+  upload_tables(mt, s);
+  // group the parts by the kernel that serves them, in order of first use
+  std::vector<PoolPlan> plans;
+  std::vector<std::vector<FwdPart>> groups;
+  for (int i = 0; i < n_parts; ++i) {
+    const mono_pool_part& p = parts[i];
+    if (p.n_rows == 0) continue;
+    const FwdPart f = fwd_part(mt, p.table, p.fids_dev, p.row_offsets_dev, p.n_rows, p.pooling, p.rows_dev, p.stride,
+                               p.col);
+    const PoolPlan pl = plan_lookup_pool(mt, f, s);
+    size_t g = 0;
+    while (g < plans.size() && !(plans[g] == pl)) ++g;
+    if (g == plans.size()) {
+      plans.push_back(pl);
+      groups.emplace_back();
+    }
+    groups[g].push_back(f);
+  }
+  if (plans.empty()) return;
+  const int rb = mt->ring.acquire();
+  char* h = mt->ring.h(rb);
+  size_t off = 0;
+  for (const auto& g : groups) {
+    std::memcpy(h + off, g.data(), sizeof(FwdPart) * g.size());
+    off += sizeof(FwdPart) * g.size();
+  }
+  static_assert(sizeof(FwdPart) * MONO_MAX_POOL_PARTS <= StageRing::kBlockBytes, "the parts fit one staged block");
+  mt->ring.commit(rb, off, s);
+  const FwdPart* d = reinterpret_cast<const FwdPart*>(mt->ring.d(rb));
+  for (size_t g = 0; g < plans.size(); ++g) {
+    FwdPart a = groups[g][0];
+    for (const FwdPart& f : groups[g]) a.n_rows = std::max(a.n_rows, f.n_rows);
+    launch_pool_plan(mt, plans[g], a, d, (int)groups[g].size(), s);
+    d += groups[g].size();
+  }
 }
 
 void launch_contains(mono_mtable* mt, int k, const int64_t* ids, int64_t n, uint8_t* out,

@@ -9,6 +9,7 @@ float32 values); the mutating methods return `self` where the reference returns 
 around the same resource handle (:419-423).
 """
 import ctypes as C
+import dataclasses
 import time
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -38,6 +39,27 @@ def _f32(t, device) -> torch.Tensor:
   if t.dtype != torch.float32 or t.device != device:
     t = t.to(device=device, dtype=torch.float32)
   return t.contiguous()
+
+
+@dataclasses.dataclass
+class PoolPart:
+  """One feature's slice of a step for pool_backward_parts: the FIDs of table `slot`, pooled by `pooling`
+  ("sum" or "mean") into rows (row_offsets: CSR [n_rows + 1] int32, None = one FID per row), and the
+  gradient rows `rows` ([n_rows, >= col + dim] float32, the table's dim floats start at column `col`)."""
+  slot: str
+  fids: torch.Tensor
+  row_offsets: Optional[torch.Tensor] = None
+  pooling: str = "sum"
+  rows: Optional[torch.Tensor] = None
+  col: int = 0
+
+  def __post_init__(self):
+    if self.pooling not in ("sum", "mean"):
+      raise ValueError(f"PoolPart.pooling must be 'sum' or 'mean', not {self.pooling!r}")
+    if not isinstance(self.col, int) or self.col < 0:
+      raise ValueError("PoolPart.col must be a non-negative int")
+    if self.rows is not None and (not isinstance(self.rows, torch.Tensor) or self.rows.dim() != 2):
+      raise ValueError("PoolPart.rows must be a 2-D tensor")
 
 
 class MultiHashTable:
@@ -340,6 +362,60 @@ class MultiHashTable:
     _lib.check(self._lib.mono_mtable_pool_backward(self._h, k, _ptr(fids), fids.numel(), _ptr(row_offsets), n_rows,
                                                    pool, _ptr(pooled_grad), stride, grad_col, lr_arr, int(req_time),
                                                    int(global_step), _stream(self._device)))
+    return self
+
+  def _parts_arr(self, parts: Sequence[PoolPart], forward: bool):
+    """-> (mono_pool_part array, tensors that must stay alive over the call, the parts' row tensors)."""
+    if len(parts) > _lib.MAX_POOL_PARTS:
+      raise ValueError(f"at most {_lib.MAX_POOL_PARTS} parts per call")
+    arr = (_lib.PoolPartC * max(len(parts), 1))()
+    keep, outs = [], []
+    for i, p in enumerate(parts):
+      if p.slot not in self._table_names:
+        raise KeyError(f"unknown table {p.slot}")
+      k = self._table_names.index(p.slot)
+      fids = _ids(p.fids, self._device)
+      ro = None
+      if p.row_offsets is not None:
+        ro = p.row_offsets.to(device=self._device, dtype=torch.int32).contiguous()
+        n_rows = ro.numel() - 1
+      else:
+        n_rows = fids.numel()
+      rows = p.rows
+      if rows is None:
+        if not forward:
+          raise ValueError("pool_backward_parts: every part needs its gradient rows")
+        rows = torch.empty(n_rows, self._dims[k], dtype=torch.float32, device=self._device)
+      if rows.dtype != torch.float32 or rows.device != self._device or rows.stride(1) != 1:
+        raise ValueError("part rows must be float32 on the table's device with unit column stride")
+      if rows.shape[0] < n_rows or rows.shape[1] < p.col + self._dims[k]:
+        raise ValueError("part rows are smaller than [n_rows, col + dim]")
+      keep += [fids, ro]
+      outs.append(rows)
+      arr[i] = _lib.PoolPartC(k, fids.data_ptr(), fids.numel(), None if ro is None else ro.data_ptr(), n_rows,
+                              {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[p.pooling], rows.data_ptr(),
+                              rows.stride(0), p.col)
+    return arr, keep, outs
+
+  def lookup_pool_parts(self, parts: Sequence[PoolPart]) -> List[torch.Tensor]:
+    """lookup_pool over many features and tables in one call (mono_mtable_lookup_pool_parts): every part's rows
+    are bit-identical to lookup_pool on that part alone; parts served by the same kernel share one launch.  A part
+    without `rows` gets a new [n_rows, dim] tensor; returns each part's rows, in part order."""
+    arr, keep, outs = self._parts_arr(parts, forward=True)
+    _lib.check(self._lib.mono_mtable_lookup_pool_parts(self._h, arr, len(parts), _stream(self._device)))
+    del keep
+    return outs
+
+  def pool_backward_parts(self, parts: Sequence[PoolPart], req_time: int = 0, global_step: int = 0):
+    """pool_backward over many features and tables in one call (mono_mtable_pool_backward_parts): the parts
+    of one table are ONE batch in part order, so a FID that several features share gets one optimizer step
+    with the sum of all its terms; the claim, sort and run list run once for the whole call."""
+    arr, keep, _ = self._parts_arr(parts, forward=False)
+    lr = self.learning_rates()
+    lr_arr = (C.c_float * max(len(lr), 1))(*lr)
+    _lib.check(self._lib.mono_mtable_pool_backward_parts(self._h, arr, len(parts), lr_arr, int(req_time),
+                                                         int(global_step), _stream(self._device)))
+    del keep
     return self
 
   def set_hash_filter(self, slot: str, capacity: int, default_threshold: int, slot_thresholds: Optional[Dict[int, int]] = None):
