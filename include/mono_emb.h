@@ -198,18 +198,36 @@ int mono_mtable_pool_backward(mono_mtable_t* t, int32_t k, const int64_t* fids_d
  * (row_offsets_dev as for mono_mtable_lookup_pool, NULL = one FID per row and then n_rows == n_fids);
  * row r is rows_dev + r*stride + col: the forward's output row, the backward's row gradient.
  *
- * mono_mtable_lookup_pool_parts: every part's output is bit-identical to mono_mtable_lookup_pool on
- * that part alone (any dim up to 512, CSR or one-FID rows, SUM or MEAN, any stride and column; parts
- * may write disjoint columns of one tensor).  Kernel launches: one per distinct kernel instantiation
- * among the parts (the kernel mono_mtable_lookup_pool would pick for each), not one per part.
+ * FIRSTN parts (pooling == MONO_POOL_FIRSTN; max_seq_len = L >= 1, read for FIRSTN parts only): a
+ * sequence feature, as the reference's FirstN combiner and the fused layout's FIRSTN branch (ref:
+ * embedding_combiners.py:72-102, RT/ops/fused_embedding_to_layout.h:251-256,334-340).  Row r owns the
+ * L*dim floats at rows_dev + r*stride + col, position j at + j*dim (a [B, L, dim] tensor is
+ * stride = L*dim, col = 0).  Let n_r be row r's FID count (1 without row offsets).
+ *   forward: position j < min(n_r, L) is the row of FID fids[offs[r] + j] (zeros for an absent FID);
+ *     positions n_r <= j < L are +0.0; occurrences at j >= L are not read.
+ *   backward: exactly the result of a one-FID-per-row SUM part over the same FIDs whose gradient row
+ *     for occurrence (r, j) is position j of row r for j < L and a row of +0.0 for j >= L.  So a FID
+ *     whose occurrences all lie beyond L is still upserted, bumped and counted by the admission
+ *     filter, and gets one optimizer step with a zero gradient (the reference's ScatterGrad leaves its
+ *     gradient row at the zero fill, and the FID stays in the ids the optimizer receives).
+ * A FIRSTN part needs n_rows * max_seq_len <= 2^31.
+ *
+ * mono_mtable_lookup_pool_parts: every SUM / MEAN part's output is bit-identical to
+ * mono_mtable_lookup_pool on that part alone (any dim up to 512, CSR or one-FID rows, SUM or MEAN, any
+ * stride and column; parts may write disjoint columns of one tensor); FIRSTN parts serve any dim up to
+ * 512 too.  Kernel launches: one per distinct kernel instantiation among the parts (for SUM / MEAN the
+ * kernel mono_mtable_lookup_pool would pick; for FIRSTN one of lookup_seq_kernel's, by the table's
+ * lane group and whether misses must be confirmed), not one per part.
  * MONO_ERR_INVALID_ARGUMENT, before any device work: n_parts outside [0, MONO_MAX_POOL_PARTS], a bad
- * table index, dim > 512, pooling other than SUM or MEAN, n_rows != n_fids without offsets.
+ * table index, dim > 512, pooling other than SUM, MEAN or FIRSTN, a FIRSTN part with max_seq_len < 1
+ * or n_rows * max_seq_len > 2^31, n_rows != n_fids without offsets.
  *
  * mono_mtable_pool_backward_parts: for every table named by some part, the occurrences
  * of all its parts are ONE batch, taken in part order and then occurrence order, as the reference's
  * per-table ScatterGrad sees them: each distinct FID of the table gets one upsert, one timestamp bump,
  * one admission-filter count and one optimizer step with the sum of its terms (a term is the part's
- * row gradient, divided by the row's n for a CSR MEAN part).  The sum is associated as for
+ * row gradient, divided by the row's n for a CSR MEAN part; for a FIRSTN part as stated above).  The
+ * sum is associated as for
  * mono_mtable_pool_backward, with the tree depth set by the table's occurrence count in the call, so
  * parts of one table with one pooling give exactly the bits of one mono_mtable_pool_backward over
  * their concatenated FIDs, stacked gradient rows and rebased row offsets.  Tables do not interact.
@@ -220,8 +238,10 @@ int mono_mtable_pool_backward(mono_mtable_t* t, int32_t k, const int64_t* fids_d
  * power of two >= max(1024, 2 M(k)), L(k) = 0 for M(k) <= 16384 occurrences, 1 up to 2^21, else 2.
  * MONO_ERR_INVALID_ARGUMENT, before any device work (no table changes): n_parts outside
  * [0, MONO_MAX_POOL_PARTS], a bad table index, a part whose table breaks the pool_backward conditions
- * (dim % 4 == 0, dim <= 128, 16-byte aligned gradient rows), pooling other than SUM or MEAN,
- * n_rows != n_fids without offsets, or more than 2^30 occurrences in total.  No host sync. */
+ * (dim % 4 == 0, dim <= 128, 16-byte aligned gradient rows; FIRSTN parts included), pooling other
+ * than SUM, MEAN or FIRSTN, a FIRSTN part with max_seq_len < 1 or n_rows * max_seq_len > 2^31,
+ * n_rows != n_fids without offsets, or more than 2^30 occurrences in total.  FIRSTN parts add no
+ * launch: the occurrence map writes their gradient-row addresses.  No host sync. */
 #define MONO_MAX_POOL_PARTS 1024
 
 typedef struct mono_pool_part {
@@ -230,10 +250,12 @@ typedef struct mono_pool_part {
   int64_t n_fids;
   const int32_t* row_offsets_dev;   /* [n_rows+1] or NULL = one FID per row                   */
   int64_t n_rows;
-  int32_t pooling;                  /* MONO_POOL_SUM | MONO_POOL_MEAN                          */
+  int32_t pooling;                  /* MONO_POOL_SUM | MONO_POOL_MEAN | MONO_POOL_FIRSTN       */
   float* rows_dev;                  /* forward: output rows; backward: pooled-row gradients   */
   int64_t stride;                   /* floats between rows                                    */
   int32_t col;                      /* first column of the table's dim(k) floats in a row     */
+  int32_t max_seq_len;              /* FIRSTN only: positions per row (in the trailing padding
+                                       of the earlier layout: the struct stays 72 bytes)      */
 } mono_pool_part;
 
 int mono_mtable_lookup_pool_parts(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,

@@ -32,7 +32,7 @@ class SliceTask(C.Structure):  # mono_slice_task
 class PoolPartC(C.Structure):  # mono_pool_part
   _fields_ = [("table", C.c_int32), ("fids_dev", C.c_void_p), ("n_fids", C.c_int64),
               ("row_offsets_dev", C.c_void_p), ("n_rows", C.c_int64), ("pooling", C.c_int32),
-              ("rows_dev", C.c_void_p), ("stride", C.c_int64), ("col", C.c_int32)]
+              ("rows_dev", C.c_void_p), ("stride", C.c_int64), ("col", C.c_int32), ("max_seq_len", C.c_int32)]
 
 
 MAX_POOL_PARTS = 1024  # MONO_MAX_POOL_PARTS

@@ -1441,13 +1441,17 @@ struct PartDev {
   int64_t stride;
   int64_t occ_begin;            // first occurrence in the table-major concatenation
   int64_t row_begin;            // first row in the concatenation of the parts' rows
-  int32_t mean, pad;            // CSR MEAN: terms divided by the row's n
+  int32_t mean;                 // CSR MEAN: terms divided by the row's n
+  int32_t seq_len;              // FIRSTN: L (0 for SUM / MEAN)
+  int32_t dim, pad;             // the table's dim: FIRSTN positions are dim floats apart
 };
 
-// One thread per row of the concatenated parts: the row's occurrences get their FID, gradient row and MEAN divisor
+// One thread per row of the concatenated parts: the row's occurrences get their FID, gradient row and MEAN divisor.
+// Occurrence j of a FIRSTN row reads position j of the row for j < L and zero_row (128 floats of +0.0) beyond it,
+// as ScatterGrad's FIRSTN branch leaves such a FID's gradient at its zero fill (fused_embedding_to_layout.h:334-340).
 __global__ void __launch_bounds__(kThreads)
 parts_occ_kernel(const PartDev* __restrict__ parts, int n_parts, int64_t n_rows, int64_t* __restrict__ fids_out,
-                 const float** __restrict__ src_out, float* __restrict__ div_out) {
+                 const float** __restrict__ src_out, float* __restrict__ div_out, const float* __restrict__ zero_row) {
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_rows; r += (int64_t)gridDim.x * blockDim.x) {
     int lo = 0, hi = n_parts - 1;  // the last part whose rows start at or before r
     while (lo < hi) {
@@ -1466,7 +1470,8 @@ parts_occ_kernel(const PartDev* __restrict__ parts, int n_parts, int64_t n_rows,
     const float dv = p.mean ? (float)(e - b) : 0.f;
     for (int64_t m = b; m < e; ++m) {
       fids_out[p.occ_begin + m] = p.fids[m];
-      src_out[p.occ_begin + m] = src;
+      const int64_t j = m - b;
+      src_out[p.occ_begin + m] = !p.seq_len ? src : j < p.seq_len ? src + j * p.dim : zero_row;
       div_out[p.occ_begin + m] = dv;
     }
   }
@@ -1487,8 +1492,10 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
   for (int i = 0; i < n_parts; ++i) {
     const mono_pool_part& p = parts[i];
     if (p.table < 0 || p.table >= K) throw ArgError("pool_backward_parts: bad table index");
-    if (p.pooling != MONO_POOL_SUM && p.pooling != MONO_POOL_MEAN) throw ArgError("pool_backward_parts: SUM or MEAN");
+    if (p.pooling != MONO_POOL_SUM && p.pooling != MONO_POOL_MEAN && p.pooling != MONO_POOL_FIRSTN)
+      throw ArgError("pool_backward_parts: SUM, MEAN or FIRSTN");
     if (p.n_fids < 0 || p.n_rows < 0) throw ArgError("pool_backward_parts: negative count");
+    check_firstn("pool_backward_parts", p);
     if (!p.row_offsets_dev && p.n_rows != p.n_fids)
       throw ArgError("pool_backward_parts: n_rows must equal n_fids without offsets");
     if (p.n_fids > 0 && (!p.fids_dev || !p.rows_dev)) throw ArgError("pool_backward_parts: null argument");
@@ -1562,6 +1569,8 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
       d.occ_begin = occ_at[k];
       d.row_begin = row_at[k];
       d.mean = p.pooling == MONO_POOL_MEAN && p.row_offsets_dev ? 1 : 0;
+      d.seq_len = p.pooling == MONO_POOL_FIRSTN ? p.max_seq_len : 0;
+      d.dim = mt->tables[k].dim;
       d.pad = 0;
       pd.push_back(d);
       occ_at[k] += p.n_fids;
@@ -1590,7 +1599,7 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
 
   // 0 occurrence map: FIDs, gradient row and MEAN divisor of every occurrence, table-major
   parts_occ_kernel<<<resident_grid(parts_occ_kernel, n_rows, kThreads), kThreads, 0, s>>>(
-      d_parts, (int)pd.size(), n_rows, w.fids, w.occ_src, w.occ_div);
+      d_parts, (int)pd.size(), n_rows, w.fids, w.occ_src, w.occ_div, mt->zero_row);
   MONO_CHECK_LAUNCH();
   // 1 claim in the occurrence's table region, resolve in that table  +  2 absent FIDs  (as run_pool_backward)
   uint32_t* miss_ctr = w.ctr + kCtrMisses;

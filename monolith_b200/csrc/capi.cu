@@ -167,6 +167,8 @@ int mono_mtable_create(const mono_table_cfg* cfgs, int32_t n_tables, int32_t dev
       MONO_CUDA(cudaStreamCreateWithFlags(&mt->own_stream, cudaStreamNonBlocking));
       MONO_CUDA(cudaHostAlloc((void**)&mt->h_flag, 256, cudaHostAllocDefault));
       MONO_CUDA(cudaMalloc((void**)&mt->d_tables, sizeof(TableDev) * n_tables));
+      MONO_CUDA(cudaMalloc((void**)&mt->zero_row, sizeof(float) * 128));
+      MONO_CUDA(cudaMemset(mt->zero_row, 0, sizeof(float) * 128));
       mt->tables.resize(n_tables);
       for (int i = 0; i < n_tables; ++i) table_init(mt, mt->tables[i], cfgs[order[i]], 0);
       MONO_CUDA(cudaDeviceSynchronize());
@@ -185,6 +187,7 @@ int mono_mtable_destroy(mono_mtable_t* t) {
   cudaDeviceSynchronize();
   for (auto& tb : t->tables) table_free(tb);
   if (t->d_tables) cudaFree(t->d_tables);
+  if (t->zero_row) cudaFree(t->zero_row);
   t->ring.destroy();
   t->ws_miss.release(); t->ws_a.release(); t->ws_b.release(); t->ws_c.release(); t->claim_set.release();
   t->ws_d.release(); t->ws_e.release(); t->ws_host_in.release(); t->ws_host_out.release();

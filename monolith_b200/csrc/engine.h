@@ -242,6 +242,7 @@ struct mono_mtable {
   mono::StageRing ring;
   mono::DevBuf ws_miss, ws_a, ws_b, ws_c, ws_d, ws_e, ws_host_in, ws_host_out;
   mono::ClaimSet claim_set;  // pool_backward's FID grouping set
+  float* zero_row = nullptr;  // 128 floats of +0.0: the gradient row of a FIRSTN occurrence beyond its sequence length
   void* pinned_in = nullptr;
   size_t pinned_in_cap = 0;
   void* pinned_out = nullptr;
@@ -447,6 +448,13 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
                        const int32_t* row_offsets, int64_t n_rows, int pooling,
                        const float* pooled_grad, int64_t grad_stride, int grad_col,
                        const float* lr_host, int64_t update_time, cudaStream_t s);
+
+// A FIRSTN part's sequence length (max_seq_len is read for FIRSTN parts only): L >= 1 and n_rows * L <= 2^31
+inline void check_firstn(const char* who, const mono_pool_part& p) {
+  if (p.pooling != MONO_POOL_FIRSTN) return;
+  if (p.max_seq_len < 1) throw ArgError(std::string(who) + ": FIRSTN needs max_seq_len >= 1");
+  if (p.n_rows > ((int64_t)1 << 31) / p.max_seq_len) throw ArgError(std::string(who) + ": n_rows * max_seq_len over 2^31");
+}
 
 void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, cudaStream_t s);
 void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, const float* lr_host,

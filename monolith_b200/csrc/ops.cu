@@ -49,8 +49,10 @@ __device__ __forceinline__ void store_vec(float* dst, int c, int D, const float4
 // CONFIRM: the call may run beside inserts of another stream (mono_mtable::lookup_must_confirm): misses are confirmed.
 // One part of a multi-feature forward (lookup_pool_parts): the one-table forward kernels take an optional array of
 // these and then serve part blockIdx.y, with exactly the arguments a single-part launch would have passed.
+// A FIRSTN part's sequence length rides in seg.lr_off (a forward has no learning rate): a field of its own would
+// change the struct's size and with it the code of every kernel that indexes the array.
 struct FwdPart {
-  CallSeg seg;                  // lookup_kernel: the part's one segment
+  CallSeg seg;                  // lookup_kernel: the part's one segment; lookup_seq_kernel: seg.lr_off = L
   const TableDev* t;
   const int64_t* fids;
   const int32_t* row_offsets;
@@ -168,6 +170,87 @@ lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ s
               store_vec(dst, cc, D, y, vec_ok);
             }
           }
+        }
+      }
+    }
+  }
+}
+
+// FIRSTN parts of lookup_pool_parts (ref: GatherEmb's FIRSTN branch, fused_embedding_to_layout.h:251-256): part
+// blockIdx.y writes n_rows x L positions of dim floats, position j of row r at out + r*out_stride + out_col + j*dim.
+// lookup_kernel<G, true>'s two phases over position slots q = r*L + j instead of ids: a slot with j < n_r probes
+// FID fids[offs[r] + j] (lane per key), a slot with j >= n_r probes nothing; phase B copies a found row and stores
+// zeros for the rest.  n_rows * L <= 2^31 (checked by the launcher), so slots divide in 32 bits.  4 blocks per SM
+// (64 registers): at 6 (40 registers) it spills, and so it does with lookup_kernel's next-tile FID prefetch.
+template <int G, bool CONFIRM>
+__global__ void __launch_bounds__(kThreads, 4)
+lookup_seq_kernel(const FwdPart* __restrict__ parts) {
+  const FwdPart& p = parts[blockIdx.y];
+  const uint32_t L = (uint32_t)p.seg.lr_off;
+  const int64_t n_total = p.n_rows * L;
+  const int32_t* __restrict__ offs = p.row_offsets;
+  const int64_t* __restrict__ fids = p.fids;
+  constexpr int RPI = 32 / G;
+  constexpr int ITERS = G;
+  constexpr int UNR = 4;
+  const int lane = threadIdx.x & 31, gl = Group<G>::gl(), grp = lane / G;
+  const int c = gl * 4;
+  const TableDev* t0 = p.t;
+  const int D0 = t0->dim;
+  const float* __restrict__ emb0 = t0->emb;
+  const uint32_t stride0 = t0->emb_stride;
+  const int64_t rs0 = p.out_stride;
+  float* const base0 = p.out + p.out_col;
+  const bool vec0 = (D0 & 3) == 0 && (rs0 & 3) == 0 && (reinterpret_cast<uintptr_t>(base0) & 15) == 0;
+  // slot q -> its row r, and its FID when position j = q - r*L holds one
+  auto slot = [&](int64_t q, int64_t& key, uint32_t& r) -> bool {
+    r = (uint32_t)q / L;
+    const uint32_t j = (uint32_t)q - r * L;
+    int64_t b = r, e = (int64_t)r + 1;
+    if (offs) {
+      b = __ldg(offs + r);
+      e = __ldg(offs + r + 1);
+    }
+    if ((int64_t)j >= e - b) return false;
+    key = __ldg(fids + b + j);
+    return true;
+  };
+  const int64_t wstride = (int64_t)gridDim.x * (kThreads / 32) * 32;
+  const int64_t wfirst = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * 32;
+  for (int64_t wbase = wfirst; wbase < n_total; wbase += wstride) {
+    // ---- phase A: lane-per-key probe ----
+    const int64_t i = wbase + lane;
+    int64_t key = 0;
+    uint32_t rq = 0;
+    const bool has = i < n_total && slot(i, key, rq);
+    uint32_t row = kEmptyRow;
+    if (has) {
+      row = probe_lane(t0, key);
+      if (CONFIRM && row == kEmptyRow) row = probe_lane_confirm_miss(t0, key);  // inserts on another stream
+    }
+    // ---- phase B: group-per-row copy, UNR rows in flight ----
+#pragma unroll
+    for (int it0 = 0; it0 < ITERS; it0 += UNR) {
+      float4 x[UNR];
+#pragma unroll
+      for (int u = 0; u < UNR; ++u) {
+        const uint32_t r = __shfl_sync(0xffffffffu, row, (it0 + u) * RPI + grp);
+        x[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (r != kEmptyRow && c < D0) x[u] = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r * stride0 + c));
+      }
+#pragma unroll
+      for (int u = 0; u < UNR; ++u) {
+        const int src_lane = (it0 + u) * RPI + grp;
+        const uint32_t r_st = __shfl_sync(0xffffffffu, row, src_lane);
+        const uint32_t rq_st = __shfl_sync(0xffffffffu, rq, src_lane);
+        const int64_t ir = wbase + src_lane;
+        if (ir >= n_total) continue;
+        float* dst = base0 + (int64_t)rq_st * rs0 + (int64_t)((uint32_t)ir - rq_st * L) * D0;
+        store_vec(dst, c, D0, x[u], vec0);
+        for (int cc = c + 4 * G; cc < D0; cc += 4 * G) {  // wide rows (dim > 128, G == 32)
+          float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (r_st != kEmptyRow) y = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r_st * stride0 + cc));
+          store_vec(dst, cc, D0, y, vec0);
         }
       }
     }
@@ -1093,8 +1176,9 @@ void launch_lookup_push(mono_mtable* mt, int k, const int64_t* ids_dev, int64_t 
 
 // The kernel that serves a lookup_pool of one table (lookup_pool_parts launches each distinct one once)
 struct PoolPlan {
-  enum Kind { kTma, kLookup, kStaged, kPool } kind;
-  int a, b, c;  // kTma: row bytes; kLookup: G, variant (0 dual, 1 no miss confirm, 2 confirm); kStaged: G; kPool: G, nv
+  enum Kind { kTma, kLookup, kStaged, kPool, kSeq } kind;
+  int a, b, c;  // kTma: row bytes; kLookup: G, variant (0 dual, 1 no miss confirm, 2 confirm); kStaged: G; kPool: G, nv;
+                // kSeq (FIRSTN, parts only): G, whether misses are confirmed
   bool operator==(const PoolPlan& o) const { return kind == o.kind && a == o.a && b == o.b && c == o.c; }
 };
 
@@ -1102,6 +1186,7 @@ static PoolPlan plan_lookup_pool(mono_mtable* mt, const FwdPart& p, cudaStream_t
   const int k = p.seg.table;
   const int D = mt->tables[k].dim;
   const int G = pick_group(D);
+  if (p.pooling == MONO_POOL_FIRSTN) return {PoolPlan::kSeq, G, mt->lookup_must_confirm(s) ? 1 : 0, 0};
   const int nv = (D + 4 * G - 1) / (4 * G);
   const int64_t n_rows = p.n_rows, out_stride = p.out_stride;
   const int out_col = p.out_col;
@@ -1118,10 +1203,28 @@ static PoolPlan plan_lookup_pool(mono_mtable* mt, const FwdPart& p, cudaStream_t
 }
 
 // a: the arguments of a single-table call (parts == null), or of any part of a parts launch whose kernels then serve
-// part blockIdx.y of `parts` (n_rows: the largest part, sizes the grid)
+// part blockIdx.y of `parts` (n_rows: the largest part's pool_work, sizes the grid)
 static void launch_pool_plan(mono_mtable* mt, const PoolPlan& pl, const FwdPart& a, const FwdPart* parts,
                              int n_parts, cudaStream_t s) {
   const int64_t n_rows = a.n_rows;
+  if (pl.kind == PoolPlan::kSeq) {
+#define LS(GG)                                                                                                      \
+  if (pl.b)                                                                                                         \
+    lookup_seq_kernel<GG, true><<<dim3(resident_grid(lookup_seq_kernel<GG, true>, n_rows, kThreads), n_parts),     \
+                                  kThreads, 0, s>>>(parts);                                                         \
+  else                                                                                                              \
+    lookup_seq_kernel<GG, false><<<dim3(resident_grid(lookup_seq_kernel<GG, false>, n_rows, kThreads), n_parts),   \
+                                   kThreads, 0, s>>>(parts)
+    switch (pl.a) {
+      case 4: LS(4); break;
+      case 8: LS(8); break;
+      case 16: LS(16); break;
+      default: LS(32); break;
+    }
+#undef LS
+    MONO_CHECK_LAUNCH();
+    return;
+  }
   if (pl.kind == PoolPlan::kTma) {
     launch_tma(pl.a, a.t, a.fids, n_rows, a.out, parts, n_parts, s);
     return;
@@ -1223,8 +1326,13 @@ void launch_lookup_pool(mono_mtable* mt, int k, const int64_t* fids_dev, const i
   launch_pool_plan(mt, plan_lookup_pool(mt, a, s), a, nullptr, 1, s);
 }
 
-// Every part exactly as lookup_pool would serve it alone, but the parts that lookup_pool would serve with the same
-// kernel share one launch: one grid row per part, the parts' arguments in one staged array.
+// The grid work of a part: its rows, or for FIRSTN its n_rows * L position slots
+static int64_t pool_work(const FwdPart& f) {
+  return f.pooling == MONO_POOL_FIRSTN ? f.n_rows * f.seg.lr_off : f.n_rows;
+}
+
+// Every SUM / MEAN part exactly as lookup_pool would serve it alone, every FIRSTN part by lookup_seq_kernel, and the
+// parts served by the same kernel share one launch: one grid row per part, the parts' arguments in one staged array.
 void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, cudaStream_t s) {
   const int K = (int)mt->tables.size();
   if (n_parts < 0 || n_parts > MONO_MAX_POOL_PARTS) throw ArgError("lookup_pool_parts: bad part count");
@@ -1232,8 +1340,10 @@ void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_p
   for (int i = 0; i < n_parts; ++i) {
     const mono_pool_part& p = parts[i];
     if (p.table < 0 || p.table >= K) throw ArgError("lookup_pool_parts: bad table index");
-    if (p.pooling != MONO_POOL_SUM && p.pooling != MONO_POOL_MEAN) throw ArgError("lookup_pool_parts: SUM or MEAN");
+    if (p.pooling != MONO_POOL_SUM && p.pooling != MONO_POOL_MEAN && p.pooling != MONO_POOL_FIRSTN)
+      throw ArgError("lookup_pool_parts: SUM, MEAN or FIRSTN");
     if (p.n_rows < 0 || p.n_fids < 0) throw ArgError("lookup_pool_parts: negative count");
+    check_firstn("lookup_pool_parts", p);
     if (!p.row_offsets_dev && p.n_rows != p.n_fids)
       throw ArgError("lookup_pool_parts: n_rows must equal n_fids without offsets");
     if (p.n_rows > 0 && (!p.rows_dev || (p.n_fids > 0 && !p.fids_dev))) throw ArgError("lookup_pool_parts: null argument");
@@ -1246,8 +1356,8 @@ void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_p
   for (int i = 0; i < n_parts; ++i) {
     const mono_pool_part& p = parts[i];
     if (p.n_rows == 0) continue;
-    const FwdPart f = fwd_part(mt, p.table, p.fids_dev, p.row_offsets_dev, p.n_rows, p.pooling, p.rows_dev, p.stride,
-                               p.col);
+    FwdPart f = fwd_part(mt, p.table, p.fids_dev, p.row_offsets_dev, p.n_rows, p.pooling, p.rows_dev, p.stride, p.col);
+    if (p.pooling == MONO_POOL_FIRSTN) f.seg.lr_off = p.max_seq_len;
     const PoolPlan pl = plan_lookup_pool(mt, f, s);
     size_t g = 0;
     while (g < plans.size() && !(plans[g] == pl)) ++g;
@@ -1270,7 +1380,7 @@ void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_p
   const FwdPart* d = reinterpret_cast<const FwdPart*>(mt->ring.d(rb));
   for (size_t g = 0; g < plans.size(); ++g) {
     FwdPart a = groups[g][0];
-    for (const FwdPart& f : groups[g]) a.n_rows = std::max(a.n_rows, f.n_rows);
+    for (const FwdPart& f : groups[g]) a.n_rows = std::max(a.n_rows, pool_work(f));
     launch_pool_plan(mt, plans[g], a, d, (int)groups[g].size(), s);
     d += groups[g].size();
   }

@@ -43,19 +43,31 @@ def _f32(t, device) -> torch.Tensor:
 
 @dataclasses.dataclass
 class PoolPart:
-  """One feature's slice of a step for pool_backward_parts: the FIDs of table `slot`, pooled by `pooling`
-  ("sum" or "mean") into rows (row_offsets: CSR [n_rows + 1] int32, None = one FID per row), and the
-  gradient rows `rows` ([n_rows, >= col + dim] float32, the table's dim floats start at column `col`)."""
+  """One feature's slice of a step for lookup_pool_parts / pool_backward_parts: the FIDs of table `slot`, pooled by
+  `pooling` ("sum", "mean" or "firstn") into rows (row_offsets: CSR [n_rows + 1] int32, None = one FID per row), and
+  the output or gradient rows `rows` ([n_rows, >= col + dim] float32, the table's dim floats start at column `col`).
+
+  "firstn" is a sequence feature (the reference's FirstN combiner): row r holds max_seq_len positions of dim floats
+  from column `col` on ([n_rows, >= col + max_seq_len * dim]; a [B, L, dim] tensor viewed as [B, L * dim] with
+  col 0), position j being the row of the row's j-th FID, zeros past the row's FIDs; FIDs past max_seq_len are not
+  looked up, and on the backward get a zero gradient.  max_seq_len is set for "firstn" only."""
   slot: str
   fids: torch.Tensor
   row_offsets: Optional[torch.Tensor] = None
   pooling: str = "sum"
   rows: Optional[torch.Tensor] = None
   col: int = 0
+  max_seq_len: int = 0
 
   def __post_init__(self):
-    if self.pooling not in ("sum", "mean"):
-      raise ValueError(f"PoolPart.pooling must be 'sum' or 'mean', not {self.pooling!r}")
+    if self.pooling not in ("sum", "mean", "firstn"):
+      raise ValueError(f"PoolPart.pooling must be 'sum', 'mean' or 'firstn', not {self.pooling!r}")
+    if not isinstance(self.max_seq_len, int) or isinstance(self.max_seq_len, bool):
+      raise ValueError("PoolPart.max_seq_len must be an int")
+    if self.pooling == "firstn" and self.max_seq_len < 1:
+      raise ValueError("PoolPart.max_seq_len must be >= 1 for 'firstn'")
+    if self.pooling != "firstn" and self.max_seq_len != 0:
+      raise ValueError("PoolPart.max_seq_len is set for 'firstn' only")
     if not isinstance(self.col, int) or self.col < 0:
       raise ValueError("PoolPart.col must be a non-negative int")
     if self.rows is not None and (not isinstance(self.rows, torch.Tensor) or self.rows.dim() != 2):
@@ -381,26 +393,30 @@ class MultiHashTable:
         n_rows = ro.numel() - 1
       else:
         n_rows = fids.numel()
+      width = self._dims[k] * (p.max_seq_len if p.pooling == "firstn" else 1)
       rows = p.rows
       if rows is None:
         if not forward:
           raise ValueError("pool_backward_parts: every part needs its gradient rows")
-        rows = torch.empty(n_rows, self._dims[k], dtype=torch.float32, device=self._device)
+        rows = torch.empty(n_rows, width, dtype=torch.float32, device=self._device)
       if rows.dtype != torch.float32 or rows.device != self._device or rows.stride(1) != 1:
         raise ValueError("part rows must be float32 on the table's device with unit column stride")
-      if rows.shape[0] < n_rows or rows.shape[1] < p.col + self._dims[k]:
-        raise ValueError("part rows are smaller than [n_rows, col + dim]")
+      if rows.shape[0] < n_rows or rows.shape[1] < p.col + width:
+        raise ValueError("part rows are smaller than [n_rows, col + dim] ([n_rows, col + max_seq_len * dim] for "
+                         "'firstn')")
       keep += [fids, ro]
       outs.append(rows)
       arr[i] = _lib.PoolPartC(k, fids.data_ptr(), fids.numel(), None if ro is None else ro.data_ptr(), n_rows,
-                              {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[p.pooling], rows.data_ptr(),
-                              rows.stride(0), p.col)
+                              {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN, "firstn": _lib.POOL_FIRSTN}[p.pooling],
+                              rows.data_ptr(), rows.stride(0), p.col, p.max_seq_len)
     return arr, keep, outs
 
   def lookup_pool_parts(self, parts: Sequence[PoolPart]) -> List[torch.Tensor]:
     """lookup_pool over many features and tables in one call (mono_mtable_lookup_pool_parts): every part's rows
-    are bit-identical to lookup_pool on that part alone; parts served by the same kernel share one launch.  A part
-    without `rows` gets a new [n_rows, dim] tensor; returns each part's rows, in part order."""
+    are bit-identical to lookup_pool on that part alone; parts served by the same kernel share one launch.  A
+    "firstn" part writes its [n_rows, max_seq_len, dim] positions (see PoolPart).  A part without `rows` gets a new
+    [n_rows, dim] tensor ([n_rows, max_seq_len * dim] for "firstn": .view(n_rows, max_seq_len, dim) gives the
+    sequence); returns each part's rows, in part order."""
     arr, keep, outs = self._parts_arr(parts, forward=True)
     _lib.check(self._lib.mono_mtable_lookup_pool_parts(self._h, arr, len(parts), _stream(self._device)))
     del keep
@@ -409,7 +425,9 @@ class MultiHashTable:
   def pool_backward_parts(self, parts: Sequence[PoolPart], req_time: int = 0, global_step: int = 0):
     """pool_backward over many features and tables in one call (mono_mtable_pool_backward_parts): the parts
     of one table are ONE batch in part order, so a FID that several features share gets one optimizer step
-    with the sum of all its terms; the claim, sort and run list run once for the whole call."""
+    with the sum of all its terms; the claim, sort and run list run once for the whole call.  A "firstn" part's
+    occurrence j of row r takes position j of the row's gradient, or zeros for j >= max_seq_len: the FID is still
+    inserted, bumped and stepped (with a zero gradient) as the reference's ScatterGrad leaves it."""
     arr, keep, _ = self._parts_arr(parts, forward=False)
     lr = self.learning_rates()
     lr_arr = (C.c_float * max(len(lr), 1))(*lr)
