@@ -15,8 +15,10 @@
 //               occurrences are summed in occurrence order (the CPU reference's order: bit-exact) and stored per run;
 //               hot FIDs are cut into run-aligned 32-occurrence blocks, combined by 0-2 levels of 128-member tree
 //               nodes (the depth follows the call's occurrence count) and a final in-order pass (deterministic,
-//               pairwise-accurate; tests/reduce_order.py restates the order)
-//   6 apply   : runs_apply_kernel streams the per-run sums and applies the optimizer, one row per run
+//               pairwise-accurate; tests/reduce_order.py restates the order).  In the fused backward the runs of
+//               <= kApplyRun (8) occurrences are left to the apply, which sums them itself
+//   6 apply   : runs_apply_kernel applies the optimizer, one row per run: it sums a run of <= 8 occurrences from
+//               the gradient rows (same order and arithmetic: same bits) and reads a longer run's sum from ugrad
 #include <algorithm>
 #include <cstring>
 
@@ -359,6 +361,10 @@ static const uint2* sort_and_runs(const SortWs& w, const uint32_t* keys, int64_t
 // gradient source and the per-row optimizer step
 // ==========================================================================================
 constexpr int kShortRun = 64;
+// runs of at most kApplyRun occurrences are summed by runs_apply_kernel, kApplyStage gradient rows in flight per lane
+constexpr int kApplyRun = 8;
+constexpr int kApplyStage = 8;
+static_assert(kApplyRun <= kShortRun, "the apply sums short runs only");
 
 __global__ void __launch_bounds__(kThreads)
 occ_row_kernel(const int32_t* __restrict__ row_offsets, int64_t n_rows, uint32_t* __restrict__ occ_row) {
@@ -416,15 +422,16 @@ __device__ __forceinline__ GradSrc make_grad_src(const BwdArgs& a, int c) {
   g.mean = a.pooling == MONO_POOL_MEAN && (a.row_offsets != nullptr || a.occ_div != nullptr);
   return g;
 }
-// gradient row of occurrence m, columns c..c+3
-__device__ __forceinline__ float4 occ_grad4(const GradSrc& gs, uint32_t m) {
+// gradient row of occurrence m, from column c (the lane's; gs.base already holds it)
+__device__ __forceinline__ const float* occ_grad_src(const GradSrc& gs, uint32_t m, int c) {
+  if (gs.occ_src) return gs.occ_src[m] + c;
+  return gs.base + (size_t)(gs.occ_row ? gs.occ_row[m] : m) * gs.stride;
+}
+// MEAN divisor of occurrence m (gs.mean only; 0 = none)
+__device__ __forceinline__ float occ_grad_div(const GradSrc& gs, uint32_t m) {
+  if (gs.occ_div) return gs.occ_div[m];
   const uint32_t r = gs.occ_row ? gs.occ_row[m] : m;
-  float4 g = __ldg(reinterpret_cast<const float4*>(gs.base + (size_t)r * gs.stride));
-  if (gs.mean) {
-    const float fn = (float)(gs.row_offsets[r + 1] - gs.row_offsets[r]);
-    g.x = __fdiv_rn(g.x, fn); g.y = __fdiv_rn(g.y, fn); g.z = __fdiv_rn(g.z, fn); g.w = __fdiv_rn(g.w, fn);
-  }
-  return g;
+  return (float)(gs.row_offsets[r + 1] - gs.row_offsets[r]);
 }
 __device__ __forceinline__ void add4(float4& a, const float4& b) {
   a.x = __fadd_rn(a.x, b.x); a.y = __fadd_rn(a.y, b.y); a.z = __fadd_rn(a.z, b.z); a.w = __fadd_rn(a.w, b.w);
@@ -638,9 +645,12 @@ __device__ __forceinline__ void fetch4(const uint32_t (&v)[32 / G], int e, uint3
 // the warp instructions per occurrence (the kernel issues ~50 of them per occurrence at VPL = 1 and can be
 // issue-bound) at the same bytes in flight (kStage / VPL rows of VPL vectors per thread).
 // PLAIN = SUM pooling over identity occurrence rows (no CSR indirection, no MEAN divisor): compiled out.
+// defer_short (the fused backward): the runs of at most kApplyRun occurrences are summed by runs_apply_kernel, which
+// reads their gradient rows itself; this kernel skips their units, so a piece without any other unit costs its item
+// loads and its meta stores only.
 template <int G, int VPL, bool PLAIN, bool AHEAD>
 __global__ void __launch_bounds__(kThreads, 3)
-seg_reduce_kernel(SegArgs sa, const PeerOut po) {
+seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short) {
   __shared__ int64_t s_start[kMaxPeers + 1];
   __shared__ char* s_base[kMaxPeers];
   extern __shared__ float4 stage_raw[];        // [kStage][kThreads]: [slot][thread], conflict-free 16-byte accesses
@@ -730,13 +740,29 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
       *reinterpret_cast<uint4*>(sa.meta + 2 * p) = *reinterpret_cast<uint4*>(&m0);
       *reinterpret_cast<uint4*>(sa.meta + 2 * p + 1) = *reinterpret_cast<uint4*>(&m1);
     }
-    if (S == 0) continue;
-    const int e_begin = __ffs(S) - 1;
+    // deferred units: SK = their elements inside the piece; the last run's continuation past the piece is deferred
+    // with it, which ends the stream at that run's head
+    uint32_t SK = 0;
+    if (defer_short) {
+      for (uint32_t rem = H; rem;) {
+        const int h = __ffs(rem) - 1;
+        rem &= rem - 1;
+        const uint32_t end = rem ? (uint32_t)(__ffs(rem) - 1) : rs_end - (uint32_t)base;  // relative, exclusive
+        if (end - (uint32_t)h <= (uint32_t)kApplyRun) {
+          SK |= end >= (uint32_t)kPiece ? ~0u << h : ((1u << end) - 1u) & (~0u << h);
+          if (end > (uint32_t)kPiece) e_stop = h;
+        }
+      }
+    }
+    const uint32_t SU = S & ~SK;  // starts of the units summed here
+    if (SU == 0) continue;
+    const int e_begin = __ffs(SU) - 1;
 
     float4 acc[VPL];
 #pragma unroll
     for (int v = 0; v < VPL; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int e0 = e_begin & ~(RS - 1); e0 < e_stop; e0 += RS) {
+      if (e0 + RS <= kPiece && ((SK >> e0) & ((1u << RS) - 1u)) == ((1u << RS) - 1u)) continue;  // all deferred
       // ---- request: up to RS gradient rows, this lane's 16-byte slices of each ----
       // (the 4-element bodies are NOT unrolled 4x more: the kernel was instruction-fetch bound when they were)
 #pragma unroll 1
@@ -756,7 +782,7 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const int e = eb + u;
-          if (e >= e_begin && e < e_stop) {
+          if (e >= e_begin && e < e_stop && !(e < kPiece && ((SK >> e) & 1u))) {
             const uint32_t r = (!PLAIN && gs.occ_row) ? gs.occ_row[m[u]] : m[u];
             const float* src = (!PLAIN && gs.occ_src) ? gs.occ_src[m[u]] + c : gs.base + (size_t)r * gs.stride;
 #pragma unroll
@@ -793,7 +819,7 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po) {
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const int e = eb + u;
-          if (e < e_begin || e >= e_stop) continue;
+          if (e < e_begin || e >= e_stop || (e < kPiece && ((SK >> e) & 1u))) continue;
 #pragma unroll
           for (int v = 0; v < VPL; ++v) {
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -923,12 +949,18 @@ long_finish_kernel(SegArgs sa, uint32_t top, const PeerOut po) {
   }
 }
 
-// Apply: group per run; rowidx[j], ugrad[j] and the row's w / state are all independent loads.
+// Apply: group per run.  A run of at most kApplyRun occurrences is summed here: its positions, then its gradient
+// rows, kApplyStage at a time with cp.async into per-thread shared-memory slots (as seg_reduce_kernel does), added
+// in occurrence order from the first row with seg_reduce_kernel's arithmetic, so the bits are those of its unit.
+// The row's w / state loads are issued first and overlap them.  A longer run reads ugrad[j] (long_finish_kernel).
+// Summing here saves those runs' ugrad store and re-load (about 120 MB per C2 step).
 // (A variant that handled two runs per group at a time needs 62 registers, which lowers occupancy.)
-// prefetch != 0: the NEXT run's row index is read one iteration ahead and its weight / state rows are pulled into L2
-// meanwhile, which takes the random row fetch from HBM off the per-iteration chain.
+// The next run's row index and run bounds are read one iteration ahead.  prefetch != 0: its weight / state rows are
+// also pulled into L2 meanwhile.
 template <int G, int OPT>
 __global__ void __launch_bounds__(kThreads) runs_apply_kernel(BwdArgs a, int prefetch) {
+  extern __shared__ float4 stage_raw[];  // [kApplyStage][kThreads]
+  float4 (*stage)[kThreads] = reinterpret_cast<float4 (*)[kThreads]>(stage_raw);
   const int gl = Group<G>::gl();
   const int c = gl * 4;
   int64_t j_lo = 0, nr = *a.n_runs;
@@ -937,13 +969,23 @@ __global__ void __launch_bounds__(kThreads) runs_apply_kernel(BwdArgs a, int pre
     nr = (int64_t)a.run_of_sorted[a.n - 1] + 1;
   }
   const int D = a.td.dim;
+  const GradSrc gs = make_grad_src(a, c);
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
   int64_t j = j_lo + (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
-  uint32_t ri_next = j < nr ? a.rowidx[j] : kEmptyRow;
+  uint32_t ri_next = kEmptyRow, rs_next = 0, re_next = 0, p0_next = 0;
+  if (j < nr) {
+    ri_next = a.rowidx[j];
+    rs_next = a.run_start[j];
+    re_next = a.run_start[j + 1];
+    p0_next = a.run_first_pos[j];
+  }
   for (; j < nr; j += gstride) {
-    const uint32_t ri = ri_next;
+    const uint32_t ri = ri_next, rs = rs_next, re = re_next, p0 = p0_next;
     if (j + gstride < nr) {
       ri_next = a.rowidx[j + gstride];
+      rs_next = a.run_start[j + gstride];
+      re_next = a.run_start[j + gstride + 1];
+      p0_next = a.run_first_pos[j + gstride];
       if (prefetch && OPT >= 0 && ri_next != kEmptyRow && !(ri_next & kFreshBit) && c < D) {
         const uint32_t row = ri_next & ~kFreshBit;
         prefetch_l2(a.td.emb + (size_t)row * a.td.emb_stride + c);
@@ -954,10 +996,37 @@ __global__ void __launch_bounds__(kThreads) runs_apply_kernel(BwdArgs a, int pre
         }
       }
     }
-    float4 g4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (c < D) g4 = __ldcs(reinterpret_cast<const float4*>(a.ugrad + (size_t)j * D + c));
     if (ri == kEmptyRow) continue;
     const RowPre pre = bwd_prefetch<G, OPT>(a, ri, c);
+    float4 g4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (re - rs > (uint32_t)kApplyRun) {
+      if (c < D) g4 = __ldcs(reinterpret_cast<const float4*>(a.ugrad + (size_t)j * D + c));
+    } else {
+      for (uint32_t k0 = rs; k0 < re; k0 += kApplyStage) {
+        const int n = (int)min(re - k0, (uint32_t)kApplyStage);
+        uint32_t m[kApplyStage];
+#pragma unroll
+        for (int u = 0; u < kApplyStage; ++u)  // the first position is p0: a one-occurrence run (most runs) has no hop
+          m[u] = u >= n ? 0u : (u == 0 && k0 == rs) ? p0 : a.sorted[k0 + u].y;
+#pragma unroll
+        for (int u = 0; u < kApplyStage; ++u)
+          if (u < n && c < D) cp_async16(&stage[u][threadIdx.x], occ_grad_src(gs, m[u], c));
+        asm volatile("cp.async.commit_group;" ::: "memory");
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+#pragma unroll
+        for (int u = 0; u < kApplyStage; ++u) {
+          if (u >= n) break;
+          float4 x = stage[u][threadIdx.x];
+          if (gs.mean) {
+            const float fn = occ_grad_div(gs, m[u]);
+            if (fn != 0.f) {
+              x.x = __fdiv_rn(x.x, fn); x.y = __fdiv_rn(x.y, fn); x.z = __fdiv_rn(x.z, fn); x.w = __fdiv_rn(x.w, fn);
+            }
+          }
+          if (k0 == rs && u == 0) g4 = x; else add4(g4, x);
+        }
+      }
+    }
     bwd_apply<G, OPT>(a, (uint32_t)j, ri, g4, c, pre);
   }
 }
@@ -1253,7 +1322,7 @@ static SegArgs seg_args(const BwdScratch& w, int64_t M, int D, const float* pool
 
 constexpr size_t kStageBytes = sizeof(float4) * kStage * kThreads;
 template <int GL, int VPL, bool PLAIN, bool AHEAD>
-static void launch_seg2(const SegArgs& sa, const PeerOut& po, cudaStream_t s) {
+static void launch_seg2(const SegArgs& sa, const PeerOut& po, bool defer_short, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
     MONO_CUDA(cudaFuncSetAttribute(seg_reduce_kernel<GL, VPL, PLAIN, AHEAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1263,17 +1332,18 @@ static void launch_seg2(const SegArgs& sa, const PeerOut& po, cudaStream_t s) {
   seg_reduce_kernel<GL, VPL, PLAIN, AHEAD>
       <<<resident_grid(seg_reduce_kernel<GL, VPL, PLAIN, AHEAD>, sa.n_pieces, (kThreads / 32) * (32 / GL), kThreads,
                        kStageBytes),
-         kThreads, kStageBytes, s>>>(sa, po);
+         kThreads, kStageBytes, s>>>(sa, po, defer_short ? 1 : 0);
   MONO_CHECK_LAUNCH();
 }
 template <int GL, int VPL, bool PLAIN>
-static void launch_seg(const SegArgs& sa, const PeerOut& po, cudaStream_t s) {
-  if (knob(KNOB_SEG_AHEAD)) launch_seg2<GL, VPL, PLAIN, true>(sa, po, s);
-  else launch_seg2<GL, VPL, PLAIN, false>(sa, po, s);
+static void launch_seg(const SegArgs& sa, const PeerOut& po, bool defer_short, cudaStream_t s) {
+  if (knob(KNOB_SEG_AHEAD)) launch_seg2<GL, VPL, PLAIN, true>(sa, po, defer_short, s);
+  else launch_seg2<GL, VPL, PLAIN, false>(sa, po, defer_short, s);
 }
 
-// per-run gradient sums -> run_dst (a.ugrad, or the owners' peer windows)
-static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, cudaStream_t s) {
+// per-run gradient sums -> run_dst (a.ugrad, or the owners' peer windows).  defer_short: runs_apply_kernel follows
+// and sums the runs of at most kApplyRun occurrences itself, so only the longer runs' sums are stored.
+static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, bool defer_short, cudaStream_t s) {
   const int64_t nr = sa.n_pieces;
   if (nr <= 0) return;
   // the tree depth follows the range's occurrence count (the whole list but for one table of a parts call)
@@ -1299,11 +1369,11 @@ static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, cudaStrea
       attr_set = true;                                                                                              \
     }                                                                                                               \
     if (two && GG >= 8) {                                                                                           \
-      if (plain) launch_seg<(GG >= 8 ? GG / 2 : GG), (GG >= 8 ? 2 : 1), true>(sa, po, s);                           \
-      else launch_seg<(GG >= 8 ? GG / 2 : GG), (GG >= 8 ? 2 : 1), false>(sa, po, s);                                \
+      if (plain) launch_seg<(GG >= 8 ? GG / 2 : GG), (GG >= 8 ? 2 : 1), true>(sa, po, defer_short, s);              \
+      else launch_seg<(GG >= 8 ? GG / 2 : GG), (GG >= 8 ? 2 : 1), false>(sa, po, defer_short, s);                   \
     } else {                                                                                                        \
-      if (plain) launch_seg<GG, 1, true>(sa, po, s);                                                                \
-      else launch_seg<GG, 1, false>(sa, po, s);                                                                     \
+      if (plain) launch_seg<GG, 1, true>(sa, po, defer_short, s);                                                   \
+      else launch_seg<GG, 1, false>(sa, po, defer_short, s);                                                        \
     }                                                                                                               \
     uint32_t stride = 1;                                                                                            \
     for (int l = 0; l < levels; ++l, stride *= kTreeFan) {                                                          \
@@ -1339,8 +1409,11 @@ static int apply_opt_sel(const HostTable& ht) {
 // the optimizer step of every run of the reduce's range (M: its occurrence count, sizes the grid)
 static void launch_apply(const BwdArgs& a, int G, int opt_sel, int64_t M, cudaStream_t s) {
   const int pf = knob(KNOB_APPLY_PF);
-#define BWD2(GG, OO)                                                                                             \
-  runs_apply_kernel<GG, OO><<<resident_grid(runs_apply_kernel<GG, OO>, M, kThreads / GG), kThreads, 0, s>>>(a, pf);  \
+  constexpr size_t smem = sizeof(float4) * kApplyStage * kThreads;
+  static_assert(smem <= 48 * 1024, "runs_apply_kernel's stage fits the default dynamic shared memory limit");
+#define BWD2(GG, OO)                                                                                              \
+  runs_apply_kernel<GG, OO><<<resident_grid(runs_apply_kernel<GG, OO>, M, kThreads / GG, kThreads, smem), kThreads, \
+                              smem, s>>>(a, pf);                                                                  \
   MONO_CHECK_LAUNCH()
 #define BWD(GG)                                                         \
   switch (opt_sel) {                                                    \
@@ -1424,7 +1497,7 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
   a.rowidx = w.sort.rowidx;
   a.lr = cb.lr;
   a.scratch = a.ugrad;
-  launch_reduce(sa, G, no_peer, s);
+  launch_reduce(sa, G, no_peer, true, s);
   // 6 apply: one streaming pass over the runs — row index, summed gradient, w / optimizer state of every distinct FID
   launch_apply(a, G, apply_opt_sel(ht), M, s);
   ht.issued_total += (uint64_t)M;
@@ -1638,7 +1711,7 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
     a.lr = cb.lr + segs[q].lr_off;
     a.scratch = a.ugrad;
     const int G = pick_group(ht.dim);
-    launch_reduce(sa, G, no_peer, s);
+    launch_reduce(sa, G, no_peer, true, s);
     launch_apply(a, G, apply_opt_sel(ht), Mk, s);
     ht.issued_total += (uint64_t)Mk;
     ht.max_update_ts = std::max<int64_t>(ht.max_update_ts, update_time);
@@ -1675,7 +1748,7 @@ void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, c
   w.sorted = sort_and_runs(w.sort, reinterpret_cast<const uint32_t*>(offs_dev), M, bits, shift, nullptr, s);
   const SegArgs sa = seg_args(w, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, w.ugrad, s);
   const int G = pick_group(D);
-  launch_reduce(sa, G, no_peer, s);
+  launch_reduce(sa, G, no_peer, false, s);
 #define EMIT(GG)                                                                                              \
   runs_emit_kernel<GG><<<resident_grid(runs_emit_kernel<GG>, M, kThreads / GG), kThreads, 0, s>>>(sa.b, shift, out_rows); \
   MONO_CHECK_LAUNCH()
@@ -1820,7 +1893,7 @@ static void grouping_reduce_impl(mono_grouping* g, const float* pooled_grad, int
   // runs are already in the bucketed order: the sums are written in place
   const SegArgs sa = seg_args(g->plan, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling,
                               out_rows, s);
-  launch_reduce(sa, pick_group(D), po, s);
+  launch_reduce(sa, pick_group(D), po, false, s);
 }
 
 // out_rows[u] = summed gradient of the u-th distinct FID of the bucketed list (ref: ScatterGrad)
