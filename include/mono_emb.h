@@ -264,6 +264,35 @@ int mono_mtable_pool_backward_parts(mono_mtable_t* t, const mono_pool_part* part
                                     const float* learning_rate_host /*[sum_k slice_size(k)]*/,
                                     int64_t update_time, int64_t global_step, void* stream);
 
+/* ---- the parts calls with bfloat16 rows ------------------------------------------------------
+ * The arguments of mono_mtable_lookup_pool_parts / mono_mtable_pool_backward_parts, but every part's
+ * rows_dev points at bfloat16 storage (a cast pointer; the struct is unchanged), and stride and col
+ * count bf16 elements (a FIRSTN part's position j sits at + j*dim bf16 elements).  Tables, optimizer
+ * state and all arithmetic stay fp32: only the rows handed in or back are bf16.
+ *
+ * mono_mtable_lookup_pool_parts_bf16: each output element is the fp32 value
+ * mono_mtable_lookup_pool_parts writes for the same part (accumulated in fp32 in the same order),
+ * rounded once to bf16 to nearest even (__float2bfloat16_rn); absent FIDs and empty FIRSTN
+ * positions are +0.0, NaN stays NaN (payload unspecified).  Any dim up to 512, any stride and
+ * column, parts writing disjoint columns of one tensor, and the same errors: as the fp32 call.
+ * Kernel launches: one per distinct bf16 kernel instantiation among the parts.  A one-FID part
+ * never takes the TMA-staged lookup (it moves rows without touching registers, and the conversion
+ * needs them): it runs the register-path lookup kernel at every dim.  The lookup_dual option does
+ * not apply.
+ *
+ * mono_mtable_pool_backward_parts_bf16: bit for bit the result of mono_mtable_pool_backward_parts
+ * on the same parts with every gradient row widened exactly to fp32 (table entries, optimizer
+ * state, timestamps, admission-filter counts, the sum's association and tree depth); the MEAN
+ * division and every add happen in fp32 after the widening.  Same launches as the fp32 call.
+ * MONO_ERR_INVALID_ARGUMENT, before any device work (no table changes): the fp32 call's conditions,
+ * with the row condition dim % 4 == 0, dim <= 128, stride % 4 == 0, col % 4 == 0 and 8-byte
+ * aligned rows. */
+int mono_mtable_lookup_pool_parts_bf16(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                       void* stream);
+int mono_mtable_pool_backward_parts_bf16(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                         const float* learning_rate_host /*[sum_k slice_size(k)]*/,
+                                         int64_t update_time, int64_t global_step, void* stream);
+
 /* ---- updates ----------------------------------------------------------------------------- */
 
 #define MONO_FLAG_IDS_UNIQUE 1u      /* caller guarantees ids unique per table within this call   */

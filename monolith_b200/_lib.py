@@ -80,6 +80,8 @@ SIGNATURES = {
     "mono_mtable_pool_backward": (C.c_int, [_p, _i32, _p, _i64, _p, _i64, _i32, _p, _i64, _i32, _p, _i64, _i64, _p]),
     "mono_mtable_lookup_pool_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p]),
     "mono_mtable_pool_backward_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p]),
+    "mono_mtable_lookup_pool_parts_bf16": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p]),
+    "mono_mtable_pool_backward_parts_bf16": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p]),
     "mono_mtable_optimize": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i64, _u32, _p]),
     "mono_mtable_fused_optimize": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i32, _u32, _p]),
     "mono_mtable_assign": (C.c_int, [_p, _p, _p, _p, _i64, _u32, _p]),

@@ -407,7 +407,8 @@ struct GradSrc {
   int64_t stride;
   const uint32_t* occ_row;
   const int32_t* row_offsets;
-  const float* const* occ_src;  // parts call: gradient row (column included) of every occurrence
+  const float* const* occ_src;  // parts call: gradient row (column included) of every occurrence; bf16 rows: a cast
+                                // pointer to the row's bf16 elements
   const float* occ_div;         // parts call: MEAN divisor of every occurrence, 0 = none
   bool mean;
 };
@@ -422,10 +423,11 @@ __device__ __forceinline__ GradSrc make_grad_src(const BwdArgs& a, int c) {
   g.mean = a.pooling == MONO_POOL_MEAN && (a.row_offsets != nullptr || a.occ_div != nullptr);
   return g;
 }
-// gradient row of occurrence m, from column c (the lane's; gs.base already holds it)
-__device__ __forceinline__ const float* occ_grad_src(const GradSrc& gs, uint32_t m, int c) {
-  if (gs.occ_src) return gs.occ_src[m] + c;
-  return gs.base + (size_t)(gs.occ_row ? gs.occ_row[m] : m) * gs.stride;
+// gradient row of occurrence m, from column c (the lane's; gs.base already holds it); T = __nv_bfloat16: occ_src only
+template <typename T>
+__device__ __forceinline__ const T* occ_grad_src(const GradSrc& gs, uint32_t m, int c) {
+  if (gs.occ_src) return reinterpret_cast<const T*>(gs.occ_src[m]) + c;
+  return reinterpret_cast<const T*>(gs.base + (size_t)(gs.occ_row ? gs.occ_row[m] : m) * gs.stride);
 }
 // MEAN divisor of occurrence m (gs.mean only; 0 = none)
 __device__ __forceinline__ float occ_grad_div(const GradSrc& gs, uint32_t m) {
@@ -648,9 +650,10 @@ __device__ __forceinline__ void fetch4(const uint32_t (&v)[32 / G], int e, uint3
 // defer_short (the fused backward): the runs of at most kApplyRun occurrences are summed by runs_apply_kernel, which
 // reads their gradient rows itself; this kernel skips their units, so a piece without any other unit costs its item
 // loads and its meta stores only.
-template <int G, int VPL, bool PLAIN, bool AHEAD>
-__global__ void __launch_bounds__(kThreads, 3)
-seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short) {
+// T: the gradient row element (float; __nv_bfloat16 for bf16 parts: each lane stages its 4 elements, 8 bytes, in the
+// first half of its 16-byte slot and widens them to fp32 when it reads the slot back).
+template <typename T, int G, int VPL, bool PLAIN, bool AHEAD>
+__device__ __forceinline__ void seg_reduce(const SegArgs& sa, const PeerOut& po, int defer_short) {
   __shared__ int64_t s_start[kMaxPeers + 1];
   __shared__ char* s_base[kMaxPeers];
   extern __shared__ float4 stage_raw[];        // [kStage][kThreads]: [slot][thread], conflict-free 16-byte accesses
@@ -784,10 +787,11 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short) {
           const int e = eb + u;
           if (e >= e_begin && e < e_stop && !(e < kPiece && ((SK >> e) & 1u))) {
             const uint32_t r = (!PLAIN && gs.occ_row) ? gs.occ_row[m[u]] : m[u];
-            const float* src = (!PLAIN && gs.occ_src) ? gs.occ_src[m[u]] + c : gs.base + (size_t)r * gs.stride;
+            const T* src = (!PLAIN && gs.occ_src) ? reinterpret_cast<const T*>(gs.occ_src[m[u]]) + c
+                                                  : reinterpret_cast<const T*>(gs.base + (size_t)r * gs.stride);
 #pragma unroll
             for (int v = 0; v < VPL; ++v)
-              if (in[v]) cp_async16(&stage[(b4 + u) * VPL + v][threadIdx.x], src + v * G * 4);
+              if (in[v]) cp_async_row4(&stage[(b4 + u) * VPL + v][threadIdx.x], src + v * G * 4);
           }
         }
       }
@@ -823,7 +827,7 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short) {
 #pragma unroll
           for (int v = 0; v < VPL; ++v) {
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (in[v]) x = stage[(b4 + u) * VPL + v][threadIdx.x];
+            if (in[v]) x = stage_row4<T>(&stage[(b4 + u) * VPL + v][threadIdx.x]);
             if (!PLAIN && gs.mean && fn[u] != 0.f) {
               x.x = __fdiv_rn(x.x, fn[u]); x.y = __fdiv_rn(x.y, fn[u]); x.z = __fdiv_rn(x.z, fn[u]); x.w = __fdiv_rn(x.w, fn[u]);
             }
@@ -843,6 +847,19 @@ seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short) {
       }
     }
   }
+}
+
+template <int G, int VPL, bool PLAIN, bool AHEAD>
+__global__ void __launch_bounds__(kThreads, 3)
+seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short) {
+  seg_reduce<float, G, VPL, PLAIN, AHEAD>(sa, po, defer_short);
+}
+
+// bf16 gradient rows of a parts call (always through the occurrence map, so there is no PLAIN form)
+template <int G, int VPL, bool AHEAD>
+__global__ void __launch_bounds__(kThreads, 3)
+bf16_seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short) {
+  seg_reduce<__nv_bfloat16, G, VPL, false, AHEAD>(sa, po, defer_short);
 }
 
 // One level of the fixed tree over the block index of the long runs: the slot of block k, k a multiple of
@@ -957,8 +974,9 @@ long_finish_kernel(SegArgs sa, uint32_t top, const PeerOut po) {
 // (A variant that handled two runs per group at a time needs 62 registers, which lowers occupancy.)
 // The next run's row index and run bounds are read one iteration ahead.  prefetch != 0: its weight / state rows are
 // also pulled into L2 meanwhile.
-template <int G, int OPT>
-__global__ void __launch_bounds__(kThreads) runs_apply_kernel(BwdArgs a, int prefetch) {
+// T: the gradient row element, as in seg_reduce.
+template <typename T, int G, int OPT>
+__device__ __forceinline__ void runs_apply(const BwdArgs& a, int prefetch) {
   extern __shared__ float4 stage_raw[];  // [kApplyStage][kThreads]
   float4 (*stage)[kThreads] = reinterpret_cast<float4 (*)[kThreads]>(stage_raw);
   const int gl = Group<G>::gl();
@@ -1010,13 +1028,13 @@ __global__ void __launch_bounds__(kThreads) runs_apply_kernel(BwdArgs a, int pre
           m[u] = u >= n ? 0u : (u == 0 && k0 == rs) ? p0 : a.sorted[k0 + u].y;
 #pragma unroll
         for (int u = 0; u < kApplyStage; ++u)
-          if (u < n && c < D) cp_async16(&stage[u][threadIdx.x], occ_grad_src(gs, m[u], c));
+          if (u < n && c < D) cp_async_row4(&stage[u][threadIdx.x], occ_grad_src<T>(gs, m[u], c));
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group 0;" ::: "memory");
 #pragma unroll
         for (int u = 0; u < kApplyStage; ++u) {
           if (u >= n) break;
-          float4 x = stage[u][threadIdx.x];
+          float4 x = stage_row4<T>(&stage[u][threadIdx.x]);
           if (gs.mean) {
             const float fn = occ_grad_div(gs, m[u]);
             if (fn != 0.f) {
@@ -1029,6 +1047,16 @@ __global__ void __launch_bounds__(kThreads) runs_apply_kernel(BwdArgs a, int pre
     }
     bwd_apply<G, OPT>(a, (uint32_t)j, ri, g4, c, pre);
   }
+}
+
+template <int G, int OPT>
+__global__ void __launch_bounds__(kThreads) runs_apply_kernel(BwdArgs a, int prefetch) {
+  runs_apply<float, G, OPT>(a, prefetch);
+}
+
+template <int G, int OPT>
+__global__ void __launch_bounds__(kThreads) bf16_runs_apply_kernel(BwdArgs a, int prefetch) {
+  runs_apply<__nv_bfloat16, G, OPT>(a, prefetch);
 }
 
 // run j of the sorted offsets -> destination row: out_rows + (sorted key << shift)
@@ -1261,13 +1289,15 @@ static BwdScratch scratch_plan(int64_t M, int D, int bits, unsigned parts, char*
   return w;
 }
 
-// The reduce reads and writes gradient rows as 16-byte vectors, one per lane of a group of at most 32 lanes.
+// The reduce reads and writes gradient rows as 4-element vectors (16 bytes; 8 of bf16 rows, elem_bytes = 2), one
+// per lane of a group of at most 32 lanes.
 static void check_grad_rows(const char* who, int D, const float* pooled_grad = nullptr, int64_t grad_stride = 0,
-                            int grad_col = 0, const float* out_rows = nullptr) {
+                            int grad_col = 0, const float* out_rows = nullptr, int elem_bytes = 4) {
   if ((D & 3) || D > 128) throw ArgError(std::string(who) + " needs dim % 4 == 0 and dim <= 128");
-  if ((grad_stride & 3) || (grad_col & 3) || (reinterpret_cast<uintptr_t>(pooled_grad) & 15) ||
-      (reinterpret_cast<uintptr_t>(out_rows) & 15))
-    throw ArgError(std::string(who) + " needs 16-byte aligned rows");
+  const uintptr_t amask = 4 * (uintptr_t)elem_bytes - 1;
+  if ((grad_stride & 3) || (grad_col & 3) || (reinterpret_cast<uintptr_t>(pooled_grad) & amask) ||
+      (reinterpret_cast<uintptr_t>(out_rows) & amask))
+    throw ArgError(std::string(who) + " needs " + std::to_string(4 * elem_bytes) + "-byte aligned rows");
 }
 
 // One table's share of a parts call: the sorted range [lo, hi) and whether any of its parts pools by MEAN
@@ -1321,29 +1351,31 @@ static SegArgs seg_args(const BwdScratch& w, int64_t M, int D, const float* pool
 }
 
 constexpr size_t kStageBytes = sizeof(float4) * kStage * kThreads;
-template <int GL, int VPL, bool PLAIN, bool AHEAD>
+// BF16: bf16_seg_reduce_kernel<GL, VPL, AHEAD> (PLAIN is then false)
+template <int GL, int VPL, bool PLAIN, bool AHEAD, bool BF16>
 static void launch_seg2(const SegArgs& sa, const PeerOut& po, bool defer_short, cudaStream_t s) {
+  void (*const kern)(SegArgs, const PeerOut, int) =
+      BF16 ? bf16_seg_reduce_kernel<GL, VPL, AHEAD> : seg_reduce_kernel<GL, VPL, PLAIN, AHEAD>;
   static bool attr_set = false;
   if (!attr_set) {
-    MONO_CUDA(cudaFuncSetAttribute(seg_reduce_kernel<GL, VPL, PLAIN, AHEAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)kStageBytes));
+    MONO_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStageBytes));
     attr_set = true;
   }
-  seg_reduce_kernel<GL, VPL, PLAIN, AHEAD>
-      <<<resident_grid(seg_reduce_kernel<GL, VPL, PLAIN, AHEAD>, sa.n_pieces, (kThreads / 32) * (32 / GL), kThreads,
-                       kStageBytes),
-         kThreads, kStageBytes, s>>>(sa, po, defer_short ? 1 : 0);
+  kern<<<resident_grid(kern, sa.n_pieces, (kThreads / 32) * (32 / GL), kThreads, kStageBytes), kThreads, kStageBytes,
+         s>>>(sa, po, defer_short ? 1 : 0);
   MONO_CHECK_LAUNCH();
 }
-template <int GL, int VPL, bool PLAIN>
+template <int GL, int VPL, bool PLAIN, bool BF16 = false>
 static void launch_seg(const SegArgs& sa, const PeerOut& po, bool defer_short, cudaStream_t s) {
-  if (knob(KNOB_SEG_AHEAD)) launch_seg2<GL, VPL, PLAIN, true>(sa, po, defer_short, s);
-  else launch_seg2<GL, VPL, PLAIN, false>(sa, po, defer_short, s);
+  if (knob(KNOB_SEG_AHEAD)) launch_seg2<GL, VPL, PLAIN, true, BF16>(sa, po, defer_short, s);
+  else launch_seg2<GL, VPL, PLAIN, false, BF16>(sa, po, defer_short, s);
 }
 
 // per-run gradient sums -> run_dst (a.ugrad, or the owners' peer windows).  defer_short: runs_apply_kernel follows
 // and sums the runs of at most kApplyRun occurrences itself, so only the longer runs' sums are stored.
-static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, bool defer_short, cudaStream_t s) {
+// bf16: the gradient rows are bf16 (parts call); the tree and finish kernels add fp32 partials either way.
+static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, bool defer_short, cudaStream_t s,
+                          bool bf16 = false) {
   const int64_t nr = sa.n_pieces;
   if (nr <= 0) return;
   // the tree depth follows the range's occurrence count (the whole list but for one table of a parts call)
@@ -1369,10 +1401,12 @@ static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, bool defe
       attr_set = true;                                                                                              \
     }                                                                                                               \
     if (two && GG >= 8) {                                                                                           \
-      if (plain) launch_seg<(GG >= 8 ? GG / 2 : GG), (GG >= 8 ? 2 : 1), true>(sa, po, defer_short, s);              \
+      if (bf16) launch_seg<(GG >= 8 ? GG / 2 : GG), (GG >= 8 ? 2 : 1), false, true>(sa, po, defer_short, s);        \
+      else if (plain) launch_seg<(GG >= 8 ? GG / 2 : GG), (GG >= 8 ? 2 : 1), true>(sa, po, defer_short, s);         \
       else launch_seg<(GG >= 8 ? GG / 2 : GG), (GG >= 8 ? 2 : 1), false>(sa, po, defer_short, s);                   \
     } else {                                                                                                        \
-      if (plain) launch_seg<GG, 1, true>(sa, po, defer_short, s);                                                   \
+      if (bf16) launch_seg<GG, 1, false, true>(sa, po, defer_short, s);                                             \
+      else if (plain) launch_seg<GG, 1, true>(sa, po, defer_short, s);                                              \
       else launch_seg<GG, 1, false>(sa, po, defer_short, s);                                                        \
     }                                                                                                               \
     uint32_t stride = 1;                                                                                            \
@@ -1406,15 +1440,18 @@ static int apply_opt_sel(const HostTable& ht) {
   return opt_sel;
 }
 
-// the optimizer step of every run of the reduce's range (M: its occurrence count, sizes the grid)
-static void launch_apply(const BwdArgs& a, int G, int opt_sel, int64_t M, cudaStream_t s) {
+// the optimizer step of every run of the reduce's range (M: its occurrence count, sizes the grid); bf16: bf16
+// gradient rows (parts call)
+static void launch_apply(const BwdArgs& a, int G, int opt_sel, int64_t M, cudaStream_t s, bool bf16 = false) {
   const int pf = knob(KNOB_APPLY_PF);
   constexpr size_t smem = sizeof(float4) * kApplyStage * kThreads;
   static_assert(smem <= 48 * 1024, "runs_apply_kernel's stage fits the default dynamic shared memory limit");
 #define BWD2(GG, OO)                                                                                              \
-  runs_apply_kernel<GG, OO><<<resident_grid(runs_apply_kernel<GG, OO>, M, kThreads / GG, kThreads, smem), kThreads, \
-                              smem, s>>>(a, pf);                                                                  \
-  MONO_CHECK_LAUNCH()
+  do {                                                                                                            \
+    void (*const kern)(BwdArgs, int) = bf16 ? bf16_runs_apply_kernel<GG, OO> : runs_apply_kernel<GG, OO>;         \
+    kern<<<resident_grid(kern, M, kThreads / GG, kThreads, smem), kThreads, smem, s>>>(a, pf);                    \
+    MONO_CHECK_LAUNCH();                                                                                          \
+  } while (0)
 #define BWD(GG)                                                         \
   switch (opt_sel) {                                                    \
     case MONO_OPT_SGD: BWD2(GG, MONO_OPT_SGD); break;                   \
@@ -1554,8 +1591,9 @@ parts_occ_kernel(const PartDev* __restrict__ parts, int n_parts, int64_t n_rows,
 // region per table, so one claim, one sort and one run list serve every table and leave each table's occurrences as
 // one contiguous sorted range; the reduce and the apply then run once per table over its range, with its row width,
 // optimizer and tree depth.  Everything is checked before the first device operation.
+// bf16: every part's rows_dev is bf16 storage (stride and col in bf16 elements); each term is widened to fp32 first.
 void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, const float* lr_host,
-                             int64_t update_time, cudaStream_t s) {
+                             int64_t update_time, cudaStream_t s, bool bf16) {
   const int K = (int)mt->tables.size();
   if (n_parts < 0 || n_parts > MONO_MAX_POOL_PARTS) throw ArgError("pool_backward_parts: bad part count");
   if ((n_parts > 0 && !parts) || !lr_host) throw ArgError("pool_backward_parts: null argument");
@@ -1572,7 +1610,8 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
     if (!p.row_offsets_dev && p.n_rows != p.n_fids)
       throw ArgError("pool_backward_parts: n_rows must equal n_fids without offsets");
     if (p.n_fids > 0 && (!p.fids_dev || !p.rows_dev)) throw ArgError("pool_backward_parts: null argument");
-    check_grad_rows("pool_backward_parts", mt->tables[p.table].dim, p.rows_dev, p.stride, p.col);
+    check_grad_rows("pool_backward_parts", mt->tables[p.table].dim, p.rows_dev, p.stride, p.col, nullptr,
+                    bf16 ? 2 : 4);
     M += p.n_fids;
     if (M > ((int64_t)1 << 30)) throw ArgError("pool_backward_parts: more than 2^30 occurrences in one call");
     if (p.n_fids == 0) continue;
@@ -1644,6 +1683,11 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
       d.mean = p.pooling == MONO_POOL_MEAN && p.row_offsets_dev ? 1 : 0;
       d.seq_len = p.pooling == MONO_POOL_FIRSTN ? p.max_seq_len : 0;
       d.dim = mt->tables[k].dim;
+      if (bf16) {  // parts_occ_kernel steps in floats: half as many floats as bf16 elements (stride, dim % 4 == 0)
+        d.rows = reinterpret_cast<const float*>(reinterpret_cast<const __nv_bfloat16*>(p.rows_dev) + p.col);
+        d.stride = p.stride / 2;
+        d.dim = d.dim / 2;
+      }
       d.pad = 0;
       pd.push_back(d);
       occ_at[k] += p.n_fids;
@@ -1711,8 +1755,8 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
     a.lr = cb.lr + segs[q].lr_off;
     a.scratch = a.ugrad;
     const int G = pick_group(ht.dim);
-    launch_reduce(sa, G, no_peer, true, s);
-    launch_apply(a, G, apply_opt_sel(ht), Mk, s);
+    launch_reduce(sa, G, no_peer, true, s, bf16);
+    launch_apply(a, G, apply_opt_sel(ht), Mk, s, bf16);
     ht.issued_total += (uint64_t)Mk;
     ht.max_update_ts = std::max<int64_t>(ht.max_update_ts, update_time);
     request_snapshot(mt, k, s);

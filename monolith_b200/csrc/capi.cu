@@ -323,7 +323,7 @@ int mono_mtable_lookup_pool_parts(mono_mtable_t* t, const mono_pool_part* parts_
                                   void* stream) {
   return guarded([&] {
     HandleGuard hg_(t);
-    run_lookup_pool_parts(t, parts_host, n_parts, (cudaStream_t)stream);
+    run_lookup_pool_parts(t, parts_host, n_parts, (cudaStream_t)stream, false);
   });
 }
 
@@ -332,7 +332,24 @@ int mono_mtable_pool_backward_parts(mono_mtable_t* t, const mono_pool_part* part
                                     int64_t /*global_step*/, void* stream) {
   return guarded([&] {
     HandleGuard hg_(t);
-    run_pool_backward_parts(t, parts_host, n_parts, learning_rate_host, update_time, (cudaStream_t)stream);
+    run_pool_backward_parts(t, parts_host, n_parts, learning_rate_host, update_time, (cudaStream_t)stream, false);
+  });
+}
+
+int mono_mtable_lookup_pool_parts_bf16(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                       void* stream) {
+  return guarded([&] {
+    HandleGuard hg_(t);
+    run_lookup_pool_parts(t, parts_host, n_parts, (cudaStream_t)stream, true);
+  });
+}
+
+int mono_mtable_pool_backward_parts_bf16(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                         const float* learning_rate_host, int64_t update_time,
+                                         int64_t /*global_step*/, void* stream) {
+  return guarded([&] {
+    HandleGuard hg_(t);
+    run_pool_backward_parts(t, parts_host, n_parts, learning_rate_host, update_time, (cudaStream_t)stream, true);
   });
 }
 

@@ -456,9 +456,10 @@ inline void check_firstn(const char* who, const mono_pool_part& p) {
   if (p.n_rows > ((int64_t)1 << 31) / p.max_seq_len) throw ArgError(std::string(who) + ": n_rows * max_seq_len over 2^31");
 }
 
-void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, cudaStream_t s);
+// bf16: the parts' rows are bfloat16 (the *_parts_bf16 calls)
+void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, cudaStream_t s, bool bf16);
 void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, const float* lr_host,
-                             int64_t update_time, cudaStream_t s);
+                             int64_t update_time, cudaStream_t s, bool bf16);
 
 void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, const int32_t* row_offsets,
                       int64_t n_rows, int pooling, const float* pooled_grad, int64_t grad_stride,

@@ -33,14 +33,15 @@ namespace mono {
 //      16-byte vectors, kRowsInFlight rows per group issued back to back before the first store.
 // Used by lookup / fused_lookup (multi-segment) and by lookup_pool when every pooled row has exactly
 // one FID (the per-slot case of Criteo/MovieLens/DCN-shaped inputs, where pooling is the identity).
-// store one 16-byte vector of a row (vector store when the row base is 16-byte aligned)
-__device__ __forceinline__ void store_vec(float* dst, int c, int D, const float4& x, bool vec_ok) {
+// store one 4-element vector of a row (vector store when the row base is aligned to 4 elements)
+template <typename T>
+__device__ __forceinline__ void store_vec(T* dst, int c, int D, const float4& x, bool vec_ok) {
   if (c >= D) return;
   if (vec_ok) {
-    __stcs(reinterpret_cast<float4*>(dst + c), x);  // streaming: written once, consumed later
+    stcs_row4(dst + c, x);  // streaming: written once, consumed later
   } else {
     const float a[4] = {x.x, x.y, x.z, x.w};
-    for (int w = 0; w < 4 && c + w < D; ++w) dst[c + w] = a[w];
+    for (int w = 0; w < 4 && c + w < D; ++w) dst[c + w] = to_row_elem(a[w], dst);
   }
 }
 
@@ -62,18 +63,20 @@ struct FwdPart {
   int32_t out_col, pooling;
 };
 
-template <int G, bool SINGLE, bool DUAL = false, bool CONFIRM = true>
-__global__ void __launch_bounds__(kThreads, SINGLE && !DUAL ? 6 : 4)
-lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ segs, int nsegs,
-              const int64_t* __restrict__ ids, int64_t n_total, float* __restrict__ out,
-              int64_t out_stride /* <= 0: rows packed at dim floats */, int out_col, int prefetch,
-              const FwdPart* __restrict__ parts = nullptr) {
+// The kernel bodies below are templates on the output row element T (float, or __nv_bfloat16 for the parts calls'
+// bf16 forms, whose FwdPart::out is then a cast pointer); the __global__ kernels instantiate them.
+template <typename T, int G, bool SINGLE, bool DUAL, bool CONFIRM>
+__device__ __forceinline__ void
+lookup_rows(const TableDev* __restrict__ tables, const CallSeg* __restrict__ segs, int nsegs,
+            const int64_t* __restrict__ ids, int64_t n_total, T* __restrict__ out,
+            int64_t out_stride /* <= 0: rows packed at dim elements */, int out_col, int prefetch,
+            const FwdPart* __restrict__ parts) {
   if (SINGLE && parts) {
     const FwdPart& p = parts[blockIdx.y];
     segs = &p.seg;
     ids = p.fids;
     n_total = p.n_rows;
-    out = p.out;
+    out = reinterpret_cast<T*>(p.out);
     out_stride = p.out_stride;
     out_col = p.out_col;
   }
@@ -88,8 +91,8 @@ lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ s
   const float* __restrict__ emb0 = t0->emb;
   const uint32_t stride0 = t0->emb_stride;
   const int64_t rs0 = out_stride > 0 ? out_stride : D0;
-  float* const base0 = out + segs[0].val_off - segs[0].id_begin * rs0 + out_col;
-  const bool vec0 = (D0 & 3) == 0 && (rs0 & 3) == 0 && (reinterpret_cast<uintptr_t>(base0) & 15) == 0;
+  T* const base0 = out + segs[0].val_off - segs[0].id_begin * rs0 + out_col;
+  const bool vec0 = (D0 & 3) == 0 && (rs0 & 3) == 0 && (reinterpret_cast<uintptr_t>(base0) & (4 * sizeof(T) - 1)) == 0;
   const int64_t wstride = (int64_t)gridDim.x * (kThreads / 32) * 32;
   const int64_t wfirst = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * 32;
   // the chain per tile is FID -> bucket -> row (one HBM latency per dependent round trip): the NEXT tile's FIDs are
@@ -144,7 +147,7 @@ lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ s
         const int s_st = SINGLE ? 0 : __shfl_sync(0xffffffffu, si, src_lane);
         if (ir >= n_total) continue;
         if (SINGLE) {
-          float* dst = base0 + ir * rs0;
+          T* dst = base0 + ir * rs0;
           store_vec(dst, c, D0, x[u], vec0);
           if (D0 > 4 * G) {  // wide rows (dim > 128, G == 32): remaining vectors of the row
             const uint32_t r = r_st;
@@ -159,8 +162,8 @@ lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ s
           const TableDev* t = tables + sg.table;
           const int D = t->dim;
           const int64_t rs = out_stride > 0 ? out_stride : D;
-          float* dst = out + sg.val_off + (ir - sg.id_begin) * rs + out_col;
-          const bool vec_ok = (D & 3) == 0 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0;
+          T* dst = out + sg.val_off + (ir - sg.id_begin) * rs + out_col;
+          const bool vec_ok = (D & 3) == 0 && (reinterpret_cast<uintptr_t>(dst) & (4 * sizeof(T) - 1)) == 0;
           store_vec(dst, c, D, x[u], vec_ok);
           if (D > 4 * G) {
             const uint32_t r = r_st;
@@ -176,15 +179,31 @@ lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ s
   }
 }
 
+template <int G, bool SINGLE, bool DUAL = false, bool CONFIRM = true>
+__global__ void __launch_bounds__(kThreads, SINGLE && !DUAL ? 6 : 4)
+lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ segs, int nsegs,
+              const int64_t* __restrict__ ids, int64_t n_total, float* __restrict__ out,
+              int64_t out_stride /* <= 0: rows packed at dim floats */, int out_col, int prefetch,
+              const FwdPart* __restrict__ parts = nullptr) {
+  lookup_rows<float, G, SINGLE, DUAL, CONFIRM>(tables, segs, nsegs, ids, n_total, out, out_stride, out_col, prefetch,
+                                               parts);
+}
+
+// one-FID parts of lookup_pool_parts_bf16 (lookup_kernel<G, true, false, CONFIRM> with bf16 rows)
+template <int G, bool CONFIRM>
+__global__ void __launch_bounds__(kThreads, 6)
+bf16_lookup_kernel(const TableDev* __restrict__ tables, int prefetch, const FwdPart* __restrict__ parts) {
+  lookup_rows<__nv_bfloat16, G, true, false, CONFIRM>(tables, nullptr, 1, nullptr, 0, nullptr, 0, 0, prefetch, parts);
+}
+
 // FIRSTN parts of lookup_pool_parts (ref: GatherEmb's FIRSTN branch, fused_embedding_to_layout.h:251-256): part
 // blockIdx.y writes n_rows x L positions of dim floats, position j of row r at out + r*out_stride + out_col + j*dim.
 // lookup_kernel<G, true>'s two phases over position slots q = r*L + j instead of ids: a slot with j < n_r probes
 // FID fids[offs[r] + j] (lane per key), a slot with j >= n_r probes nothing; phase B copies a found row and stores
 // zeros for the rest.  n_rows * L <= 2^31 (checked by the launcher), so slots divide in 32 bits.  4 blocks per SM
 // (64 registers): at 6 (40 registers) it spills, and so it does with lookup_kernel's next-tile FID prefetch.
-template <int G, bool CONFIRM>
-__global__ void __launch_bounds__(kThreads, 4)
-lookup_seq_kernel(const FwdPart* __restrict__ parts) {
+template <typename T, int G, bool CONFIRM>
+__device__ __forceinline__ void seq_rows(const FwdPart* __restrict__ parts) {
   const FwdPart& p = parts[blockIdx.y];
   const uint32_t L = (uint32_t)p.seg.lr_off;
   const int64_t n_total = p.n_rows * L;
@@ -200,8 +219,8 @@ lookup_seq_kernel(const FwdPart* __restrict__ parts) {
   const float* __restrict__ emb0 = t0->emb;
   const uint32_t stride0 = t0->emb_stride;
   const int64_t rs0 = p.out_stride;
-  float* const base0 = p.out + p.out_col;
-  const bool vec0 = (D0 & 3) == 0 && (rs0 & 3) == 0 && (reinterpret_cast<uintptr_t>(base0) & 15) == 0;
+  T* const base0 = reinterpret_cast<T*>(p.out) + p.out_col;
+  const bool vec0 = (D0 & 3) == 0 && (rs0 & 3) == 0 && (reinterpret_cast<uintptr_t>(base0) & (4 * sizeof(T) - 1)) == 0;
   // slot q -> its row r, and its FID when position j = q - r*L holds one
   auto slot = [&](int64_t q, int64_t& key, uint32_t& r) -> bool {
     r = (uint32_t)q / L;
@@ -245,7 +264,7 @@ lookup_seq_kernel(const FwdPart* __restrict__ parts) {
         const uint32_t rq_st = __shfl_sync(0xffffffffu, rq, src_lane);
         const int64_t ir = wbase + src_lane;
         if (ir >= n_total) continue;
-        float* dst = base0 + (int64_t)rq_st * rs0 + (int64_t)((uint32_t)ir - rq_st * L) * D0;
+        T* dst = base0 + (int64_t)rq_st * rs0 + (int64_t)((uint32_t)ir - rq_st * L) * D0;
         store_vec(dst, c, D0, x[u], vec0);
         for (int cc = c + 4 * G; cc < D0; cc += 4 * G) {  // wide rows (dim > 128, G == 32)
           float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -255,6 +274,18 @@ lookup_seq_kernel(const FwdPart* __restrict__ parts) {
       }
     }
   }
+}
+
+template <int G, bool CONFIRM>
+__global__ void __launch_bounds__(kThreads, 4)
+lookup_seq_kernel(const FwdPart* __restrict__ parts) {
+  seq_rows<float, G, CONFIRM>(parts);
+}
+
+template <int G, bool CONFIRM>
+__global__ void __launch_bounds__(kThreads, 4)
+bf16_seq_kernel(const FwdPart* __restrict__ parts) {
+  seq_rows<__nv_bfloat16, G, CONFIRM>(parts);
 }
 
 // Owner lookup fused with the row exchange of the sharded forward (replaces FusedLookup + the
@@ -488,12 +519,11 @@ lookup_entry_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ 
 // vectors of the embedding row and accumulate in registers; one coalesced store per output row.
 // Terms are added in FID order => bit-exact with the CPU reference's pooling
 // (ref: OptimizedSumpooling, fused_embedding_to_layout.cc:26-59; ReduceSumOp, reduce_op.cc:29-51).
-template <int G, int NV, int U>  // NV = 16-byte vectors per lane (dim <= 4*G*NV); U = rows in flight
-__global__ void __launch_bounds__(kThreads)
-lookup_pool_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ fids,
-                   const int32_t* __restrict__ row_offsets, int64_t n_rows, int pooling,
-                   float* __restrict__ out, int64_t out_stride, int out_col,
-                   const FwdPart* __restrict__ parts = nullptr) {
+template <typename T, int G, int NV, int U>  // NV = 16-byte vectors per lane (dim <= 4*G*NV); U = rows in flight
+__device__ __forceinline__ void
+pool_rows(const TableDev* __restrict__ t, const int64_t* __restrict__ fids, const int32_t* __restrict__ row_offsets,
+          int64_t n_rows, int pooling, T* __restrict__ out, int64_t out_stride, int out_col,
+          const FwdPart* __restrict__ parts) {
   if (parts) {
     const FwdPart& p = parts[blockIdx.y];
     t = p.t;
@@ -501,7 +531,7 @@ lookup_pool_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ f
     row_offsets = p.row_offsets;
     n_rows = p.n_rows;
     pooling = p.pooling;
-    out = p.out;
+    out = reinterpret_cast<T*>(p.out);
     out_stride = p.out_stride;
     out_col = p.out_col;
   }
@@ -588,21 +618,36 @@ lookup_pool_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ f
 #pragma unroll
     for (int q = 0; q < U; ++q) {
       if (r[q] >= n_rows) continue;
-      float* dst = out + r[q] * out_stride + out_col;
-      const bool vec_ok = (D & 3) == 0 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0;
+      T* dst = out + r[q] * out_stride + out_col;
+      const bool vec_ok = (D & 3) == 0 && (reinterpret_cast<uintptr_t>(dst) & (4 * sizeof(T) - 1)) == 0;
 #pragma unroll
       for (int v = 0; v < NV; ++v) {
         const int c = (v * G + gl) * 4;
         if (c >= D) continue;
         if (vec_ok) {
-          __stcs(reinterpret_cast<float4*>(dst + c), acc[q][v]);  // streaming: written once, read later
+          stcs_row4(dst + c, acc[q][v]);  // streaming: written once, read later
         } else {
           const float a[4] = {acc[q][v].x, acc[q][v].y, acc[q][v].z, acc[q][v].w};
-          for (int w = 0; w < 4 && c + w < D; ++w) dst[c + w] = a[w];
+          for (int w = 0; w < 4 && c + w < D; ++w) dst[c + w] = to_row_elem(a[w], dst);
         }
       }
     }
   }
+}
+
+template <int G, int NV, int U>
+__global__ void __launch_bounds__(kThreads)
+lookup_pool_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ fids,
+                   const int32_t* __restrict__ row_offsets, int64_t n_rows, int pooling,
+                   float* __restrict__ out, int64_t out_stride, int out_col,
+                   const FwdPart* __restrict__ parts = nullptr) {
+  pool_rows<float, G, NV, U>(t, fids, row_offsets, n_rows, pooling, out, out_stride, out_col, parts);
+}
+
+template <int G, int NV, int U>
+__global__ void __launch_bounds__(kThreads)
+bf16_pool_kernel(const FwdPart* __restrict__ parts) {
+  pool_rows<__nv_bfloat16, G, NV, U>(nullptr, nullptr, nullptr, 0, 0, nullptr, 0, 0, parts);
 }
 
 // CSR pooling, staged: the round-1 kernel above walks a pooled row's FIDs one at a time (FID -> bucket -> row per step:
@@ -612,13 +657,12 @@ lookup_pool_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ f
 // into per-thread shared-memory slots (this lane's 16-byte slice of each row), and the sums run in FID order out of
 // shared memory: three round trips per 16 FIDs instead of two per FID.  Longer lists are walked in chunks of 16 with
 // the accumulators carried.  Terms are added in FID order: bit-exact with the CPU reference's pooling.
-template <int G>
-__global__ void __launch_bounds__(kThreads, 2)
-lookup_pool_staged_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ fids,
-                          const int32_t* __restrict__ row_offsets, int64_t n_rows, int pooling,
-                          float* __restrict__ out, int64_t out_stride, int out_col,
-                          const FwdPart* __restrict__ parts = nullptr) {
-  constexpr int U = 4;
+// T = __nv_bfloat16: the output base only needs 8-byte alignment (4 elements), as the fp32 form's 16.
+template <typename T, int G, int U>  // U: pooled rows per lane group
+__device__ __forceinline__ void
+pool_staged_rows(const TableDev* __restrict__ t, const int64_t* __restrict__ fids,
+                 const int32_t* __restrict__ row_offsets, int64_t n_rows, int pooling, T* __restrict__ out,
+                 int64_t out_stride, int out_col, const FwdPart* __restrict__ parts) {
   if (parts) {
     const FwdPart& p = parts[blockIdx.y];
     t = p.t;
@@ -626,7 +670,7 @@ lookup_pool_staged_kernel(const TableDev* __restrict__ t, const int64_t* __restr
     row_offsets = p.row_offsets;
     n_rows = p.n_rows;
     pooling = p.pooling;
-    out = p.out;
+    out = reinterpret_cast<T*>(p.out);
     out_stride = p.out_stride;
     out_col = p.out_col;
   }
@@ -726,10 +770,27 @@ lookup_pool_staged_kernel(const TableDev* __restrict__ t, const int64_t* __restr
 #pragma unroll
     for (int q = 0; q < U; ++q) {
       if (r0 + q >= n_rows || !in) continue;
-      float* dst = out + (r0 + q) * out_stride + out_col;
-      __stcs(reinterpret_cast<float4*>(dst + c), acc[q]);  // an empty row pools to zeros
+      T* dst = out + (r0 + q) * out_stride + out_col;
+      stcs_row4(dst + c, acc[q]);  // an empty row pools to zeros
     }
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads, 2)
+lookup_pool_staged_kernel(const TableDev* __restrict__ t, const int64_t* __restrict__ fids,
+                          const int32_t* __restrict__ row_offsets, int64_t n_rows, int pooling,
+                          float* __restrict__ out, int64_t out_stride, int out_col,
+                          const FwdPart* __restrict__ parts = nullptr) {
+  constexpr int U = 4;
+  pool_staged_rows<float, G, U>(t, fids, row_offsets, n_rows, pooling, out, out_stride, out_col, parts);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads, 2)
+bf16_pool_staged_kernel(const FwdPart* __restrict__ parts) {
+  constexpr int U = 4;
+  pool_staged_rows<__nv_bfloat16, G, U>(nullptr, nullptr, nullptr, 0, 0, nullptr, 0, 0, parts);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1179,8 +1240,90 @@ struct PoolPlan {
   enum Kind { kTma, kLookup, kStaged, kPool, kSeq } kind;
   int a, b, c;  // kTma: row bytes; kLookup: G, variant (0 dual, 1 no miss confirm, 2 confirm); kStaged: G; kPool: G, nv;
                 // kSeq (FIRSTN, parts only): G, whether misses are confirmed
-  bool operator==(const PoolPlan& o) const { return kind == o.kind && a == o.a && b == o.b && c == o.c; }
+  bool bf16;    // bf16 output rows (lookup_pool_parts_bf16): the bf16_* kernels
+  bool operator==(const PoolPlan& o) const {
+    return kind == o.kind && a == o.a && b == o.b && c == o.c && bf16 == o.bf16;
+  }
 };
+
+// bf16 output rows: the register-path kernels only (the TMA lookup never touches registers, and the conversion needs
+// them), so a one-FID part takes the lookup kernel at any dim; the lookup_dual knob does not apply.
+static PoolPlan plan_lookup_pool_bf16(mono_mtable* mt, const FwdPart& p, cudaStream_t s) {
+  const int D = mt->tables[p.seg.table].dim;
+  const int G = pick_group(D);
+  const bool confirm = mt->lookup_must_confirm(s);
+  const int nv = (D + 4 * G - 1) / (4 * G);
+  PoolPlan pl;
+  if (p.pooling == MONO_POOL_FIRSTN) pl = {PoolPlan::kSeq, G, confirm ? 1 : 0, 0};
+  else if (p.row_offsets == nullptr) pl = {PoolPlan::kLookup, G, confirm ? 2 : 1, 0};
+  else if ((D & 3) == 0 && D <= 128 && (p.out_stride & 3) == 0 && (p.out_col & 3) == 0 &&
+           (reinterpret_cast<uintptr_t>(p.out) & 7) == 0 && p.n_rows < ((int64_t)1 << 31))
+    pl = {PoolPlan::kStaged, G, 0, 0};
+  else pl = {PoolPlan::kPool, G, nv <= 2 ? nv : 4, 0};
+  pl.bf16 = true;
+  return pl;
+}
+
+// a parts launch of a bf16 plan (launch_pool_plan's grids and instantiation choices, bf16 kernels)
+static void launch_pool_plan_bf16(mono_mtable* mt, const PoolPlan& pl, int64_t n_rows, const FwdPart* parts,
+                                  int n_parts, cudaStream_t s) {
+  const dim3 blk(kThreads);
+#define GRID(K, PER, SMEM) dim3(resident_grid(K, n_rows, PER, kThreads, SMEM), n_parts)
+#define BY_G(M)            \
+  switch (pl.a) {          \
+    case 4: M(4); break;   \
+    case 8: M(8); break;   \
+    case 16: M(16); break; \
+    default: M(32); break; \
+  }
+  if (pl.kind == PoolPlan::kSeq) {
+#define LS(GG)                                                                                                  \
+  if (pl.b) bf16_seq_kernel<GG, true><<<GRID((bf16_seq_kernel<GG, true>), kThreads, 0), blk, 0, s>>>(parts);      \
+  else bf16_seq_kernel<GG, false><<<GRID((bf16_seq_kernel<GG, false>), kThreads, 0), blk, 0, s>>>(parts)
+    BY_G(LS)
+#undef LS
+  } else if (pl.kind == PoolPlan::kLookup) {
+    const int pf = knob(KNOB_LOOKUP_PF);
+#define LL(GG)                                                                                                   \
+  if (pl.b == 2)                                                                                                 \
+    bf16_lookup_kernel<GG, true><<<GRID((bf16_lookup_kernel<GG, true>), kThreads, 0), blk, 0, s>>>(mt->d_tables, pf, \
+                                                                                               parts);          \
+  else                                                                                                           \
+    bf16_lookup_kernel<GG, false><<<GRID((bf16_lookup_kernel<GG, false>), kThreads, 0), blk, 0, s>>>(mt->d_tables,  \
+                                                                                                 pf, parts)
+    BY_G(LL)
+#undef LL
+  } else if (pl.kind == PoolPlan::kStaged) {
+    constexpr size_t kStageBytes = sizeof(float4) * kStage * kThreads;
+#define LPS(GG)                                                                                                    \
+  do {                                                                                                             \
+    static bool attr_set = false;                                                                                  \
+    if (!attr_set) {                                                                                               \
+      MONO_CUDA(cudaFuncSetAttribute(bf16_pool_staged_kernel<GG>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
+                                     (int)kStageBytes));                                                           \
+      attr_set = true;                                                                                             \
+    }                                                                                                              \
+    bf16_pool_staged_kernel<GG><<<GRID((bf16_pool_staged_kernel<GG>), (kThreads / GG) * 4, kStageBytes), blk,        \
+                                  kStageBytes, s>>>(parts);                                                        \
+  } while (0)
+    BY_G(LPS)
+#undef LPS
+  } else {
+#define LP(GG, NV, UU) \
+  bf16_pool_kernel<GG, NV, UU><<<GRID((bf16_pool_kernel<GG, NV, UU>), (kThreads / GG) * UU, 0), blk, 0, s>>>(parts)
+    const int G = pl.a, nv = pl.b;
+    if (G == 4) LP(4, 1, 4);
+    else if (G == 8) LP(8, 1, 4);
+    else if (G == 16) LP(16, 1, 4);
+    else if (nv == 1) LP(32, 1, 4);
+    else if (nv == 2) LP(32, 2, 2);
+    else LP(32, 4, 1);
+#undef LP
+  }
+#undef BY_G
+#undef GRID
+  MONO_CHECK_LAUNCH();
+}
 
 static PoolPlan plan_lookup_pool(mono_mtable* mt, const FwdPart& p, cudaStream_t s) {
   const int k = p.seg.table;
@@ -1333,7 +1476,8 @@ static int64_t pool_work(const FwdPart& f) {
 
 // Every SUM / MEAN part exactly as lookup_pool would serve it alone, every FIRSTN part by lookup_seq_kernel, and the
 // parts served by the same kernel share one launch: one grid row per part, the parts' arguments in one staged array.
-void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, cudaStream_t s) {
+// bf16: rows_dev of every part is bf16 storage (stride and col in bf16 elements), served by the bf16_* kernels.
+void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, cudaStream_t s, bool bf16) {
   const int K = (int)mt->tables.size();
   if (n_parts < 0 || n_parts > MONO_MAX_POOL_PARTS) throw ArgError("lookup_pool_parts: bad part count");
   if (n_parts > 0 && !parts) throw ArgError("lookup_pool_parts: null argument");
@@ -1358,7 +1502,7 @@ void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_p
     if (p.n_rows == 0) continue;
     FwdPart f = fwd_part(mt, p.table, p.fids_dev, p.row_offsets_dev, p.n_rows, p.pooling, p.rows_dev, p.stride, p.col);
     if (p.pooling == MONO_POOL_FIRSTN) f.seg.lr_off = p.max_seq_len;
-    const PoolPlan pl = plan_lookup_pool(mt, f, s);
+    const PoolPlan pl = bf16 ? plan_lookup_pool_bf16(mt, f, s) : plan_lookup_pool(mt, f, s);
     size_t g = 0;
     while (g < plans.size() && !(plans[g] == pl)) ++g;
     if (g == plans.size()) {
@@ -1381,7 +1525,8 @@ void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_p
   for (size_t g = 0; g < plans.size(); ++g) {
     FwdPart a = groups[g][0];
     for (const FwdPart& f : groups[g]) a.n_rows = std::max(a.n_rows, pool_work(f));
-    launch_pool_plan(mt, plans[g], a, d, (int)groups[g].size(), s);
+    if (plans[g].bf16) launch_pool_plan_bf16(mt, plans[g], a.n_rows, d, (int)groups[g].size(), s);
+    else launch_pool_plan(mt, plans[g], a, d, (int)groups[g].size(), s);
     d += groups[g].size();
   }
 }

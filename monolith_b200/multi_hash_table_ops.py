@@ -45,7 +45,9 @@ def _f32(t, device) -> torch.Tensor:
 class PoolPart:
   """One feature's slice of a step for lookup_pool_parts / pool_backward_parts: the FIDs of table `slot`, pooled by
   `pooling` ("sum", "mean" or "firstn") into rows (row_offsets: CSR [n_rows + 1] int32, None = one FID per row), and
-  the output or gradient rows `rows` ([n_rows, >= col + dim] float32, the table's dim floats start at column `col`).
+  the output or gradient rows `rows` ([n_rows, >= col + dim] float32 or bfloat16, the table's dim values start at
+  column `col`).  bfloat16 rows go to the engine's bf16 calls: the tables and all arithmetic stay float32, outputs are
+  rounded once to bfloat16 (nearest even) and gradients are widened exactly to float32.
 
   "firstn" is a sequence feature (the reference's FirstN combiner): row r holds max_seq_len positions of dim floats
   from column `col` on ([n_rows, >= col + max_seq_len * dim]; a [B, L, dim] tensor viewed as [B, L * dim] with
@@ -376,10 +378,24 @@ class MultiHashTable:
                                                    int(global_step), _stream(self._device)))
     return self
 
-  def _parts_arr(self, parts: Sequence[PoolPart], forward: bool):
-    """-> (mono_pool_part array, tensors that must stay alive over the call, the parts' row tensors)."""
+  @staticmethod
+  def _parts_dtype(parts: Sequence[PoolPart], dtype=None):
+    """The row dtype of a parts call: `dtype` if given, else the one dtype of the rows passed in, else float32."""
+    if dtype is None:
+      given = {p.rows.dtype for p in parts if p.rows is not None}
+      if len(given) > 1:
+        raise ValueError(f"part rows mix dtypes {sorted(str(d) for d in given)}")
+      dtype = given.pop() if given else torch.float32
+    if dtype not in (torch.float32, torch.bfloat16):
+      raise ValueError(f"part rows must be float32 or bfloat16, not {dtype}")
+    return dtype
+
+  def _parts_arr(self, parts: Sequence[PoolPart], forward: bool, dtype=None):
+    """-> (mono_pool_part array, tensors that must stay alive over the call, the parts' row tensors); rows of the
+    call's dtype (_parts_dtype)."""
     if len(parts) > _lib.MAX_POOL_PARTS:
       raise ValueError(f"at most {_lib.MAX_POOL_PARTS} parts per call")
+    dtype = self._parts_dtype(parts, dtype)
     arr = (_lib.PoolPartC * max(len(parts), 1))()
     keep, outs = [], []
     for i, p in enumerate(parts):
@@ -398,9 +414,11 @@ class MultiHashTable:
       if rows is None:
         if not forward:
           raise ValueError("pool_backward_parts: every part needs its gradient rows")
-        rows = torch.empty(n_rows, width, dtype=torch.float32, device=self._device)
-      if rows.dtype != torch.float32 or rows.device != self._device or rows.stride(1) != 1:
-        raise ValueError("part rows must be float32 on the table's device with unit column stride")
+        rows = torch.empty(n_rows, width, dtype=dtype, device=self._device)
+      if rows.dtype != dtype:
+        raise ValueError(f"part rows are {rows.dtype}, the call's rows are {dtype}")
+      if rows.device != self._device or rows.stride(1) != 1:
+        raise ValueError("part rows must be on the table's device with unit column stride")
       if rows.shape[0] < n_rows or rows.shape[1] < p.col + width:
         raise ValueError("part rows are smaller than [n_rows, col + dim] ([n_rows, col + max_seq_len * dim] for "
                          "'firstn')")
@@ -411,14 +429,20 @@ class MultiHashTable:
                               rows.data_ptr(), rows.stride(0), p.col, p.max_seq_len)
     return arr, keep, outs
 
-  def lookup_pool_parts(self, parts: Sequence[PoolPart]) -> List[torch.Tensor]:
+  def lookup_pool_parts(self, parts: Sequence[PoolPart], dtype: Optional[torch.dtype] = None) -> List[torch.Tensor]:
     """lookup_pool over many features and tables in one call (mono_mtable_lookup_pool_parts): every part's rows
     are bit-identical to lookup_pool on that part alone; parts served by the same kernel share one launch.  A
     "firstn" part writes its [n_rows, max_seq_len, dim] positions (see PoolPart).  A part without `rows` gets a new
     [n_rows, dim] tensor ([n_rows, max_seq_len * dim] for "firstn": .view(n_rows, max_seq_len, dim) gives the
-    sequence); returns each part's rows, in part order."""
-    arr, keep, outs = self._parts_arr(parts, forward=True)
-    _lib.check(self._lib.mono_mtable_lookup_pool_parts(self._h, arr, len(parts), _stream(self._device)))
+    sequence); returns each part's rows, in part order.
+
+    The call's row dtype is `dtype` if given, else that of the rows passed in (all alike), else float32.  With
+    torch.bfloat16 (mono_mtable_lookup_pool_parts_bf16) every row is the float32 result rounded once to bfloat16."""
+    dtype = self._parts_dtype(parts, dtype)
+    arr, keep, outs = self._parts_arr(parts, forward=True, dtype=dtype)
+    fn = (self._lib.mono_mtable_lookup_pool_parts_bf16 if dtype == torch.bfloat16 else
+          self._lib.mono_mtable_lookup_pool_parts)
+    _lib.check(fn(self._h, arr, len(parts), _stream(self._device)))
     del keep
     return outs
 
@@ -427,12 +451,17 @@ class MultiHashTable:
     of one table are ONE batch in part order, so a FID that several features share gets one optimizer step
     with the sum of all its terms; the claim, sort and run list run once for the whole call.  A "firstn" part's
     occurrence j of row r takes position j of the row's gradient, or zeros for j >= max_seq_len: the FID is still
-    inserted, bumped and stepped (with a zero gradient) as the reference's ScatterGrad leaves it."""
-    arr, keep, _ = self._parts_arr(parts, forward=False)
+    inserted, bumped and stepped (with a zero gradient) as the reference's ScatterGrad leaves it.
+
+    Every part's rows share one dtype, float32 or bfloat16; bfloat16 gradients (mono_mtable_pool_backward_parts_bf16)
+    give exactly the bits of this call on the rows widened to float32."""
+    dtype = self._parts_dtype(parts)
+    arr, keep, _ = self._parts_arr(parts, forward=False, dtype=dtype)
     lr = self.learning_rates()
     lr_arr = (C.c_float * max(len(lr), 1))(*lr)
-    _lib.check(self._lib.mono_mtable_pool_backward_parts(self._h, arr, len(parts), lr_arr, int(req_time),
-                                                         int(global_step), _stream(self._device)))
+    fn = (self._lib.mono_mtable_pool_backward_parts_bf16 if dtype == torch.bfloat16 else
+          self._lib.mono_mtable_pool_backward_parts)
+    _lib.check(fn(self._h, arr, len(parts), lr_arr, int(req_time), int(global_step), _stream(self._device)))
     del keep
     return self
 
