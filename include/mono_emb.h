@@ -470,8 +470,20 @@ typedef struct mono_slice_task {
 } mono_slice_task;
 
 /* emb_ptrs_dev: device array of `n_emb` device pointers (one per (table, shard) list, index1 of
- * fid_offset); emb_strides_host[n_emb] = PtrWrapper.offset of each list (1 in v3/v4/v5).
- * out_ptrs_dev: device array of output tensor pointers (zero-filled by this call). */
+ * fid_offset); emb_strides_dev[n_emb] = PtrWrapper.offset of each list (1 in v3/v4/v5).
+ * nfl_offset_dev holds the reference's uint32 words (bit 31 = shared feature), one per entry;
+ * fid_offset_dev the reference's uint64 words.
+ * out_ptrs_dev: device array of output tensor pointers.  The output sizes are not passed: the
+ * forward writes exactly the elements its tasks cover (for every sample b < batch_size, floats
+ * out_col .. out_col + dim of row b, out_col + max_seq_len * dim for FIRSTN, zeros where a sample
+ * has no FIDs or a FIRSTN row is shorter than max_seq_len) and leaves every other element as it
+ * was.  The grad call accumulates into emb_grad_ptrs_dev with float atomics: those buffers must
+ * arrive zero-filled, and elements no FID refers to are left as they are.
+ * Both calls return MONO_ERR_INVALID_ARGUMENT, before any device work, for a task with nfl_idx
+ * outside [0, total_nfl), dim <= 0, a negative slice_start, out_col or out_tensor, an unknown
+ * pooling, FIRSTN with max_seq_len <= 0 or accumulate set, out_row_stride < out_col + dim
+ * (out_col + max_seq_len * dim for FIRSTN); and, once the device is selected, for ADDN members of
+ * one output slice with unequal dims. */
 int mono_embedding_to_layout(int32_t device, const float* const* emb_ptrs_dev,
                              const int32_t* emb_strides_dev, int32_t n_emb,
                              const uint64_t* fid_offset_dev, int64_t total_fid,

@@ -760,6 +760,7 @@ int mono_embedding_to_layout(int32_t device, const float* const* emb_ptrs_dev,
                              const mono_slice_task* tasks_host, int32_t n_tasks,
                              float* const* out_ptrs_dev, void* stream) {
   return guarded([&] {
+    check_layout_tasks(tasks_host, n_tasks, total_nfl);
     MONO_CUDA(cudaSetDevice(device));
     launch_layout(false, const_cast<float* const*>(emb_ptrs_dev), emb_strides_dev, n_emb, fid_offset_dev,
                   total_fid, feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size,
@@ -776,6 +777,7 @@ int mono_embedding_to_layout_grad(int32_t device, float* const* emb_grad_ptrs_de
                                   int32_t n_tasks, const float* const* out_grad_ptrs_dev,
                                   void* stream) {
   return guarded([&] {
+    check_layout_tasks(tasks_host, n_tasks, total_nfl);
     MONO_CUDA(cudaSetDevice(device));
     launch_layout(true, emb_grad_ptrs_dev, emb_strides_dev, n_emb, fid_offset_dev, total_fid,
                   feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host,

@@ -479,6 +479,7 @@ void launch_gather_pool(const float* fused_emb, const int32_t* emb_offset, const
 void launch_gather_pool_grad(const float* pooled_grad, int64_t grad_stride, int grad_col,
                              const int32_t* emb_offset, const int32_t* row_offsets, int64_t n_rows,
                              int dim, int pooling, float* grad_fused, cudaStream_t s);
+void check_layout_tasks(const mono_slice_task* tasks, int n_tasks, int total_nfl);
 void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb_strides_dev,
                    int n_emb, const uint64_t* fid_offset, int64_t total_fid,
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,

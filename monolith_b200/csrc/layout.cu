@@ -311,6 +311,29 @@ __global__ void __launch_bounds__(kThreads) layout_bwd_kernel(LayoutArgs a, int 
   }
 }
 
+// Host-side checks of the tasks: the kernels index with every field unchecked.
+void check_layout_tasks(const mono_slice_task* tasks, int n_tasks, int total_nfl) {
+  if (n_tasks <= 0) return;
+  if (tasks == nullptr) throw ArgError("layout: tasks is null");
+  for (int i = 0; i < n_tasks; ++i) {
+    const mono_slice_task& t = tasks[i];
+    if (t.nfl_idx < 0 || t.nfl_idx >= total_nfl) throw ArgError("layout: task nfl_idx outside [0, total_nfl)");
+    if (t.dim <= 0) throw ArgError("layout: task dim must be positive");
+    if (t.slice_start < 0 || t.out_col < 0 || t.out_tensor < 0)
+      throw ArgError("layout: task slice_start, out_col and out_tensor must be >= 0");
+    if (t.pooling != MONO_POOL_SUM && t.pooling != MONO_POOL_MEAN && t.pooling != MONO_POOL_FIRSTN)
+      throw ArgError("layout: task pooling must be SUM, MEAN or FIRSTN");
+    int64_t width = t.dim;
+    if (t.pooling == MONO_POOL_FIRSTN) {
+      if (t.max_seq_len <= 0) throw ArgError("layout: FIRSTN task needs max_seq_len >= 1");
+      if (t.accumulate) throw ArgError("layout: FIRSTN task cannot accumulate (ADDN)");
+      width *= t.max_seq_len;
+    }
+    if ((int64_t)t.out_row_stride < (int64_t)t.out_col + width)
+      throw ArgError("layout: task out_row_stride < out_col + dim (+ max_seq_len * dim for FIRSTN)");
+  }
+}
+
 void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb_strides_dev,
                    int n_emb, const uint64_t* fid_offset, int64_t total_fid,
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,

@@ -84,8 +84,9 @@ def sharding_sparse_fids(features: Dict[str, Tuple[torch.Tensor, torch.Tensor]],
                    each feature's distinct FIDs of that shard in first-occurrence order
     fid_offset     int64[M] holding the reference's uint64: (table_index * N + shard) << 32 | float offset of the
                    FID's row inside that (table, shard) list, rows of feature f being dims_sum[f] floats wide
-    feature_offset int32[#(feature, row) + 1]; nfl_offset int64[#features + 1] (bit 31 = shared), features in
-                   sorted-name order — exactly what mono_embedding_to_layout consumes
+    feature_offset int32[#(feature, row) + 1]; nfl_offset int32[#features + 1] holding the reference's uint32 bits
+                   (bit 31 = shared, so a shared feature's entry is negative), features in sorted-name order — all
+                   three are what fused_embedding_to_layout[_grad] takes as they are
   The dedup / shard / offset work is ONE FusedReorderByIndices launch over the features as lists (per-list
   dims = dims_sum, shard-major / list-minor output, bit-exact kernel); the rest is index arithmetic on device.
   (The reference dedups per (feature, shard); FIDs carry their slot, so features never share a FID.)"""
@@ -143,7 +144,8 @@ def sharding_sparse_fids(features: Dict[str, Tuple[torch.Tensor, torch.Tensor]],
   fid_offset = torch.cat(pieces) if pieces else torch.empty(0, dtype=torch.int64, device=device)
   return {"fid_list": fid_list, "fid_offset": fid_offset,
           "feature_offset": torch.as_tensor(feature_offset, dtype=torch.int32, device=device),
-          "nfl_offset": torch.as_tensor(nfl_offset, dtype=torch.int64, device=device),
+          "nfl_offset": torch.as_tensor([v - (1 << 32) if v >> 31 else v for v in nfl_offset], dtype=torch.int32,
+                                        device=device),
           "table_names": tables, "feature_names": names}
 
 
@@ -359,13 +361,36 @@ def _ptr_table(tensors: Sequence[torch.Tensor], device):
   return torch.tensor([t.data_ptr() for t in tensors], dtype=torch.int64, device=device)
 
 
+def _check_layout_inputs(fid_offset, feature_offset, nfl_offset, rows, rows_name):
+  """-> the device of the index tensors.  The C ABI reads fid_offset as uint64, feature_offset as int32 and
+  nfl_offset as uint32 words: a tensor of another dtype would be silently reinterpreted, so it is refused."""
+  want = (("fid_offset", fid_offset, torch.int64), ("feature_offset", feature_offset, torch.int32),
+          ("nfl_offset", nfl_offset, torch.int32))
+  for name, t, dt in want:
+    if not isinstance(t, torch.Tensor) or t.dtype != dt:
+      raise ValueError(f"{name} must be a {dt} tensor, not {getattr(t, 'dtype', type(t).__name__)}")
+  dev = fid_offset.device
+  for name, t, _ in want:
+    if t.device.type != "cuda" or t.device != dev:
+      raise ValueError(f"{name} must be a CUDA tensor on {dev if dev.type == 'cuda' else 'a CUDA device'}, "
+                       f"not on {t.device}")
+    if not t.is_contiguous():
+      raise ValueError(f"{name} must be contiguous")
+  for t in rows:
+    if t.dtype != torch.float32 or t.device != dev:
+      raise ValueError(f"{rows_name} must be float32 tensors on {dev}, not {t.dtype} on {t.device}")
+  return dev
+
+
 def fused_embedding_to_layout(embeddings_list: Sequence[torch.Tensor], emb_strides: Sequence[int],
                               fid_offset: torch.Tensor, feature_offset: torch.Tensor, nfl_offset: torch.Tensor,
                               batch_size: int, tasks: Sequence[SliceTask], out_shapes: Sequence[Sequence[int]]):
   """ref: distribution_ops.fused_embedding_to_layout (versions 3/4/5) -> MonolithEmbeddingToLayoutV*.
-  fid_offset: uint64 viewed as int64 tensor; nfl_offset: uint32 viewed as int32 tensor."""
+  fid_offset: uint64 viewed as int64 tensor; nfl_offset: uint32 viewed as int32 tensor (sharding_sparse_fids'
+  outputs as they are).  Raises ValueError for any other dtype, a non-CUDA or non-contiguous index tensor, or
+  embeddings that are not float32 on the same device."""
+  dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, embeddings_list, "embeddings_list")
   lib = _lib.load()
-  dev = fid_offset.device
   outs = [torch.zeros(*s, dtype=torch.float32, device=dev) for s in out_shapes]
   embs = [e.contiguous() for e in embeddings_list]
   ep, op = _ptr_table(embs, dev), _ptr_table(outs, dev)
@@ -380,9 +405,10 @@ def fused_embedding_to_layout(embeddings_list: Sequence[torch.Tensor], emb_strid
 def fused_embedding_to_layout_grad(emb_sizes: Sequence[int], emb_strides: Sequence[int], fid_offset: torch.Tensor,
                                    feature_offset: torch.Tensor, nfl_offset: torch.Tensor, batch_size: int,
                                    tasks: Sequence[SliceTask], out_grads: Sequence[torch.Tensor]):
-  """ref: MonolithEmbeddingToLayoutGradV* (fused_embedding_to_layout.cc:697-948)."""
+  """ref: MonolithEmbeddingToLayoutGradV* (fused_embedding_to_layout.cc:697-948).  The index tensors as in
+  fused_embedding_to_layout; out_grads float32 on their device."""
+  dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, out_grads, "out_grads")
   lib = _lib.load()
-  dev = fid_offset.device
   grads = [torch.zeros(n, dtype=torch.float32, device=dev) for n in emb_sizes]
   og = [g.contiguous() for g in out_grads]
   gp, op = _ptr_table(grads, dev), _ptr_table(og, dev)
