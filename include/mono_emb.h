@@ -382,6 +382,14 @@ int mono_mtable_note_update_ts(mono_mtable_t* t, int32_t k, int64_t ts);
  *                                  buffer (rows laid out in `output` order, list m has dims[m] floats)
  * The two small arrays are produced on the device (sizes_dev, int32[N + N*K]) and also copied to
  * the host pointers when those are non-NULL (SYNC in that case).  n_unique likewise.
+ * Limits, checked on the host before the device is selected (MONO_ERR_INVALID_ARGUMENT, nothing launched):
+ *   1 <= K <= 2^25 lists, 1 <= N <= 64 shards (N >= 2 with rank0_empty), id_split[0] == 0 and non-decreasing,
+ *   M = id_split[K] <= 2^30 ids (the scratch set for more would not fit in 80 GB), every dims[m] > 0
+ *   (dims[0] only for K == 1).
+ * The float offsets are int32, as in the reference: sum over (shard, list) of sizes x dims must be <= 2^31 - 1.
+ * The call checks the exact sum after its synchronisation (K > 1 or any host output requested) and then
+ * returns MONO_ERR_INVALID_ARGUMENT; the device outputs are undefined and the host outputs are not written.
+ * K == 1 without host outputs does not synchronise and is rejected up front when M * dims[0] > 2^31 - 1.
  */
 int mono_reorder_by_indices(int32_t device, const int64_t* ids_dev, const int64_t* id_split_host,
                             int32_t num_lists, int32_t num_shards, const int32_t* dims_host,
@@ -392,7 +400,7 @@ int mono_reorder_by_indices(int32_t device, const int64_t* ids_dev, const int64_
 
 /* Single-list dedup used by the fused single-GPU train step: unique FIDs in first-occurrence
  * order + the inverse map (occurrence -> unique ordinal).  n_unique_dev is an int32 on device;
- * n_unique_host (optional) forces a SYNC. */
+ * n_unique_host (optional) forces a SYNC.  n <= 2^30 (MONO_ERR_INVALID_ARGUMENT otherwise, nothing launched). */
 int mono_dedup(int32_t device, const int64_t* ids_dev, int64_t n, int64_t* unique_out_dev,
                int32_t* inverse_out_dev, int32_t* n_unique_dev, int64_t* n_unique_host,
                void* stream);

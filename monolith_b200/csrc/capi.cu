@@ -562,7 +562,9 @@ int mono_grouping_build(mono_grouping_t* g, const int64_t* fids_dev, int64_t n_f
                         int32_t dim, int64_t* uniq_out_dev, int32_t* occ_offset_out_dev,
                         int32_t* shard_counts_host, int64_t* n_unique_host, void* stream) {
   return guarded([&] {
-    require(g && fids_dev && uniq_out_dev && occ_offset_out_dev && shard_counts_host, "grouping_build: null argument");
+    // an empty batch may come with a null FID pointer (an empty tensor has no storage)
+    require(g && (fids_dev || n_fids == 0) && uniq_out_dev && occ_offset_out_dev && shard_counts_host,
+            "grouping_build: null argument");
     grouping_build(g, fids_dev, n_fids, num_shards, dim, uniq_out_dev, occ_offset_out_dev, shard_counts_host,
                    n_unique_host, (cudaStream_t)stream);
   });

@@ -25,6 +25,8 @@
 namespace mono {
 
 constexpr int kMaxShards = 64;
+constexpr int kMaxLists = 1 << 25;                  // (shard, list) keys cls * K + m stay below 2^31
+constexpr int64_t kMaxIds = (int64_t)1 << 30;       // the scratch set holds 2^31 16-byte slots at most
 constexpr int kTileItems = 8;                       // ids per thread per tile
 constexpr int kTile = kThreads * kTileItems;        // ids per block tile
 
@@ -127,7 +129,8 @@ dd_rank_kernel(const int64_t* __restrict__ ids, int64_t M, const int64_t* __rest
       if (cls >= 0 && lane == (__ffs(same) - 1)) wcnt[w][cls] += __popc(same);
       if (MODE == 0) {
         // per (shard, list) totals: aggregate lanes that share both, one atomic per distinct pair
-        const int pair = cls >= 0 ? cls * 65536 + m : -1;
+        // (cls * K + m < 64 * K <= 2^31 for K <= kMaxLists: the key is unique per pair)
+        const int pair = cls >= 0 ? cls * K + m : -1;
         const uint32_t same2 = __match_any_sync(0xffffffffu, pair);
         if (cls >= 0 && lane == (__ffs(same2) - 1)) atomicAdd(tb.sizes + cls * K + m, __popc(same2));
       }
@@ -266,17 +269,30 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
                  int32_t* fused_emb_offset_dev, int32_t* shard_sizes_host,
                  int32_t* sharded_slot_sizes_host, int64_t* n_unique_host, int32_t* n_unique_dev,
                  cudaStream_t s) {
-  MONO_CUDA(cudaSetDevice(device));
+  // every argument check runs before the device is touched
   if (K <= 0 || N <= 0) throw ArgError("num_lists and num_shards must be positive");
+  if (K > kMaxLists) throw ArgError("num_lists > 2^25 is not supported");
   if (N > kMaxShards) throw ArgError("num_shards > 64 is not supported");
   if (rank0_empty && N < 2) throw ArgError("rank0_empty needs at least 2 shards");
-  const int64_t M = id_split_host[K] - id_split_host[0];
   if (id_split_host[0] != 0) throw ArgError("id_split must start at 0");
-  if (M >= ((int64_t)1 << 31)) throw ArgError("more than 2^31 ids in one call");
+  for (int m = 0; m < K; ++m)
+    if (id_split_host[m + 1] < id_split_host[m]) throw ArgError("id_split must not decrease");
+  const int64_t M = id_split_host[K];
+  if (M > kMaxIds) throw ArgError("more than 2^30 ids in one call");
+  for (int m = 0; m < (K > 1 ? K : 1); ++m)
+    if (dims_host[m] <= 0) throw ArgError("dims must be positive");
+  const int dim0 = dims_host[0];
+  const bool want_host = shard_sizes_host || sharded_slot_sizes_host || n_unique_host;
+  // The pageable H2D sources (id_split_host, dims_host; K > 1 only) and the host outputs must stay valid until the
+  // copies have run: synchronise in those cases.  K == 1 without host outputs (mono_dedup in the fused train step)
+  // stays fully asynchronous, so its float offsets (< M * dim0) are bounded up front instead of checked afterwards.
+  const bool sync = K > 1 || want_host;
+  if (!sync && M * (int64_t)dim0 > INT32_MAX) throw ArgError("ids x dim exceeds 2^31 - 1 float offsets");
+  MONO_CUDA(cudaSetDevice(device));
   const int n_eff = N - (rank0_empty ? 1 : 0);
   const int nblk = (int)std::max<int64_t>(1, (M + kTile - 1) / kTile);
 
-  // one scratch allocation (stream-ordered)
+  // one scratch allocation (stream-ordered); M <= 2^30 keeps cap <= 2^31
   uint32_t cap = 1024;
   while (cap < 2 * (uint64_t)std::max<int64_t>(M, 1)) cap <<= 1;
   const size_t NK = (size_t)N * K;
@@ -312,7 +328,6 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
     MONO_CUDA(cudaMemcpyAsync(split_dev, id_split_host, sizeof(int64_t) * (K + 1), cudaMemcpyHostToDevice, s));
     MONO_CUDA(cudaMemcpyAsync(dims_dev, dims_host, sizeof(int32_t) * K, cudaMemcpyHostToDevice, s));
   }
-  const int dim0 = dims_host[0];
   MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(DSet) * cap, s));
   MONO_CUDA(cudaMemsetAsync(small, 0, sizeof(int32_t) * (4 * NK + N + 8), s));
 
@@ -340,18 +355,20 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
   }
   if (n_unique_dev)
     MONO_CUDA(cudaMemcpyAsync(n_unique_dev, tb.n_unique, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
-  const bool want_host = shard_sizes_host || sharded_slot_sizes_host || n_unique_host;
   std::vector<int32_t> h(NK + N + 1);
-  if (want_host) {
+  if (sync) {
     MONO_CUDA(cudaMemcpyAsync(h.data(), tb.shard_sz, sizeof(int32_t) * N, cudaMemcpyDeviceToHost, s));
     MONO_CUDA(cudaMemcpyAsync(h.data() + N, tb.sizes, sizeof(int32_t) * NK, cudaMemcpyDeviceToHost, s));
     MONO_CUDA(cudaMemcpyAsync(h.data() + N + NK, tb.n_unique, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   }
   MONO_CUDA(cudaFreeAsync(ws, s));
-  // The pageable H2D sources (id_split_host, dims_host; K > 1 only) and `h` must stay valid until
-  // the copies have run: synchronise in those cases.  K == 1 without host outputs (mono_dedup in
-  // the fused train step) stays fully asynchronous.
-  if (K > 1 || want_host) MONO_CUDA(cudaStreamSynchronize(s));
+  if (sync) {
+    MONO_CUDA(cudaStreamSynchronize(s));
+    // the device accumulates the float offsets in int32: the exact sum of sizes x dims must fit
+    int64_t floats = 0;
+    for (size_t nm = 0; nm < NK; ++nm) floats += (int64_t)h[N + nm] * (K > 1 ? dims_host[nm % K] : dim0);
+    if (floats > INT32_MAX) throw ArgError("float offsets exceed 2^31 - 1 (sum of unique ids x dims)");
+  }
   if (want_host) {
     if (shard_sizes_host) std::memcpy(shard_sizes_host, h.data(), sizeof(int32_t) * N);
     if (sharded_slot_sizes_host) std::memcpy(sharded_slot_sizes_host, h.data() + N, sizeof(int32_t) * NK);
