@@ -460,6 +460,37 @@ int mono_scatter_grad_rows(int32_t device, const float* pooled_grad_dev, int64_t
                            int32_t pooling, float* grad_fused_dev, int64_t total_floats,
                            void* stream);
 
+/* ---- the gather calls with bfloat16 pooled rows ----------------------------------------------
+ * The arguments of their fp32 twins above, but the tower-side rows are bfloat16: out_dev /
+ * pooled_grad_dev point at bf16 storage (cast pointers) and out_stride / out_col, grad_stride /
+ * grad_col count bf16 elements.  fused_emb_dev and grad_fused_dev stay fp32, as does all arithmetic.
+ *
+ * mono_gather_pool_bf16: each output element is the fp32 value mono_gather_pool writes (accumulated in
+ * fp32 in the same order), rounded once to nearest even (__float2bfloat16_rn); NaN stays NaN (payload
+ * unspecified).  One kernel launch: the row copy when row_offsets_dev is NULL, dim % 4 == 0,
+ * dim <= 4 * lane-group width, out_stride % 4 == 0, out_col % 4 == 0, fused_emb_dev 16-byte and out_dev
+ * 8-byte aligned; the pooling kernel otherwise.
+ *
+ * mono_gather_pool_grad_bf16 / mono_scatter_grad_rows_bf16: bit for bit the fp32 twin's result on the
+ * pooled gradients widened exactly to fp32 (the MEAN division and every add happen in fp32 after the
+ * widening).  gather_pool_grad: one kernel launch.  scatter_grad_rows: the fp32 twin's launches
+ * (3 per radix pass and 3 for the run list, 1 occurrence -> row map when row_offsets_dev is given, the
+ * reduce, one per tree level and the finish, then the emit); MONO_ERR_INVALID_ARGUMENT before any
+ * device work unless dim % 4 == 0, dim <= 128, grad_stride % 4 == 0, grad_col % 4 == 0, pooled_grad_dev
+ * 8-byte and grad_fused_dev 16-byte aligned. */
+int mono_gather_pool_bf16(int32_t device, const float* fused_emb_dev, const int32_t* emb_offset_dev,
+                          const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim, int32_t pooling,
+                          float* out_dev, int64_t out_stride, int32_t out_col, void* stream);
+int mono_gather_pool_grad_bf16(int32_t device, const float* pooled_grad_dev, int64_t grad_stride,
+                               int32_t grad_col, const int32_t* emb_offset_dev,
+                               const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim,
+                               int32_t pooling, float* grad_fused_dev, void* stream);
+int mono_scatter_grad_rows_bf16(int32_t device, const float* pooled_grad_dev, int64_t grad_stride,
+                                int32_t grad_col, const int32_t* emb_offset_dev, int64_t n_occurrences,
+                                const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim,
+                                int32_t pooling, float* grad_fused_dev, int64_t total_floats,
+                                void* stream);
+
 /* ---- generic fused layout op -------------------------------------------------------------- */
 
 /* ref: MonolithEmbeddingToLayoutV3/V4/V5 and its grad, RT/ops/fused_embedding_to_layout.{h,cc,cu.cc}.
@@ -507,6 +538,30 @@ int mono_embedding_to_layout_grad(int32_t device, float* const* emb_grad_ptrs_de
                                   int32_t batch_size, const mono_slice_task* tasks_host,
                                   int32_t n_tasks, const float* const* out_grad_ptrs_dev,
                                   void* stream);
+
+/* The layout calls with bfloat16 tower-side tensors: the arguments of mono_embedding_to_layout /
+ * _grad, but out_ptrs_dev / out_grad_ptrs_dev point at bf16 tensors and every task's out_row_stride
+ * and out_col count bf16 elements.  The embedding inputs and the embedding gradients stay fp32.
+ * Forward: every covered element is the fp32 call's value (accumulated in fp32 in the same order)
+ * rounded once to nearest even; NaN stays NaN (payload unspecified); absent rows and empty FIRSTN
+ * positions are +0.0; uncovered elements keep their bits.  Grad: bit for bit the fp32 call on the
+ * gradients widened exactly to fp32 (MEAN division and atomics in fp32).  The same task validation and
+ * error codes as the fp32 calls, in the same order.  One kernel launch per call, as the fp32 calls. */
+int mono_embedding_to_layout_bf16(int32_t device, const float* const* emb_ptrs_dev,
+                                  const int32_t* emb_strides_dev, int32_t n_emb,
+                                  const uint64_t* fid_offset_dev, int64_t total_fid,
+                                  const int32_t* feature_offset_dev, int32_t total_feature,
+                                  const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                  const mono_slice_task* tasks_host, int32_t n_tasks,
+                                  float* const* out_ptrs_dev, void* stream);
+int mono_embedding_to_layout_grad_bf16(int32_t device, float* const* emb_grad_ptrs_dev,
+                                       const int32_t* emb_strides_dev, int32_t n_emb,
+                                       const uint64_t* fid_offset_dev, int64_t total_fid,
+                                       const int32_t* feature_offset_dev, int32_t total_feature,
+                                       const uint32_t* nfl_offset_dev, int32_t total_nfl,
+                                       int32_t batch_size, const mono_slice_task* tasks_host,
+                                       int32_t n_tasks, const float* const* out_grad_ptrs_dev,
+                                       void* stream);
 
 /* ---- NVLink peer window: the exchange steps of the sharded path as peer stores ---------------
  * ref: the all-to-alls of the reference's synchronous multi-GPU path (distributed_ps_sync.py:92-118

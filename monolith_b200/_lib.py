@@ -115,6 +115,13 @@ SIGNATURES = {
                                            C.POINTER(SliceTask), _i32, _p, _p]),
     "mono_embedding_to_layout_grad": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
                                                 C.POINTER(SliceTask), _i32, _p, _p]),
+    "mono_gather_pool_bf16": (C.c_int, [_i32, _p, _p, _p, _i64, _i32, _i32, _p, _i64, _i32, _p]),
+    "mono_gather_pool_grad_bf16": (C.c_int, [_i32, _p, _i64, _i32, _p, _p, _i64, _i32, _i32, _p, _p]),
+    "mono_scatter_grad_rows_bf16": (C.c_int, [_i32, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _i32, _p, _i64, _p]),
+    "mono_embedding_to_layout_bf16": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
+                                                C.POINTER(SliceTask), _i32, _p, _p]),
+    "mono_embedding_to_layout_grad_bf16": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
+                                                     C.POINTER(SliceTask), _i32, _p, _p]),
     "mono_mtable_note_update_ts": (C.c_int, [_p, _i32, _i64]),
     "mono_ckpt_last_error": (C.c_char_p, []),
     "mono_ckpt_writer_open": (C.c_int, [C.c_char_p, C.c_char_p, _i32, C.POINTER(_p)]),

@@ -403,7 +403,7 @@ struct BwdArgs {
 // Where the gradient rows come from: copied out of the kernel parameters once per thread so that the
 // inner loops do not re-read the constant bank (ncu showed LDCU stalls inside the unrolled loads).
 struct GradSrc {
-  const float* base;            // pooled_grad + grad_col + lane column
+  const float* base;            // pooled_grad + grad_col + lane column, counted in row elements (T of the kernel)
   int64_t stride;
   const uint32_t* occ_row;
   const int32_t* row_offsets;
@@ -412,9 +412,11 @@ struct GradSrc {
   const float* occ_div;         // parts call: MEAN divisor of every occurrence, 0 = none
   bool mean;
 };
+// T: the gradient row element; a bf16 pooled_grad is a cast pointer whose stride and column count bf16 elements
+template <typename T>
 __device__ __forceinline__ GradSrc make_grad_src(const BwdArgs& a, int c) {
   GradSrc g;
-  g.base = a.pooled_grad + a.grad_col + c;
+  g.base = reinterpret_cast<const float*>(reinterpret_cast<const T*>(a.pooled_grad) + a.grad_col + c);
   g.stride = a.grad_stride;
   g.occ_row = a.occ_row;
   g.row_offsets = a.row_offsets;
@@ -423,11 +425,11 @@ __device__ __forceinline__ GradSrc make_grad_src(const BwdArgs& a, int c) {
   g.mean = a.pooling == MONO_POOL_MEAN && (a.row_offsets != nullptr || a.occ_div != nullptr);
   return g;
 }
-// gradient row of occurrence m, from column c (the lane's; gs.base already holds it); T = __nv_bfloat16: occ_src only
+// gradient row of occurrence m, from column c (the lane's; gs.base already holds it)
 template <typename T>
 __device__ __forceinline__ const T* occ_grad_src(const GradSrc& gs, uint32_t m, int c) {
   if (gs.occ_src) return reinterpret_cast<const T*>(gs.occ_src[m]) + c;
-  return reinterpret_cast<const T*>(gs.base + (size_t)(gs.occ_row ? gs.occ_row[m] : m) * gs.stride);
+  return reinterpret_cast<const T*>(gs.base) + (size_t)(gs.occ_row ? gs.occ_row[m] : m) * gs.stride;
 }
 // MEAN divisor of occurrence m (gs.mean only; 0 = none)
 __device__ __forceinline__ float occ_grad_div(const GradSrc& gs, uint32_t m) {
@@ -672,7 +674,7 @@ __device__ __forceinline__ void seg_reduce(const SegArgs& sa, const PeerOut& po,
 #pragma unroll
   for (int v = 0; v < VPL; ++v) in[v] = c + v * G * 4 < D;
   const int64_t M = a.n;
-  const GradSrc gs = make_grad_src(a, c);
+  const GradSrc gs = make_grad_src<T>(a, c);
   const uint32_t* __restrict__ run_start = a.run_start;
   const int64_t wstride = (int64_t)gridDim.x * (kThreads / 32) * RPI;
   for (int64_t p0 = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * RPI; p0 < sa.n_pieces; p0 += wstride) {
@@ -788,7 +790,7 @@ __device__ __forceinline__ void seg_reduce(const SegArgs& sa, const PeerOut& po,
           if (e >= e_begin && e < e_stop && !(e < kPiece && ((SK >> e) & 1u))) {
             const uint32_t r = (!PLAIN && gs.occ_row) ? gs.occ_row[m[u]] : m[u];
             const T* src = (!PLAIN && gs.occ_src) ? reinterpret_cast<const T*>(gs.occ_src[m[u]]) + c
-                                                  : reinterpret_cast<const T*>(gs.base + (size_t)r * gs.stride);
+                                                  : reinterpret_cast<const T*>(gs.base) + (size_t)r * gs.stride;
 #pragma unroll
             for (int v = 0; v < VPL; ++v)
               if (in[v]) cp_async_row4(&stage[(b4 + u) * VPL + v][threadIdx.x], src + v * G * 4);
@@ -987,7 +989,7 @@ __device__ __forceinline__ void runs_apply(const BwdArgs& a, int prefetch) {
     nr = (int64_t)a.run_of_sorted[a.n - 1] + 1;
   }
   const int D = a.td.dim;
-  const GradSrc gs = make_grad_src(a, c);
+  const GradSrc gs = make_grad_src<T>(a, c);
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
   int64_t j = j_lo + (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
   uint32_t ri_next = kEmptyRow, rs_next = 0, re_next = 0, p0_next = 0;
@@ -1768,14 +1770,21 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
 // fused_embedding_to_layout.h:286-347): out_rows[offs[m] : +dim] = sum over the occurrences m with that
 // offset of pooled_grad[row(m)] (or /n for MEAN), in the reduce's order (occurrence order for <= 64
 // occurrences).  Rows of out_rows that no occurrence points at are left untouched.
+// bf16: pooled_grad is a cast pointer to bf16 rows (grad_stride and grad_col count bf16 elements); the reduce
+// widens them exactly and the sums, the tree and out_rows stay fp32 (bf16_seg_reduce_kernel, then the same kernels).
 void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, const int32_t* row_offsets,
                       int64_t n_rows, int pooling, const float* pooled_grad, int64_t grad_stride,
-                      int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s) {
+                      int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s, bool bf16) {
   MONO_CUDA(cudaSetDevice(device));
   if (M <= 0) return;
   if (M >= ((int64_t)1 << 31) || total_floats >= ((int64_t)1 << 31)) throw ArgError("scatter_rows: sizes exceed 2^31");
   if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN) throw ArgError("scatter_rows: SUM or MEAN");
-  check_grad_rows("scatter_rows", dim, pooled_grad, grad_stride, grad_col, out_rows);
+  if (bf16) {  // bf16 pooled gradient rows (8-byte aligned), fp32 destination rows (16-byte aligned)
+    check_grad_rows("scatter_rows", dim, pooled_grad, grad_stride, grad_col, nullptr, 2);
+    check_grad_rows("scatter_rows", dim, nullptr, 0, 0, out_rows);
+  } else {
+    check_grad_rows("scatter_rows", dim, pooled_grad, grad_stride, grad_col, out_rows);
+  }
   const int D = dim;
   // offsets are multiples of 4 floats (16-byte aligned rows; every dim in the fused buffer is a multiple
   // of 4): drop the two zero bits from the sort key
@@ -1792,7 +1801,7 @@ void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, c
   w.sorted = sort_and_runs(w.sort, reinterpret_cast<const uint32_t*>(offs_dev), M, bits, shift, nullptr, s);
   const SegArgs sa = seg_args(w, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, w.ugrad, s);
   const int G = pick_group(D);
-  launch_reduce(sa, G, no_peer, false, s);
+  launch_reduce(sa, G, no_peer, false, s, bf16);
 #define EMIT(GG)                                                                                              \
   runs_emit_kernel<GG><<<resident_grid(runs_emit_kernel<GG>, M, kThreads / GG), kThreads, 0, s>>>(sa.b, shift, out_rows); \
   MONO_CHECK_LAUNCH()

@@ -787,6 +787,77 @@ int mono_embedding_to_layout_grad(int32_t device, float* const* emb_grad_ptrs_de
   });
 }
 
+int mono_gather_pool_bf16(int32_t device, const float* fused_emb_dev, const int32_t* emb_offset_dev,
+                          const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim, int32_t pooling,
+                          float* out_dev, int64_t out_stride, int32_t out_col, void* stream) {
+  return guarded([&] {
+    MONO_CUDA(cudaSetDevice(device));
+    require(dim > 0, "dim must be positive");
+    launch_gather_pool_bf16(fused_emb_dev, emb_offset_dev, row_offsets_dev, n_rows, dim, pooling,
+                            reinterpret_cast<__nv_bfloat16*>(out_dev), out_stride, out_col, (cudaStream_t)stream);
+  });
+}
+
+int mono_gather_pool_grad_bf16(int32_t device, const float* pooled_grad_dev, int64_t grad_stride,
+                               int32_t grad_col, const int32_t* emb_offset_dev,
+                               const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim,
+                               int32_t pooling, float* grad_fused_dev, void* stream) {
+  return guarded([&] {
+    MONO_CUDA(cudaSetDevice(device));
+    require(dim > 0, "dim must be positive");
+    launch_gather_pool_grad_bf16(reinterpret_cast<const __nv_bfloat16*>(pooled_grad_dev), grad_stride, grad_col,
+                                 emb_offset_dev, row_offsets_dev, n_rows, dim, pooling, grad_fused_dev,
+                                 (cudaStream_t)stream);
+  });
+}
+
+int mono_scatter_grad_rows_bf16(int32_t device, const float* pooled_grad_dev, int64_t grad_stride,
+                                int32_t grad_col, const int32_t* emb_offset_dev, int64_t n_occurrences,
+                                const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim,
+                                int32_t pooling, float* grad_fused_dev, int64_t total_floats,
+                                void* stream) {
+  return guarded([&] {
+    require(pooled_grad_dev && emb_offset_dev && grad_fused_dev, "scatter_grad_rows: null argument");
+    require(row_offsets_dev != nullptr || n_rows == n_occurrences, "scatter_grad_rows: n_rows != n_occurrences");
+    run_scatter_rows(device, emb_offset_dev, n_occurrences, dim, row_offsets_dev, n_rows, pooling,
+                     pooled_grad_dev, grad_stride, grad_col, grad_fused_dev, total_floats, (cudaStream_t)stream,
+                     true);
+  });
+}
+
+int mono_embedding_to_layout_bf16(int32_t device, const float* const* emb_ptrs_dev,
+                                  const int32_t* emb_strides_dev, int32_t n_emb,
+                                  const uint64_t* fid_offset_dev, int64_t total_fid,
+                                  const int32_t* feature_offset_dev, int32_t total_feature,
+                                  const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                  const mono_slice_task* tasks_host, int32_t n_tasks,
+                                  float* const* out_ptrs_dev, void* stream) {
+  return guarded([&] {
+    check_layout_tasks(tasks_host, n_tasks, total_nfl);
+    MONO_CUDA(cudaSetDevice(device));
+    launch_layout(false, const_cast<float* const*>(emb_ptrs_dev), emb_strides_dev, n_emb, fid_offset_dev,
+                  total_fid, feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size,
+                  tasks_host, n_tasks, out_ptrs_dev, (cudaStream_t)stream, true);
+  });
+}
+
+int mono_embedding_to_layout_grad_bf16(int32_t device, float* const* emb_grad_ptrs_dev,
+                                       const int32_t* emb_strides_dev, int32_t n_emb,
+                                       const uint64_t* fid_offset_dev, int64_t total_fid,
+                                       const int32_t* feature_offset_dev, int32_t total_feature,
+                                       const uint32_t* nfl_offset_dev, int32_t total_nfl,
+                                       int32_t batch_size, const mono_slice_task* tasks_host,
+                                       int32_t n_tasks, const float* const* out_grad_ptrs_dev,
+                                       void* stream) {
+  return guarded([&] {
+    check_layout_tasks(tasks_host, n_tasks, total_nfl);
+    MONO_CUDA(cudaSetDevice(device));
+    launch_layout(true, emb_grad_ptrs_dev, emb_strides_dev, n_emb, fid_offset_dev, total_fid,
+                  feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host,
+                  n_tasks, const_cast<float* const*>(out_grad_ptrs_dev), (cudaStream_t)stream, true);
+  });
+}
+
 // ---- host-buffer entry points --------------------------------------------------------------
 int mono_mtable_lookup_host(mono_mtable_t* t, const int64_t* ids_host, const int64_t* id_split_host,
                             float* emb_out_host) {

@@ -1,6 +1,7 @@
 // engine.h — host-side state of the engine (one mono_mtable = K tables on one device).
 #pragma once
 
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -463,7 +464,7 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
 
 void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, const int32_t* row_offsets,
                       int64_t n_rows, int pooling, const float* pooled_grad, int64_t grad_stride,
-                      int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s);
+                      int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s, bool bf16 = false);
 
 // dedup.cu
 void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_host, int K, int N,
@@ -479,11 +480,17 @@ void launch_gather_pool(const float* fused_emb, const int32_t* emb_offset, const
 void launch_gather_pool_grad(const float* pooled_grad, int64_t grad_stride, int grad_col,
                              const int32_t* emb_offset, const int32_t* row_offsets, int64_t n_rows,
                              int dim, int pooling, float* grad_fused, cudaStream_t s);
+void launch_gather_pool_bf16(const float* fused_emb, const int32_t* emb_offset, const int32_t* row_offsets,
+                             int64_t n_rows, int dim, int pooling, __nv_bfloat16* out, int64_t out_stride,
+                             int out_col, cudaStream_t s);
+void launch_gather_pool_grad_bf16(const __nv_bfloat16* pooled_grad, int64_t grad_stride, int grad_col,
+                                  const int32_t* emb_offset, const int32_t* row_offsets, int64_t n_rows, int dim,
+                                  int pooling, float* grad_fused, cudaStream_t s);
 void check_layout_tasks(const mono_slice_task* tasks, int n_tasks, int total_nfl);
 void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb_strides_dev,
                    int n_emb, const uint64_t* fid_offset, int64_t total_fid,
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,
                    int total_nfl, int batch_size, const mono_slice_task* tasks_host, int n_tasks,
-                   float* const* out_ptrs_dev, cudaStream_t s);
+                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16 = false);
 
 }  // namespace mono

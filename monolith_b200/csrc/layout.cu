@@ -13,14 +13,16 @@
 #include <vector>
 
 #include "engine.h"
+#include "rowelem.cuh"
 
 namespace mono {
 
-template <int G>
-__global__ void __launch_bounds__(kThreads)
-gather_pool_kernel(const float* __restrict__ fused, const int32_t* __restrict__ emb_offset,
-                   const int32_t* __restrict__ row_offsets, int64_t n_rows, int dim, int pooling,
-                   float* __restrict__ out, int64_t out_stride, int out_col) {
+// T: element type of the pooled rows (float, or bf16 for the *_bf16 calls); the fused row buffer is always fp32 and
+// every add and division runs in fp32, so a bf16 element is the fp32 result rounded once.
+template <typename T, int G>
+__device__ __forceinline__ void gather_pool(const float* __restrict__ fused, const int32_t* __restrict__ emb_offset,
+                                            const int32_t* __restrict__ row_offsets, int64_t n_rows, int dim,
+                                            int pooling, T* __restrict__ out, int64_t out_stride, int out_col) {
   const int gl = Group<G>::gl();
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
   const bool src_vec = (dim & 3) == 0 && (reinterpret_cast<uintptr_t>(fused) & 15) == 0;
@@ -29,8 +31,9 @@ gather_pool_kernel(const float* __restrict__ fused, const int32_t* __restrict__ 
     const int64_t e = row_offsets ? row_offsets[r + 1] : r + 1;
     const int n = (int)(e - b);
     const float fn = (float)n;
-    float* dst = out + r * out_stride + out_col;
-    const bool dst_vec = src_vec && (reinterpret_cast<uintptr_t>(dst) & 15) == 0;
+    T* dst = out + r * out_stride + out_col;
+    // 4 elements per vector store: 16 bytes of fp32, 8 of bf16
+    const bool dst_vec = src_vec && (reinterpret_cast<uintptr_t>(dst) & (4 * sizeof(T) - 1)) == 0;
     if (dst_vec) {
       for (int c = gl * 4; c < dim; c += G * 4) {
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -54,7 +57,7 @@ gather_pool_kernel(const float* __restrict__ fused, const int32_t* __restrict__ 
             acc.z = __fadd_rn(acc.z, x.z); acc.w = __fadd_rn(acc.w, x.w);
           }
         }
-        *reinterpret_cast<float4*>(dst + c) = acc;
+        store_row4(dst + c, acc);
       }
     } else {
       for (int c = gl; c < dim; c += G) {
@@ -64,20 +67,37 @@ gather_pool_kernel(const float* __restrict__ fused, const int32_t* __restrict__ 
           if (pooling == MONO_POOL_MEAN) x = __fdiv_rn(x, fn);
           acc = j == 0 ? x : __fadd_rn(acc, x);
         }
-        dst[c] = acc;
+        dst[c] = to_row_elem(acc, dst);
       }
     }
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+gather_pool_kernel(const float* __restrict__ fused, const int32_t* __restrict__ emb_offset,
+                   const int32_t* __restrict__ row_offsets, int64_t n_rows, int dim, int pooling,
+                   float* __restrict__ out, int64_t out_stride, int out_col) {
+  gather_pool<float, G>(fused, emb_offset, row_offsets, n_rows, dim, pooling, out, out_stride, out_col);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+bf16_gather_pool_kernel(const float* __restrict__ fused, const int32_t* __restrict__ emb_offset,
+                        const int32_t* __restrict__ row_offsets, int64_t n_rows, int dim, int pooling,
+                        __nv_bfloat16* __restrict__ out, int64_t out_stride, int out_col) {
+  gather_pool<__nv_bfloat16, G>(fused, emb_offset, row_offsets, n_rows, dim, pooling, out, out_stride, out_col);
 }
 
 // One occurrence per output row (row_offsets == NULL: FusedGatherKernel proper) with 16-byte aligned rows:
 // the same two-phase shape as the table lookup (ops.cu lookup_kernel): a lane fetches one offset
 // (32 coalesced, independent loads per warp), then G lanes move one row with 128-bit accesses, 4 rows in
 // flight per lane before the first store.  Pooling over a single row is the identity for SUM and MEAN.
-template <int G>
-__global__ void __launch_bounds__(kThreads, 4)
-gather_rows_kernel(const float* __restrict__ fused, const int32_t* __restrict__ emb_offset, int64_t n_rows,
-                   int dim, float* __restrict__ out, int64_t out_stride, int out_col) {
+// T = bf16: the same fp32 loads, one 8-byte streaming store of 4 rounded elements per lane.
+template <typename T, int G>
+__device__ __forceinline__ void gather_rows(const float* __restrict__ fused, const int32_t* __restrict__ emb_offset,
+                                            int64_t n_rows, int dim, T* __restrict__ out, int64_t out_stride,
+                                            int out_col) {
   constexpr int RPI = 32 / G, ITERS = G, UNR = 4;
   const int lane = threadIdx.x & 31, gl = Group<G>::gl(), grp = lane / G;
   const int c = gl * 4;
@@ -103,19 +123,34 @@ gather_rows_kernel(const float* __restrict__ fused, const int32_t* __restrict__ 
 #pragma unroll
       for (int u = 0; u < UNR; ++u) {
         const int64_t ir = wbase + (it0 + u) * RPI + grp;
-        if (ir < n_rows && c < dim) __stcs(reinterpret_cast<float4*>(out + ir * out_stride + out_col + c), x[u]);
+        if (ir < n_rows && c < dim) stcs_row4(out + ir * out_stride + out_col + c, x[u]);
       }
     }
   }
 }
 
+template <int G>
+__global__ void __launch_bounds__(kThreads, 4)
+gather_rows_kernel(const float* __restrict__ fused, const int32_t* __restrict__ emb_offset, int64_t n_rows,
+                   int dim, float* __restrict__ out, int64_t out_stride, int out_col) {
+  gather_rows<float, G>(fused, emb_offset, n_rows, dim, out, out_stride, out_col);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads, 4)
+bf16_gather_rows_kernel(const float* __restrict__ fused, const int32_t* __restrict__ emb_offset, int64_t n_rows,
+                        int dim, __nv_bfloat16* __restrict__ out, int64_t out_stride, int out_col) {
+  gather_rows<__nv_bfloat16, G>(fused, emb_offset, n_rows, dim, out, out_stride, out_col);
+}
+
 // grad_fused[offset[m] : +dim] += g_row   (float atomics: several occurrences may share a row,
 // exactly like the reference's FusedGatherGradKernel atomicAdd, map_id_to_embedding.cu.cc:75-118)
-template <int G>
-__global__ void __launch_bounds__(kThreads)
-gather_pool_grad_kernel(const float* __restrict__ pooled_grad, int64_t grad_stride, int grad_col,
-                        const int32_t* __restrict__ emb_offset, const int32_t* __restrict__ row_offsets,
-                        int64_t n_rows, int dim, int pooling, float* __restrict__ grad_fused) {
+// T = bf16: the pooled gradient is widened exactly, then divided and added in fp32.
+template <typename T, int G>
+__device__ __forceinline__ void gather_pool_grad(const T* __restrict__ pooled_grad, int64_t grad_stride, int grad_col,
+                                                 const int32_t* __restrict__ emb_offset,
+                                                 const int32_t* __restrict__ row_offsets, int64_t n_rows, int dim,
+                                                 int pooling, float* __restrict__ grad_fused) {
   const int gl = Group<G>::gl();
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
   for (int64_t r = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G; r < n_rows; r += gstride) {
@@ -123,13 +158,31 @@ gather_pool_grad_kernel(const float* __restrict__ pooled_grad, int64_t grad_stri
     const int64_t e = row_offsets ? row_offsets[r + 1] : r + 1;
     const int n = (int)(e - b);
     const float fn = (float)n;
-    const float* g = pooled_grad + r * grad_stride + grad_col;
+    const T* g = pooled_grad + r * grad_stride + grad_col;
     for (int c = gl; c < dim; c += G) {
-      float x = __ldg(g + c);
+      float x = row_elem_f32(__ldg(g + c));
       if (pooling == MONO_POOL_MEAN) x = __fdiv_rn(x, fn);
       for (int j = 0; j < n; ++j) atomicAdd(grad_fused + emb_offset[b + j] + c, x);
     }
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+gather_pool_grad_kernel(const float* __restrict__ pooled_grad, int64_t grad_stride, int grad_col,
+                        const int32_t* __restrict__ emb_offset, const int32_t* __restrict__ row_offsets,
+                        int64_t n_rows, int dim, int pooling, float* __restrict__ grad_fused) {
+  gather_pool_grad<float, G>(pooled_grad, grad_stride, grad_col, emb_offset, row_offsets, n_rows, dim, pooling,
+                             grad_fused);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+bf16_gather_pool_grad_kernel(const __nv_bfloat16* __restrict__ pooled_grad, int64_t grad_stride, int grad_col,
+                             const int32_t* __restrict__ emb_offset, const int32_t* __restrict__ row_offsets,
+                             int64_t n_rows, int dim, int pooling, float* __restrict__ grad_fused) {
+  gather_pool_grad<__nv_bfloat16, G>(pooled_grad, grad_stride, grad_col, emb_offset, row_offsets, n_rows, dim, pooling,
+                                     grad_fused);
 }
 
 static int pick_group(int dim) {
@@ -176,6 +229,45 @@ void launch_gather_pool_grad(const float* pooled_grad, int64_t grad_stride, int 
   MONO_CHECK_LAUNCH();
 }
 
+// bf16 pooled rows: launch_gather_pool's rules, with 8-byte aligned output rows for the row copy
+void launch_gather_pool_bf16(const float* fused_emb, const int32_t* emb_offset, const int32_t* row_offsets,
+                             int64_t n_rows, int dim, int pooling, __nv_bfloat16* out, int64_t out_stride,
+                             int out_col, cudaStream_t s) {
+  if (n_rows <= 0) return;
+  if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN) throw ArgError("gather_pool: SUM or MEAN");
+  if (row_offsets == nullptr) pooling = MONO_POOL_SUM;
+  const int G = pick_group(dim);
+  if (row_offsets == nullptr && (dim & 3) == 0 && dim <= 4 * G && (out_stride & 3) == 0 && (out_col & 3) == 0 &&
+      (reinterpret_cast<uintptr_t>(fused_emb) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0) {
+#define BR(GG) bf16_gather_rows_kernel<GG><<<resident_grid(bf16_gather_rows_kernel<GG>, n_rows, kThreads), kThreads, 0, \
+      s>>>(fused_emb, emb_offset, n_rows, dim, out, out_stride, out_col)
+    switch (G) { case 4: BR(4); break; case 8: BR(8); break; case 16: BR(16); break; default: BR(32); }
+#undef BR
+    MONO_CHECK_LAUNCH();
+    return;
+  }
+  const int grid = grid_for(n_rows, kThreads / G);
+#define BP(GG) bf16_gather_pool_kernel<GG><<<grid, kThreads, 0, s>>>(fused_emb, emb_offset, row_offsets, n_rows, dim, \
+      pooling, out, out_stride, out_col)
+  switch (G) { case 4: BP(4); break; case 8: BP(8); break; case 16: BP(16); break; default: BP(32); }
+#undef BP
+  MONO_CHECK_LAUNCH();
+}
+
+void launch_gather_pool_grad_bf16(const __nv_bfloat16* pooled_grad, int64_t grad_stride, int grad_col,
+                                  const int32_t* emb_offset, const int32_t* row_offsets, int64_t n_rows, int dim,
+                                  int pooling, float* grad_fused, cudaStream_t s) {
+  if (n_rows <= 0) return;
+  if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN) throw ArgError("gather_pool_grad: SUM or MEAN");
+  const int G = std::min(32, std::max(4, pick_group(dim * 4)));
+  const int grid = grid_for(n_rows, kThreads / G);
+#define BG(GG) bf16_gather_pool_grad_kernel<GG><<<grid, kThreads, 0, s>>>(pooled_grad, grad_stride, grad_col, \
+      emb_offset, row_offsets, n_rows, dim, pooling, grad_fused)
+  switch (G) { case 4: BG(4); break; case 8: BG(8); break; case 16: BG(16); break; default: BG(32); }
+#undef BG
+  MONO_CHECK_LAUNCH();
+}
+
 // ------------------------------------------------------------------------------------------
 // generic layout op
 // ------------------------------------------------------------------------------------------
@@ -214,8 +306,9 @@ __device__ __forceinline__ void fid_range(const LayoutArgs& a, int feature_idx, 
 // Forward.  A "chain" is the list of slice tasks that write the same destination (length 1 except
 // for ADDN outputs, where the reference sums the slices in config order:
 // ForwardTaskRunImpl, fused_embedding_to_layout.cc:468-540).
-template <int G>
-__global__ void __launch_bounds__(kThreads) layout_fwd_kernel(LayoutArgs a) {
+// T: element type of the outputs (a.out_ptrs point at T storage; out_row_stride and out_col count T elements).
+template <typename T, int G>
+__device__ __forceinline__ void layout_fwd(const LayoutArgs& a) {
   const int gl = Group<G>::gl();
   const int64_t total = (int64_t)a.n_chains * a.batch_size;
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
@@ -224,7 +317,8 @@ __global__ void __launch_bounds__(kThreads) layout_fwd_kernel(LayoutArgs a) {
     const int b = (int)(u % a.batch_size);
     const int t0 = a.chain_start[ch], t1 = a.chain_start[ch + 1];
     const mono_slice_task first = a.tasks[t0];
-    float* dst = a.out_ptrs[first.out_tensor] + (int64_t)b * first.out_row_stride + first.out_col;
+    T* dst = reinterpret_cast<T* const*>(a.out_ptrs)[first.out_tensor] + (int64_t)b * first.out_row_stride +
+             first.out_col;
     if (first.pooling == MONO_POOL_FIRSTN) {
       // out[seq_idx, :] = row of the seq_idx-th fid (zeros past the end)
       bool shared; int off, num;
@@ -238,7 +332,7 @@ __global__ void __launch_bounds__(kThreads) layout_fwd_kernel(LayoutArgs a) {
           const int i1 = (int)(fo >> 32), i2 = (int)(fo & 0xffffffffu);
           src = a.emb_ptrs[i1] + (int64_t)i2 * a.emb_strides[i1] + first.slice_start;
         }
-        for (int c = gl; c < first.dim; c += G) dst[q * first.dim + c] = src ? src[c] : 0.0f;
+        for (int c = gl; c < first.dim; c += G) dst[q * first.dim + c] = to_row_elem(src ? src[c] : 0.0f, dst);
       }
       continue;
     }
@@ -274,15 +368,26 @@ __global__ void __launch_bounds__(kThreads) layout_fwd_kernel(LayoutArgs a) {
         }
         if (via_tmp) acc = __fadd_rn(acc, tmp);
       }
-      dst[c] = acc;
+      dst[c] = to_row_elem(acc, dst);
     }
   }
 }
 
+template <int G>
+__global__ void __launch_bounds__(kThreads) layout_fwd_kernel(LayoutArgs a) {
+  layout_fwd<float, G>(a);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads) bf16_layout_fwd_kernel(LayoutArgs a) {
+  layout_fwd<__nv_bfloat16, G>(a);
+}
+
 // Backward: ScatterGrad (ref: fused_embedding_to_layout.h:286-347) with float atomics, as the
 // reference GPU kernel does (BackwardBatchKernel, cu.cc:337-381).
-template <int G>
-__global__ void __launch_bounds__(kThreads) layout_bwd_kernel(LayoutArgs a, int n_tasks) {
+// T: element type of the output gradients, widened exactly; the division and the atomics run in fp32.
+template <typename T, int G>
+__device__ __forceinline__ void layout_bwd(const LayoutArgs& a, int n_tasks) {
   const int gl = Group<G>::gl();
   const int64_t total = (int64_t)n_tasks * a.batch_size;
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
@@ -295,7 +400,7 @@ __global__ void __launch_bounds__(kThreads) layout_bwd_kernel(LayoutArgs a, int 
     if (!num) continue;
     int start, fnum;
     fid_range(a, shared ? off : off + b, &start, &fnum);
-    const float* g = a.out_ptrs[tk.out_tensor] + (int64_t)b * tk.out_row_stride + tk.out_col;
+    const T* g = reinterpret_cast<T* const*>(a.out_ptrs)[tk.out_tensor] + (int64_t)b * tk.out_row_stride + tk.out_col;
     const float fn = (float)fnum;
     for (int f = 0; f < fnum; ++f) {
       if (tk.pooling == MONO_POOL_FIRSTN && f >= tk.max_seq_len) break;
@@ -303,12 +408,22 @@ __global__ void __launch_bounds__(kThreads) layout_bwd_kernel(LayoutArgs a, int 
       const int i1 = (int)(fo >> 32), i2 = (int)(fo & 0xffffffffu);
       float* dst = a.emb_ptrs[i1] + (int64_t)i2 * a.emb_strides[i1] + tk.slice_start;
       for (int c = gl; c < tk.dim; c += G) {
-        float x = tk.pooling == MONO_POOL_FIRSTN ? g[f * tk.dim + c] : g[c];
+        float x = row_elem_f32(tk.pooling == MONO_POOL_FIRSTN ? g[f * tk.dim + c] : g[c]);
         if (tk.pooling == MONO_POOL_MEAN) x = __fdiv_rn(x, fn);
         atomicAdd(dst + c, x);
       }
     }
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads) layout_bwd_kernel(LayoutArgs a, int n_tasks) {
+  layout_bwd<float, G>(a, n_tasks);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads) bf16_layout_bwd_kernel(LayoutArgs a, int n_tasks) {
+  layout_bwd<__nv_bfloat16, G>(a, n_tasks);
 }
 
 // Host-side checks of the tasks: the kernels index with every field unchecked.
@@ -334,11 +449,18 @@ void check_layout_tasks(const mono_slice_task* tasks, int n_tasks, int total_nfl
   }
 }
 
+// the bf16 twins of layout_fwd_kernel / layout_bwd_kernel at lane-group width G
+template <int G>
+static void launch_bf16_layout(bool backward, int grid, const LayoutArgs& a, int n_tasks, cudaStream_t s) {
+  if (backward) bf16_layout_bwd_kernel<G><<<grid, kThreads, 0, s>>>(a, n_tasks);
+  else bf16_layout_fwd_kernel<G><<<grid, kThreads, 0, s>>>(a);
+}
+
 void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb_strides_dev,
                    int n_emb, const uint64_t* fid_offset, int64_t total_fid,
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,
                    int total_nfl, int batch_size, const mono_slice_task* tasks_host, int n_tasks,
-                   float* const* out_ptrs_dev, cudaStream_t s) {
+                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16) {
   (void)n_emb;
   if (n_tasks <= 0 || batch_size <= 0) return;
   // chains: consecutive grouping of tasks by destination (accumulate tasks with equal destination)
@@ -391,7 +513,14 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
   while (G < max_dim && G < 32) G <<= 1;  // one float per lane
   const int64_t units = (int64_t)(backward ? (int)ordered.size() : n_chains) * batch_size;
   const int grid = grid_for(units, kThreads / G);
-  if (!backward) {
+  if (bf16) {
+    switch (G) {
+      case 4: launch_bf16_layout<4>(backward, grid, a, (int)ordered.size(), s); break;
+      case 8: launch_bf16_layout<8>(backward, grid, a, (int)ordered.size(), s); break;
+      case 16: launch_bf16_layout<16>(backward, grid, a, (int)ordered.size(), s); break;
+      default: launch_bf16_layout<32>(backward, grid, a, (int)ordered.size(), s); break;
+    }
+  } else if (!backward) {
     switch (G) {
       case 4: layout_fwd_kernel<4><<<grid, kThreads, 0, s>>>(a); break;
       case 8: layout_fwd_kernel<8><<<grid, kThreads, 0, s>>>(a); break;

@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 
 #include "engine.h"
+#include "rowelem.cuh"
 
 namespace mono {
 
@@ -528,38 +529,12 @@ __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
 }
 
-// ---- row element types of the caller's rows: float, or bf16 (the *_parts_bf16 calls) ----
-// A lane moves 4 consecutive elements of a row (16 bytes of fp32, 8 of bf16); every add, division and optimizer
-// step runs in fp32.  bf16 -> fp32 is exact; fp32 -> bf16 rounds to nearest even.
-__device__ __forceinline__ float4 widen_bf16x4(uint2 u) {
-  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
-                     __uint_as_float(u.y & 0xFFFF0000u));
-}
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
 // cp.async of a lane's 4 elements into its 16-byte stage slot (a bf16 row fills the slot's first 8 bytes)
 __device__ __forceinline__ void cp_async_row4(void* smem_dst, const float* gsrc) { cp_async16(smem_dst, gsrc); }
 __device__ __forceinline__ void cp_async_row4(void* smem_dst, const __nv_bfloat16* gsrc) {
   const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(d), "l"(gsrc) : "memory");
 }
-// the 4 elements a lane staged with cp_async_row4, as fp32
-template <typename T>
-__device__ __forceinline__ float4 stage_row4(const float4* slot) { return *slot; }
-template <>
-__device__ __forceinline__ float4 stage_row4<__nv_bfloat16>(const float4* slot) {
-  return widen_bf16x4(*reinterpret_cast<const uint2*>(slot));
-}
-// streaming store of 4 elements (dst aligned to 4 elements)
-__device__ __forceinline__ void stcs_row4(float* dst, const float4& x) { __stcs(reinterpret_cast<float4*>(dst), x); }
-__device__ __forceinline__ void stcs_row4(__nv_bfloat16* dst, const float4& x) {
-  __stcs(reinterpret_cast<uint2*>(dst), make_uint2(pack_bf16x2(x.x, x.y), pack_bf16x2(x.z, x.w)));
-}
-__device__ __forceinline__ float to_row_elem(float x, const float*) { return x; }
-__device__ __forceinline__ __nv_bfloat16 to_row_elem(float x, const __nv_bfloat16*) { return __float2bfloat16_rn(x); }
-
 // ---- host helpers implemented in ops.cu ----
 struct CallBlob {  // device pointers into the staged per-call descriptor block
   const CallSeg* segs;

@@ -56,7 +56,8 @@ class CudaBackend:
 
   def gather_pool_grad_into(self, grad_buf, pooled_grad, offs, dim, row_offsets, pooling):
     """Fills grad_buf (pre-zeroed, shared by all tables of the step).  dim % 4 == 0 and <= 128: the
-    deterministic sort-based scatter; otherwise the float-atomic kernel (like the reference GPU path)."""
+    deterministic sort-based scatter; otherwise the float-atomic kernel (like the reference GPU path).
+    pooled_grad is float32 or bfloat16 (the bf16 kernels widen it exactly); grad_buf is float32."""
     if self.vec_ok and dim <= 128:
       self.dops.scatter_grad_rows(pooled_grad, offs, dim, grad_buf, row_offsets, pooling)
       return
@@ -66,10 +67,10 @@ class CudaBackend:
     n_rows = offs.numel() if row_offsets is None else row_offsets.numel() - 1
     pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
     ro = None if row_offsets is None else C.c_void_p(row_offsets.data_ptr())
-    _lib.check(lib.mono_gather_pool_grad(pooled_grad.device.index, C.c_void_p(pooled_grad.data_ptr()),
-                                         pooled_grad.stride(0), 0, C.c_void_p(offs.data_ptr()), ro, n_rows, dim, pool,
-                                         C.c_void_p(grad_buf.data_ptr()),
-                                         C.c_void_p(torch.cuda.current_stream(pooled_grad.device).cuda_stream)))
+    fn = lib.mono_gather_pool_grad_bf16 if pooled_grad.dtype == torch.bfloat16 else lib.mono_gather_pool_grad
+    _lib.check(fn(pooled_grad.device.index, C.c_void_p(pooled_grad.data_ptr()), pooled_grad.stride(0), 0,
+                  C.c_void_p(offs.data_ptr()), ro, n_rows, dim, pool, C.c_void_p(grad_buf.data_ptr()),
+                  C.c_void_p(torch.cuda.current_stream(pooled_grad.device).cuda_stream)))
 
   def zeros(self, n, like):
     return torch.zeros(n, dtype=torch.float32, device=like.device)
@@ -150,8 +151,12 @@ class PartitionedHashTable:
     return [sum(slot_sizes[n * self.K + k] * self.dims[k] for k in range(self.K)) for n in range(self.N)]
 
   def lookup(self, slot_to_fids: Dict[str, torch.Tensor], row_offsets: Optional[Dict[str, torch.Tensor]] = None,
-             pooling: Optional[Dict[str, str]] = None, outs: Optional[Dict[str, torch.Tensor]] = None):
-    """Forward steps 1-6.  Returns ({table: pooled [rows, D]}, ctx)."""
+             pooling: Optional[Dict[str, str]] = None, outs: Optional[Dict[str, torch.Tensor]] = None,
+             dtype: torch.dtype = torch.float32):
+    """Forward steps 1-6.  Returns ({table: pooled [rows, D]}, ctx).  dtype: of the pooled rows this call
+    allocates, float32 or bfloat16 (the float32 rows rounded once; the exchanged rows stay float32)."""
+    if dtype not in (torch.float32, torch.bfloat16):
+      raise ValueError(f"dtype must be torch.float32 or torch.bfloat16, not {dtype}")
     be, N, K = self.backend, self.N, self.K
     row_offsets = row_offsets or {}
     pooling = pooling or {}
@@ -192,8 +197,10 @@ class PartitionedHashTable:
       occ_splits.append((pos, pos + n_occ))
       if name in slot_to_fids:
         ro = row_offsets.get(name)
-        pooled[name] = be.gather_pool(recv_rows, offs[pos:pos + n_occ], self.dims[k], ro, pooling.get(name, "sum"),
-                                      None if outs is None else outs.get(name))
+        out = None if outs is None else outs.get(name)
+        if out is None and dtype != torch.float32:
+          out = torch.empty(n_occ if ro is None else ro.numel() - 1, self.dims[k], dtype=dtype, device=dev)
+        pooled[name] = be.gather_pool(recv_rows, offs[pos:pos + n_occ], self.dims[k], ro, pooling.get(name, "sum"), out)
       pos += n_occ
     ph.mark("f6_gather_pool")
     ctx = StepContext()
@@ -204,7 +211,7 @@ class PartitionedHashTable:
     return pooled, ctx
 
   def apply_gradients(self, ctx: StepContext, pooled_grads: Dict[str, torch.Tensor], req_time: int = 0):
-    """Backward steps 7-9."""
+    """Backward steps 7-9.  pooled_grads are float32 or bfloat16; the exchanged row gradients are float32."""
     be, N = self.backend, self.N
     some = next(iter(pooled_grads.values()))
     ph = self.phases

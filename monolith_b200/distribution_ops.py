@@ -21,6 +21,16 @@ def _stream(device):
   return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+_TOWER_DTYPES = (torch.float32, torch.bfloat16)
+
+
+def _tower_dtype(dtype, what):
+  """The dtype of the tensors a tower reads or writes: float32, or bfloat16 (the *_bf16 kernels)."""
+  if dtype not in _TOWER_DTYPES:
+    raise ValueError(f"{what} must be torch.float32 or torch.bfloat16, not {dtype}")
+  return dtype
+
+
 def fused_reorder_by_indices(inputs: Sequence[torch.Tensor], num_of_shards: int, dim_sizes: Sequence[int],
                              rank0_empty_shard: Optional[bool] = None):
   """ref: distribution_ops.py:218-258 / FusedReorderByIndices (runtime/ops/fused_reorder_by_indices.cc).
@@ -151,9 +161,12 @@ def sharding_sparse_fids(features: Dict[str, Tuple[torch.Tensor, torch.Tensor]],
 
 def gather_pool(fused_embeddings: torch.Tensor, fused_embedding_offsets: torch.Tensor, dim: int,
                 row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum",
-                out: Optional[torch.Tensor] = None, out_col: int = 0) -> torch.Tensor:
+                out: Optional[torch.Tensor] = None, out_col: int = 0, dtype: torch.dtype = torch.float32) -> torch.Tensor:
   """out[r] = pool_{m in row r} fused_embeddings[offsets[m]:offsets[m]+dim]
-  (ref: FusedGatherKernel, runtime/ops/map_id_to_embedding.cu.cc:30-74, + per-row pool)."""
+  (ref: FusedGatherKernel, runtime/ops/map_id_to_embedding.cu.cc:30-74, + per-row pool).
+  The pooled rows are float32 or bfloat16: out's dtype when out is given, else `dtype`.  bfloat16 rows are the
+  float32 results rounded once to nearest even; the fused buffer stays float32."""
+  dtype = _tower_dtype(out.dtype if out is not None else dtype, "gather_pool's output")
   lib = _lib.load()
   dev = fused_embeddings.device
   offs = fused_embedding_offsets.to(torch.int32).contiguous()
@@ -161,9 +174,10 @@ def gather_pool(fused_embeddings: torch.Tensor, fused_embedding_offsets: torch.T
   if row_offsets is not None:
     row_offsets = row_offsets.to(torch.int32).contiguous()
   if out is None:
-    out = torch.empty(n_rows, dim, dtype=torch.float32, device=dev)
+    out = torch.empty(n_rows, dim, dtype=dtype, device=dev)
   pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-  _lib.check(lib.mono_gather_pool(dev.index, _ptr(fused_embeddings), _ptr(offs), _ptr(row_offsets), n_rows, dim,
+  fn = lib.mono_gather_pool_bf16 if dtype == torch.bfloat16 else lib.mono_gather_pool
+  _lib.check(fn(dev.index, _ptr(fused_embeddings), _ptr(offs), _ptr(row_offsets), n_rows, dim,
                                   pool, _ptr(out), out.stride(0), out_col, _stream(dev)))
   return out
 
@@ -171,7 +185,9 @@ def gather_pool(fused_embeddings: torch.Tensor, fused_embedding_offsets: torch.T
 def gather_pool_grad(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.Tensor, dim: int, total_floats: int,
                      row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum", grad_col: int = 0):
   """Backward of gather_pool: scatter-add pooled grads to the fused row buffer
-  (ref: FusedGatherGradKernel, map_id_to_embedding.cu.cc:75-118)."""
+  (ref: FusedGatherGradKernel, map_id_to_embedding.cu.cc:75-118).  pooled_grad is float32 or bfloat16 (widened
+  exactly); the returned buffer is float32."""
+  bf16 = _tower_dtype(pooled_grad.dtype, "pooled_grad") == torch.bfloat16
   lib = _lib.load()
   dev = pooled_grad.device
   offs = fused_embedding_offsets.to(torch.int32).contiguous()
@@ -180,8 +196,9 @@ def gather_pool_grad(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.T
     row_offsets = row_offsets.to(torch.int32).contiguous()
   grad = torch.zeros(total_floats, dtype=torch.float32, device=dev)
   pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-  _lib.check(lib.mono_gather_pool_grad(dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs),
-                                       _ptr(row_offsets), n_rows, dim, pool, _ptr(grad), _stream(dev)))
+  fn = lib.mono_gather_pool_grad_bf16 if bf16 else lib.mono_gather_pool_grad
+  _lib.check(fn(dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs), _ptr(row_offsets), n_rows,
+                dim, pool, _ptr(grad), _stream(dev)))
   return grad
 
 
@@ -189,7 +206,11 @@ def scatter_grad_rows(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.
                       grad_fused: torch.Tensor, row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum",
                       grad_col: int = 0):
   """Deterministic (sort-based, atomics-free) scatter of pooled-row grads into the fused row buffer
-  `grad_fused` (written in place; rows nobody refers to are left as they are)."""
+  `grad_fused` (written in place; rows nobody refers to are left as they are).  pooled_grad is float32 or
+  bfloat16 (widened exactly); grad_fused must be float32."""
+  bf16 = _tower_dtype(pooled_grad.dtype, "pooled_grad") == torch.bfloat16
+  if grad_fused.dtype != torch.float32:
+    raise ValueError(f"grad_fused must be torch.float32, not {grad_fused.dtype}")
   lib = _lib.load()
   dev = pooled_grad.device
   offs = fused_embedding_offsets.to(torch.int32).contiguous()
@@ -197,9 +218,9 @@ def scatter_grad_rows(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.
   if row_offsets is not None:
     row_offsets = row_offsets.to(torch.int32).contiguous()
   pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-  _lib.check(lib.mono_scatter_grad_rows(dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs),
-                                        offs.numel(), _ptr(row_offsets), n_rows, dim, pool, _ptr(grad_fused),
-                                        grad_fused.numel(), _stream(dev)))
+  fn = lib.mono_scatter_grad_rows_bf16 if bf16 else lib.mono_scatter_grad_rows
+  _lib.check(fn(dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs), offs.numel(),
+                _ptr(row_offsets), n_rows, dim, pool, _ptr(grad_fused), grad_fused.numel(), _stream(dev)))
   return grad_fused
 
 
@@ -361,7 +382,7 @@ def _ptr_table(tensors: Sequence[torch.Tensor], device):
   return torch.tensor([t.data_ptr() for t in tensors], dtype=torch.int64, device=device)
 
 
-def _check_layout_inputs(fid_offset, feature_offset, nfl_offset, rows, rows_name):
+def _check_layout_inputs(fid_offset, feature_offset, nfl_offset, rows, rows_name, rows_dtype=torch.float32):
   """-> the device of the index tensors.  The C ABI reads fid_offset as uint64, feature_offset as int32 and
   nfl_offset as uint32 words: a tensor of another dtype would be silently reinterpreted, so it is refused."""
   want = (("fid_offset", fid_offset, torch.int64), ("feature_offset", feature_offset, torch.int32),
@@ -377,28 +398,31 @@ def _check_layout_inputs(fid_offset, feature_offset, nfl_offset, rows, rows_name
     if not t.is_contiguous():
       raise ValueError(f"{name} must be contiguous")
   for t in rows:
-    if t.dtype != torch.float32 or t.device != dev:
-      raise ValueError(f"{rows_name} must be float32 tensors on {dev}, not {t.dtype} on {t.device}")
+    if t.dtype != rows_dtype or t.device != dev:
+      raise ValueError(f"{rows_name} must be {rows_dtype} tensors on {dev}, not {t.dtype} on {t.device}")
   return dev
 
 
 def fused_embedding_to_layout(embeddings_list: Sequence[torch.Tensor], emb_strides: Sequence[int],
                               fid_offset: torch.Tensor, feature_offset: torch.Tensor, nfl_offset: torch.Tensor,
-                              batch_size: int, tasks: Sequence[SliceTask], out_shapes: Sequence[Sequence[int]]):
+                              batch_size: int, tasks: Sequence[SliceTask], out_shapes: Sequence[Sequence[int]],
+                              dtype: torch.dtype = torch.float32):
   """ref: distribution_ops.fused_embedding_to_layout (versions 3/4/5) -> MonolithEmbeddingToLayoutV*.
   fid_offset: uint64 viewed as int64 tensor; nfl_offset: uint32 viewed as int32 tensor (sharding_sparse_fids'
   outputs as they are).  Raises ValueError for any other dtype, a non-CUDA or non-contiguous index tensor, or
-  embeddings that are not float32 on the same device."""
+  embeddings that are not float32 on the same device.  dtype: of the outputs, float32 or bfloat16 (the float32
+  results rounded once to nearest even; the tasks' strides and columns then count bfloat16 elements)."""
+  bf16 = _tower_dtype(dtype, "dtype") == torch.bfloat16
   dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, embeddings_list, "embeddings_list")
   lib = _lib.load()
-  outs = [torch.zeros(*s, dtype=torch.float32, device=dev) for s in out_shapes]
+  outs = [torch.zeros(*s, dtype=dtype, device=dev) for s in out_shapes]
   embs = [e.contiguous() for e in embeddings_list]
   ep, op = _ptr_table(embs, dev), _ptr_table(outs, dev)
   st = torch.tensor(list(emb_strides), dtype=torch.int32, device=dev)
-  _lib.check(lib.mono_embedding_to_layout(dev.index, _ptr(ep), _ptr(st), len(embs), _ptr(fid_offset),
-                                          fid_offset.numel(), _ptr(feature_offset), feature_offset.numel(),
-                                          _ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks),
-                                          len(tasks), _ptr(op), _stream(dev)))
+  fn = lib.mono_embedding_to_layout_bf16 if bf16 else lib.mono_embedding_to_layout
+  _lib.check(fn(dev.index, _ptr(ep), _ptr(st), len(embs), _ptr(fid_offset), fid_offset.numel(), _ptr(feature_offset),
+                feature_offset.numel(), _ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks), len(tasks),
+                _ptr(op), _stream(dev)))
   return outs
 
 
@@ -406,15 +430,19 @@ def fused_embedding_to_layout_grad(emb_sizes: Sequence[int], emb_strides: Sequen
                                    feature_offset: torch.Tensor, nfl_offset: torch.Tensor, batch_size: int,
                                    tasks: Sequence[SliceTask], out_grads: Sequence[torch.Tensor]):
   """ref: MonolithEmbeddingToLayoutGradV* (fused_embedding_to_layout.cc:697-948).  The index tensors as in
-  fused_embedding_to_layout; out_grads float32 on their device."""
-  dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, out_grads, "out_grads")
+  fused_embedding_to_layout; out_grads all float32 or all bfloat16 (widened exactly) on their device.  The
+  returned embedding gradients are float32."""
+  dtype = _tower_dtype(out_grads[0].dtype if len(out_grads) else torch.float32, "out_grads")
+  if any(g.dtype != dtype for g in out_grads):
+    raise ValueError(f"out_grads must be all torch.float32 or all torch.bfloat16, not {[g.dtype for g in out_grads]}")
+  dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, out_grads, "out_grads", dtype)
   lib = _lib.load()
   grads = [torch.zeros(n, dtype=torch.float32, device=dev) for n in emb_sizes]
   og = [g.contiguous() for g in out_grads]
   gp, op = _ptr_table(grads, dev), _ptr_table(og, dev)
   st = torch.tensor(list(emb_strides), dtype=torch.int32, device=dev)
-  _lib.check(lib.mono_embedding_to_layout_grad(dev.index, _ptr(gp), _ptr(st), len(grads), _ptr(fid_offset),
-                                               fid_offset.numel(), _ptr(feature_offset), feature_offset.numel(),
-                                               _ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks),
-                                               len(tasks), _ptr(op), _stream(dev)))
+  fn = lib.mono_embedding_to_layout_grad_bf16 if dtype == torch.bfloat16 else lib.mono_embedding_to_layout_grad
+  _lib.check(fn(dev.index, _ptr(gp), _ptr(st), len(grads), _ptr(fid_offset), fid_offset.numel(), _ptr(feature_offset),
+                feature_offset.numel(), _ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks), len(tasks),
+                _ptr(op), _stream(dev)))
   return grads
