@@ -24,13 +24,7 @@ namespace mono {
 // ref: MultiHashTableLookupOp::Compute / FusedLookupOp (multi_hash_table_lookup_op.cc:37-88,143-197)
 // One launch serves every (shard, table) segment of the call.
 //
-// Two phases per warp-tile of 32 ids, designed for memory-level parallelism (the op is a chain of
-// dependent random HBM reads: FID -> 64 B bucket -> 128 B row):
-//   A. lane-per-key probe: every lane resolves its own FID (4 x LDG.128 = the whole 64-byte bucket),
-//      so a warp keeps 32 independent bucket reads in flight with ~10 live registers per lane;
-//      the few lanes that miss probe the alternate bucket (and the stash when non-empty).
-//   B. group-per-row copy: row indices are handed around with shuffles; G lanes move one row with
-//      16-byte vectors, kRowsInFlight rows per group issued back to back before the first store.
+// Two phases per warp-tile of 32 ids (rowops.cuh lookup_tiles): a lane-per-key probe, then a group-per-row copy.
 // Used by lookup / fused_lookup (multi-segment) and by lookup_pool when every pooled row has exactly
 // one FID (the per-slot case of Criteo/MovieLens/DCN-shaped inputs, where pooling is the identity).
 // store one 4-element vector of a row (vector store when the row base is aligned to 4 elements)
@@ -44,6 +38,17 @@ __device__ __forceinline__ void store_vec(T* dst, int c, int D, const float4& x,
     for (int w = 0; w < 4 && c + w < D; ++w) dst[c + w] = to_row_elem(a[w], dst);
   }
 }
+
+// lookup_tiles sink: row ir at base + ir * rs, streaming stores (store_vec)
+template <typename T>
+struct StreamRows {
+  T* base;
+  int64_t rs;
+  int D;
+  bool vec;
+  __device__ __forceinline__ T* row(int64_t ir, uint32_t) const { return base + ir * rs; }
+  __device__ __forceinline__ void store(T* dst, int c, const float4& x) const { store_vec(dst, c, D, x, vec); }
+};
 
 // SINGLE: the call has one segment (one table): table fields and the output base are warp-uniform
 // and hoisted, which keeps the kernel at ~40 registers => 6 resident blocks (48 warps) per SM.
@@ -80,45 +85,36 @@ lookup_rows(const TableDev* __restrict__ tables, const CallSeg* __restrict__ seg
     out_stride = p.out_stride;
     out_col = p.out_col;
   }
-  constexpr int RPI = 32 / G;   // rows copied per iteration of a warp
-  constexpr int ITERS = G;      // iterations to drain the 32 resolved rows
-  constexpr int UNR = 4;        // row loads in flight per lane
+  if constexpr (SINGLE) {  // hoisted table / output description
+    const TileLanes<G> ln;
+    const TableRows tab = table_rows(tables + segs[0].table);
+    const int64_t rs0 = out_stride > 0 ? out_stride : tab.D;
+    T* const base0 = out + segs[0].val_off - segs[0].id_begin * rs0 + out_col;
+    const bool vec0 = (tab.D & 3) == 0 && (rs0 & 3) == 0 && (reinterpret_cast<uintptr_t>(base0) & (4 * sizeof(T) - 1)) == 0;
+    lookup_tiles<T, G, DUAL, CONFIRM>(ln, IdKeys<true>{tab, n_total, ids, prefetch}, StreamRows<T>{base0, rs0, tab.D, vec0});
+    return;
+  }
+  // several segments: the tile loop of lookup_tiles with the table, output base and stride of each position's segment
+  constexpr int RPI = 32 / G;
+  constexpr int ITERS = G;
+  constexpr int UNR = 4;
   const int lane = threadIdx.x & 31, gl = Group<G>::gl(), grp = lane / G;
   const int c = gl * 4;
-  // SINGLE: hoisted table / output description
-  const TableDev* t0 = tables + segs[0].table;
-  const int D0 = t0->dim;
-  const float* __restrict__ emb0 = t0->emb;
-  const uint32_t stride0 = t0->emb_stride;
-  const int64_t rs0 = out_stride > 0 ? out_stride : D0;
-  T* const base0 = out + segs[0].val_off - segs[0].id_begin * rs0 + out_col;
-  const bool vec0 = (D0 & 3) == 0 && (rs0 & 3) == 0 && (reinterpret_cast<uintptr_t>(base0) & (4 * sizeof(T) - 1)) == 0;
   const int64_t wstride = (int64_t)gridDim.x * (kThreads / 32) * 32;
   const int64_t wfirst = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * 32;
-  // the chain per tile is FID -> bucket -> row (one HBM latency per dependent round trip): the NEXT tile's FIDs are
-  // requested one iteration ahead, which takes that round trip off the chain
   int64_t key_next = wfirst + lane < n_total ? __ldg(ids + wfirst + lane) : 0;
   for (int64_t wbase = wfirst; wbase < n_total; wbase += wstride) {
-    // ---- phase A: lane-per-key probe ----
     const int64_t i = wbase + lane;
     const int64_t key = key_next;
-    if (i + wstride < n_total) {
-      key_next = __ldg(ids + i + wstride);
-      if (SINGLE && prefetch) {  // knob lookup_pf: the next tile's first buckets into L2
-        uint32_t b1, b2;
-        bucket_pair(key_next, t0->num_buckets, b1, b2);
-        prefetch_l2(t0->buckets + (size_t)b1 * kBucketSlots);
-      }
-    }
+    if (i + wstride < n_total) key_next = __ldg(ids + i + wstride);
     int si = 0;
     uint32_t row = kEmptyRow;
     if (i < n_total) {
-      if (!SINGLE) si = find_seg(segs, nsegs, i);
-      const TableDev* tk = SINGLE ? t0 : tables + segs[si].table;
+      si = find_seg(segs, nsegs, i);
+      const TableDev* tk = tables + segs[si].table;
       row = probe_lane<DUAL>(tk, key);
       if (CONFIRM && row == kEmptyRow) row = probe_lane_confirm_miss(tk, key);  // inserts on another stream
     }
-    // ---- phase B: group-per-row copy, UNR rows in flight ----
 #pragma unroll
     for (int it0 = 0; it0 < ITERS; it0 += UNR) {
       float4 x[UNR];
@@ -127,15 +123,10 @@ lookup_rows(const TableDev* __restrict__ tables, const CallSeg* __restrict__ seg
         const int src_lane = (it0 + u) * RPI + grp;
         const uint32_t r = __shfl_sync(0xffffffffu, row, src_lane);
         x[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (SINGLE) {
-          if (r != kEmptyRow && c < D0)
-            x[u] = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r * stride0 + c));
-        } else {
-          const int s_r = __shfl_sync(0xffffffffu, si, src_lane);
-          if (r != kEmptyRow) {
-            const TableDev* t = tables + segs[s_r].table;
-            if (c < t->dim) x[u] = __ldg(reinterpret_cast<const float4*>(t->emb + (size_t)r * t->emb_stride + c));
-          }
+        const int s_r = __shfl_sync(0xffffffffu, si, src_lane);
+        if (r != kEmptyRow) {
+          const TableDev* t = tables + segs[s_r].table;
+          if (c < t->dim) x[u] = __ldg(reinterpret_cast<const float4*>(t->emb + (size_t)r * t->emb_stride + c));
         }
       }
 #pragma unroll
@@ -144,34 +135,20 @@ lookup_rows(const TableDev* __restrict__ tables, const CallSeg* __restrict__ seg
         const int64_t ir = wbase + src_lane;
         // shuffles read lanes outside the group: all 32 lanes take part, before any divergence
         const uint32_t r_st = __shfl_sync(0xffffffffu, row, src_lane);
-        const int s_st = SINGLE ? 0 : __shfl_sync(0xffffffffu, si, src_lane);
+        const int s_st = __shfl_sync(0xffffffffu, si, src_lane);
         if (ir >= n_total) continue;
-        if (SINGLE) {
-          T* dst = base0 + ir * rs0;
-          store_vec(dst, c, D0, x[u], vec0);
-          if (D0 > 4 * G) {  // wide rows (dim > 128, G == 32): remaining vectors of the row
-            const uint32_t r = r_st;
-            for (int cc = c + 4 * G; cc < D0; cc += 4 * G) {
-              float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (r != kEmptyRow) y = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r * stride0 + cc));
-              store_vec(dst, cc, D0, y, vec0);
-            }
-          }
-        } else {
-          const CallSeg sg = segs[s_st];
-          const TableDev* t = tables + sg.table;
-          const int D = t->dim;
-          const int64_t rs = out_stride > 0 ? out_stride : D;
-          T* dst = out + sg.val_off + (ir - sg.id_begin) * rs + out_col;
-          const bool vec_ok = (D & 3) == 0 && (reinterpret_cast<uintptr_t>(dst) & (4 * sizeof(T) - 1)) == 0;
-          store_vec(dst, c, D, x[u], vec_ok);
-          if (D > 4 * G) {
-            const uint32_t r = r_st;
-            for (int cc = c + 4 * G; cc < D; cc += 4 * G) {
-              float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (r != kEmptyRow) y = __ldg(reinterpret_cast<const float4*>(t->emb + (size_t)r * t->emb_stride + cc));
-              store_vec(dst, cc, D, y, vec_ok);
-            }
+        const CallSeg sg = segs[s_st];
+        const TableDev* t = tables + sg.table;
+        const int D = t->dim;
+        const int64_t rs = out_stride > 0 ? out_stride : D;
+        T* dst = out + sg.val_off + (ir - sg.id_begin) * rs + out_col;
+        const bool vec_ok = (D & 3) == 0 && (reinterpret_cast<uintptr_t>(dst) & (4 * sizeof(T) - 1)) == 0;
+        store_vec(dst, c, D, x[u], vec_ok);
+        if (D > 4 * G) {
+          for (int cc = c + 4 * G; cc < D; cc += 4 * G) {
+            float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (r_st != kEmptyRow) y = __ldg(reinterpret_cast<const float4*>(t->emb + (size_t)r_st * t->emb_stride + cc));
+            store_vec(dst, cc, D, y, vec_ok);
           }
         }
       }
@@ -196,6 +173,37 @@ bf16_lookup_kernel(const TableDev* __restrict__ tables, int prefetch, const FwdP
   lookup_rows<__nv_bfloat16, G, true, false, CONFIRM>(tables, nullptr, 1, nullptr, 0, nullptr, 0, 0, prefetch, parts);
 }
 
+// lookup_tiles source: slot q -> its row r (the tag), and its FID when position j = q - r*L holds one
+struct SeqKeys {
+  static constexpr bool kAhead = false, kTag = true;
+  TableRows tab;
+  int64_t n;
+  const int64_t* __restrict__ fids;
+  const int32_t* __restrict__ offs;
+  uint32_t L;
+  __device__ __forceinline__ bool key(int64_t q, int64_t& key, uint32_t& r) const {
+    r = (uint32_t)q / L;
+    const uint32_t j = (uint32_t)q - r * L;
+    int64_t b = r, e = (int64_t)r + 1;
+    if (offs) {
+      b = __ldg(offs + r);
+      e = __ldg(offs + r + 1);
+    }
+    if ((int64_t)j >= e - b) return false;
+    key = __ldg(fids + b + j);
+    return true;
+  }
+};
+
+// lookup_tiles sink: position j of row r at base + r * rs + j * D
+template <typename T>
+struct SeqRows : StreamRows<T> {
+  uint32_t L;
+  __device__ __forceinline__ T* row(int64_t ir, uint32_t r) const {
+    return this->base + (int64_t)r * this->rs + (int64_t)((uint32_t)ir - r * L) * this->D;
+  }
+};
+
 // FIRSTN parts of lookup_pool_parts (ref: GatherEmb's FIRSTN branch, fused_embedding_to_layout.h:251-256): part
 // blockIdx.y writes n_rows x L positions of dim floats, position j of row r at out + r*out_stride + out_col + j*dim.
 // lookup_kernel<G, true>'s two phases over position slots q = r*L + j instead of ids: a slot with j < n_r probes
@@ -209,71 +217,12 @@ __device__ __forceinline__ void seq_rows(const FwdPart* __restrict__ parts) {
   const int64_t n_total = p.n_rows * L;
   const int32_t* __restrict__ offs = p.row_offsets;
   const int64_t* __restrict__ fids = p.fids;
-  constexpr int RPI = 32 / G;
-  constexpr int ITERS = G;
-  constexpr int UNR = 4;
-  const int lane = threadIdx.x & 31, gl = Group<G>::gl(), grp = lane / G;
-  const int c = gl * 4;
-  const TableDev* t0 = p.t;
-  const int D0 = t0->dim;
-  const float* __restrict__ emb0 = t0->emb;
-  const uint32_t stride0 = t0->emb_stride;
+  const TileLanes<G> ln;
+  const TableRows tab = table_rows(p.t);
   const int64_t rs0 = p.out_stride;
   T* const base0 = reinterpret_cast<T*>(p.out) + p.out_col;
-  const bool vec0 = (D0 & 3) == 0 && (rs0 & 3) == 0 && (reinterpret_cast<uintptr_t>(base0) & (4 * sizeof(T) - 1)) == 0;
-  // slot q -> its row r, and its FID when position j = q - r*L holds one
-  auto slot = [&](int64_t q, int64_t& key, uint32_t& r) -> bool {
-    r = (uint32_t)q / L;
-    const uint32_t j = (uint32_t)q - r * L;
-    int64_t b = r, e = (int64_t)r + 1;
-    if (offs) {
-      b = __ldg(offs + r);
-      e = __ldg(offs + r + 1);
-    }
-    if ((int64_t)j >= e - b) return false;
-    key = __ldg(fids + b + j);
-    return true;
-  };
-  const int64_t wstride = (int64_t)gridDim.x * (kThreads / 32) * 32;
-  const int64_t wfirst = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * 32;
-  for (int64_t wbase = wfirst; wbase < n_total; wbase += wstride) {
-    // ---- phase A: lane-per-key probe ----
-    const int64_t i = wbase + lane;
-    int64_t key = 0;
-    uint32_t rq = 0;
-    const bool has = i < n_total && slot(i, key, rq);
-    uint32_t row = kEmptyRow;
-    if (has) {
-      row = probe_lane(t0, key);
-      if (CONFIRM && row == kEmptyRow) row = probe_lane_confirm_miss(t0, key);  // inserts on another stream
-    }
-    // ---- phase B: group-per-row copy, UNR rows in flight ----
-#pragma unroll
-    for (int it0 = 0; it0 < ITERS; it0 += UNR) {
-      float4 x[UNR];
-#pragma unroll
-      for (int u = 0; u < UNR; ++u) {
-        const uint32_t r = __shfl_sync(0xffffffffu, row, (it0 + u) * RPI + grp);
-        x[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (r != kEmptyRow && c < D0) x[u] = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r * stride0 + c));
-      }
-#pragma unroll
-      for (int u = 0; u < UNR; ++u) {
-        const int src_lane = (it0 + u) * RPI + grp;
-        const uint32_t r_st = __shfl_sync(0xffffffffu, row, src_lane);
-        const uint32_t rq_st = __shfl_sync(0xffffffffu, rq, src_lane);
-        const int64_t ir = wbase + src_lane;
-        if (ir >= n_total) continue;
-        T* dst = base0 + (int64_t)rq_st * rs0 + (int64_t)((uint32_t)ir - rq_st * L) * D0;
-        store_vec(dst, c, D0, x[u], vec0);
-        for (int cc = c + 4 * G; cc < D0; cc += 4 * G) {  // wide rows (dim > 128, G == 32)
-          float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (r_st != kEmptyRow) y = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r_st * stride0 + cc));
-          store_vec(dst, cc, D0, y, vec0);
-        }
-      }
-    }
-  }
+  const bool vec0 = (tab.D & 3) == 0 && (rs0 & 3) == 0 && (reinterpret_cast<uintptr_t>(base0) & (4 * sizeof(T) - 1)) == 0;
+  lookup_tiles<T, G, false, CONFIRM>(ln, SeqKeys{tab, n_total, fids, offs, L}, SeqRows<T>{{base0, rs0, tab.D, vec0}, L});
 }
 
 template <int G, bool CONFIRM>
@@ -288,62 +237,30 @@ bf16_seq_kernel(const FwdPart* __restrict__ parts) {
   seq_rows<__nv_bfloat16, G, CONFIRM>(parts);
 }
 
+// lookup_tiles sink: row ir into the window of the part that holds ir
+struct PeerRows : PlainStore {
+  const int64_t* start;  // the part boundaries (shared memory)
+  const PeerOut& po;
+  __device__ __forceinline__ float* row(int64_t ir, uint32_t) const {
+    const int pr = peer_part(start, po.n, ir);
+    return reinterpret_cast<float*>(po.base[pr]) + (ir - start[pr]) * D;
+  }
+};
+
 // Owner lookup fused with the row exchange of the sharded forward (replaces FusedLookup + the
 // embedding all-to-all, ref: distributed_ps_sync.py:100-118): ids[] is the concatenation of the FID
 // buckets the requesters stored into this rank's window; the row of id i is written straight into the
 // window of the requester that asked for it (one 128-bit NVLink store per lane, a whole row per group).
-// Same two phases as lookup_kernel<G, true>.
+// Same two phases as lookup_kernel<G, true>, every miss confirmed.
 template <int G>
 __global__ void __launch_bounds__(kThreads, 6)
 lookup_push_kernel(const TableDev* __restrict__ t0, const int64_t* __restrict__ ids, int64_t n_total,
                    const PeerOut po) {
   __shared__ int64_t s_start[kMaxPeers + 1];
   peer_starts(po, s_start);
-  constexpr int RPI = 32 / G;
-  constexpr int ITERS = G;
-  constexpr int UNR = 4;
-  const int lane = threadIdx.x & 31, gl = Group<G>::gl(), grp = lane / G;
-  const int c = gl * 4;
-  const int D0 = t0->dim;
-  const float* __restrict__ emb0 = t0->emb;
-  const uint32_t stride0 = t0->emb_stride;
-  const int64_t wstride = (int64_t)gridDim.x * (kThreads / 32) * 32;
-  for (int64_t wbase = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * 32;
-       wbase < n_total; wbase += wstride) {
-    const int64_t i = wbase + lane;
-    uint32_t row = kEmptyRow;
-    if (i < n_total) {
-      const int64_t key = __ldg(ids + i);
-      row = probe_lane(t0, key);
-      if (row == kEmptyRow) row = probe_lane_confirm_miss(t0, key);
-    }
-#pragma unroll
-    for (int it0 = 0; it0 < ITERS; it0 += UNR) {
-      float4 x[UNR];
-#pragma unroll
-      for (int u = 0; u < UNR; ++u) {
-        const uint32_t r = __shfl_sync(0xffffffffu, row, (it0 + u) * RPI + grp);
-        x[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (r != kEmptyRow && c < D0)
-          x[u] = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r * stride0 + c));
-      }
-#pragma unroll
-      for (int u = 0; u < UNR; ++u) {
-        const int src_lane = (it0 + u) * RPI + grp;
-        const int64_t ir = wbase + src_lane;
-        const uint32_t r_st = __shfl_sync(0xffffffffu, row, src_lane);
-        if (ir >= n_total) continue;
-        const int pr = peer_part(s_start, po.n, ir);
-        float* dst = reinterpret_cast<float*>(po.base[pr]) + (ir - s_start[pr]) * D0;
-        if (c < D0) *reinterpret_cast<float4*>(dst + c) = x[u];
-        for (int cc = c + 4 * G; cc < D0; cc += 4 * G) {  // wide rows (dim > 128)
-          float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (r_st != kEmptyRow) y = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r_st * stride0 + cc));
-          *reinterpret_cast<float4*>(dst + cc) = y;
-        }
-      }
-    }
-  }
+  const TileLanes<G> ln;
+  const TableRows tab = table_rows(t0);
+  lookup_tiles<float, G, false, true>(ln, IdKeys<false>{tab, n_total, ids, 0}, PeerRows{{tab.D}, s_start, po});
 }
 
 // ------------------------------------------------------------------------------------------

@@ -371,6 +371,10 @@ __device__ __forceinline__ void apply_row(const TableDev* __restrict__ t, uint32
   }
 }
 
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
+
 __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -468,6 +472,136 @@ static __device__ __noinline__ uint32_t probe_lane_confirm_miss(const TableDev* 
   return kEmptyRow;
 }
 
+// The register-path lookup of one table (lookup_kernel, bf16_lookup_kernel, the seq kernels, the push kernels): two
+// phases per warp tile of 32 positions, designed for memory-level parallelism (the op is a chain of dependent random
+// HBM reads: FID -> 64 B bucket -> row):
+//   A. lane-per-key probe: every lane resolves its own FID (4 x LDG.128 = the whole 64-byte bucket), so a warp keeps
+//      32 independent bucket reads in flight with ~10 live registers per lane; the few lanes that miss probe the
+//      alternate bucket (and the stash when non-empty).  CONFIRM: the call may run beside inserts of another stream
+//      (mono_mtable::lookup_must_confirm): misses are confirmed.
+//   B. group-per-row copy: row indices are handed around with shuffles; G lanes move one row with 16-byte vectors,
+//      UNR rows per group issued back to back before the first store; rows wider than 4 * G floats (G == 32) finish
+//      in a tail loop.  An absent row is stored as zeros.
+// Src: tab (the table, TableRows), n (positions), bool key(i, key&, tag&) (whether position i holds a key, and
+//   the key).  kAhead: every position below n holds one, and the NEXT tile's keys are requested one iteration early,
+//   which takes that round trip off the FID -> bucket -> row chain (it costs registers); ahead(key) sees each of them.
+//   kTag: key() also sets a 32-bit tag that phase B shuffles to the sink with the row.
+// Sink: T* row(ir, tag) is where the row of position ir goes; store(dst, c, x) stores elements c..c+3 of it
+//   (nothing when c >= the row's dim).
+// The caller sets up the thread's lanes (TileLanes) and then the table (table_rows), before any loop around
+// lookup_tiles, in that order: the kernels' register allocation and spills depend on it.
+template <int G>
+struct TileLanes {
+  int lane = threadIdx.x & 31, gl = Group<G>::gl(), grp = lane / G;
+  int c = gl * 4;
+};
+struct TableRows {
+  const TableDev* t;
+  int D;
+  const float* __restrict__ emb;
+  uint32_t stride;
+};
+__device__ __forceinline__ TableRows table_rows(const TableDev* t) { return {t, t->dim, t->emb, t->emb_stride}; }
+
+template <typename T, int G, bool DUAL, bool CONFIRM, class Src, class Sink>
+__device__ __forceinline__ void lookup_tiles(const TileLanes<G>& ln, const Src& src, const Sink& sink) {
+  static_assert(!(Src::kAhead && Src::kTag), "a tag is set with its key, in the tile that uses it");
+  constexpr int RPI = 32 / G;   // rows copied per iteration of a warp
+  constexpr int ITERS = G;      // iterations to drain the 32 resolved rows
+  constexpr int UNR = 4;        // row loads in flight per lane
+  const int lane = ln.lane, grp = ln.grp, c = ln.c;
+  const TableRows tab = src.tab;
+  const int64_t n_total = src.n;
+  const int64_t wstride = (int64_t)gridDim.x * (kThreads / 32) * 32;
+  const int64_t wfirst = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * 32;
+  int64_t key_next = 0;
+  uint32_t no_tag;
+  if (Src::kAhead && wfirst + lane < n_total) src.key(wfirst + lane, key_next, no_tag);
+  for (int64_t wbase = wfirst; wbase < n_total; wbase += wstride) {
+    // ---- phase A: lane-per-key probe ----
+    const int64_t i = wbase + lane;
+    int64_t key = key_next;
+    uint32_t tag = 0;
+    bool has;
+    if constexpr (Src::kAhead) {
+      if (i + wstride < n_total) {
+        src.key(i + wstride, key_next, no_tag);
+        src.ahead(key_next);
+      }
+      has = i < n_total;
+    } else {
+      has = i < n_total && src.key(i, key, tag);
+    }
+    uint32_t row = kEmptyRow;
+    if (has) {
+      row = probe_lane<DUAL>(tab.t, key);
+      if (CONFIRM && row == kEmptyRow) row = probe_lane_confirm_miss(tab.t, key);  // inserts on another stream
+    }
+    // ---- phase B: group-per-row copy, UNR rows in flight ----
+#pragma unroll
+    for (int it0 = 0; it0 < ITERS; it0 += UNR) {
+      float4 x[UNR];
+#pragma unroll
+      for (int u = 0; u < UNR; ++u) {
+        const uint32_t r = __shfl_sync(0xffffffffu, row, (it0 + u) * RPI + grp);
+        x[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (r != kEmptyRow && c < tab.D) x[u] = __ldg(reinterpret_cast<const float4*>(tab.emb + (size_t)r * tab.stride + c));
+      }
+#pragma unroll
+      for (int u = 0; u < UNR; ++u) {
+        const int src_lane = (it0 + u) * RPI + grp;
+        // shuffles read lanes outside the group: all 32 lanes take part, before any divergence.  ir is taken before
+        // them, or after them when there is a tag: either order is the one that keeps its kernels' registers and spills
+        int64_t ir = 0;
+        if constexpr (!Src::kTag) ir = wbase + src_lane;
+        const uint32_t r_st = __shfl_sync(0xffffffffu, row, src_lane);
+        uint32_t tag_st = 0;
+        if constexpr (Src::kTag) {
+          tag_st = __shfl_sync(0xffffffffu, tag, src_lane);
+          ir = wbase + src_lane;
+        }
+        if (ir >= n_total) continue;
+        T* dst = sink.row(ir, tag_st);
+        sink.store(dst, c, x[u]);
+        for (int cc = c + 4 * G; cc < tab.D; cc += 4 * G) {  // wide rows (dim > 128, G == 32)
+          float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (r_st != kEmptyRow) y = __ldg(reinterpret_cast<const float4*>(tab.emb + (size_t)r_st * tab.stride + cc));
+          sink.store(dst, cc, y);
+        }
+      }
+    }
+  }
+}
+
+// lookup_tiles source: keys ids[0, n).  LDG: read through the non-coherent path (__ldg); false where peers write the
+// list while the kernel runs.  prefetch (knob lookup_pf, AHEAD only): the early keys' first buckets into L2.
+template <bool AHEAD, bool LDG = true>
+struct IdKeys {
+  static constexpr bool kAhead = AHEAD, kTag = false;
+  TableRows tab;
+  int64_t n;
+  const int64_t* ids;
+  int prefetch;
+  __device__ __forceinline__ bool key(int64_t i, int64_t& k, uint32_t&) const {
+    k = LDG ? __ldg(ids + i) : ids[i];
+    return true;
+  }
+  __device__ __forceinline__ void ahead(int64_t k) const {
+    if (prefetch) {
+      uint32_t b1, b2;
+      bucket_pair(k, tab.t->num_buckets, b1, b2);
+      prefetch_l2(tab.t->buckets + (size_t)b1 * kBucketSlots);
+    }
+  }
+};
+
+struct PlainStore {  // lookup_tiles sink part: plain 16-byte stores of rows of D floats
+  int D;
+  __device__ __forceinline__ void store(float* dst, int c, float4 x) const {
+    if (c < D) *reinterpret_cast<float4*>(dst + c) = x;
+  }
+};
+
 constexpr uint32_t kFreshBit = 0x80000000u;
 
 // probe that also returns the matching entry's address (for the timestamp bump)
@@ -517,10 +651,6 @@ __device__ __forceinline__ uint32_t probe_lane_slot(const TableDev* __restrict__
   return kEmptyRow;
 }
 
-
-__device__ __forceinline__ void prefetch_l2(const void* p) {
-  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-}
 
 // ---- cp.async staging: rows requested kStage at a time into per-thread shared-memory slots (zero register cost) ----
 constexpr int kStage = 16;

@@ -117,22 +117,22 @@ __global__ void __launch_bounds__(32) xwait_kernel(XWin w, int phase, uint64_t s
   wait_flag(w.flags(w.me) + kFlagSlot0 + 16 * phase + r, seq, timeout_ns, phase, r);
 }
 
+// lookup_tiles sink: row ir at rows + ir * D
+struct WindowRows : PlainStore {
+  float* rows;
+  __device__ __forceinline__ float* row(int64_t ir, uint32_t) const { return rows + ir * D; }
+};
+
 // 2 owner: lookup fused with the row exchange, source by source as the FID buckets arrive.  Every block visits all
 // sources (starting at a block-dependent one, taking whichever has arrived first) and grid-strides over the
 // source's warp tiles; rows go straight into the requester's rows_in (one 128-bit NVLink store per lane).
 template <int G, bool CONFIRM>
 __global__ void __launch_bounds__(kThreads, 6)
 xlookup_push_kernel(const TableDev* __restrict__ t0, XWin w, int par, uint64_t seq, uint64_t timeout_ns) {
-  constexpr int RPI = 32 / G;
-  constexpr int ITERS = G;
-  constexpr int UNR = 4;
   __shared__ uint32_t s_src;
   __shared__ uint64_t s_hdr;
-  const int lane = threadIdx.x & 31, gl = Group<G>::gl(), grp = lane / G;
-  const int c = gl * 4;
-  const int D0 = t0->dim;
-  const float* __restrict__ emb0 = t0->emb;
-  const uint32_t stride0 = t0->emb_stride;
+  const TileLanes<G> ln;
+  const TableRows tab = table_rows(t0);
   const uint64_t* myf = w.flags(w.me);
   uint32_t done = 0;  // block-uniform: sources already served
   for (int served = 0; served < w.N; ++served) {
@@ -161,45 +161,9 @@ xlookup_push_kernel(const TableDev* __restrict__ t0, XWin w, int par, uint64_t s
     const int64_t dst_off = (int64_t)(s_hdr & 0xFFFFFFFFull);
     __syncthreads();
     done |= 1u << src;
-    const int64_t* __restrict__ ids = w.ids_in(w.me, par, src);
-    float* __restrict__ dst_rows = w.rows_in(src) + dst_off * D0;
-    const int64_t wstride = (int64_t)gridDim.x * (kThreads / 32) * 32;
-    const int64_t wfirst = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * 32;
-    int64_t key_next = wfirst + lane < n_src ? ids[wfirst + lane] : 0;  // next tile's FIDs one iteration ahead
-    for (int64_t wbase = wfirst; wbase < n_src; wbase += wstride) {
-      const int64_t i = wbase + lane;
-      const int64_t key = key_next;
-      if (i + wstride < n_src) key_next = ids[i + wstride];
-      uint32_t row = kEmptyRow;
-      if (i < n_src) {
-        row = probe_lane(t0, key);
-        if (CONFIRM && row == kEmptyRow) row = probe_lane_confirm_miss(t0, key);  // inserts on another stream (rowops.cuh)
-      }
-#pragma unroll
-      for (int it0 = 0; it0 < ITERS; it0 += UNR) {
-        float4 x[UNR];
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) {
-          const uint32_t r = __shfl_sync(0xffffffffu, row, (it0 + u) * RPI + grp);
-          x[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (r != kEmptyRow && c < D0) x[u] = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r * stride0 + c));
-        }
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) {
-          const int src_lane = (it0 + u) * RPI + grp;
-          const int64_t ir = wbase + src_lane;
-          const uint32_t r_st = __shfl_sync(0xffffffffu, row, src_lane);
-          if (ir >= n_src) continue;
-          float* dst = dst_rows + ir * D0;
-          if (c < D0) *reinterpret_cast<float4*>(dst + c) = x[u];
-          for (int cc = c + 4 * G; cc < D0; cc += 4 * G) {  // wide rows (dim > 128)
-            float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (r_st != kEmptyRow) y = __ldg(reinterpret_cast<const float4*>(emb0 + (size_t)r_st * stride0 + cc));
-            *reinterpret_cast<float4*>(dst + cc) = y;
-          }
-        }
-      }
-    }
+    // the FIDs load coherently: peers write the window while the kernel runs
+    lookup_tiles<float, G, false, CONFIRM>(ln, IdKeys<true, false>{tab, n_src, w.ids_in(w.me, par, src), 0},
+                                           WindowRows{{tab.D}, w.rows_in(src) + dst_off * tab.D});
   }
 }
 
