@@ -405,6 +405,51 @@ int mono_dedup(int32_t device, const int64_t* ids_dev, int64_t n, int64_t* uniqu
                int32_t* inverse_out_dev, int32_t* n_unique_dev, int64_t* n_unique_host,
                void* stream);
 
+/* ---- ShardingSparseFids (requester side, fused-layout path) ----------------------------------
+ * ref: ShardingSparseFidsOp, NT/data/kernels/parse_sparse_feature.cc:187-330 (FillFidList, CreateOffsetTensor),
+ * version 4 outputs parse_sparse_feature.h:714-765, 763-835, 860-920; Python model
+ * NT/data/parse_sparse_feature_test.py:89-301.
+ * One record per feature, features in sorted-name order; the feature's FIDs and row splits are its slices of
+ * fids_dev (n_fids entries) and row_splits_dev (n_rows + 1 entries), concatenated in that order. */
+typedef struct mono_sharding_feature {
+  int64_t n_fids;   /* occurrences */
+  int64_t n_rows;   /* rows of the feature's CSR (1 for a shared feature) */
+  int32_t table;    /* table index, tables in sorted-name order */
+  int32_t dims_sum; /* floats of one FID's row, > 0 */
+  int32_t shared;   /* nonzero: bit 31 of the feature's nfl_offset */
+} mono_sharding_feature;
+
+/* F features over K tables and N shards; shard = (uint64)fid % N.  unique != 0: each (feature, shard) keeps its
+ * distinct FIDs in first-occurrence order (MultiShardUniqHashTable); unique == 0: every occurrence keeps a row of its
+ * own, ranked in input order inside its (feature, shard).  Lists are table-major, feature-minor.  Outputs, all on
+ * the device (M = sum n_fids, R = sum n_rows):
+ *   fid_list_dev          int64[max(M, 1)]  version-4 fid_list: shard-major, table-minor, feature-minor; the first
+ *                                           sum(shard_row_length) entries are written.  The version-3 list
+ *                                           (table k, shard n) is its contiguous slice.
+ *   fid_offset_dev        uint64[M]  in feature order: (k * N + shard) << 32 | (ordinal * dims_sum + float offset
+ *                                    of the feature's block inside its (table, shard) list)
+ *   feature_offset_dev    int32[R + 1]   every feature's row splits shifted by the occurrences before it
+ *   nfl_offset_dev        uint32[F + 1]  first feature_offset entry of every feature, bit 31 = shared
+ *   fid_list_row_splits_dev int64[N * (F + K)]  [shard][table][0, c1, c1 + c2, ...] FID counts of the table's features
+ *   table_row_length_dev  int32[N * K]  FIDs of list (shard n, table k) at n * K + k
+ *   shard_row_length_dev  int32[N]
+ *   emb_row_length_dev    int32[N * K]  floats of list (n, k): sum of counts x dims_sum
+ *   bad_row_splits_dev    int32[1], optional: 1 when a feature's row splits do not start at 0, decrease, or do not
+ *                         end at its n_fids (checked on the device), else 0
+ * table_row_length_host (int32[N * K], optional) is the only output that synchronises; the call then also returns
+ * MONO_ERR_INVALID_ARGUMENT for malformed row splits.  Without it the call makes no host round trip: the records
+ * reach the device by one stream-ordered copy.
+ * Limits, checked on the host before anything launches (MONO_ERR_INVALID_ARGUMENT): 1 <= F <= 2^25,
+ * 1 <= K, 1 <= N <= 64, M <= 2^30, R < 2^31 - 1, every table in [0, K), every dims_sum > 0, and
+ * sum n_fids x dims_sum <= 2^31 - 1 (the reference's offsets are 32-bit). */
+int mono_sharding_sparse_fids(int32_t device, const int64_t* fids_dev, const int64_t* row_splits_dev,
+                              const mono_sharding_feature* features, int32_t num_features, int32_t num_tables,
+                              int32_t num_shards, int32_t unique, int64_t* fid_list_dev, uint64_t* fid_offset_dev,
+                              int32_t* feature_offset_dev, uint32_t* nfl_offset_dev, int64_t* fid_list_row_splits_dev,
+                              int32_t* table_row_length_dev, int32_t* shard_row_length_dev,
+                              int32_t* emb_row_length_dev, int32_t* bad_row_splits_dev,
+                              int32_t* table_row_length_host, void* stream);
+
 /* ---- owner grouping: one grouping per batch shared by the sharded forward and backward -------
  * Replaces FusedReorderByIndices (ref: RT/ops/fused_reorder_by_indices.cc:38-123) + the float-atomic
  * FusedGatherGrad scatter (ref: RT/ops/map_id_to_embedding.cu.cc:75-118) for ONE id list on the

@@ -35,6 +35,11 @@ class PoolPartC(C.Structure):  # mono_pool_part
               ("rows_dev", C.c_void_p), ("stride", C.c_int64), ("col", C.c_int32), ("max_seq_len", C.c_int32)]
 
 
+class ShardingFeature(C.Structure):  # mono_sharding_feature
+  _fields_ = [("n_fids", C.c_int64), ("n_rows", C.c_int64), ("table", C.c_int32), ("dims_sum", C.c_int32),
+              ("shared", C.c_int32)]
+
+
 MAX_POOL_PARTS = 1024  # MONO_MAX_POOL_PARTS
 OPT_SGD, OPT_ADAGRAD, OPT_FTRL, OPT_ADAM = 0, 1, 2, 3
 OPT_MOMENTUM, OPT_RMSPROP, OPT_RMSPROPV2, OPT_ADADELTA, OPT_AMSGRAD = 4, 5, 6, 7, 8
@@ -93,6 +98,8 @@ SIGNATURES = {
     "mono_mtable_restore_rows": (C.c_int, [_p, _i32, _p, _i64, _p, _p]),
     "mono_reorder_by_indices": (C.c_int, [_i32, _p, _p, _i32, _i32, _p, _i32, _p, _p, _p, _p, _p, _p, _p]),
     "mono_dedup": (C.c_int, [_i32, _p, _i64, _p, _p, _p, _p, _p]),
+    "mono_sharding_sparse_fids": (C.c_int, [_i32, _p, _p, C.POINTER(ShardingFeature), _i32, _i32, _i32, _i32, _p, _p,
+                                            _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "mono_grouping_create": (C.c_int, [_i32, C.POINTER(_p)]),
     "mono_grouping_destroy": (C.c_int, [_p]),
     "mono_grouping_build": (C.c_int, [_p, _p, _i64, _i32, _i32, _p, _p, _p, C.POINTER(_i64), _p]),

@@ -585,6 +585,24 @@ int mono_reorder_by_indices(int32_t device, const int64_t* ids_dev, const int64_
   });
 }
 
+int mono_sharding_sparse_fids(int32_t device, const int64_t* fids_dev, const int64_t* row_splits_dev,
+                              const mono_sharding_feature* features, int32_t num_features, int32_t num_tables,
+                              int32_t num_shards, int32_t unique, int64_t* fid_list_dev, uint64_t* fid_offset_dev,
+                              int32_t* feature_offset_dev, uint32_t* nfl_offset_dev, int64_t* fid_list_row_splits_dev,
+                              int32_t* table_row_length_dev, int32_t* shard_row_length_dev,
+                              int32_t* emb_row_length_dev, int32_t* bad_row_splits_dev,
+                              int32_t* table_row_length_host, void* stream) {
+  return guarded([&] {
+    require(features && row_splits_dev && fid_list_dev && fid_offset_dev && feature_offset_dev && nfl_offset_dev &&
+                fid_list_row_splits_dev && table_row_length_dev && shard_row_length_dev && emb_row_length_dev,
+            "sharding_sparse_fids: null argument");
+    run_sharding(device, fids_dev, row_splits_dev, features, num_features, num_tables, num_shards, unique,
+                 fid_list_dev, fid_offset_dev, feature_offset_dev, nfl_offset_dev, fid_list_row_splits_dev,
+                 table_row_length_dev, shard_row_length_dev, emb_row_length_dev, bad_row_splits_dev,
+                 table_row_length_host, (cudaStream_t)stream);
+  });
+}
+
 int mono_dedup(int32_t device, const int64_t* ids_dev, int64_t n, int64_t* unique_out_dev,
                int32_t* inverse_out_dev, int32_t* n_unique_dev, int64_t* n_unique_host, void* stream) {
   return guarded([&] {

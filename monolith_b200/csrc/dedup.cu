@@ -18,6 +18,7 @@
 //   5 offsets : every occurrence -> fused_emb_offset[]
 #include <algorithm>
 #include <cstring>
+#include <numeric>
 #include <vector>
 
 #include "engine.h"
@@ -264,6 +265,25 @@ dd_offsets_kernel(const int64_t* __restrict__ ids, int64_t M, const int64_t* __r
   }
 }
 
+// passes 2-5 over M > 0 ids, once slot_of and the scratch set's first positions are written
+static void rank_passes(const int64_t* ids_dev, int64_t M, const int64_t* split_dev, int K, int N, int n_eff,
+                        int rank0_empty, const DSet* set, const uint32_t* slot_of, int32_t* blk_cnt, int nblk,
+                        const int32_t* dims_dev, int dim0, DDTables tb, int64_t* output_dev, int32_t* rank,
+                        int32_t* fused_emb_offset_dev, cudaStream_t s) {
+  const int g = std::min(nblk, device_sms() * 8);
+  dd_rank_kernel<0><<<g, kThreads, 0, s>>>(ids_dev, M, split_dev, K, N, n_eff, rank0_empty, set, slot_of, blk_cnt,
+                                          nblk, tb, output_dev, rank);
+  MONO_CHECK_LAUNCH();
+  dd_scan_kernel<<<1, 1024, 0, s>>>(blk_cnt, nblk, N, K, dims_dev, dim0, tb);
+  MONO_CHECK_LAUNCH();
+  dd_rank_kernel<1><<<g, kThreads, 0, s>>>(ids_dev, M, split_dev, K, N, n_eff, rank0_empty, set, slot_of, blk_cnt,
+                                          nblk, tb, output_dev, rank);
+  MONO_CHECK_LAUNCH();
+  dd_offsets_kernel<<<grid_for(M, kThreads), kThreads, 0, s>>>(ids_dev, M, split_dev, K, N, n_eff, rank0_empty, set,
+                                                              slot_of, rank, dims_dev, dim0, tb, fused_emb_offset_dev);
+  MONO_CHECK_LAUNCH();
+}
+
 void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_host, int K, int N,
                  const int32_t* dims_host, int rank0_empty, int64_t* output_dev, int32_t* sizes_dev,
                  int32_t* fused_emb_offset_dev, int32_t* shard_sizes_host,
@@ -334,19 +354,8 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
   if (M > 0) {
     dd_claim_kernel<<<grid_for(M, kThreads), kThreads, 0, s>>>(ids_dev, M, split_dev, K, set, cap - 1, slot_of);
     MONO_CHECK_LAUNCH();
-    const int g = std::min(nblk, device_sms() * 8);
-    dd_rank_kernel<0><<<g, kThreads, 0, s>>>(ids_dev, M, split_dev, K, N, n_eff, rank0_empty ? 1 : 0, set,
-                                            slot_of, blk_cnt, nblk, tb, output_dev, rank);
-    MONO_CHECK_LAUNCH();
-    dd_scan_kernel<<<1, 1024, 0, s>>>(blk_cnt, nblk, N, K, dims_dev, dim0, tb);
-    MONO_CHECK_LAUNCH();
-    dd_rank_kernel<1><<<g, kThreads, 0, s>>>(ids_dev, M, split_dev, K, N, n_eff, rank0_empty ? 1 : 0, set,
-                                            slot_of, blk_cnt, nblk, tb, output_dev, rank);
-    MONO_CHECK_LAUNCH();
-    dd_offsets_kernel<<<grid_for(M, kThreads), kThreads, 0, s>>>(ids_dev, M, split_dev, K, N, n_eff,
-                                                                rank0_empty ? 1 : 0, set, slot_of, rank,
-                                                                dims_dev, dim0, tb, fused_emb_offset_dev);
-    MONO_CHECK_LAUNCH();
+    rank_passes(ids_dev, M, split_dev, K, N, n_eff, rank0_empty ? 1 : 0, set, slot_of, blk_cnt, nblk, dims_dev, dim0, tb,
+                output_dev, rank, fused_emb_offset_dev, s);
   }
   // results: sizes_dev = [shard_sizes (N) | sharded_slot_sizes (N*K)]
   if (sizes_dev) {
@@ -373,6 +382,257 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
     if (shard_sizes_host) std::memcpy(shard_sizes_host, h.data(), sizeof(int32_t) * N);
     if (sharded_slot_sizes_host) std::memcpy(sharded_slot_sizes_host, h.data() + N, sizeof(int32_t) * NK);
     if (n_unique_host) *n_unique_host = h[N + NK];
+  }
+}
+
+// ---- ShardingSparseFids (ref: parse_sparse_feature.cc:187-330, parse_sparse_feature.h:714-920) ----------------
+//
+// The features arrive in sorted-name order ("name order", index f); the reference's lists are table-major,
+// feature-minor ("list order", index j).  The FIDs are gathered into list order and run through the reorder's
+// claim / count / scan / scatter / offsets passes with one list per feature: its output buffer is then the
+// version-4 fid_list (shard-major, table-minor, feature-minor), tb.sizes the per-(shard, feature) counts and
+// tb.emb_base the float offset of every (shard, feature) block.  unique = false replaces the claim by an identity
+// grouping (every occurrence its own first occurrence), so the same passes keep every occurrence, ranked in input
+// order inside its (feature, shard).  Three small kernels then write the remaining outputs.
+
+// Per-call tables staged from the host (one H2D copy), all indexed as named.
+struct ShardStage {
+  int64_t* split_lo;   // [F + 1] occurrence start of list j in the gathered (list-order) FIDs
+  int64_t* split_in;   // [F + 1] occurrence start of feature f in the caller's (name-order) FIDs
+  int64_t* row_start;  // [F + 1] first feature_offset entry of feature f; row_start[F] = R
+  int32_t* list_of_f;  // [F]     list index of feature f
+  int32_t* feat_of_j;  // [F]     feature index of list j
+  int32_t* table_of_j; // [F]
+  int32_t* dims_lo;    // [F]     dims_sum of list j
+  int32_t* first_j;    // [K + 1] first list of table k
+  uint32_t* nfl;       // [F + 1] nfl_offset (bit 31 = shared)
+};
+
+// list-order FIDs; unique = false also writes the identity grouping the rank passes read
+__global__ void __launch_bounds__(kThreads)
+sh_gather_kernel(const int64_t* __restrict__ fids, int64_t M, int F, ShardStage st, int identity,
+                 int64_t* __restrict__ ids_lo, DSet* __restrict__ set, uint32_t* __restrict__ slot_of) {
+  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < M; p += (int64_t)gridDim.x * blockDim.x) {
+    const int j = F > 1 ? list_of(st.split_lo, F, p) : 0;
+    ids_lo[p] = fids[st.split_in[st.feat_of_j[j]] + (p - st.split_lo[j])];
+    if (identity) {
+      slot_of[p] = (uint32_t)p;
+      set[p].first_pos = (int32_t)p;
+    }
+  }
+}
+
+// one thread per (shard n, table k): version-4 row splits [n][k][0, c1, c1 + c2, ...], table and embedding row
+// lengths ([n * K + k]); the k == 0 thread writes the shard row length
+__global__ void __launch_bounds__(kThreads)
+sh_tables_kernel(int N, int K, int F, ShardStage st, DDTables tb, int64_t* __restrict__ row_splits,
+                 int32_t* __restrict__ table_len, int32_t* __restrict__ shard_len, int32_t* __restrict__ emb_len) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= N * K) return;
+  const int n = idx / K, k = idx % K;
+  const int j0 = st.first_j[k], j1 = st.first_j[k + 1];
+  int64_t* rs = row_splits + (size_t)n * (F + K) + j0 + k;
+  int32_t cnt = 0, emb = 0;
+  rs[0] = 0;
+  for (int j = j0; j < j1; ++j) {
+    const int32_t c = tb.sizes[(size_t)n * F + j];
+    cnt += c;
+    emb += c * st.dims_lo[j];
+    rs[j - j0 + 1] = cnt;
+  }
+  table_len[idx] = cnt;
+  emb_len[idx] = emb;
+  if (k == 0) shard_len[n] = tb.shard_sz[n];
+}
+
+// every occurrence, in name order: (table * N + shard) << 32 | float offset of its row inside its (table, shard)
+// list (ref: parse_sparse_feature.cc:199-240)
+__global__ void __launch_bounds__(kThreads)
+sh_fid_offset_kernel(const int64_t* __restrict__ fids, int64_t M, int N, int F, ShardStage st, DDTables tb,
+                     const int32_t* __restrict__ offs_lo, uint64_t* __restrict__ fid_offset) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < M; i += (int64_t)gridDim.x * blockDim.x) {
+    const int f = F > 1 ? list_of(st.split_in, F, i) : 0;
+    const int j = st.list_of_f[f];
+    const int k = st.table_of_j[j];
+    const int n = (int)((uint64_t)fids[i] % (uint64_t)N);
+    const int32_t local = offs_lo[st.split_lo[j] + (i - st.split_in[f])] - tb.emb_base[(size_t)n * F + st.first_j[k]];
+    fid_offset[i] = ((uint64_t)(k * N + n) << 32) | (uint32_t)local;
+  }
+}
+
+// feature_offset[R + 1]: every feature's row splits shifted by the occurrences before it; nfl_offset[F + 1] from
+// the staged table.  Checks every feature's row splits: 0 first, non-decreasing, n_fids last (bad = 1 otherwise).
+__global__ void __launch_bounds__(kThreads)
+sh_feature_offset_kernel(const int64_t* __restrict__ rs_in, int64_t R, int F, ShardStage st,
+                         int32_t* __restrict__ feature_offset, uint32_t* __restrict__ nfl_offset,
+                         int32_t* __restrict__ bad) {
+  const int64_t items = (R > F ? R : F) + 1;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < items; r += (int64_t)gridDim.x * blockDim.x) {
+    if (r <= F) {
+      nfl_offset[r] = st.nfl[r];
+      if (r < F && st.row_start[r + 1] == st.row_start[r]) {  // a feature without rows: its splits are [0]
+        if (rs_in[st.row_start[r] + r] != 0 || st.split_in[r + 1] != st.split_in[r]) *bad = 1;
+      }
+    }
+    if (r > R) continue;
+    if (r == R) {
+      feature_offset[r] = (int32_t)st.split_in[F];
+      continue;
+    }
+    const int f = F > 1 ? list_of(st.row_start, F, r) : 0;
+    const int64_t local = r - st.row_start[f];
+    const int64_t at = st.row_start[f] + f + local;  // feature f's splits start after f earlier end entries
+    const int64_t v = rs_in[at], next = rs_in[at + 1];
+    if ((local == 0 && v != 0) || next < v ||
+        (r + 1 == st.row_start[f + 1] && next != st.split_in[f + 1] - st.split_in[f]))
+      *bad = 1;
+    feature_offset[r] = (int32_t)(st.split_in[f] + v);
+  }
+}
+
+void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits_dev,
+                  const mono_sharding_feature* feats, int F, int K, int N, int unique, int64_t* fid_list_dev,
+                  uint64_t* fid_offset_dev, int32_t* feature_offset_dev, uint32_t* nfl_offset_dev,
+                  int64_t* row_splits_out_dev, int32_t* table_len_dev, int32_t* shard_len_dev, int32_t* emb_len_dev,
+                  int32_t* bad_row_splits_dev, int32_t* table_len_host, cudaStream_t s) {
+  // every argument check runs before the device is touched
+  if (F <= 0 || K <= 0 || N <= 0) throw ArgError("num_features, num_tables and num_shards must be positive");
+  if (F > kMaxLists) throw ArgError("num_features > 2^25 is not supported");
+  if (N > kMaxShards) throw ArgError("num_shards > 64 is not supported");
+  int64_t M = 0, R = 0, floats = 0;
+  for (int f = 0; f < F; ++f) {
+    const mono_sharding_feature& a = feats[f];
+    if (a.n_fids < 0 || a.n_rows < 0) throw ArgError("n_fids and n_rows must not be negative");
+    if (a.table < 0 || a.table >= K) throw ArgError("table index out of range");
+    if (a.dims_sum <= 0) throw ArgError("dims_sum must be positive");
+    M += a.n_fids;
+    R += a.n_rows;
+    if (M > kMaxIds) throw ArgError("more than 2^30 ids in one call");
+    if (R >= INT32_MAX) throw ArgError("more than 2^31 - 2 rows in one call");
+    floats += a.n_fids * a.dims_sum;
+    if (floats > INT32_MAX) throw ArgError("sum of n_fids x dims_sum exceeds 2^31 - 1 float offsets");
+  }
+  MONO_CUDA(cudaSetDevice(device));
+
+  // staged tables: name order -> list order is a stable sort by table
+  std::vector<int32_t> feat_of_j(F);
+  std::iota(feat_of_j.begin(), feat_of_j.end(), 0);
+  std::stable_sort(feat_of_j.begin(), feat_of_j.end(), [&](int a, int b) { return feats[a].table < feats[b].table; });
+  size_t off = 0;
+  auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 15) & ~(size_t)15; return o; };
+  const size_t o_split_lo = take(sizeof(int64_t) * (F + 1)), o_split_in = take(sizeof(int64_t) * (F + 1)),
+               o_row = take(sizeof(int64_t) * (F + 1)), o_list = take(sizeof(int32_t) * F),
+               o_feat = take(sizeof(int32_t) * F), o_tab = take(sizeof(int32_t) * F), o_dims = take(sizeof(int32_t) * F),
+               o_first = take(sizeof(int32_t) * (K + 1)), o_nfl = take(sizeof(uint32_t) * (F + 1));
+  const size_t stage_bytes = off;
+  std::vector<char> h(stage_bytes);
+  auto H = [&](size_t o, auto* type) { return reinterpret_cast<decltype(type)>(h.data() + o); };
+  int64_t* split_lo = H(o_split_lo, (int64_t*)nullptr);
+  int64_t* split_in = H(o_split_in, (int64_t*)nullptr);
+  int64_t* row_start = H(o_row, (int64_t*)nullptr);
+  int32_t* list_of_f = H(o_list, (int32_t*)nullptr);
+  int32_t* table_of_j = H(o_tab, (int32_t*)nullptr);
+  int32_t* dims_lo = H(o_dims, (int32_t*)nullptr);
+  int32_t* first_j = H(o_first, (int32_t*)nullptr);
+  uint32_t* nfl = H(o_nfl, (uint32_t*)nullptr);
+  std::memcpy(h.data() + o_feat, feat_of_j.data(), sizeof(int32_t) * F);
+  split_lo[0] = split_in[0] = row_start[0] = 0;
+  for (int f = 0; f < F; ++f) {
+    split_in[f + 1] = split_in[f] + feats[f].n_fids;
+    row_start[f + 1] = row_start[f] + feats[f].n_rows;
+    nfl[f] = (uint32_t)row_start[f] | (feats[f].shared ? 0x80000000u : 0u);
+  }
+  nfl[F] = (uint32_t)(R + 1);
+  for (int k = 0; k <= K; ++k) first_j[k] = F;
+  for (int j = F - 1; j >= 0; --j) {
+    const mono_sharding_feature& a = feats[feat_of_j[j]];
+    list_of_f[feat_of_j[j]] = j;
+    table_of_j[j] = a.table;
+    dims_lo[j] = a.dims_sum;
+    first_j[a.table] = j;
+  }
+  for (int k = K - 1; k >= 0; --k) first_j[k] = std::min(first_j[k], first_j[k + 1]);  // tables without features
+  for (int j = 0; j < F; ++j) split_lo[j + 1] = split_lo[j] + feats[feat_of_j[j]].n_fids;
+
+  // one stream-ordered scratch allocation: the reorder's scratch, the gathered FIDs and offsets, the staged tables
+  const int nblk = (int)std::max<int64_t>(1, (M + kTile - 1) / kTile);
+  const size_t M1 = (size_t)std::max<int64_t>(M, 1);
+  const uint32_t cap = unique ? claim_set_slots(std::max<int64_t>(M, 1)) : (uint32_t)M1;
+  const size_t NF = (size_t)N * F;
+  off = 0;
+  auto take256 = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_set = take256(sizeof(DSet) * cap), o_slot = take256(sizeof(uint32_t) * M1),
+               o_rank = take256(sizeof(int32_t) * M1), o_blk = take256(sizeof(int32_t) * (size_t)N * nblk),
+               o_ids = take256(sizeof(int64_t) * M1), o_offs = take256(sizeof(int32_t) * M1),
+               o_small = take256(sizeof(int32_t) * (4 * NF + N + 8)), o_stage = take256(stage_bytes);
+  char* ws = nullptr;
+  MONO_CUDA(cudaMallocAsync((void**)&ws, off, s));
+  DSet* set = reinterpret_cast<DSet*>(ws + o_set);
+  uint32_t* slot_of = reinterpret_cast<uint32_t*>(ws + o_slot);
+  int32_t* rank = reinterpret_cast<int32_t*>(ws + o_rank);
+  int32_t* blk_cnt = reinterpret_cast<int32_t*>(ws + o_blk);
+  int64_t* ids_lo = reinterpret_cast<int64_t*>(ws + o_ids);
+  int32_t* offs_lo = reinterpret_cast<int32_t*>(ws + o_offs);
+  int32_t* small = reinterpret_cast<int32_t*>(ws + o_small);
+  char* stage = ws + o_stage;
+  DDTables tb;
+  tb.sizes = small;
+  tb.shard_sz = small + NF;
+  tb.out_base = tb.shard_sz + N;
+  tb.emb_base = tb.out_base + NF;
+  tb.list_rank0 = tb.emb_base + NF;
+  tb.n_unique = tb.list_rank0 + NF;
+  int32_t* bad = tb.n_unique + 1;
+  ShardStage st;
+  st.split_lo = reinterpret_cast<int64_t*>(stage + o_split_lo);
+  st.split_in = reinterpret_cast<int64_t*>(stage + o_split_in);
+  st.row_start = reinterpret_cast<int64_t*>(stage + o_row);
+  st.list_of_f = reinterpret_cast<int32_t*>(stage + o_list);
+  st.feat_of_j = reinterpret_cast<int32_t*>(stage + o_feat);
+  st.table_of_j = reinterpret_cast<int32_t*>(stage + o_tab);
+  st.dims_lo = reinterpret_cast<int32_t*>(stage + o_dims);
+  st.first_j = reinterpret_cast<int32_t*>(stage + o_first);
+  st.nfl = reinterpret_cast<uint32_t*>(stage + o_nfl);
+
+  // a pageable H2D copy is staged by the driver before the call returns: h may go out of scope after it
+  MONO_CUDA(cudaMemcpyAsync(stage, h.data(), stage_bytes, cudaMemcpyHostToDevice, s));
+  if (unique) MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(DSet) * cap, s));
+  MONO_CUDA(cudaMemsetAsync(small, 0, sizeof(int32_t) * (4 * NF + N + 8), s));
+
+  if (M > 0) {
+    sh_gather_kernel<<<grid_for(M, kThreads), kThreads, 0, s>>>(fids_dev, M, F, st, unique ? 0 : 1, ids_lo, set,
+                                                               slot_of);
+    MONO_CHECK_LAUNCH();
+    if (unique) {
+      dd_claim_kernel<<<grid_for(M, kThreads), kThreads, 0, s>>>(ids_lo, M, st.split_lo, F, set, cap - 1, slot_of);
+      MONO_CHECK_LAUNCH();
+    }
+    rank_passes(ids_lo, M, st.split_lo, F, N, N, 0, set, slot_of, blk_cnt, nblk, st.dims_lo, dims_lo[0], tb,
+                fid_list_dev, rank, offs_lo, s);
+  }
+  sh_tables_kernel<<<(N * K + kThreads - 1) / kThreads, kThreads, 0, s>>>(N, K, F, st, tb, row_splits_out_dev,
+                                                                         table_len_dev, shard_len_dev, emb_len_dev);
+  MONO_CHECK_LAUNCH();
+  if (M > 0) {
+    sh_fid_offset_kernel<<<grid_for(M, kThreads), kThreads, 0, s>>>(fids_dev, M, N, F, st, tb, offs_lo,
+                                                                   fid_offset_dev);
+    MONO_CHECK_LAUNCH();
+  }
+  sh_feature_offset_kernel<<<grid_for(std::max<int64_t>(R, F) + 1, kThreads), kThreads, 0, s>>>(
+      row_splits_dev, R, F, st, feature_offset_dev, nfl_offset_dev, bad);
+  MONO_CHECK_LAUNCH();
+  if (bad_row_splits_dev)
+    MONO_CUDA(cudaMemcpyAsync(bad_row_splits_dev, bad, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+  std::vector<int32_t> back((size_t)N * K + 1);
+  if (table_len_host) {
+    MONO_CUDA(cudaMemcpyAsync(back.data(), table_len_dev, sizeof(int32_t) * N * K, cudaMemcpyDeviceToHost, s));
+    MONO_CUDA(cudaMemcpyAsync(back.data() + (size_t)N * K, bad, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  }
+  MONO_CUDA(cudaFreeAsync(ws, s));
+  if (table_len_host) {
+    MONO_CUDA(cudaStreamSynchronize(s));
+    if (back[(size_t)N * K]) throw ArgError("row splits must start at 0, not decrease and end at the feature's n_fids");
+    std::memcpy(table_len_host, back.data(), sizeof(int32_t) * N * K);
   }
 }
 

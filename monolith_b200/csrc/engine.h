@@ -504,6 +504,11 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
                  int32_t* fused_emb_offset_dev, int32_t* shard_sizes_host,
                  int32_t* sharded_slot_sizes_host, int64_t* n_unique_host, int32_t* n_unique_dev,
                  cudaStream_t s);
+void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits_dev,
+                  const mono_sharding_feature* feats, int F, int K, int N, int unique, int64_t* fid_list_dev,
+                  uint64_t* fid_offset_dev, int32_t* feature_offset_dev, uint32_t* nfl_offset_dev,
+                  int64_t* row_splits_out_dev, int32_t* table_len_dev, int32_t* shard_len_dev, int32_t* emb_len_dev,
+                  int32_t* bad_row_splits_dev, int32_t* table_len_host, cudaStream_t s);
 
 // layout.cu; T: element type of the pooled rows, float or __nv_bfloat16
 template <typename T>

@@ -82,28 +82,42 @@ def unique_with_inverse(ids: torch.Tensor, sync: bool = True):
 
 def sharding_sparse_fids(features: Dict[str, Tuple[torch.Tensor, torch.Tensor]], feature_table: Dict[str, str],
                          feature_dims_sum: Dict[str, int], num_of_shards: int, shared_features: Sequence[str] = (),
-                         reorder_fn=None):
-  """Outputs of the reference's ShardingSparseFids (version 3+, unique = true) from per-feature FID lists —
-  ref: ShardingSparseFidsOp::FillFidList / CreateOffsetTensor, NT/data/kernels/parse_sparse_feature.cc:187-330;
-  Python model: NT/data/parse_sparse_feature_test.py:87-240 (SURVEY §8 row a2).
+                         reorder_fn=None, *, unique: bool = True, sync: bool = True):
+  """Outputs of the reference's ShardingSparseFids (versions 3 and 4) from per-feature FID lists —
+  ref: ShardingSparseFidsOp::FillFidList / CreateOffsetTensor, NT/data/kernels/parse_sparse_feature.cc:187-330,
+  version 4: parse_sparse_feature.h:714-920; Python model: NT/data/parse_sparse_feature_test.py:87-301 (SURVEY §8
+  row a2).
 
   features[name] = (fids int64[n], row_splits int64[rows + 1]) — CSR over the samples of the batch (a shared
   feature has ONE row).  Returns a dict:
     fid_list       list of K*N int64 tensors, index = table_index * N + shard (tables in sorted-name order): the
                    (table, shard) list is the concatenation, over the table's features in sorted-name order, of
-                   each feature's distinct FIDs of that shard in first-occurrence order
+                   each feature's FIDs of that shard: its distinct FIDs in first-occurrence order (unique=True) or
+                   every occurrence in input order (unique=False).  None with sync=False (its sizes are on the device)
     fid_offset     int64[M] holding the reference's uint64: (table_index * N + shard) << 32 | float offset of the
                    FID's row inside that (table, shard) list, rows of feature f being dims_sum[f] floats wide
     feature_offset int32[#(feature, row) + 1]; nfl_offset int32[#features + 1] holding the reference's uint32 bits
                    (bit 31 = shared, so a shared feature's entry is negative), features in sorted-name order — all
                    three are what fused_embedding_to_layout[_grad] takes as they are
-  The dedup / shard / offset work is ONE FusedReorderByIndices launch over the features as lists (per-list
-  dims = dims_sum, shard-major / list-minor output, bit-exact kernel); the rest is index arithmetic on device.
+  and, for CUDA inputs without reorder_fn (one mono_sharding_sparse_fids call, all outputs made on the device):
+    fid_list_row_splits        K*N int64 tensors [0, c1, c1 + c2, ...], FID counts of the (table, shard) list's features
+    fid_list_fused             the version-4 fid_list: the lists shard-major, table-minor, in one int64 tensor; with
+                               sync=False its first sum(fid_list_shard_row_length) of M entries
+    fid_list_table_row_length  int32[N*K], list (shard n, table k) at n * K + k
+    fid_list_shard_row_length  int32[N]
+    fid_list_emb_row_length    int32[N*K], floats of each list
+  sync=True reads the N*K list lengths back to slice fid_list (one synchronisation); sync=False makes no host round
+  trip.  reorder_fn (the CPU twin: lists, N, dims -> fused_reorder_by_indices' outputs) keeps the version-3
+  unique outputs only and the adapter's own index arithmetic.
   (The reference dedups per (feature, shard); FIDs carry their slot, so features never share a FID.)"""
   N = int(num_of_shards)
+  names = sorted(features)
+  if reorder_fn is None and names and features[names[0]][0].is_cuda:
+    return _sharding_sparse_fids_device(features, feature_table, feature_dims_sum, N, shared_features, unique, sync)
+  if not unique or not sync:
+    raise ValueError("unique=False and sync=False need CUDA inputs and no reorder_fn")
   if reorder_fn is None:
     reorder_fn = lambda lists, n, dims: fused_reorder_by_indices(lists, n, dims, rank0_empty_shard=False)
-  names = sorted(features)
   tables = sorted({feature_table[n] for n in names})
   t_idx = {t: i for i, t in enumerate(tables)}
   order = sorted(names, key=lambda n: (t_idx[feature_table[n]], n))      # table-major, feature-minor
@@ -157,6 +171,57 @@ def sharding_sparse_fids(features: Dict[str, Tuple[torch.Tensor, torch.Tensor]],
           "nfl_offset": torch.as_tensor([v - (1 << 32) if v >> 31 else v for v in nfl_offset], dtype=torch.int32,
                                         device=device),
           "table_names": tables, "feature_names": names}
+
+
+def _sharding_sparse_fids_device(features, feature_table, feature_dims_sum, N, shared_features, unique, sync):
+  lib = _lib.load()
+  names = sorted(features)
+  tables = sorted({feature_table[n] for n in names})
+  t_idx = {t: i for i, t in enumerate(tables)}
+  F, K = len(names), len(tables)
+  device = features[names[0]][0].device
+  fids = [features[n][0].reshape(-1).to(torch.int64) for n in names]
+  splits = [features[n][1].reshape(-1).to(device=device, dtype=torch.int64) for n in names]
+  shared = set(shared_features)
+  recs = (_lib.ShardingFeature * F)()
+  for i, n in enumerate(names):
+    recs[i].n_fids, recs[i].n_rows = fids[i].numel(), splits[i].numel() - 1
+    recs[i].table, recs[i].dims_sum, recs[i].shared = t_idx[feature_table[n]], int(feature_dims_sum[n]), n in shared
+  M, R = sum(t.numel() for t in fids), sum(t.numel() - 1 for t in splits)
+  fids, splits = torch.cat(fids), torch.cat(splits)
+  i32 = dict(dtype=torch.int32, device=device)
+  fused = torch.empty(max(M, 1), dtype=torch.int64, device=device)
+  fid_offset = torch.empty(max(M, 1), dtype=torch.int64, device=device)
+  feature_offset, nfl_offset = torch.empty(R + 1, **i32), torch.empty(F + 1, **i32)
+  row_splits = torch.empty(N * (F + K), dtype=torch.int64, device=device)
+  table_len, shard_len, emb_len = torch.empty(N * K, **i32), torch.empty(N, **i32), torch.empty(N * K, **i32)
+  host_len = (C.c_int32 * (N * K))() if sync else None
+  _lib.check(lib.mono_sharding_sparse_fids(device.index, _ptr(fids), _ptr(splits), recs, F, K, N, 1 if unique else 0,
+                                           _ptr(fused), _ptr(fid_offset), _ptr(feature_offset), _ptr(nfl_offset),
+                                           _ptr(row_splits), _ptr(table_len), _ptr(shard_len), _ptr(emb_len), None,
+                                           host_len, _stream(device)))
+  # lists of table k: features first[k] .. first[k + 1] - 1 in table-major order; row splits block of (n, k) at
+  # n * (F + K) + first[k] + k
+  per_table = [sum(1 for n in names if t_idx[feature_table[n]] == k) for k in range(K)]
+  first = [0]
+  for c in per_table:
+    first.append(first[-1] + c)
+  rs_list = [row_splits[n * (F + K) + first[k] + k:n * (F + K) + first[k + 1] + k + 1] for k in range(K)
+             for n in range(N)]
+  fid_list = None
+  if sync:
+    lens = list(host_len)
+    starts = [0]
+    for x in lens:
+      starts.append(starts[-1] + x)
+    fid_list = [fused[starts[n * K + k]:starts[n * K + k + 1]] for k in range(K) for n in range(N)]
+    fused = fused[:starts[-1]]
+  else:
+    fused = fused[:M]
+  return {"fid_list": fid_list, "fid_offset": fid_offset[:M], "feature_offset": feature_offset, "nfl_offset": nfl_offset,
+          "table_names": tables, "feature_names": names, "fid_list_row_splits": rs_list, "fid_list_fused": fused,
+          "fid_list_table_row_length": table_len, "fid_list_shard_row_length": shard_len,
+          "fid_list_emb_row_length": emb_len}
 
 
 def gather_pool(fused_embeddings: torch.Tensor, fused_embedding_offsets: torch.Tensor, dim: int,
