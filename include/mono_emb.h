@@ -127,6 +127,11 @@ const char* mono_mtable_table_name(const mono_mtable_t* t, int32_t k);
 int32_t mono_mtable_dim(const mono_mtable_t* t, int32_t k);
 int32_t mono_mtable_slice_size(const mono_mtable_t* t, int32_t k);
 int mono_mtable_size(mono_mtable_t* t, int32_t k, int64_t* out_size, void* stream); /* SYNC */
+/* Diagnostics: copies the first min(n, 16) counter words of table k to out_host, as they are (no error check).
+ * Word 0 rows handed out by the bump allocator, 1 rows on the free list, 2 live keys, 3 stash entries (live and
+ * deleted), 4 sticky error bits (1 stash overflow, 2 row slab overflow, 4 a cuckoo displacement lost its marked
+ * slot), 8 cuckoo displacements made, 9 entries an insert currently carries outside the table.  SYNC */
+int mono_mtable_counters(mono_mtable_t* t, int32_t k, uint32_t* out_host, int32_t n, void* stream);
 /* ref: EmbeddingHashTableTfBridge::max_update_ts_sec_ (tf_bridge.cc:202-206,262-263) */
 int64_t mono_mtable_max_update_ts(const mono_mtable_t* t, int32_t k);
 

@@ -76,6 +76,7 @@ SIGNATURES = {
     "mono_mtable_state_floats": (_i32, [_p, _i32]),
     "mono_mtable_size": (C.c_int, [_p, _i32, C.POINTER(_i64), _p]),
     "mono_mtable_max_update_ts": (_i64, [_p, _i32]),
+    "mono_mtable_counters": (C.c_int, [_p, _i32, _p, _i32, _p]),
     "mono_mtable_lookup": (C.c_int, [_p, _p, _p, _p, _p]),
     "mono_mtable_fused_offsets": (C.c_int, [_p, _p, _i32, _p, _p, _p]),
     "mono_mtable_fused_lookup": (C.c_int, [_p, _p, _p, _i32, _i64, _p, _p]),

@@ -275,6 +275,17 @@ int mono_mtable_size(mono_mtable_t* t, int32_t k, int64_t* out_size, void* strea
   });
 }
 
+int mono_mtable_counters(mono_mtable_t* t, int32_t k, uint32_t* out_host, int32_t n, void* stream) {
+  return guarded([&] {
+    require(k >= 0 && k < (int)t->tables.size(), "bad table index");
+    require(out_host != nullptr && n > 0, "counters: bad arguments");
+    HandleGuard hg_(t);
+    uint32_t c[kNumCtrs];
+    copy_counters_sync(t, k, (cudaStream_t)stream, c);
+    std::memcpy(out_host, c, sizeof(uint32_t) * (size_t)std::min<int32_t>(n, kNumCtrs));
+  });
+}
+
 int mono_mtable_lookup(mono_mtable_t* t, const int64_t* ids_dev, const int64_t* id_split_host,
                        float* emb_out_dev, void* stream) {
   return guarded([&] {

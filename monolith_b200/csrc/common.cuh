@@ -47,7 +47,7 @@ enum Ctr {
   kCtrFree = 1,      // entries on the free list
   kCtrSize = 2,      // live keys
   kCtrStash = 3,     // live + tomb entries in the stash
-  kCtrError = 4,     // sticky error bits (1 = stash overflow, 2 = row slab overflow)
+  kCtrError = 4,     // sticky error bits (1 = stash overflow, 2 = row slab overflow, 4 = lost a marked slot)
   kCtrMiss = 5,      // scratch: misses of the current upsert call
   kCtrAux = 6,       // scratch
   kCtrMaxTs = 7,     // max update time seen (low 32 bits; ref tf_bridge.cc:202-206 truncates to int)

@@ -450,6 +450,8 @@ void upload_tables(mono_mtable* mt, cudaStream_t s);
 // make room for n_new more keys in table k (grows row slabs / rehashes buckets when needed)
 void ensure_capacity(mono_mtable* mt, int k, uint64_t n_new, cudaStream_t s);
 void request_snapshot(mono_mtable* mt, int k, cudaStream_t s);
+// the table's counter words as they are (no error check); read_counters_sync also raises on every error bit
+void copy_counters_sync(mono_mtable* mt, int k, cudaStream_t s, uint32_t* out /*kNumCtrs*/);
 void read_counters_sync(mono_mtable* mt, int k, cudaStream_t s, uint32_t* out /*kNumCtrs*/);
 void evict_table(mono_mtable* mt, int k, int64_t max_update_time, cudaStream_t s);
 int64_t export_rows(mono_mtable* mt, int k, int64_t* cursor, int64_t max_n, int64_t* ids_out,

@@ -330,14 +330,21 @@ void upload_tables(mono_mtable* mt, cudaStream_t s) {
   mt->tables_dirty = false;
 }
 
-void read_counters_sync(mono_mtable* mt, int k, cudaStream_t s, uint32_t* out) {
+void copy_counters_sync(mono_mtable* mt, int k, cudaStream_t s, uint32_t* out) {
   HostTable& t = mt->tables[k];
   MONO_CUDA(cudaMemcpyAsync(mt->h_flag, t.dev.ctrs, kNumCtrs * sizeof(uint32_t),
                             cudaMemcpyDeviceToHost, s));
   MONO_CUDA(cudaStreamSynchronize(s));
   std::memcpy(out, mt->h_flag, kNumCtrs * sizeof(uint32_t));
-  if (out[kCtrError] & 1u) throw CudaError("table '" + t.name + "': stash overflow (insert failed)");
-  if (out[kCtrError] & 2u) throw CudaError("table '" + t.name + "': row slab overflow");
+}
+
+void read_counters_sync(mono_mtable* mt, int k, cudaStream_t s, uint32_t* out) {
+  copy_counters_sync(mt, k, s, out);
+  const std::string& name = mt->tables[k].name;
+  if (out[kCtrError] & 1u) throw CudaError("table '" + name + "': stash overflow (insert failed)");
+  if (out[kCtrError] & 2u) throw CudaError("table '" + name + "': row slab overflow");
+  if (out[kCtrError] & 4u)
+    throw CudaError("table '" + name + "': cuckoo displacement lost a marked slot (table changed under an insert)");
 }
 
 void request_snapshot(mono_mtable* mt, int k, cudaStream_t s) {

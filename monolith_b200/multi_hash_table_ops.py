@@ -156,6 +156,18 @@ class MultiHashTable:
       res[n] = v.value
     return res[name] if name else res
 
+  COUNTER_WORDS = {"bump": 0, "free": 1, "size": 2, "stash": 3, "error": 4, "moves": 8, "inflight": 9}
+
+  def counters(self, slot: str) -> Dict[str, int]:
+    """The table's allocator and cuckoo counters by name, as they are (mono_mtable_counters): rows handed out by the
+    bump allocator, rows on the free list, live keys, stash entries, sticky error bits, displacements made and
+    entries an insert carries outside the table.  Between calls bump - free == size and inflight == 0.  Synchronises;
+    raises on nothing (size() raises on the error bits)."""
+    words = (C.c_uint32 * 16)()
+    _lib.check(self._lib.mono_mtable_counters(self._h, self._table_names.index(slot), words, 16,
+                                              _stream(self._device)))
+    return {n: int(words[i]) for n, i in MultiHashTable.COUNTER_WORDS.items()}
+
   # ---- ragged packing (ref: get_ragged_id / get_flat_value / get_embeddings :528-548) -------
   def get_ragged_id(self, slot_to_id: Dict[str, torch.Tensor]) -> Tuple[torch.Tensor, List[int]]:
     parts, splits = [], [0]

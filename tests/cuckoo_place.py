@@ -135,3 +135,73 @@ def colliding_keys(nb, b1, b2, n, rng, stash_start=None, slots=None):
         if len(keys) == n:
           break
   return np.asarray(keys, np.int64)
+
+
+# ------------------------------------------------------------------------------------------------
+# groups aimed at the write side (cuckoo_insert, rehash_kernel)
+# ------------------------------------------------------------------------------------------------
+BUCKET_SLOTS = 4          # common.cuh kBucketSlots
+
+
+def stable_keys(nb, b1, b2, n, rng, levels=2):
+  """n keys that share one bucket pair at nb, 2·nb, ..., 2^levels·nb: both hash halves are drawn inside one bucket
+  of the 2^levels·nb table, whose buckets are nested in those of every smaller one (umulhi(w, nb) ==
+  umulhi(w, 2·nb) >> 1).  A closed group of more than 8 such keys keeps its excess in the stash through every rehash
+  that doubles the bucket count (table.cu rehash: max(2·nb, buckets_for(keys)) = 2·nb while that is larger).
+  b1, b2 are buckets of the 2^levels·nb table; the caller keeps b1 >> j != b2 >> j for every j <= levels so that no
+  level needs the b2 == b1 fix-up."""
+  for j in range(levels + 1):
+    assert (b1 >> j) != (b2 >> j), "the pair collapses at some level"
+  return colliding_keys(nb << levels, b1, b2, n, rng)
+
+
+def avoiding(keys, used, nbs):
+  """The keys none of whose bucket pairs, at any nb of `nbs`, meets a bucket in used[nb]."""
+  keys = np.asarray(keys, np.int64)
+  ok = np.ones(keys.size, bool)
+  for nb in nbs:
+    b1, b2 = bucket_pair(keys, nb)
+    u = np.asarray(sorted(used.get(nb, ())), np.int64)
+    ok &= ~np.isin(b1, u) & ~np.isin(b2, u)
+  return keys[ok]
+
+
+class BucketPicker:
+  """Distinct buckets of an nb-bucket table (optionally at the finest level of a stable_keys group, whose images
+  at every coarser level must be distinct as well)."""
+
+  def __init__(self, nb, rng, levels=0):
+    self.nb, self.rng, self.levels = nb, rng, levels
+    self.used = [set() for _ in range(levels + 1)]   # used[j]: buckets taken in the table of nb << (levels - j)
+
+  def take(self):
+    fine = self.nb << self.levels
+    while True:
+      b = int(self.rng.integers(0, fine))
+      imgs = [b >> j for j in range(self.levels + 1)]
+      if all(i not in u for i, u in zip(imgs, self.used)):
+        for i, u in zip(imgs, self.used):
+          u.add(i)
+        return b
+
+
+def copy_first_group(nb, picker, rng):
+  """Keys that make one insert move an entry copy-first (the displacement that succeeds, common.cuh cuckoo_insert
+  step 2): `fill` = 4 keys whose first bucket is A and 4 whose first bucket is B, each with its own otherwise empty
+  alternate bucket; `newcomer` has the pair (A, B).  Once `fill` is in the table (an earlier call: 4 keys in 4 empty
+  slots of their first bucket), both of the newcomer's buckets are full, so its insert marks a victim in A and copies
+  it into the victim's alternate bucket, which has room: ctrs[kCtrMoves] rises and nothing reaches the stash.
+  -> (fill, newcomer, buckets used)"""
+  A, B = picker.take(), picker.take()
+  fill = []
+  for first in (A, B):
+    for _ in range(BUCKET_SLOTS):
+      fill += colliding_keys(nb, first, picker.take(), 1, rng).tolist()
+  newcomer = colliding_keys(nb, A, B, 1, rng)
+  return np.asarray(fill, np.int64), newcomer
+
+
+def predicted_stash(group_sizes):
+  """Stash entries that closed, disjoint bucket pairs leave: the two buckets hold 2·kBucketSlots keys, every further
+  key of the pair ends in the stash (and nothing else can move into or out of the pair)."""
+  return sum(max(0, int(n) - 2 * BUCKET_SLOTS) for n in group_sizes)
