@@ -166,7 +166,10 @@ int mono_mtable_contains(mono_mtable_t* t, int32_t k, const int64_t* ids_dev, in
  * occurrences (no dedup pass is needed on the forward).  Replaces, for one table,
  *   MultiHashTable.lookup -> embedding_combiners.ReduceSum/ReduceMean
  *   (ref: multi_hash_table_ops.py:382-390, embedding_combiners.py:41-70, RT/ops/reduce_op.cc:29-87)
- * and, in the fused-layout path, lookup -> GatherEmb (ref: RT/ops/fused_embedding_to_layout.h:204-261).
+ * with the fused-layout path's arithmetic, lookup -> GatherEmb (ref: RT/ops/fused_embedding_to_layout.h:204-261):
+ * not bit for bit ReduceSum / ReduceMean.  SUM here starts from the first term (ReduceSum from +0.0: a row of -0.0
+ * terms is -0.0 here, +0.0 there), MEAN divides each term (ReduceMean multiplies the sum by 1/n).
+ * mono_reduce_and_split after mono_mtable_lookup gives ReduceSum's and ReduceMean's bits.
  * fids_dev[row_offsets[r]:row_offsets[r+1]] are the FIDs pooled into output row r
  * (row_offsets_dev == NULL means exactly one FID per pooled row).  Terms are accumulated in FID
  * order (deterministic, no atomics).  MEAN divides each term by n (fused-layout semantics,
@@ -612,6 +615,58 @@ int mono_embedding_to_layout_grad_bf16(int32_t device, float* const* emb_grad_pt
                                        int32_t batch_size, const mono_slice_task* tasks_host,
                                        int32_t n_tasks, const float* const* out_grad_ptrs_dev,
                                        void* stream);
+
+/* ---- ReduceSum / ReduceMean / FusedReduceAndSplitGPU: pooling of per-occurrence rows ----------
+ * ref: MonolithFusedReduceAndSplitGPU[Grad] (RT/ops/reduce_op.cu.cc:290-378, 478-680), MonolithReduceSum /
+ * MonolithReduceMean and their gradients (reduce_op.cc:29-89, 124-180), MonolithFusedReduceSumAndSplit[Gradient]
+ * (reduce_op.cc:232-330): the default (not fused-layout) pooling of feature.create_embedding_slices.
+ * One record per feature.  Sample b of the feature owns the occurrence rows splits[b] .. splits[b + 1] - 1 of
+ * rows_dev (row i at rows_dev + i * row_stride, dim floats); the feature's dim columns are cut, in order, into its
+ * slices, and slice s of sample b is the row at out_dev + b * stride.
+ *   forward (mono_reduce_and_split): slice row b = +0.0 + e_lo + e_lo+1 + ... over the slice's columns, in
+ *     occurrence order with fp32 adds (the CPU ops' and the reference kernel's order).  MEAN then multiplies the
+ *     sum by (float)(1.0 / (double)(float)n), as ReduceMeanOp does: an empty MEAN row is 0 * inf = NaN.
+ *   grad (mono_reduce_and_split_grad): occurrence row i of sample b is written with sample b's slice gradients,
+ *     copied (SUM) or each multiplied by the same factor as the forward (MEAN).  rows_dev is the output; a row that
+ *     no sample's range covers is not written.
+ * The _bf16 calls take bf16 slice rows (out_dev points at bf16 storage, stride counts bf16 elements): a forward
+ * element is the fp32 result rounded once to nearest even (NaN stays NaN, payload unspecified), a gradient element
+ * is widened exactly before the fp32 multiply.  rows_dev stays fp32.
+ * Every feature of one call has the same batch_size.  bad_splits_dev (int32[1], optional) is set to 1 when some
+ * feature's splits do not start at 0, decrease, or do not end at n_rows, else 0; a sample whose range lies outside
+ * [0, n_rows] or decreases is pooled as empty and its occurrence rows are not written, so no kernel touches memory
+ * outside the given buffers.  No host synchronisation: the records reach the device by one stream-ordered copy.
+ * Kernel launches: one per lane-group width (4, 8, 16 or 32, from the feature's widest slice) among the features.
+ * MONO_ERR_INVALID_ARGUMENT, before any device work: num_features outside [0, 2^20], batch sizes that differ,
+ * are negative or exceed 2^31 - 2, features x batch_size > 2^33, a null splits or rows pointer (when batch_size > 0),
+ * dim <= 0, n_rows outside [0, 2^31 - 1], row_stride < dim, pooling other than SUM or MEAN, no slices, a slice with
+ * dim <= 0, a null slice pointer or stride < dim, slice dims that do not add up to dim. */
+typedef struct mono_reduce_slice {
+  int32_t dim;
+  float* out_dev;   /* forward: the slice's output rows; grad: its gradient rows (bf16 in the _bf16 calls) */
+  int64_t stride;   /* elements between consecutive samples */
+} mono_reduce_slice;
+
+typedef struct mono_reduce_feature {
+  const int32_t* splits_dev;        /* [batch_size + 1] */
+  int64_t batch_size;
+  float* rows_dev;                  /* forward: occurrence rows (read); grad: their gradients (written) */
+  int64_t n_rows;                   /* occurrences */
+  int64_t row_stride;               /* floats between occurrence rows */
+  int32_t dim;
+  int32_t pooling;                  /* MONO_POOL_SUM | MONO_POOL_MEAN */
+  const mono_reduce_slice* slices;  /* host array of n_slices */
+  int32_t n_slices;
+} mono_reduce_feature;
+
+int mono_reduce_and_split(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                          int32_t* bad_splits_dev, void* stream);
+int mono_reduce_and_split_grad(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                               int32_t* bad_splits_dev, void* stream);
+int mono_reduce_and_split_bf16(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                               int32_t* bad_splits_dev, void* stream);
+int mono_reduce_and_split_grad_bf16(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                                    int32_t* bad_splits_dev, void* stream);
 
 /* ---- NVLink peer window: the exchange steps of the sharded path as peer stores ---------------
  * ref: the all-to-alls of the reference's synchronous multi-GPU path (distributed_ps_sync.py:92-118

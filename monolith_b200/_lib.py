@@ -40,6 +40,16 @@ class ShardingFeature(C.Structure):  # mono_sharding_feature
               ("shared", C.c_int32)]
 
 
+class ReduceSlice(C.Structure):  # mono_reduce_slice
+  _fields_ = [("dim", C.c_int32), ("out_dev", C.c_void_p), ("stride", C.c_int64)]
+
+
+class ReduceFeature(C.Structure):  # mono_reduce_feature
+  _fields_ = [("splits_dev", C.c_void_p), ("batch_size", C.c_int64), ("rows_dev", C.c_void_p), ("n_rows", C.c_int64),
+              ("row_stride", C.c_int64), ("dim", C.c_int32), ("pooling", C.c_int32),
+              ("slices", C.POINTER(ReduceSlice)), ("n_slices", C.c_int32)]
+
+
 MAX_POOL_PARTS = 1024  # MONO_MAX_POOL_PARTS
 OPT_SGD, OPT_ADAGRAD, OPT_FTRL, OPT_ADAM = 0, 1, 2, 3
 OPT_MOMENTUM, OPT_RMSPROP, OPT_RMSPROPV2, OPT_ADADELTA, OPT_AMSGRAD = 4, 5, 6, 7, 8
@@ -130,6 +140,10 @@ SIGNATURES = {
                                                 C.POINTER(SliceTask), _i32, _p, _p]),
     "mono_embedding_to_layout_grad_bf16": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
                                                      C.POINTER(SliceTask), _i32, _p, _p]),
+    "mono_reduce_and_split": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
+    "mono_reduce_and_split_grad": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
+    "mono_reduce_and_split_bf16": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
+    "mono_reduce_and_split_grad_bf16": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
     "mono_mtable_note_update_ts": (C.c_int, [_p, _i32, _i64]),
     "mono_ckpt_last_error": (C.c_char_p, []),
     "mono_ckpt_writer_open": (C.c_int, [C.c_char_p, C.c_char_p, _i32, C.POINTER(_p)]),

@@ -155,6 +155,16 @@ int layout_entry(bool backward, int32_t device, float* const* emb_ptrs_dev, cons
                   (cudaStream_t)stream, bf16);
   });
 }
+
+template <typename T>
+int reduce_split_entry(bool backward, int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                       int32_t* bad_splits_dev, void* stream) {
+  return guarded([&] {
+    check_reduce_split(features, num_features);
+    MONO_CUDA(cudaSetDevice(device));
+    launch_reduce_split<T>(backward, features, num_features, bad_splits_dev, (cudaStream_t)stream);
+  });
+}
 }  // namespace
 
 extern "C" {
@@ -845,6 +855,23 @@ int mono_embedding_to_layout_grad(int32_t device, float* const* emb_grad_ptrs_de
   return layout_entry(true, device, emb_grad_ptrs_dev, emb_strides_dev, n_emb, fid_offset_dev, total_fid,
                       feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host, n_tasks,
                       const_cast<float* const*>(out_grad_ptrs_dev), stream, false);
+}
+
+int mono_reduce_and_split(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                          int32_t* bad_splits_dev, void* stream) {
+  return reduce_split_entry<float>(false, device, features, num_features, bad_splits_dev, stream);
+}
+int mono_reduce_and_split_grad(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                               int32_t* bad_splits_dev, void* stream) {
+  return reduce_split_entry<float>(true, device, features, num_features, bad_splits_dev, stream);
+}
+int mono_reduce_and_split_bf16(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                               int32_t* bad_splits_dev, void* stream) {
+  return reduce_split_entry<__nv_bfloat16>(false, device, features, num_features, bad_splits_dev, stream);
+}
+int mono_reduce_and_split_grad_bf16(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                                    int32_t* bad_splits_dev, void* stream) {
+  return reduce_split_entry<__nv_bfloat16>(true, device, features, num_features, bad_splits_dev, stream);
 }
 
 int mono_gather_pool_bf16(int32_t device, const float* fused_emb_dev, const int32_t* emb_offset_dev,

@@ -527,5 +527,10 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,
                    int total_nfl, int batch_size, const mono_slice_task* tasks_host, int n_tasks,
                    float* const* out_ptrs_dev, cudaStream_t s, bool bf16 = false);
+// mono_reduce_and_split[_grad]; T: element type of the slice rows
+void check_reduce_split(const mono_reduce_feature* feats, int n_features);
+template <typename T>
+void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int n_features, int32_t* bad_splits_dev,
+                         cudaStream_t s);
 
 }  // namespace mono

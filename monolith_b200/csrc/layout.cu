@@ -498,4 +498,286 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
   MONO_CUDA(cudaStreamSynchronize(s));
 }
 
+// ------------------------------------------------------------------------------------------
+// ReduceSum / ReduceMean / FusedReduceAndSplitGPU (ref: RT/ops/reduce_op.cc:29-89,124-180,232-330,
+// reduce_op.cu.cc:290-378): per-occurrence rows pooled per sample and cut into slices.  The reference GPU kernel
+// runs one thread per output element with a dependent scalar load chain (cu.cc:308-316); here one lane group per
+// (feature, sample), lanes across the slice's columns, occurrence rows staged kRsStage at a time with cp.async and
+// added strictly in occurrence order.  Every group handles exactly one (feature, sample): the block scheduler hands
+// out blocks as SMs free up, so a long row holds up only its own block (a row cannot be split without changing the
+// order of its adds).
+// ------------------------------------------------------------------------------------------
+struct RsFeat {
+  const int32_t* splits;
+  float* rows;
+  int64_t n_rows, row_stride;
+  int32_t pooling, slice0, n_slices;
+};
+struct RsSlice {
+  void* ptr;       // T rows of the slice (forward: written; grad: read)
+  int64_t stride;  // T elements between samples
+  int32_t dim, col;  // col: first column of the slice in the feature's rows
+};
+struct RsArgs {
+  const RsFeat* feats;
+  const RsSlice* slices;
+  const int32_t* order;  // the features of this launch's lane-group width
+  int64_t units;         // features of this launch x batch
+  int64_t batch;
+  int32_t* bad;          // optional malformed-splits flag
+};
+
+constexpr int kRsStage = 8;  // occurrence rows in flight per lane (8 x 16 B x 256 threads = 32 KB per block)
+
+__device__ __forceinline__ void rs_cp_async16(void* smem_dst, const void* gsrc) {
+  const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void rs_cp_async4(void* smem_dst, const void* gsrc) {
+  const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(d), "l"(gsrc) : "memory");
+}
+
+// Sample b's occurrences [*lo, *lo + n) of feature f.  A range outside [0, n_rows] or decreasing is empty; it, and
+// splits that do not start at 0 or end at n_rows, raise the flag.
+__device__ __forceinline__ int rs_range(const RsFeat& f, int64_t b, int64_t batch, int32_t* bad, int* lo) {
+  int l = __ldg(f.splits + b), h = __ldg(f.splits + b + 1);
+  const bool ok = l >= 0 && h >= l && h <= f.n_rows;
+  if (bad && (!ok || (b == 0 && l != 0) || (b == batch - 1 && h != f.n_rows))) *bad = 1;
+  if (!ok) l = h = 0;
+  *lo = l;
+  return h - l;
+}
+
+// ReduceMeanOp's factor: float multiply = 1.0 / static_cast<float>(count) (reduce_op.cc:81, :172), a double
+// division rounded to float; n == 0 gives +inf
+__device__ __forceinline__ float rs_mean_factor(int n) { return __double2float_rn(__drcp_rn((double)(float)n)); }
+
+__device__ __forceinline__ float4 rs_load4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ float4 rs_load4(const __nv_bfloat16* p) {
+  return widen_bf16x4(*reinterpret_cast<const uint2*>(p));
+}
+
+// A lane owns 4 columns of a slice per pass: c .. c + 3 when the slice's rows allow 16-byte source and 4-element
+// destination accesses, else c, c + G, c + 2G, c + 3G (odd dims, 1-column slices, unaligned columns).
+template <typename T>
+__device__ __forceinline__ bool rs_vec(const RsFeat& f, const RsSlice& sl, const T* tower_row) {
+  return ((sl.dim | sl.col) & 3) == 0 && (f.row_stride & 3) == 0 && (reinterpret_cast<uintptr_t>(f.rows) & 15) == 0 &&
+         (sl.stride & 3) == 0 && (reinterpret_cast<uintptr_t>(tower_row) & (4 * sizeof(T) - 1)) == 0;
+}
+
+template <typename T, int G>
+__device__ __forceinline__ void reduce_split_fwd(const RsArgs& a) {
+  __shared__ float4 stage[kRsStage][kThreads];
+  const int64_t u = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
+  if (u >= a.units) return;
+  const RsFeat f = a.feats[a.order[u / a.batch]];
+  const int64_t b = u % a.batch;
+  int lo;
+  const int n = rs_range(f, b, a.batch, a.bad, &lo);
+  const int gl = Group<G>::gl();
+  const float* occ = f.rows + (int64_t)lo * f.row_stride;
+  const int64_t rstride = f.row_stride;
+  for (int s = f.slice0; s < f.slice0 + f.n_slices; ++s) {
+    const RsSlice sl = a.slices[s];
+    T* dst = reinterpret_cast<T*>(sl.ptr) + b * sl.stride;
+    const bool vec = rs_vec(f, sl, reinterpret_cast<T*>(sl.ptr));
+    const int step = vec ? 1 : G;
+    float* slot = reinterpret_cast<float*>(&stage[0][threadIdx.x]);
+    for (int c = vec ? gl * 4 : gl; c < sl.dim; c += 4 * G) {
+      const float* p = occ + sl.col + c;
+      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);  // ReduceSumOp's zero-filled output (reduce_op.cc:44)
+      for (int j0 = 0; j0 < n; j0 += kRsStage) {
+        const int m = min(kRsStage, n - j0);
+        for (int k = 0; k < m; ++k, p += rstride) {
+          if (vec) {
+            rs_cp_async16(slot + k * kThreads * 4, p);
+          } else {
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+              if (c + i * G < sl.dim) rs_cp_async4(slot + k * kThreads * 4 + i, p + i * G);
+          }
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        for (int k = 0; k < m; ++k) {
+          const float4 x = stage[k][threadIdx.x];
+          acc.x = __fadd_rn(acc.x, x.x); acc.y = __fadd_rn(acc.y, x.y);
+          acc.z = __fadd_rn(acc.z, x.z); acc.w = __fadd_rn(acc.w, x.w);
+        }
+      }
+      if (f.pooling == MONO_POOL_MEAN) {
+        const float mult = rs_mean_factor(n);
+        acc.x = __fmul_rn(acc.x, mult); acc.y = __fmul_rn(acc.y, mult);
+        acc.z = __fmul_rn(acc.z, mult); acc.w = __fmul_rn(acc.w, mult);
+      }
+      if (vec) {
+        store_row4(dst + c, acc);
+      } else {
+        dst[c] = to_row_elem(acc.x, dst);
+        if (c + step < sl.dim) dst[c + step] = to_row_elem(acc.y, dst);
+        if (c + 2 * step < sl.dim) dst[c + 2 * step] = to_row_elem(acc.z, dst);
+        if (c + 3 * step < sl.dim) dst[c + 3 * step] = to_row_elem(acc.w, dst);
+      }
+    }
+  }
+}
+
+// Every occurrence row of sample b gets b's slice gradients: copied (SUM) or times the forward's factor (MEAN).
+template <typename T, int G>
+__device__ __forceinline__ void reduce_split_bwd(const RsArgs& a) {
+  const int64_t u = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
+  if (u >= a.units) return;
+  const RsFeat f = a.feats[a.order[u / a.batch]];
+  const int64_t b = u % a.batch;
+  int lo;
+  const int n = rs_range(f, b, a.batch, a.bad, &lo);
+  if (n == 0) return;
+  const float mult = rs_mean_factor(n);
+  const bool mean = f.pooling == MONO_POOL_MEAN;
+  const int gl = Group<G>::gl();
+  float* occ = f.rows + (int64_t)lo * f.row_stride;
+  for (int s = f.slice0; s < f.slice0 + f.n_slices; ++s) {
+    const RsSlice sl = a.slices[s];
+    const T* g = reinterpret_cast<const T*>(sl.ptr) + b * sl.stride;
+    const bool vec = rs_vec(f, sl, reinterpret_cast<const T*>(sl.ptr));
+    for (int c = vec ? gl * 4 : gl; c < sl.dim; c += 4 * G) {
+      float* dst = occ + sl.col + c;
+      if (vec) {
+        float4 x = rs_load4(g + c);
+        if (mean) {
+          x.x = __fmul_rn(x.x, mult); x.y = __fmul_rn(x.y, mult);
+          x.z = __fmul_rn(x.z, mult); x.w = __fmul_rn(x.w, mult);
+        }
+        for (int j = 0; j < n; ++j) *reinterpret_cast<float4*>(dst + (int64_t)j * f.row_stride) = x;
+      } else {
+        float x[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          x[i] = c + i * G < sl.dim ? row_elem_f32(g[c + i * G]) : 0.f;
+          if (mean) x[i] = __fmul_rn(x[i], mult);
+        }
+        for (int j = 0; j < n; ++j) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            if (c + i * G < sl.dim) dst[(int64_t)j * f.row_stride + i * G] = x[i];
+        }
+      }
+    }
+  }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads, 4) reduce_split_fwd_kernel(RsArgs a) {
+  reduce_split_fwd<float, G>(a);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads, 4) bf16_reduce_split_fwd_kernel(RsArgs a) {
+  reduce_split_fwd<__nv_bfloat16, G>(a);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads) reduce_split_bwd_kernel(RsArgs a) {
+  reduce_split_bwd<float, G>(a);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads) bf16_reduce_split_bwd_kernel(RsArgs a) {
+  reduce_split_bwd<__nv_bfloat16, G>(a);
+}
+
+// Host-side checks of the records: the kernels index with every field unchecked.
+void check_reduce_split(const mono_reduce_feature* feats, int F) {
+  if (F < 0 || F > (1 << 20)) throw ArgError("reduce_and_split: num_features outside [0, 2^20]");
+  if (F > 0 && feats == nullptr) throw ArgError("reduce_and_split: features is null");
+  for (int i = 0; i < F; ++i) {
+    const mono_reduce_feature& f = feats[i];
+    if (f.batch_size < 0 || f.batch_size > INT32_MAX - 1)
+      throw ArgError("reduce_and_split: batch_size outside [0, 2^31 - 2]");
+    if (f.batch_size != feats[0].batch_size) throw ArgError("reduce_and_split: features with different batch sizes");
+    if (f.dim <= 0) throw ArgError("reduce_and_split: dim must be positive");
+    if (f.n_rows < 0 || f.n_rows > INT32_MAX) throw ArgError("reduce_and_split: n_rows outside [0, 2^31 - 1]");
+    if (f.row_stride < f.dim) throw ArgError("reduce_and_split: row_stride < dim");
+    if (f.batch_size > 0 && (f.splits_dev == nullptr || (f.rows_dev == nullptr && f.n_rows > 0)))
+      throw ArgError("reduce_and_split: null splits or rows");
+    if (f.pooling != MONO_POOL_SUM && f.pooling != MONO_POOL_MEAN)
+      throw ArgError("reduce_and_split: pooling must be SUM or MEAN");
+    if (f.n_slices <= 0 || f.slices == nullptr) throw ArgError("reduce_and_split: a feature needs slices");
+    int64_t cols = 0;
+    for (int s = 0; s < f.n_slices; ++s) {
+      const mono_reduce_slice& sl = f.slices[s];
+      if (sl.dim <= 0) throw ArgError("reduce_and_split: slice dim must be positive");
+      if (sl.stride < sl.dim) throw ArgError("reduce_and_split: slice stride < slice dim");
+      if (sl.out_dev == nullptr && f.batch_size > 0) throw ArgError("reduce_and_split: null slice pointer");
+      cols += sl.dim;
+    }
+    if (cols != f.dim) throw ArgError("reduce_and_split: slice dims must add up to dim");
+  }
+  if (F > 0 && (int64_t)F * feats[0].batch_size > ((int64_t)1 << 33))
+    throw ArgError("reduce_and_split: features x batch_size over 2^33");
+}
+
+template <typename T>
+void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int F, int32_t* bad_dev, cudaStream_t s) {
+  if (bad_dev) MONO_CUDA(cudaMemsetAsync(bad_dev, 0, sizeof(int32_t), s));
+  const int64_t B = F > 0 ? feats[0].batch_size : 0;
+  if (F == 0 || B == 0) return;
+  // staged tables: features, slices, then the features ordered by lane-group width
+  int S = 0;
+  for (int i = 0; i < F; ++i) S += feats[i].n_slices;
+  const size_t fb = sizeof(RsFeat) * F, sb = sizeof(RsSlice) * S, ob = sizeof(int32_t) * F;
+  const size_t o_sl = (fb + 15) & ~(size_t)15, o_ord = (o_sl + sb + 15) & ~(size_t)15, bytes = o_ord + ob;
+  std::vector<char> h(bytes);
+  RsFeat* hf = reinterpret_cast<RsFeat*>(h.data());
+  RsSlice* hs = reinterpret_cast<RsSlice*>(h.data() + o_sl);
+  int32_t* ho = reinterpret_cast<int32_t*>(h.data() + o_ord);
+  std::vector<int> width(F);
+  int count[4] = {0, 0, 0, 0};  // features per width 4, 8, 16, 32
+  for (int i = 0, s0 = 0; i < F; ++i) {
+    const mono_reduce_feature& f = feats[i];
+    hf[i] = RsFeat{f.splits_dev, f.rows_dev, f.n_rows, f.row_stride, f.pooling, s0, f.n_slices};
+    int col = 0, widest = 0;
+    for (int j = 0; j < f.n_slices; ++j, ++s0) {
+      hs[s0] = RsSlice{f.slices[j].out_dev, f.slices[j].stride, f.slices[j].dim, col};
+      col += f.slices[j].dim;
+      widest = std::max(widest, f.slices[j].dim);
+    }
+    width[i] = pick_group(widest);  // 4 columns per lane
+    ++count[__builtin_ctz(width[i]) - 2];
+  }
+  int start[5] = {0, 0, 0, 0, 0};
+  for (int w = 0; w < 4; ++w) start[w + 1] = start[w] + count[w];
+  int fill[4] = {start[0], start[1], start[2], start[3]};
+  for (int i = 0; i < F; ++i) ho[fill[__builtin_ctz(width[i]) - 2]++] = i;
+
+  char* ws = nullptr;
+  MONO_CUDA(cudaMallocAsync((void**)&ws, bytes, s));
+  // a pageable H2D copy is staged by the driver before the call returns: h may go out of scope after it
+  MONO_CUDA(cudaMemcpyAsync(ws, h.data(), bytes, cudaMemcpyHostToDevice, s));
+  for (int w = 0; w < 4; ++w) {
+    if (count[w] == 0) continue;
+    RsArgs a;
+    a.feats = reinterpret_cast<const RsFeat*>(ws);
+    a.slices = reinterpret_cast<const RsSlice*>(ws + o_sl);
+    a.order = reinterpret_cast<const int32_t*>(ws + o_ord) + start[w];
+    a.units = (int64_t)count[w] * B;
+    a.batch = B;
+    a.bad = bad_dev;
+    by_group(4 << w, [&](auto g) {
+      constexpr int GG = decltype(g)::value;
+      const int64_t grid = (a.units + kThreads / GG - 1) / (kThreads / GG);
+      if (!backward) by_elem<T>(reduce_split_fwd_kernel<GG>, bf16_reduce_split_fwd_kernel<GG>)
+                         <<<(unsigned)grid, kThreads, 0, s>>>(a);
+      else by_elem<T>(reduce_split_bwd_kernel<GG>, bf16_reduce_split_bwd_kernel<GG>)
+               <<<(unsigned)grid, kThreads, 0, s>>>(a);
+    });
+    MONO_CHECK_LAUNCH();
+  }
+  MONO_CUDA(cudaFreeAsync(ws, s));
+}
+
+template void launch_reduce_split<float>(bool, const mono_reduce_feature*, int, int32_t*, cudaStream_t);
+template void launch_reduce_split<__nv_bfloat16>(bool, const mono_reduce_feature*, int, int32_t*, cudaStream_t);
+
 }  // namespace mono

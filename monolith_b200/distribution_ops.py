@@ -289,6 +289,182 @@ def scatter_grad_rows(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.
   return grad_fused
 
 
+# ---- ReduceSum / ReduceMean / FusedReduceSumAndSplit / FusedReduceAndSplitGPU ------------------------------------
+# ref: distribution_ops.py:689-884 and RT/ops/reduce_op.{cc,cu.cc}.  Every function below is one call of
+# mono_reduce_and_split[_grad][_bf16]: see include/mono_emb.h for the arithmetic.
+
+_POOLINGS = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}
+
+
+def _poolings(pooling, n):
+  ps = [pooling] * n if isinstance(pooling, str) else list(pooling)
+  if len(ps) != n or any(p not in _POOLINGS for p in ps):
+    raise ValueError(f"pooling must be 'sum', 'mean' or one of them per feature, not {pooling!r}")
+  return ps
+
+
+def _rows2d(t, what):
+  if t.dim() != 2 or t.dtype != torch.float32 or (t.size(0) > 1 and t.stride(1) != 1):
+    raise ValueError(f"{what} must be a 2-D float32 tensor with unit column stride")
+  return t
+
+
+def _reduce_split_call(backward, splits, rows, slices, poolings, bad_splits):
+  """splits[f]: int32 [B + 1]; rows[f]: [n_f, D_f] float32 (read forward, written backward); slices[f]: the 2-D
+  tensors of feature f's slices (written forward, read backward), all float32 or all bfloat16."""
+  lib = _lib.load()
+  F = len(splits)
+  flat = [t for s in slices for t in s]
+  dtype = _tower_dtype(flat[0].dtype if flat else torch.float32, "the slice tensors")
+  if any(t.dtype != dtype or t.dim() != 2 or (t.size(0) > 1 and t.stride(1) != 1) for t in flat):
+    raise ValueError("the slice tensors must be 2-D with unit column stride and all float32 or all bfloat16")
+  dev = splits[0].device if F else torch.device("cuda", torch.cuda.current_device())
+  keep = []
+  recs = (_lib.ReduceFeature * max(F, 1))()
+  for f in range(F):
+    sl = (_lib.ReduceSlice * max(len(slices[f]), 1))()
+    for j, t in enumerate(slices[f]):
+      sl[j].dim, sl[j].out_dev, sl[j].stride = t.size(1), t.data_ptr(), t.stride(0)
+    keep.append(sl)
+    r = rows[f]
+    recs[f].splits_dev, recs[f].batch_size = splits[f].data_ptr(), splits[f].numel() - 1
+    recs[f].rows_dev, recs[f].n_rows, recs[f].row_stride = r.data_ptr(), r.size(0), r.stride(0) if r.size(0) > 1 else r.size(1)
+    recs[f].dim, recs[f].pooling = r.size(1), _POOLINGS[poolings[f]]
+    recs[f].slices, recs[f].n_slices = sl, len(slices[f])
+  bf16 = dtype == torch.bfloat16
+  fn = {(False, False): lib.mono_reduce_and_split, (True, False): lib.mono_reduce_and_split_grad,
+        (False, True): lib.mono_reduce_and_split_bf16, (True, True): lib.mono_reduce_and_split_grad_bf16}[backward, bf16]
+  _lib.check(fn(dev.index, recs, F, _ptr(bad_splits), _stream(dev)))
+
+
+def _splits32(splits):
+  s = splits.reshape(-1)
+  return s if s.dtype == torch.int32 and s.is_contiguous() else s.to(torch.int32).contiguous()
+
+
+def fused_reduce_and_split_gpu(splits: Sequence[torch.Tensor], embeddings: Sequence[torch.Tensor],
+                               slice_dims: Sequence[Sequence[int]], *, pooling="sum", dtype: torch.dtype = torch.float32,
+                               bad_splits: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
+  """ref: fused_reduce_and_split_gpu (distribution_ops.py:838-872, MonolithFusedReduceAndSplitGPU).  Feature f's
+  per-occurrence rows embeddings[f] ([n_f, D_f] float32) are pooled per sample by its row splits splits[f] ([B + 1])
+  and cut into slices of slice_dims[f].  Returns the flat list of [B, s] slices, feature by feature, in `dtype`
+  (float32, or bfloat16: the float32 result rounded once).  pooling: 'sum' (the reference op), 'mean'
+  (ReduceMean's multiply), or one per feature.  bad_splits (int32 [1] on the device, optional) becomes 1 when some
+  feature's splits are malformed (such samples pool as empty); no host round trip."""
+  dtype = _tower_dtype(dtype, "fused_reduce_and_split_gpu's dtype")
+  F = len(splits)
+  if len(embeddings) != F or len(slice_dims) != F:
+    raise ValueError("splits, embeddings and slice_dims must have the same length")
+  sp = [_splits32(s) for s in splits]
+  rows = [_rows2d(e, "embeddings[%d]" % f) for f, e in enumerate(embeddings)]
+  outs = [[torch.empty(s.numel() - 1, d, dtype=dtype, device=s.device) for d in dims] for s, dims in zip(sp, slice_dims)]
+  _reduce_split_call(False, sp, rows, outs, _poolings(pooling, F), bad_splits)
+  return [t for o in outs for t in o]
+
+
+def fused_reduce_and_split_gpu_grad(splits: Sequence[torch.Tensor], embeddings: Sequence[torch.Tensor],
+                                    grads: Sequence[torch.Tensor], slice_dims: Sequence[Sequence[int]], *,
+                                    pooling="sum", out: Optional[Sequence[torch.Tensor]] = None,
+                                    bad_splits: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
+  """ref: MonolithFusedReduceAndSplitGPUGrad (reduce_op.cu.cc:478-680).  grads is the flat list of slice gradients
+  (all float32 or all bfloat16, widened exactly).  Returns feature f's occurrence-row gradients [n_f, D_f] float32:
+  sample b's slice gradients copied (SUM) or times ReduceMean's factor (MEAN) into each of b's rows.  out[f], when
+  given, is written instead (a [n_f, D_f] view, e.g. of the flat gradient buffer raw_apply_gradients takes); rows
+  no sample covers are left as they are.  embeddings only give the shapes (as in the reference gradient)."""
+  F = len(splits)
+  sp = [_splits32(s) for s in splits]
+  shapes = [(e.size(0), e.size(1)) for e in embeddings]
+  if out is None:
+    out = [torch.empty(n, d, dtype=torch.float32, device=s.device) for (n, d), s in zip(shapes, sp)]
+  rows = [_rows2d(o, "out[%d]" % f) for f, o in enumerate(out)]
+  if [tuple(o.shape) for o in rows] != shapes:
+    raise ValueError("out must have the shapes of embeddings")
+  it = iter(grads)
+  per = [[next(it) for _ in dims] for dims in slice_dims]
+  if sum(len(d) for d in slice_dims) != len(grads):
+    raise ValueError("grads must hold one tensor per slice")
+  _reduce_split_call(True, sp, rows, per, _poolings(pooling, F), bad_splits)
+  return list(rows)
+
+
+def _batch_size(id_dense_shape):
+  if isinstance(id_dense_shape, int):
+    return id_dense_shape
+  return int(torch.as_tensor(id_dense_shape).reshape(-1)[0])
+
+
+def _splits_from_indices(id_indices, B, sync):
+  """Row splits [B + 1] (int32, on the device) of the non-decreasing sample indices in [0, B) the reference's
+  callers pass (fused_value_rowids).  The reference CPU ops accept any order; these calls do not: with sync=True
+  unsorted or out-of-range indices raise ValueError, with sync=False nothing is checked on the host (the kernel
+  still reads and writes only inside the given buffers)."""
+  idx = id_indices[:, 0] if id_indices.dim() == 2 else id_indices.reshape(-1)
+  idx = idx.to(torch.int64).contiguous()
+  if sync and idx.numel():
+    bad = (idx[0] < 0) | (idx[-1] >= B)
+    if idx.numel() > 1:
+      bad = bad | (idx[1:] < idx[:-1]).any()
+    if bool(bad):
+      raise ValueError(f"id_indices must be non-decreasing and in [0, {B})")
+  q = torch.arange(B + 1, dtype=torch.int64, device=idx.device)
+  return torch.searchsorted(idx, q, out_int32=True)
+
+
+def _reduce(id_indices, id_values, B, split_dims, pooling, dtype, sync):
+  splits = _splits_from_indices(id_indices, B, sync)
+  return fused_reduce_and_split_gpu([splits], [id_values], [split_dims], pooling=pooling, dtype=dtype)
+
+
+def _reduce_grad(id_indices, grads, split_dims, pooling, sync, B=None):
+  B = grads[0].size(0) if B is None else B
+  splits = _splits_from_indices(id_indices, B, sync)
+  out = torch.empty(id_indices.size(0), sum(split_dims), dtype=torch.float32, device=splits.device)
+  return fused_reduce_and_split_gpu_grad([splits], [out], grads, [split_dims], pooling=pooling, out=[out])[0]
+
+
+def reduce_sum(id_indices: torch.Tensor, id_values: torch.Tensor, id_dense_shape, *,
+               dtype: torch.dtype = torch.float32, sync: bool = True) -> torch.Tensor:
+  """ref: reduce_sum (distribution_ops.py:726-741, MonolithReduceSum): [B, D] with row b = +0.0 + the id_values rows
+  whose index is b, in order.  B = id_dense_shape[0]; id_indices [n, 1] (or [n]), non-decreasing in [0, B)."""
+  return _reduce(id_indices, id_values, _batch_size(id_dense_shape), [id_values.size(1)], "sum", dtype, sync)[0]
+
+
+def reduce_mean(id_indices: torch.Tensor, id_values: torch.Tensor, id_dense_shape, *,
+                dtype: torch.dtype = torch.float32, sync: bool = True) -> torch.Tensor:
+  """ref: reduce_mean (distribution_ops.py:689-700, MonolithReduceMean): reduce_sum's rows times
+  (float)(1.0 / (float)n); an empty row is NaN (0 * inf), as in the reference."""
+  return _reduce(id_indices, id_values, _batch_size(id_dense_shape), [id_values.size(1)], "mean", dtype, sync)[0]
+
+
+def reduce_sum_gradient(id_indices: torch.Tensor, grads: torch.Tensor, *, sync: bool = True) -> torch.Tensor:
+  """ref: MonolithReduceSumGradient (reduce_op.cc:124-148): row i is grads[id_indices[i]] ([n, D] float32)."""
+  return _reduce_grad(id_indices, [grads], [grads.size(1)], "sum", sync)
+
+
+def reduce_mean_gradient(id_indices: torch.Tensor, grads: torch.Tensor, *, sync: bool = True) -> torch.Tensor:
+  """ref: MonolithReduceMeanGradient (reduce_op.cc:150-180): row i is grads[b] times the forward's factor for
+  b = id_indices[i], counted per sample (the reference sizes its counter by the dim, reduce_op.cc:166)."""
+  return _reduce_grad(id_indices, [grads], [grads.size(1)], "mean", sync)
+
+
+def fused_reduce_sum_and_split(id_indices: torch.Tensor, id_values: torch.Tensor, id_length, split_dims: Sequence[int],
+                               *, dtype: torch.dtype = torch.float32, sync: bool = True) -> List[torch.Tensor]:
+  """ref: fused_reduce_sum_and_split (distribution_ops.py:802-826, MonolithFusedReduceSumAndSplit): reduce_sum over
+  id_length samples, cut into [id_length, split_dims[i]] tensors."""
+  if sum(split_dims) != id_values.size(1):
+    raise ValueError("split_dims must add up to id_values.size(1)")
+  return _reduce(id_indices, id_values, _batch_size(id_length), list(split_dims), "sum", dtype, sync)
+
+
+def fused_reduce_sum_and_split_gradient(id_indices: torch.Tensor, grads: Sequence[torch.Tensor],
+                                        split_dims: Sequence[int], *, sync: bool = True) -> torch.Tensor:
+  """ref: MonolithFusedReduceSumAndSplitGradient (reduce_op.cc:282-330): [n, sum(split_dims)] float32, row i the
+  concatenated slice gradients of sample id_indices[i]."""
+  if [g.size(1) for g in grads] != list(split_dims):
+    raise ValueError("grads must have the split_dims widths")
+  return _reduce_grad(id_indices, list(grads), list(split_dims), "sum", sync)
+
+
 class Grouping:
   """One grouping of a batch's FID occurrences, shared by the sharded forward and backward
   (mono_grouping_*).  build(): dedup + bucket by owner = fid mod num_shards; reduce(): deterministic

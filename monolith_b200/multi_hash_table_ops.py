@@ -349,8 +349,11 @@ class MultiHashTable:
 
   def lookup_pool(self, slot: str, fids: torch.Tensor, row_offsets: Optional[torch.Tensor] = None,
                   pooling: str = "sum", out: Optional[torch.Tensor] = None, out_col: int = 0) -> torch.Tensor:
-    """Fused probe + gather + SUM/MEAN pool (one kernel): the hot forward.  Equivalent to
-    lookup() followed by embedding_combiners.ReduceSum/ReduceMean (ref: embedding_combiners.py:41-70)."""
+    """Fused probe + gather + SUM/MEAN pool (one kernel): the hot forward.  It replaces lookup() followed by
+    embedding_combiners.ReduceSum/ReduceMean (ref: embedding_combiners.py:41-70), with the fused-layout arithmetic:
+    SUM starts from the first term (ReduceSum starts from +0.0, so a row of -0.0 terms differs in sign) and MEAN
+    divides every term by n (ReduceMean multiplies the sum by 1/n).  distribution_ops.reduce_sum / reduce_mean after
+    lookup() give ReduceSum's and ReduceMean's bits."""
     k = self._table_names.index(slot)
     fids = _ids(fids, self._device)
     if row_offsets is not None:
