@@ -668,6 +668,94 @@ int mono_reduce_and_split_bf16(int32_t device, const mono_reduce_feature* featur
 int mono_reduce_and_split_grad_bf16(int32_t device, const mono_reduce_feature* features, int32_t num_features,
                                     int32_t* bad_splits_dev, void* stream);
 
+/* ---- clip by global norm: the norm, the scale, and the scale fused into the sparse backward ---
+ * ref: GlobalL2Reduce (RT/ops/global_norm.cu.cc), ClipByGlobalNorm's scale (RT/ops/clip_by_global_norm.h:42-49),
+ * feature_utils.apply_gradients_with_var_optimizer (NT/feature_utils.py:209-333), grad_scale of
+ * PartitionedHashTable.apply_gradients (NT/distributed_ps.py:1283-1329) and layout_tensors_grad_scale
+ * (NT/distribution_ops.py:544-550).
+ *
+ * mono_global_norm: norm = the L2 norm of all elements of all tensors (fp32 and bf16 device buffers in any mix; bf16
+ * elements are widened exactly), written to *norm_dev as fp32; with clip_norm > 0 also the scale
+ * scale = norm > clip_norm ? clip_norm / norm : 1.0f (IEEE fp32 divide) to *scale_dev: a NaN norm gives 1, an
+ * infinite norm +0.0.  clip_norm == 0: the norm only (scale_dev may be NULL and is not written).
+ * Arithmetic, bit for bit and independent of the device and the launch grid:
+ *   every square is (double)x * (double)x (exact).  The squares are summed in fp64 in chunks of 8192 elements that
+ *   never cross a tensor boundary (chunk c of a tensor is elements 8192 c ... 8192 c + 8191, the last chunk shorter;
+ *   an empty tensor has none): thread t (0 <= t < 256) adds the squares of the chunk's elements t + 256 i in
+ *   increasing i, starting from +0.0; then s[t] += s[t + h] for h = 128, 64, ..., 1, and s[0] is the chunk's partial.
+ *   The partials, in (tensor, chunk) order, are summed by the same rule (chunks of 8192 partials) level after level
+ *   until one value is left: the sum (+0.0 without any element).  norm = sqrtf((float)sum).
+ * Sizes are int64 throughout (a tensor may exceed 2^31 elements).  Two kernel launches (one without elements); no
+ * host synchronisation: the descriptors reach the device by one stream-ordered copy, the partials live in
+ * stream-ordered scratch.
+ * MONO_ERR_INVALID_ARGUMENT, before any device work: n_tensors outside [0, MONO_MAX_NORM_TENSORS], a null
+ * tensors_host with n_tensors > 0, a negative n, a null data_dev with n > 0, an unknown dtype, a NULL norm_dev, a
+ * negative, NaN or infinite clip_norm, clip_norm > 0 with scale_dev == NULL. */
+#define MONO_MAX_NORM_TENSORS 4096
+
+typedef enum mono_dtype { MONO_DTYPE_F32 = 0, MONO_DTYPE_BF16 = 1 } mono_dtype;
+
+typedef struct mono_norm_tensor {
+  const void* data_dev;
+  int64_t n;        /* elements */
+  int32_t dtype;    /* mono_dtype */
+} mono_norm_tensor;
+
+int mono_global_norm(int32_t device, const mono_norm_tensor* tensors_host, int32_t n_tensors, float clip_norm,
+                     float* norm_dev, float* scale_dev, void* stream);
+
+/* The _scaled backward calls: the arguments of the call they are named after, then grad_scale_dev (one device
+ * float, read on the device), then the stream.  Semantics, for all eight:
+ *   a scaled call is bit for bit the unscaled call on gradient rows pre-multiplied by s = *grad_scale_dev in fp32
+ *   (g * s, round to nearest), which is what the reference computes, because it multiplies before the op:
+ *   - MEAN divides the scaled term: (g * s) / n;
+ *   - FIRSTN positions at or beyond max_seq_len stay +0.0 (they are not part of the gradient rows);
+ *   - bf16 rows are widened exactly and then multiplied in fp32, so a bf16 scaled call equals the fp32 scaled call
+ *     on the widened rows (not the unscaled call on bf16 rows scaled and rounded to bf16);
+ *   - NaN stays NaN (payload unspecified).
+ * grad_scale_dev == NULL is the unscaled call.  No host synchronisation beyond the unscaled call's, and the same
+ * kernel launches: the multiply sits where the gradient rows are loaded, in scaled_ twins of the unscaled kernels.
+ * Errors are the unscaled call's. */
+int mono_mtable_pool_backward_parts_scaled(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                           const float* learning_rate_host, int64_t update_time,
+                                           int64_t global_step, const float* grad_scale_dev, void* stream);
+int mono_mtable_pool_backward_parts_bf16_scaled(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                                const float* learning_rate_host, int64_t update_time,
+                                                int64_t global_step, const float* grad_scale_dev, void* stream);
+int mono_embedding_to_layout_grad_scaled(int32_t device, float* const* emb_grad_ptrs_dev,
+                                         const int32_t* emb_strides_dev, int32_t n_emb,
+                                         const uint64_t* fid_offset_dev, int64_t total_fid,
+                                         const int32_t* feature_offset_dev, int32_t total_feature,
+                                         const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                         const mono_slice_task* tasks_host, int32_t n_tasks,
+                                         const float* const* out_grad_ptrs_dev, const float* grad_scale_dev,
+                                         void* stream);
+int mono_embedding_to_layout_grad_bf16_scaled(int32_t device, float* const* emb_grad_ptrs_dev,
+                                              const int32_t* emb_strides_dev, int32_t n_emb,
+                                              const uint64_t* fid_offset_dev, int64_t total_fid,
+                                              const int32_t* feature_offset_dev, int32_t total_feature,
+                                              const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                              const mono_slice_task* tasks_host, int32_t n_tasks,
+                                              const float* const* out_grad_ptrs_dev, const float* grad_scale_dev,
+                                              void* stream);
+int mono_gather_pool_grad_scaled(int32_t device, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                                 const int32_t* emb_offset_dev, const int32_t* row_offsets_dev, int64_t n_rows,
+                                 int32_t dim, int32_t pooling, float* grad_fused_dev, const float* grad_scale_dev,
+                                 void* stream);
+int mono_gather_pool_grad_bf16_scaled(int32_t device, const float* pooled_grad_dev, int64_t grad_stride,
+                                      int32_t grad_col, const int32_t* emb_offset_dev, const int32_t* row_offsets_dev,
+                                      int64_t n_rows, int32_t dim, int32_t pooling, float* grad_fused_dev,
+                                      const float* grad_scale_dev, void* stream);
+int mono_scatter_grad_rows_scaled(int32_t device, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                                  const int32_t* emb_offset_dev, int64_t n_occurrences, const int32_t* row_offsets_dev,
+                                  int64_t n_rows, int32_t dim, int32_t pooling, float* grad_fused_dev,
+                                  int64_t total_floats, const float* grad_scale_dev, void* stream);
+int mono_scatter_grad_rows_bf16_scaled(int32_t device, const float* pooled_grad_dev, int64_t grad_stride,
+                                       int32_t grad_col, const int32_t* emb_offset_dev, int64_t n_occurrences,
+                                       const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim, int32_t pooling,
+                                       float* grad_fused_dev, int64_t total_floats, const float* grad_scale_dev,
+                                       void* stream);
+
 /* ---- NVLink peer window: the exchange steps of the sharded path as peer stores ---------------
  * ref: the all-to-alls of the reference's synchronous multi-GPU path (distributed_ps_sync.py:92-118
  * forward ids + embeddings, :531-573 backward gradients; SURVEY.md §8e).  One window per rank

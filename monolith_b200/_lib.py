@@ -50,7 +50,13 @@ class ReduceFeature(C.Structure):  # mono_reduce_feature
               ("slices", C.POINTER(ReduceSlice)), ("n_slices", C.c_int32)]
 
 
+class NormTensor(C.Structure):  # mono_norm_tensor
+  _fields_ = [("data_dev", C.c_void_p), ("n", C.c_int64), ("dtype", C.c_int32)]
+
+
 MAX_POOL_PARTS = 1024  # MONO_MAX_POOL_PARTS
+MAX_NORM_TENSORS = 4096  # MONO_MAX_NORM_TENSORS
+DTYPE_F32, DTYPE_BF16 = 0, 1
 OPT_SGD, OPT_ADAGRAD, OPT_FTRL, OPT_ADAM = 0, 1, 2, 3
 OPT_MOMENTUM, OPT_RMSPROP, OPT_RMSPROPV2, OPT_ADADELTA, OPT_AMSGRAD = 4, 5, 6, 7, 8
 OPT_MOVING_AVERAGE, OPT_GROUP_ADAGRAD = 9, 10
@@ -145,6 +151,20 @@ SIGNATURES = {
     "mono_reduce_and_split_bf16": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
     "mono_reduce_and_split_grad_bf16": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
     "mono_mtable_note_update_ts": (C.c_int, [_p, _i32, _i64]),
+    "mono_global_norm": (C.c_int, [_i32, C.POINTER(NormTensor), _i32, C.c_float, _p, _p, _p]),
+    "mono_mtable_pool_backward_parts_scaled": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p, _p]),
+    "mono_mtable_pool_backward_parts_bf16_scaled": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p,
+                                                              _p]),
+    "mono_embedding_to_layout_grad_scaled": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
+                                                       C.POINTER(SliceTask), _i32, _p, _p, _p]),
+    "mono_embedding_to_layout_grad_bf16_scaled": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
+                                                            C.POINTER(SliceTask), _i32, _p, _p, _p]),
+    "mono_gather_pool_grad_scaled": (C.c_int, [_i32, _p, _i64, _i32, _p, _p, _i64, _i32, _i32, _p, _p, _p]),
+    "mono_gather_pool_grad_bf16_scaled": (C.c_int, [_i32, _p, _i64, _i32, _p, _p, _i64, _i32, _i32, _p, _p, _p]),
+    "mono_scatter_grad_rows_scaled": (C.c_int, [_i32, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _i32, _p, _i64, _p,
+                                                _p]),
+    "mono_scatter_grad_rows_bf16_scaled": (C.c_int, [_i32, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _i32, _p, _i64,
+                                                     _p, _p]),
     "mono_ckpt_last_error": (C.c_char_p, []),
     "mono_ckpt_writer_open": (C.c_int, [C.c_char_p, C.c_char_p, _i32, C.POINTER(_p)]),
     "mono_ckpt_writer_begin_table": (C.c_int, [_p, C.c_char_p, C.POINTER(SegmentCfg), _i32]),

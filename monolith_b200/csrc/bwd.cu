@@ -437,6 +437,15 @@ __device__ __forceinline__ float occ_grad_div(const GradSrc& gs, uint32_t m) {
   const uint32_t r = gs.occ_row ? gs.occ_row[m] : m;
   return (float)(gs.row_offsets[r + 1] - gs.row_offsets[r]);
 }
+// The gradient scale of the scaled_ kernels: every gradient term is g * *scale in fp32 (before a MEAN division),
+// except a FIRSTN position past max_seq_len (its occurrence's source is zero_row), which stays +0.0.
+struct GradScale {
+  const float* scale;
+  const float* zero_row;
+};
+__device__ __forceinline__ void mul4(float4& x, float s) {
+  x.x = __fmul_rn(x.x, s); x.y = __fmul_rn(x.y, s); x.z = __fmul_rn(x.z, s); x.w = __fmul_rn(x.w, s);
+}
 __device__ __forceinline__ void add4(float4& a, const float4& b) {
   a.x = __fadd_rn(a.x, b.x); a.y = __fadd_rn(a.y, b.y); a.z = __fadd_rn(a.z, b.z); a.w = __fadd_rn(a.w, b.w);
 }
@@ -654,8 +663,10 @@ __device__ __forceinline__ void fetch4(const uint32_t (&v)[32 / G], int e, uint3
 // loads and its meta stores only.
 // T: the gradient row element (float; __nv_bfloat16 for bf16 parts: each lane stages its 4 elements, 8 bytes, in the
 // first half of its 16-byte slot and widens them to fp32 when it reads the slot back).
-template <typename T, int G, int VPL, bool PLAIN, bool AHEAD>
-__device__ __forceinline__ void seg_reduce(const SegArgs& sa, const PeerOut& po, int defer_short) {
+// SCALED (scaled_ kernels): each term is multiplied by *sc.scale where it is read back, before the MEAN division.
+template <typename T, int G, int VPL, bool PLAIN, bool AHEAD, bool SCALED = false>
+__device__ __forceinline__ void seg_reduce(const SegArgs& sa, const PeerOut& po, int defer_short,
+                                           GradScale sc = GradScale{}) {
   __shared__ int64_t s_start[kMaxPeers + 1];
   __shared__ char* s_base[kMaxPeers];
   extern __shared__ float4 stage_raw[];        // [kStage][kThreads]: [slot][thread], conflict-free 16-byte accesses
@@ -675,6 +686,7 @@ __device__ __forceinline__ void seg_reduce(const SegArgs& sa, const PeerOut& po,
   for (int v = 0; v < VPL; ++v) in[v] = c + v * G * 4 < D;
   const int64_t M = a.n;
   const GradSrc gs = make_grad_src<T>(a, c);
+  const float gscale = SCALED ? *sc.scale : 1.f;
   const uint32_t* __restrict__ run_start = a.run_start;
   const int64_t wstride = (int64_t)gridDim.x * (kThreads / 32) * RPI;
   for (int64_t p0 = ((int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5)) * RPI; p0 < sa.n_pieces; p0 += wstride) {
@@ -768,6 +780,7 @@ __device__ __forceinline__ void seg_reduce(const SegArgs& sa, const PeerOut& po,
     for (int v = 0; v < VPL; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int e0 = e_begin & ~(RS - 1); e0 < e_stop; e0 += RS) {
       if (e0 + RS <= kPiece && ((SK >> e0) & ((1u << RS) - 1u)) == ((1u << RS) - 1u)) continue;  // all deferred
+      uint32_t unscaled = 0;  // SCALED: the stage slots holding a FIRSTN position past L (zero_row)
       // ---- request: up to RS gradient rows, this lane's 16-byte slices of each ----
       // (the 4-element bodies are NOT unrolled 4x more: the kernel was instruction-fetch bound when they were)
 #pragma unroll 1
@@ -794,6 +807,7 @@ __device__ __forceinline__ void seg_reduce(const SegArgs& sa, const PeerOut& po,
 #pragma unroll
             for (int v = 0; v < VPL; ++v)
               if (in[v]) cp_async_row4(&stage[(b4 + u) * VPL + v][threadIdx.x], src + v * G * 4);
+            if (SCALED && !PLAIN && gs.occ_src && gs.occ_src[m[u]] == sc.zero_row) unscaled |= 1u << (b4 + u);
           }
         }
       }
@@ -830,6 +844,7 @@ __device__ __forceinline__ void seg_reduce(const SegArgs& sa, const PeerOut& po,
           for (int v = 0; v < VPL; ++v) {
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
             if (in[v]) x = stage_row4<T>(&stage[(b4 + u) * VPL + v][threadIdx.x]);
+            if (SCALED && !((unscaled >> (b4 + u)) & 1u)) mul4(x, gscale);
             if (!PLAIN && gs.mean && fn[u] != 0.f) {
               x.x = __fdiv_rn(x.x, fn[u]); x.y = __fdiv_rn(x.y, fn[u]); x.z = __fdiv_rn(x.z, fn[u]); x.w = __fdiv_rn(x.w, fn[u]);
             }
@@ -862,6 +877,18 @@ template <int G, int VPL, bool AHEAD>
 __global__ void __launch_bounds__(kThreads, 3)
 bf16_seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short) {
   seg_reduce<__nv_bfloat16, G, VPL, false, AHEAD>(sa, po, defer_short);
+}
+
+// the two above with every gradient term multiplied by *sc.scale (the calls' grad_scale_dev)
+template <int G, int VPL, bool PLAIN, bool AHEAD>
+__global__ void __launch_bounds__(kThreads, 3)
+scaled_seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short, GradScale sc) {
+  seg_reduce<float, G, VPL, PLAIN, AHEAD, true>(sa, po, defer_short, sc);
+}
+template <int G, int VPL, bool AHEAD>
+__global__ void __launch_bounds__(kThreads, 3)
+scaled_bf16_seg_reduce_kernel(SegArgs sa, const PeerOut po, int defer_short, GradScale sc) {
+  seg_reduce<__nv_bfloat16, G, VPL, false, AHEAD, true>(sa, po, defer_short, sc);
 }
 
 // One level of the fixed tree over the block index of the long runs: the slot of block k, k a multiple of
@@ -976,9 +1003,9 @@ long_finish_kernel(SegArgs sa, uint32_t top, const PeerOut po) {
 // (A variant that handled two runs per group at a time needs 62 registers, which lowers occupancy.)
 // The next run's row index and run bounds are read one iteration ahead.  prefetch != 0: its weight / state rows are
 // also pulled into L2 meanwhile.
-// T: the gradient row element, as in seg_reduce.
-template <typename T, int G, int OPT>
-__device__ __forceinline__ void runs_apply(const BwdArgs& a, int prefetch) {
+// T: the gradient row element, as in seg_reduce.  SCALED: each term of a short run times *sc.scale, as in seg_reduce.
+template <typename T, int G, int OPT, bool SCALED = false>
+__device__ __forceinline__ void runs_apply(const BwdArgs& a, int prefetch, GradScale sc = GradScale{}) {
   extern __shared__ float4 stage_raw[];  // [kApplyStage][kThreads]
   float4 (*stage)[kThreads] = reinterpret_cast<float4 (*)[kThreads]>(stage_raw);
   const int gl = Group<G>::gl();
@@ -990,6 +1017,7 @@ __device__ __forceinline__ void runs_apply(const BwdArgs& a, int prefetch) {
   }
   const int D = a.td.dim;
   const GradSrc gs = make_grad_src<T>(a, c);
+  const float gscale = SCALED ? *sc.scale : 1.f;
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
   int64_t j = j_lo + (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
   uint32_t ri_next = kEmptyRow, rs_next = 0, re_next = 0, p0_next = 0;
@@ -1031,12 +1059,19 @@ __device__ __forceinline__ void runs_apply(const BwdArgs& a, int prefetch) {
 #pragma unroll
         for (int u = 0; u < kApplyStage; ++u)
           if (u < n && c < D) cp_async_row4(&stage[u][threadIdx.x], occ_grad_src<T>(gs, m[u], c));
+        uint32_t unscaled = 0;  // SCALED: the occurrences that are FIRSTN positions past L (zero_row)
+        if (SCALED && gs.occ_src) {
+#pragma unroll
+          for (int u = 0; u < kApplyStage; ++u)
+            if (u < n && gs.occ_src[m[u]] == sc.zero_row) unscaled |= 1u << u;
+        }
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group 0;" ::: "memory");
 #pragma unroll
         for (int u = 0; u < kApplyStage; ++u) {
           if (u >= n) break;
           float4 x = stage_row4<T>(&stage[u][threadIdx.x]);
+          if (SCALED && !((unscaled >> u) & 1u)) mul4(x, gscale);
           if (gs.mean) {
             const float fn = occ_grad_div(gs, m[u]);
             if (fn != 0.f) {
@@ -1059,6 +1094,16 @@ __global__ void __launch_bounds__(kThreads) runs_apply_kernel(BwdArgs a, int pre
 template <int G, int OPT>
 __global__ void __launch_bounds__(kThreads) bf16_runs_apply_kernel(BwdArgs a, int prefetch) {
   runs_apply<__nv_bfloat16, G, OPT>(a, prefetch);
+}
+
+template <int G, int OPT>
+__global__ void __launch_bounds__(kThreads) scaled_runs_apply_kernel(BwdArgs a, int prefetch, GradScale sc) {
+  runs_apply<float, G, OPT, true>(a, prefetch, sc);
+}
+
+template <int G, int OPT>
+__global__ void __launch_bounds__(kThreads) scaled_bf16_runs_apply_kernel(BwdArgs a, int prefetch, GradScale sc) {
+  runs_apply<__nv_bfloat16, G, OPT, true>(a, prefetch, sc);
 }
 
 // run j of the sorted offsets -> destination row: out_rows + (sorted key << shift)
@@ -1353,9 +1398,25 @@ static SegArgs seg_args(const BwdScratch& w, int64_t M, int D, const float* pool
 }
 
 constexpr size_t kStageBytes = sizeof(float4) * kStage * kThreads;
-// BF16: bf16_seg_reduce_kernel<GL, VPL, AHEAD> (PLAIN is then false)
+
+// A reduce as the host launches it: the kernel arguments and the gradient scale (null: the unscaled kernels; else
+// their scaled_ twins, which take *sc as one more argument)
+struct SegLaunch : SegArgs {
+  const GradScale* sc;
+  SegLaunch(const SegArgs& a, const GradScale* scale = nullptr) : SegArgs(a), sc(scale) {}
+};
+// BF16: bf16_seg_reduce_kernel<GL, VPL, AHEAD> (PLAIN is then false); sc != null: their scaled_ twins
 template <int GL, int VPL, bool PLAIN, bool AHEAD, bool BF16>
-static void launch_seg2(const SegArgs& sa, const PeerOut& po, bool defer_short, cudaStream_t s) {
+static void launch_seg2(const SegLaunch& sa, const PeerOut& po, bool defer_short, cudaStream_t s) {
+  if (sa.sc) {
+    constexpr void (*kern)(SegArgs, const PeerOut, int, GradScale) =
+        BF16 ? scaled_bf16_seg_reduce_kernel<GL, VPL, AHEAD> : scaled_seg_reduce_kernel<GL, VPL, PLAIN, AHEAD>;
+    set_max_dynamic_smem<kern>(kStageBytes);
+    kern<<<resident_grid(kern, sa.n_pieces, (kThreads / 32) * (32 / GL), kThreads, kStageBytes), kThreads, kStageBytes,
+           s>>>(sa, po, defer_short ? 1 : 0, *sa.sc);
+    MONO_CHECK_LAUNCH();
+    return;
+  }
   constexpr void (*kern)(SegArgs, const PeerOut, int) =
       BF16 ? bf16_seg_reduce_kernel<GL, VPL, AHEAD> : seg_reduce_kernel<GL, VPL, PLAIN, AHEAD>;
   set_max_dynamic_smem<kern>(kStageBytes);
@@ -1364,7 +1425,7 @@ static void launch_seg2(const SegArgs& sa, const PeerOut& po, bool defer_short, 
   MONO_CHECK_LAUNCH();
 }
 template <int GL, int VPL, bool PLAIN, bool BF16 = false>
-static void launch_seg(const SegArgs& sa, const PeerOut& po, bool defer_short, cudaStream_t s) {
+static void launch_seg(const SegLaunch& sa, const PeerOut& po, bool defer_short, cudaStream_t s) {
   if (knob(KNOB_SEG_AHEAD)) launch_seg2<GL, VPL, PLAIN, true, BF16>(sa, po, defer_short, s);
   else launch_seg2<GL, VPL, PLAIN, false, BF16>(sa, po, defer_short, s);
 }
@@ -1372,7 +1433,8 @@ static void launch_seg(const SegArgs& sa, const PeerOut& po, bool defer_short, c
 // per-run gradient sums -> run_dst (a.ugrad, or the owners' peer windows).  defer_short: runs_apply_kernel follows
 // and sums the runs of at most kApplyRun occurrences itself, so only the longer runs' sums are stored.
 // bf16: the gradient rows are bf16 (parts call); the tree and finish kernels add fp32 partials either way.
-static void launch_reduce(const SegArgs& sa, int G, const PeerOut& po, bool defer_short, cudaStream_t s,
+// sa.sc != null: the reduce multiplies every gradient term by the scale (the tree and finish add scaled partials).
+static void launch_reduce(const SegLaunch& sa, int G, const PeerOut& po, bool defer_short, cudaStream_t s,
                           bool bf16 = false) {
   const int64_t nr = sa.n_pieces;
   if (nr <= 0) return;
@@ -1426,14 +1488,22 @@ static int apply_opt_sel(const HostTable& ht) {
 }
 
 // the optimizer step of every run of the reduce's range (M: its occurrence count, sizes the grid); bf16: bf16
-// gradient rows (parts call)
-static void launch_apply(const BwdArgs& a, int G, int opt_sel, int64_t M, cudaStream_t s, bool bf16 = false) {
+// gradient rows (parts call); sc != null: the scaled_ twins
+static void launch_apply(const BwdArgs& a, int G, int opt_sel, int64_t M, cudaStream_t s, bool bf16 = false,
+                         const GradScale* sc = nullptr) {
   const int pf = knob(KNOB_APPLY_PF);
   constexpr size_t smem = sizeof(float4) * kApplyStage * kThreads;
   static_assert(smem <= 48 * 1024, "runs_apply_kernel's stage fits the default dynamic shared memory limit");
   by_group(G, [&](auto g) {
     auto launch = [&](auto o) {
       constexpr int GG = decltype(g)::value, OO = decltype(o)::value;
+      if (sc) {
+        void (*const kern)(BwdArgs, int, GradScale) =
+            bf16 ? scaled_bf16_runs_apply_kernel<GG, OO> : scaled_runs_apply_kernel<GG, OO>;
+        kern<<<resident_grid(kern, M, kThreads / GG, kThreads, smem), kThreads, smem, s>>>(a, pf, *sc);
+        MONO_CHECK_LAUNCH();
+        return;
+      }
       void (*const kern)(BwdArgs, int) = bf16 ? bf16_runs_apply_kernel<GG, OO> : runs_apply_kernel<GG, OO>;
       kern<<<resident_grid(kern, M, kThreads / GG, kThreads, smem), kThreads, smem, s>>>(a, pf);
       MONO_CHECK_LAUNCH();
@@ -1495,7 +1565,7 @@ static void claim_insert_sort(mono_mtable* mt, const CallBlob& cb, BwdScratch* w
 
 // 5 reduce + 6 apply over the runs of table k (sa: the reduce's arguments, M: the occurrences it covers): one
 // streaming pass over the runs — row index, summed gradient, w / optimizer state of every distinct FID
-static void reduce_and_apply(mono_mtable* mt, int k, const BwdScratch& w, SegArgs sa, const int64_t* fids,
+static void reduce_and_apply(mono_mtable* mt, int k, const BwdScratch& w, SegLaunch sa, const int64_t* fids,
                              const float* lr, int64_t M, int64_t update_time, cudaStream_t s, bool bf16) {
   const HostTable& ht = mt->tables[k];
   BwdArgs& a = sa.b;
@@ -1507,7 +1577,8 @@ static void reduce_and_apply(mono_mtable* mt, int k, const BwdScratch& w, SegArg
   a.scratch = a.ugrad;
   const int G = pick_group(ht.dim);
   launch_reduce(sa, G, no_peer, true, s, bf16);
-  launch_apply(a, G, apply_opt_sel(ht), M, s, bf16);
+  if (!sa.sc) launch_apply(a, G, apply_opt_sel(ht), M, s, bf16);
+  else launch_apply(a, G, apply_opt_sel(ht), M, s, bf16, sa.sc);
   note_issued(mt, k, (uint64_t)M, update_time, s);
 }
 
@@ -1595,7 +1666,7 @@ parts_occ_kernel(const PartDev* __restrict__ parts, int n_parts, int64_t n_rows,
 // optimizer and tree depth.  Everything is checked before the first device operation.
 // bf16: every part's rows_dev is bf16 storage (stride and col in bf16 elements); each term is widened to fp32 first.
 void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, const float* lr_host,
-                             int64_t update_time, cudaStream_t s, bool bf16) {
+                             int64_t update_time, cudaStream_t s, bool bf16, const float* grad_scale) {
   const int K = (int)mt->tables.size();
   if (n_parts < 0 || n_parts > MONO_MAX_POOL_PARTS) throw ArgError("pool_backward_parts: bad part count");
   if ((n_parts > 0 && !parts) || !lr_host) throw ArgError("pool_backward_parts: null argument");
@@ -1722,11 +1793,13 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
   cr.regions = d_ct;
   cr.n_regions = T;
   claim_insert_sort(mt, cb, &w, w.fids, M, set, cap, epoch, cr, update_time, s);
+  const GradScale gsc{grad_scale, mt->zero_row};
   // 5 reduce + 6 apply, per table over its range
   for (int q = 0; q < T; ++q) {
     const int k = ct[q].table;
     const SortedRange rg = {ct[q].occ_begin, ct[q].occ_end, mean[k] != 0};
-    const SegArgs sa = seg_args(w, M, mt->tables[k].dim, nullptr, 0, 0, nullptr, 0, MONO_POOL_SUM, w.ugrad, s, &rg);
+    const SegLaunch sa(seg_args(w, M, mt->tables[k].dim, nullptr, 0, 0, nullptr, 0, MONO_POOL_SUM, w.ugrad, s, &rg),
+                       grad_scale ? &gsc : nullptr);
     reduce_and_apply(mt, k, w, sa, w.fids, cb.lr + segs[q].lr_off, rg.hi - rg.lo, update_time, s, bf16);
   }
 }
@@ -1740,7 +1813,8 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
 // widens them exactly and the sums, the tree and out_rows stay fp32 (bf16_seg_reduce_kernel, then the same kernels).
 void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, const int32_t* row_offsets,
                       int64_t n_rows, int pooling, const float* pooled_grad, int64_t grad_stride,
-                      int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s, bool bf16) {
+                      int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s, bool bf16,
+                      const float* grad_scale) {
   MONO_CUDA(cudaSetDevice(device));
   if (M <= 0) return;
   if (M >= ((int64_t)1 << 31) || total_floats >= ((int64_t)1 << 31)) throw ArgError("scatter_rows: sizes exceed 2^31");
@@ -1767,7 +1841,8 @@ void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, c
   w.sorted = sort_and_runs(w.sort, reinterpret_cast<const uint32_t*>(offs_dev), M, bits, shift, nullptr, s);
   const SegArgs sa = seg_args(w, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, w.ugrad, s);
   const int G = pick_group(D);
-  launch_reduce(sa, G, no_peer, false, s, bf16);
+  const GradScale gsc{grad_scale, nullptr};
+  launch_reduce(SegLaunch(sa, grad_scale ? &gsc : nullptr), G, no_peer, false, s, bf16);
   by_group(G, [&](auto g) {
     constexpr int GG = decltype(g)::value;
     runs_emit_kernel<GG><<<resident_grid(runs_emit_kernel<GG>, M, kThreads / GG), kThreads, 0, s>>>(sa.b, shift,

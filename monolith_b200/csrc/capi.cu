@@ -121,24 +121,24 @@ int gather_pool_entry(int32_t device, const float* fused_emb_dev, const int32_t*
 template <typename T>
 int gather_pool_grad_entry(int32_t device, const T* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
                      const int32_t* emb_offset_dev, const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim,
-                     int32_t pooling, float* grad_fused_dev, void* stream) {
+                     int32_t pooling, float* grad_fused_dev, void* stream, const float* grad_scale = nullptr) {
   return guarded([&] {
     MONO_CUDA(cudaSetDevice(device));
     require(dim > 0, "dim must be positive");
     launch_gather_pool_grad(pooled_grad_dev, grad_stride, grad_col, emb_offset_dev, row_offsets_dev, n_rows, dim,
-                            pooling, grad_fused_dev, (cudaStream_t)stream);
+                            pooling, grad_fused_dev, (cudaStream_t)stream, grad_scale);
   });
 }
 
 int scatter_grad_rows_entry(int32_t device, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
                       const int32_t* emb_offset_dev, int64_t n_occurrences, const int32_t* row_offsets_dev,
                       int64_t n_rows, int32_t dim, int32_t pooling, float* grad_fused_dev, int64_t total_floats,
-                      void* stream, bool bf16) {
+                      void* stream, bool bf16, const float* grad_scale = nullptr) {
   return guarded([&] {
     require(pooled_grad_dev && emb_offset_dev && grad_fused_dev, "scatter_grad_rows: null argument");
     require(row_offsets_dev != nullptr || n_rows == n_occurrences, "scatter_grad_rows: n_rows != n_occurrences");
     run_scatter_rows(device, emb_offset_dev, n_occurrences, dim, row_offsets_dev, n_rows, pooling, pooled_grad_dev,
-                     grad_stride, grad_col, grad_fused_dev, total_floats, (cudaStream_t)stream, bf16);
+                     grad_stride, grad_col, grad_fused_dev, total_floats, (cudaStream_t)stream, bf16, grad_scale);
   });
 }
 
@@ -146,13 +146,13 @@ int layout_entry(bool backward, int32_t device, float* const* emb_ptrs_dev, cons
                  int32_t n_emb, const uint64_t* fid_offset_dev, int64_t total_fid, const int32_t* feature_offset_dev,
                  int32_t total_feature, const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
                  const mono_slice_task* tasks_host, int32_t n_tasks, float* const* out_ptrs_dev, void* stream,
-                 bool bf16) {
+                 bool bf16, const float* grad_scale = nullptr) {
   return guarded([&] {
     check_layout_tasks(tasks_host, n_tasks, total_nfl);
     MONO_CUDA(cudaSetDevice(device));
     launch_layout(backward, emb_ptrs_dev, emb_strides_dev, n_emb, fid_offset_dev, total_fid, feature_offset_dev,
                   total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host, n_tasks, out_ptrs_dev,
-                  (cudaStream_t)stream, bf16);
+                  (cudaStream_t)stream, bf16, grad_scale);
   });
 }
 
@@ -922,6 +922,99 @@ int mono_embedding_to_layout_grad_bf16(int32_t device, float* const* emb_grad_pt
   return layout_entry(true, device, emb_grad_ptrs_dev, emb_strides_dev, n_emb, fid_offset_dev, total_fid,
                       feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host, n_tasks,
                       const_cast<float* const*>(out_grad_ptrs_dev), stream, true);
+}
+
+// ---- the scaled backward calls: the unscaled call's arguments, then grad_scale_dev (NULL = the unscaled call) ----
+int mono_mtable_pool_backward_parts_scaled(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                           const float* learning_rate_host, int64_t update_time,
+                                           int64_t /*global_step*/, const float* grad_scale_dev, void* stream) {
+  return guarded([&] {
+    HandleGuard hg_(t);
+    run_pool_backward_parts(t, parts_host, n_parts, learning_rate_host, update_time, (cudaStream_t)stream, false,
+                            grad_scale_dev);
+  });
+}
+
+int mono_mtable_pool_backward_parts_bf16_scaled(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                                                const float* learning_rate_host, int64_t update_time,
+                                                int64_t /*global_step*/, const float* grad_scale_dev, void* stream) {
+  return guarded([&] {
+    HandleGuard hg_(t);
+    run_pool_backward_parts(t, parts_host, n_parts, learning_rate_host, update_time, (cudaStream_t)stream, true,
+                            grad_scale_dev);
+  });
+}
+
+int mono_gather_pool_grad_scaled(int32_t device, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                                 const int32_t* emb_offset_dev, const int32_t* row_offsets_dev, int64_t n_rows,
+                                 int32_t dim, int32_t pooling, float* grad_fused_dev, const float* grad_scale_dev,
+                                 void* stream) {
+  return gather_pool_grad_entry(device, pooled_grad_dev, grad_stride, grad_col, emb_offset_dev, row_offsets_dev, n_rows,
+                                dim, pooling, grad_fused_dev, stream, grad_scale_dev);
+}
+
+int mono_gather_pool_grad_bf16_scaled(int32_t device, const float* pooled_grad_dev, int64_t grad_stride,
+                                      int32_t grad_col, const int32_t* emb_offset_dev, const int32_t* row_offsets_dev,
+                                      int64_t n_rows, int32_t dim, int32_t pooling, float* grad_fused_dev,
+                                      const float* grad_scale_dev, void* stream) {
+  return gather_pool_grad_entry(device, reinterpret_cast<const __nv_bfloat16*>(pooled_grad_dev), grad_stride,
+                                grad_col, emb_offset_dev, row_offsets_dev, n_rows, dim, pooling, grad_fused_dev,
+                                stream, grad_scale_dev);
+}
+
+int mono_scatter_grad_rows_scaled(int32_t device, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                                  const int32_t* emb_offset_dev, int64_t n_occurrences, const int32_t* row_offsets_dev,
+                                  int64_t n_rows, int32_t dim, int32_t pooling, float* grad_fused_dev,
+                                  int64_t total_floats, const float* grad_scale_dev, void* stream) {
+  return scatter_grad_rows_entry(device, pooled_grad_dev, grad_stride, grad_col, emb_offset_dev, n_occurrences,
+                                 row_offsets_dev, n_rows, dim, pooling, grad_fused_dev, total_floats, stream, false,
+                                 grad_scale_dev);
+}
+
+int mono_scatter_grad_rows_bf16_scaled(int32_t device, const float* pooled_grad_dev, int64_t grad_stride,
+                                       int32_t grad_col, const int32_t* emb_offset_dev, int64_t n_occurrences,
+                                       const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim, int32_t pooling,
+                                       float* grad_fused_dev, int64_t total_floats, const float* grad_scale_dev,
+                                       void* stream) {
+  return scatter_grad_rows_entry(device, pooled_grad_dev, grad_stride, grad_col, emb_offset_dev, n_occurrences,
+                                 row_offsets_dev, n_rows, dim, pooling, grad_fused_dev, total_floats, stream, true,
+                                 grad_scale_dev);
+}
+
+int mono_embedding_to_layout_grad_scaled(int32_t device, float* const* emb_grad_ptrs_dev,
+                                         const int32_t* emb_strides_dev, int32_t n_emb,
+                                         const uint64_t* fid_offset_dev, int64_t total_fid,
+                                         const int32_t* feature_offset_dev, int32_t total_feature,
+                                         const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                         const mono_slice_task* tasks_host, int32_t n_tasks,
+                                         const float* const* out_grad_ptrs_dev, const float* grad_scale_dev,
+                                         void* stream) {
+  return layout_entry(true, device, emb_grad_ptrs_dev, emb_strides_dev, n_emb, fid_offset_dev, total_fid,
+                      feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host, n_tasks,
+                      const_cast<float* const*>(out_grad_ptrs_dev), stream, false, grad_scale_dev);
+}
+
+int mono_embedding_to_layout_grad_bf16_scaled(int32_t device, float* const* emb_grad_ptrs_dev,
+                                              const int32_t* emb_strides_dev, int32_t n_emb,
+                                              const uint64_t* fid_offset_dev, int64_t total_fid,
+                                              const int32_t* feature_offset_dev, int32_t total_feature,
+                                              const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                              const mono_slice_task* tasks_host, int32_t n_tasks,
+                                              const float* const* out_grad_ptrs_dev, const float* grad_scale_dev,
+                                              void* stream) {
+  return layout_entry(true, device, emb_grad_ptrs_dev, emb_strides_dev, n_emb, fid_offset_dev, total_fid,
+                      feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host, n_tasks,
+                      const_cast<float* const*>(out_grad_ptrs_dev), stream, true, grad_scale_dev);
+}
+
+// ---- global norm + clip scale ----------------------------------------------------------------
+int mono_global_norm(int32_t device, const mono_norm_tensor* tensors_host, int32_t n_tensors, float clip_norm,
+                     float* norm_dev, float* scale_dev, void* stream) {
+  return guarded([&] {
+    check_global_norm(tensors_host, n_tensors, clip_norm, norm_dev, scale_dev);
+    MONO_CUDA(cudaSetDevice(device));
+    launch_global_norm(tensors_host, n_tensors, clip_norm, norm_dev, scale_dev, (cudaStream_t)stream);
+  });
 }
 
 // ---- host-buffer entry points --------------------------------------------------------------

@@ -493,12 +493,15 @@ inline void check_firstn(const char* who, const mono_pool_part& p) {
 
 // bf16: the parts' rows are bfloat16 (the *_parts_bf16 calls)
 void run_lookup_pool_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, cudaStream_t s, bool bf16);
+// grad_scale (device float, or null): every gradient row is multiplied by it in fp32 where it is loaded (the scaled_
+// kernels; null runs the unscaled kernels)
 void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n_parts, const float* lr_host,
-                             int64_t update_time, cudaStream_t s, bool bf16);
+                             int64_t update_time, cudaStream_t s, bool bf16, const float* grad_scale = nullptr);
 
 void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, const int32_t* row_offsets,
                       int64_t n_rows, int pooling, const float* pooled_grad, int64_t grad_stride,
-                      int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s, bool bf16 = false);
+                      int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s, bool bf16 = false,
+                      const float* grad_scale = nullptr);
 
 // dedup.cu
 void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_host, int K, int N,
@@ -520,17 +523,23 @@ void launch_gather_pool(const float* fused_emb, const int32_t* emb_offset, const
 template <typename T>
 void launch_gather_pool_grad(const T* pooled_grad, int64_t grad_stride, int grad_col, const int32_t* emb_offset,
                              const int32_t* row_offsets, int64_t n_rows, int dim, int pooling, float* grad_fused,
-                             cudaStream_t s);
+                             cudaStream_t s, const float* grad_scale = nullptr);
 void check_layout_tasks(const mono_slice_task* tasks, int n_tasks, int total_nfl);
 void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb_strides_dev,
                    int n_emb, const uint64_t* fid_offset, int64_t total_fid,
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,
                    int total_nfl, int batch_size, const mono_slice_task* tasks_host, int n_tasks,
-                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16 = false);
+                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16 = false, const float* grad_scale = nullptr);
 // mono_reduce_and_split[_grad]; T: element type of the slice rows
 void check_reduce_split(const mono_reduce_feature* feats, int n_features);
 template <typename T>
 void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int n_features, int32_t* bad_splits_dev,
                          cudaStream_t s);
+
+// clip.cu
+void check_global_norm(const mono_norm_tensor* tensors, int n_tensors, float clip_norm, const float* norm_dev,
+                       const float* scale_dev);
+void launch_global_norm(const mono_norm_tensor* tensors, int n_tensors, float clip_norm, float* norm_dev,
+                        float* scale_dev, cudaStream_t s);
 
 }  // namespace mono

@@ -146,12 +146,15 @@ bf16_gather_rows_kernel(const float* __restrict__ fused, const int32_t* __restri
 // grad_fused[offset[m] : +dim] += g_row   (float atomics: several occurrences may share a row,
 // exactly like the reference's FusedGatherGradKernel atomicAdd, map_id_to_embedding.cu.cc:75-118)
 // T = bf16: the pooled gradient is widened exactly, then divided and added in fp32.
-template <typename T, int G>
+// SCALED (scaled_ kernels): x * *scale in fp32 before the MEAN division (FusedGatherGradKernel's input * scale).
+template <typename T, int G, bool SCALED = false>
 __device__ __forceinline__ void gather_pool_grad(const T* __restrict__ pooled_grad, int64_t grad_stride, int grad_col,
                                                  const int32_t* __restrict__ emb_offset,
                                                  const int32_t* __restrict__ row_offsets, int64_t n_rows, int dim,
-                                                 int pooling, float* __restrict__ grad_fused) {
+                                                 int pooling, float* __restrict__ grad_fused,
+                                                 const float* __restrict__ scale = nullptr) {
   const int gl = Group<G>::gl();
+  const float gscale = SCALED ? *scale : 1.f;
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
   for (int64_t r = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G; r < n_rows; r += gstride) {
     const int64_t b = row_offsets ? row_offsets[r] : r;
@@ -161,6 +164,7 @@ __device__ __forceinline__ void gather_pool_grad(const T* __restrict__ pooled_gr
     const T* g = pooled_grad + r * grad_stride + grad_col;
     for (int c = gl; c < dim; c += G) {
       float x = row_elem_f32(__ldg(g + c));
+      if (SCALED) x = __fmul_rn(x, gscale);
       if (pooling == MONO_POOL_MEAN) x = __fdiv_rn(x, fn);
       for (int j = 0; j < n; ++j) atomicAdd(grad_fused + emb_offset[b + j] + c, x);
     }
@@ -183,6 +187,26 @@ bf16_gather_pool_grad_kernel(const __nv_bfloat16* __restrict__ pooled_grad, int6
                              int64_t n_rows, int dim, int pooling, float* __restrict__ grad_fused) {
   gather_pool_grad<__nv_bfloat16, G>(pooled_grad, grad_stride, grad_col, emb_offset, row_offsets, n_rows, dim, pooling,
                                      grad_fused);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+scaled_gather_pool_grad_kernel(const float* __restrict__ pooled_grad, int64_t grad_stride, int grad_col,
+                               const int32_t* __restrict__ emb_offset, const int32_t* __restrict__ row_offsets,
+                               int64_t n_rows, int dim, int pooling, float* __restrict__ grad_fused,
+                               const float* __restrict__ scale) {
+  gather_pool_grad<float, G, true>(pooled_grad, grad_stride, grad_col, emb_offset, row_offsets, n_rows, dim, pooling,
+                                   grad_fused, scale);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+scaled_bf16_gather_pool_grad_kernel(const __nv_bfloat16* __restrict__ pooled_grad, int64_t grad_stride, int grad_col,
+                                    const int32_t* __restrict__ emb_offset, const int32_t* __restrict__ row_offsets,
+                                    int64_t n_rows, int dim, int pooling, float* __restrict__ grad_fused,
+                                    const float* __restrict__ scale) {
+  gather_pool_grad<__nv_bfloat16, G, true>(pooled_grad, grad_stride, grad_col, emb_offset, row_offsets, n_rows, dim,
+                                           pooling, grad_fused, scale);
 }
 
 // The kernel of an fp32 / bf16 pair for pooled rows of element type T
@@ -224,12 +248,19 @@ void launch_gather_pool(const float* fused_emb, const int32_t* emb_offset, const
 template <typename T>
 void launch_gather_pool_grad(const T* pooled_grad, int64_t grad_stride, int grad_col, const int32_t* emb_offset,
                              const int32_t* row_offsets, int64_t n_rows, int dim, int pooling, float* grad_fused,
-                             cudaStream_t s) {
+                             cudaStream_t s, const float* grad_scale) {
   if (n_rows <= 0) return;
   if (pooling != MONO_POOL_SUM && pooling != MONO_POOL_MEAN) throw ArgError("gather_pool_grad: SUM or MEAN");
   const int G = pick_group(dim * 4);  // one float per lane
   by_group(G, [&](auto g) {
     constexpr int GG = decltype(g)::value;
+    if (grad_scale) {
+      const auto kern = by_elem<T>(scaled_gather_pool_grad_kernel<GG>, scaled_bf16_gather_pool_grad_kernel<GG>);
+      kern<<<grid_for(n_rows, kThreads / G), kThreads, 0, s>>>(pooled_grad, grad_stride, grad_col, emb_offset,
+                                                              row_offsets, n_rows, dim, pooling, grad_fused,
+                                                              grad_scale);
+      return;
+    }
     const auto kern = by_elem<T>(gather_pool_grad_kernel<GG>, bf16_gather_pool_grad_kernel<GG>);
     kern<<<grid_for(n_rows, kThreads / G), kThreads, 0, s>>>(pooled_grad, grad_stride, grad_col, emb_offset,
                                                             row_offsets, n_rows, dim, pooling, grad_fused);
@@ -242,9 +273,10 @@ template void launch_gather_pool<float>(const float*, const int32_t*, const int3
 template void launch_gather_pool<__nv_bfloat16>(const float*, const int32_t*, const int32_t*, int64_t, int, int,
                                                 __nv_bfloat16*, int64_t, int, cudaStream_t);
 template void launch_gather_pool_grad<float>(const float*, int64_t, int, const int32_t*, const int32_t*, int64_t,
-                                             int, int, float*, cudaStream_t);
+                                             int, int, float*, cudaStream_t, const float*);
 template void launch_gather_pool_grad<__nv_bfloat16>(const __nv_bfloat16*, int64_t, int, const int32_t*,
-                                                     const int32_t*, int64_t, int, int, float*, cudaStream_t);
+                                                     const int32_t*, int64_t, int, int, float*, cudaStream_t,
+                                                     const float*);
 
 // ------------------------------------------------------------------------------------------
 // generic layout op
@@ -364,9 +396,12 @@ __global__ void __launch_bounds__(kThreads) bf16_layout_fwd_kernel(LayoutArgs a)
 // Backward: ScatterGrad (ref: fused_embedding_to_layout.h:286-347) with float atomics, as the
 // reference GPU kernel does (BackwardBatchKernel, cu.cc:337-381).
 // T: element type of the output gradients, widened exactly; the division and the atomics run in fp32.
-template <typename T, int G>
-__device__ __forceinline__ void layout_bwd(const LayoutArgs& a, int n_tasks) {
+// SCALED (scaled_ kernels): each gradient element times *scale in fp32 before the MEAN division
+// (layout_tensors_grad_scale * grad, ref: distribution_ops.py:544-550).
+template <typename T, int G, bool SCALED = false>
+__device__ __forceinline__ void layout_bwd(const LayoutArgs& a, int n_tasks, const float* scale = nullptr) {
   const int gl = Group<G>::gl();
+  const float gscale = SCALED ? *scale : 1.f;
   const int64_t total = (int64_t)n_tasks * a.batch_size;
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
   for (int64_t u = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G; u < total; u += gstride) {
@@ -387,6 +422,7 @@ __device__ __forceinline__ void layout_bwd(const LayoutArgs& a, int n_tasks) {
       float* dst = a.emb_ptrs[i1] + (int64_t)i2 * a.emb_strides[i1] + tk.slice_start;
       for (int c = gl; c < tk.dim; c += G) {
         float x = row_elem_f32(tk.pooling == MONO_POOL_FIRSTN ? g[f * tk.dim + c] : g[c]);
+        if (SCALED) x = __fmul_rn(x, gscale);
         if (tk.pooling == MONO_POOL_MEAN) x = __fdiv_rn(x, fn);
         atomicAdd(dst + c, x);
       }
@@ -402,6 +438,17 @@ __global__ void __launch_bounds__(kThreads) layout_bwd_kernel(LayoutArgs a, int 
 template <int G>
 __global__ void __launch_bounds__(kThreads) bf16_layout_bwd_kernel(LayoutArgs a, int n_tasks) {
   layout_bwd<__nv_bfloat16, G>(a, n_tasks);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads) scaled_layout_bwd_kernel(LayoutArgs a, int n_tasks, const float* scale) {
+  layout_bwd<float, G, true>(a, n_tasks, scale);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+scaled_bf16_layout_bwd_kernel(LayoutArgs a, int n_tasks, const float* scale) {
+  layout_bwd<__nv_bfloat16, G, true>(a, n_tasks, scale);
 }
 
 // Host-side checks of the tasks: the kernels index with every field unchecked.
@@ -431,7 +478,7 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
                    int n_emb, const uint64_t* fid_offset, int64_t total_fid,
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,
                    int total_nfl, int batch_size, const mono_slice_task* tasks_host, int n_tasks,
-                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16) {
+                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16, const float* grad_scale) {
   (void)n_emb;
   if (n_tasks <= 0 || batch_size <= 0) return;
   // chains: consecutive grouping of tasks by destination (accumulate tasks with equal destination)
@@ -489,6 +536,8 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
     constexpr int GG = decltype(g)::value;
     if (!backward && !bf16) layout_fwd_kernel<GG><<<grid, kThreads, 0, s>>>(a);
     else if (!backward) bf16_layout_fwd_kernel<GG><<<grid, kThreads, 0, s>>>(a);
+    else if (grad_scale && !bf16) scaled_layout_bwd_kernel<GG><<<grid, kThreads, 0, s>>>(a, nt, grad_scale);
+    else if (grad_scale) scaled_bf16_layout_bwd_kernel<GG><<<grid, kThreads, 0, s>>>(a, nt, grad_scale);
     else if (!bf16) layout_bwd_kernel<GG><<<grid, kThreads, 0, s>>>(a, nt);
     else bf16_layout_bwd_kernel<GG><<<grid, kThreads, 0, s>>>(a, nt);
   });

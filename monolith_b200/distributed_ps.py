@@ -54,12 +54,14 @@ class CudaBackend:
   def gather_pool(self, rows, offs, dim, row_offsets, pooling, out):
     return self.dops.gather_pool(rows, offs, dim, row_offsets, pooling, out=out)
 
-  def gather_pool_grad_into(self, grad_buf, pooled_grad, offs, dim, row_offsets, pooling):
+  def gather_pool_grad_into(self, grad_buf, pooled_grad, offs, dim, row_offsets, pooling, scale=None):
     """Fills grad_buf (pre-zeroed, shared by all tables of the step).  dim % 4 == 0 and <= 128: the
     deterministic sort-based scatter; otherwise the float-atomic kernel (like the reference GPU path).
-    pooled_grad is float32 or bfloat16 (the bf16 kernels widen it exactly); grad_buf is float32."""
+    pooled_grad is float32 or bfloat16 (the bf16 kernels widen it exactly); grad_buf is float32.  scale (a
+    one-element float32 device tensor, or None): pooled_grad is multiplied by it in float32 first (the _scaled
+    kernels, no extra pass)."""
     if self.vec_ok and dim <= 128:
-      self.dops.scatter_grad_rows(pooled_grad, offs, dim, grad_buf, row_offsets, pooling)
+      self.dops.scatter_grad_rows(pooled_grad, offs, dim, grad_buf, row_offsets, pooling, scale=scale)
       return
     import ctypes as C
     from . import _lib
@@ -67,10 +69,16 @@ class CudaBackend:
     n_rows = offs.numel() if row_offsets is None else row_offsets.numel() - 1
     pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
     ro = None if row_offsets is None else C.c_void_p(row_offsets.data_ptr())
-    fn = lib.mono_gather_pool_grad_bf16 if pooled_grad.dtype == torch.bfloat16 else lib.mono_gather_pool_grad
-    _lib.check(fn(pooled_grad.device.index, C.c_void_p(pooled_grad.data_ptr()), pooled_grad.stride(0), 0,
-                  C.c_void_p(offs.data_ptr()), ro, n_rows, dim, pool, C.c_void_p(grad_buf.data_ptr()),
-                  C.c_void_p(torch.cuda.current_stream(pooled_grad.device).cuda_stream)))
+    args = (pooled_grad.device.index, C.c_void_p(pooled_grad.data_ptr()), pooled_grad.stride(0), 0,
+            C.c_void_p(offs.data_ptr()), ro, n_rows, dim, pool, C.c_void_p(grad_buf.data_ptr()))
+    stream = C.c_void_p(torch.cuda.current_stream(pooled_grad.device).cuda_stream)
+    bf16 = pooled_grad.dtype == torch.bfloat16
+    if scale is None:
+      fn = lib.mono_gather_pool_grad_bf16 if bf16 else lib.mono_gather_pool_grad
+      _lib.check(fn(*args, stream))
+    else:
+      fn = lib.mono_gather_pool_grad_bf16_scaled if bf16 else lib.mono_gather_pool_grad_scaled
+      _lib.check(fn(*args, C.c_void_p(scale.data_ptr()), stream))
 
   def zeros(self, n, like):
     return torch.zeros(n, dtype=torch.float32, device=like.device)
@@ -210,10 +218,18 @@ class PartitionedHashTable:
     ctx.row_offsets, ctx.poolings, ctx.occ_splits = row_offsets, pooling, occ_splits
     return pooled, ctx
 
-  def apply_gradients(self, ctx: StepContext, pooled_grads: Dict[str, torch.Tensor], req_time: int = 0):
-    """Backward steps 7-9.  pooled_grads are float32 or bfloat16; the exchanged row gradients are float32."""
+  def apply_gradients(self, ctx: StepContext, pooled_grads: Dict[str, torch.Tensor], req_time: int = 0,
+                      grad_scale: Optional[torch.Tensor] = None):
+    """Backward steps 7-9.  pooled_grads are float32 or bfloat16; the exchanged row gradients are float32.
+    grad_scale (ref: PartitionedHashTable.apply_gradients' grad_scale, distributed_ps.py:1283-1329): a one-element
+    float32 tensor on the gradients' device, e.g. clip_ops.global_norm_scale's scale.  Every pooled gradient is then
+    multiplied by it in float32 inside the scatter of step 7; the backend receives it only when it is given."""
     be, N = self.backend, self.N
     some = next(iter(pooled_grads.values()))
+    if grad_scale is not None:
+      from .clip_ops import scale_ptr
+      scale_ptr(grad_scale, some.device, "grad_scale")
+    extra = {} if grad_scale is None else {"scale": grad_scale}
     ph = self.phases
     ph.mark("bwd_start")
     # 7 scatter pooled grads to the unique rows, in the layout of the received row buffer
@@ -223,7 +239,7 @@ class PartitionedHashTable:
         continue
       lo, hi = ctx.occ_splits[k]
       be.gather_pool_grad_into(grad_rows, pooled_grads[name], ctx.offs[lo:hi], self.dims[k], ctx.row_offsets.get(name),
-                               ctx.poolings.get(name, "sum"))
+                               ctx.poolings.get(name, "sum"), **extra)
     ph.mark("b7_scatter_grads")
     # 8 grads to the owners (reverse of step 5)
     owner_grads = torch.empty(sum(ctx.send_row_splits), dtype=torch.float32, device=grad_rows.device)

@@ -248,44 +248,62 @@ def gather_pool(fused_embeddings: torch.Tensor, fused_embedding_offsets: torch.T
 
 
 def gather_pool_grad(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.Tensor, dim: int, total_floats: int,
-                     row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum", grad_col: int = 0):
+                     row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum", grad_col: int = 0,
+                     scale: Optional[torch.Tensor] = None):
   """Backward of gather_pool: scatter-add pooled grads to the fused row buffer
   (ref: FusedGatherGradKernel, map_id_to_embedding.cu.cc:75-118).  pooled_grad is float32 or bfloat16 (widened
-  exactly); the returned buffer is float32."""
+  exactly); the returned buffer is float32.  scale: a one-element float32 tensor on pooled_grad's device (the
+  reference kernel's `input * scale`): each gradient element is multiplied by it in float32 before the MEAN
+  division (mono_gather_pool_grad[_bf16]_scaled)."""
+  from .clip_ops import scale_ptr
   bf16 = _tower_dtype(pooled_grad.dtype, "pooled_grad") == torch.bfloat16
   lib = _lib.load()
   dev = pooled_grad.device
+  sp = scale_ptr(scale, dev, "scale")
   offs = fused_embedding_offsets.to(torch.int32).contiguous()
   n_rows = offs.numel() if row_offsets is None else row_offsets.numel() - 1
   if row_offsets is not None:
     row_offsets = row_offsets.to(torch.int32).contiguous()
   grad = torch.zeros(total_floats, dtype=torch.float32, device=dev)
   pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-  fn = lib.mono_gather_pool_grad_bf16 if bf16 else lib.mono_gather_pool_grad
-  _lib.check(fn(dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs), _ptr(row_offsets), n_rows,
-                dim, pool, _ptr(grad), _stream(dev)))
+  args = (dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs), _ptr(row_offsets), n_rows, dim,
+          pool, _ptr(grad))
+  if sp is None:
+    fn = lib.mono_gather_pool_grad_bf16 if bf16 else lib.mono_gather_pool_grad
+    _lib.check(fn(*args, _stream(dev)))
+  else:
+    fn = lib.mono_gather_pool_grad_bf16_scaled if bf16 else lib.mono_gather_pool_grad_scaled
+    _lib.check(fn(*args, sp, _stream(dev)))
   return grad
 
 
 def scatter_grad_rows(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.Tensor, dim: int,
                       grad_fused: torch.Tensor, row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum",
-                      grad_col: int = 0):
+                      grad_col: int = 0, scale: Optional[torch.Tensor] = None):
   """Deterministic (sort-based, atomics-free) scatter of pooled-row grads into the fused row buffer
   `grad_fused` (written in place; rows nobody refers to are left as they are).  pooled_grad is float32 or
-  bfloat16 (widened exactly); grad_fused must be float32."""
+  bfloat16 (widened exactly); grad_fused must be float32.  scale: as gather_pool_grad's; the result is bit for bit
+  this call on pooled_grad multiplied by it in float32 (mono_scatter_grad_rows[_bf16]_scaled)."""
+  from .clip_ops import scale_ptr
   bf16 = _tower_dtype(pooled_grad.dtype, "pooled_grad") == torch.bfloat16
   if grad_fused.dtype != torch.float32:
     raise ValueError(f"grad_fused must be torch.float32, not {grad_fused.dtype}")
   lib = _lib.load()
   dev = pooled_grad.device
+  sp = scale_ptr(scale, dev, "scale")
   offs = fused_embedding_offsets.to(torch.int32).contiguous()
   n_rows = offs.numel() if row_offsets is None else row_offsets.numel() - 1
   if row_offsets is not None:
     row_offsets = row_offsets.to(torch.int32).contiguous()
   pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-  fn = lib.mono_scatter_grad_rows_bf16 if bf16 else lib.mono_scatter_grad_rows
-  _lib.check(fn(dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs), offs.numel(),
-                _ptr(row_offsets), n_rows, dim, pool, _ptr(grad_fused), grad_fused.numel(), _stream(dev)))
+  args = (dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs), offs.numel(), _ptr(row_offsets),
+          n_rows, dim, pool, _ptr(grad_fused), grad_fused.numel())
+  if sp is None:
+    fn = lib.mono_scatter_grad_rows_bf16 if bf16 else lib.mono_scatter_grad_rows
+    _lib.check(fn(*args, _stream(dev)))
+  else:
+    fn = lib.mono_scatter_grad_rows_bf16_scaled if bf16 else lib.mono_scatter_grad_rows_scaled
+    _lib.check(fn(*args, sp, _stream(dev)))
   return grad_fused
 
 
@@ -669,21 +687,32 @@ def fused_embedding_to_layout(embeddings_list: Sequence[torch.Tensor], emb_strid
 
 def fused_embedding_to_layout_grad(emb_sizes: Sequence[int], emb_strides: Sequence[int], fid_offset: torch.Tensor,
                                    feature_offset: torch.Tensor, nfl_offset: torch.Tensor, batch_size: int,
-                                   tasks: Sequence[SliceTask], out_grads: Sequence[torch.Tensor]):
+                                   tasks: Sequence[SliceTask], out_grads: Sequence[torch.Tensor],
+                                   layout_tensors_grad_scale: Optional[torch.Tensor] = None):
   """ref: MonolithEmbeddingToLayoutGradV* (fused_embedding_to_layout.cc:697-948).  The index tensors as in
   fused_embedding_to_layout; out_grads all float32 or all bfloat16 (widened exactly) on their device.  The
-  returned embedding gradients are float32."""
+  returned embedding gradients are float32.  layout_tensors_grad_scale: a one-element float32 tensor on that device
+  (the reference's `layout_tensors_grad_scale * grad`, distribution_ops.py:544-550): every gradient element is
+  multiplied by it in float32 before the MEAN division (mono_embedding_to_layout_grad[_bf16]_scaled)."""
+  from .clip_ops import scale_ptr
   dtype = _tower_dtype(out_grads[0].dtype if len(out_grads) else torch.float32, "out_grads")
   if any(g.dtype != dtype for g in out_grads):
     raise ValueError(f"out_grads must be all torch.float32 or all torch.bfloat16, not {[g.dtype for g in out_grads]}")
   dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, out_grads, "out_grads", dtype)
+  sp = scale_ptr(layout_tensors_grad_scale, dev, "layout_tensors_grad_scale")
   lib = _lib.load()
   grads = [torch.zeros(n, dtype=torch.float32, device=dev) for n in emb_sizes]
   og = [g.contiguous() for g in out_grads]
   gp, op = _ptr_table(grads, dev), _ptr_table(og, dev)
   st = torch.tensor(list(emb_strides), dtype=torch.int32, device=dev)
-  fn = lib.mono_embedding_to_layout_grad_bf16 if dtype == torch.bfloat16 else lib.mono_embedding_to_layout_grad
-  _lib.check(fn(dev.index, _ptr(gp), _ptr(st), len(grads), _ptr(fid_offset), fid_offset.numel(), _ptr(feature_offset),
-                feature_offset.numel(), _ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks), len(tasks),
-                _ptr(op), _stream(dev)))
+  args = (dev.index, _ptr(gp), _ptr(st), len(grads), _ptr(fid_offset), fid_offset.numel(), _ptr(feature_offset),
+          feature_offset.numel(), _ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks), len(tasks),
+          _ptr(op))
+  if sp is None:
+    fn = lib.mono_embedding_to_layout_grad_bf16 if dtype == torch.bfloat16 else lib.mono_embedding_to_layout_grad
+    _lib.check(fn(*args, _stream(dev)))
+  else:
+    fn = (lib.mono_embedding_to_layout_grad_bf16_scaled if dtype == torch.bfloat16 else
+          lib.mono_embedding_to_layout_grad_scaled)
+    _lib.check(fn(*args, sp, _stream(dev)))
   return grads

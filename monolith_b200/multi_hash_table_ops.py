@@ -461,7 +461,8 @@ class MultiHashTable:
     del keep
     return outs
 
-  def pool_backward_parts(self, parts: Sequence[PoolPart], req_time: int = 0, global_step: int = 0):
+  def pool_backward_parts(self, parts: Sequence[PoolPart], req_time: int = 0, global_step: int = 0,
+                          grad_scale: Optional[torch.Tensor] = None):
     """pool_backward over many features and tables in one call (mono_mtable_pool_backward_parts): the parts
     of one table are ONE batch in part order, so a FID that several features share gets one optimizer step
     with the sum of all its terms; the claim, sort and run list run once for the whole call.  A "firstn" part's
@@ -469,14 +470,25 @@ class MultiHashTable:
     inserted, bumped and stepped (with a zero gradient) as the reference's ScatterGrad leaves it.
 
     Every part's rows share one dtype, float32 or bfloat16; bfloat16 gradients (mono_mtable_pool_backward_parts_bf16)
-    give exactly the bits of this call on the rows widened to float32."""
+    give exactly the bits of this call on the rows widened to float32.
+
+    grad_scale: a one-element float32 tensor on the table's device (clip_ops.global_norm_scale's scale), read on the
+    device: the call is then bit for bit this call on every gradient row multiplied by it in float32 first
+    (mono_mtable_pool_backward_parts[_bf16]_scaled; a bfloat16 row is widened before the multiply)."""
+    from .clip_ops import scale_ptr
     dtype = self._parts_dtype(parts)
+    sp = scale_ptr(grad_scale, self._device, "grad_scale")
     arr, keep, _ = self._parts_arr(parts, forward=False, dtype=dtype)
     lr = self.learning_rates()
     lr_arr = (C.c_float * max(len(lr), 1))(*lr)
-    fn = (self._lib.mono_mtable_pool_backward_parts_bf16 if dtype == torch.bfloat16 else
-          self._lib.mono_mtable_pool_backward_parts)
-    _lib.check(fn(self._h, arr, len(parts), lr_arr, int(req_time), int(global_step), _stream(self._device)))
+    if sp is None:
+      fn = (self._lib.mono_mtable_pool_backward_parts_bf16 if dtype == torch.bfloat16 else
+            self._lib.mono_mtable_pool_backward_parts)
+      _lib.check(fn(self._h, arr, len(parts), lr_arr, int(req_time), int(global_step), _stream(self._device)))
+    else:
+      fn = (self._lib.mono_mtable_pool_backward_parts_bf16_scaled if dtype == torch.bfloat16 else
+            self._lib.mono_mtable_pool_backward_parts_scaled)
+      _lib.check(fn(self._h, arr, len(parts), lr_arr, int(req_time), int(global_step), sp, _stream(self._device)))
     del keep
     return self
 
