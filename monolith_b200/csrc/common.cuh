@@ -226,6 +226,45 @@ __device__ __forceinline__ Entry exch_entry(Entry* addr, const Entry& val) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// first-occurrence set: the lowest position of every distinct (key, tag) of a call, in a scratch
+// open-addressing set of power-of-two size memset to 0xFF (tag -1 = empty; tags are >= 0).  Which
+// slot a key lands in decides no output: first_pos alone does.
+// ---------------------------------------------------------------------------------------------
+struct FirstOcc {  // viewed as an Entry for the 128-bit CAS: row = tag, ts = first_pos
+  int64_t key;
+  int32_t tag;
+  int32_t first_pos;
+};
+static_assert(sizeof(FirstOcc) == sizeof(Entry), "a set entry is one 128-bit word");
+
+__device__ __forceinline__ uint32_t first_occ_slot(int64_t key, int tag, uint32_t mask) {
+  return (uint32_t)(mix64((uint64_t)key * 0x9E3779B97F4A7C15ULL + (uint64_t)tag) >> 20) & mask;
+}
+
+// Position pos claims or joins the slot of (key, tag), probing linearly from slot s; returns that slot.
+__device__ __forceinline__ uint32_t claim_first_occ(FirstOcc* set, uint32_t mask, uint32_t s, int64_t key, int tag,
+                                                    int32_t pos) {
+  while (true) {
+    const Entry e = ld_entry_cg(reinterpret_cast<Entry*>(set + s));
+    if ((int32_t)e.row == -1) {  // empty
+      Entry v;
+      v.key = key;
+      v.row = (uint32_t)tag;
+      v.ts = (uint32_t)pos;
+      if (cas_entry(reinterpret_cast<Entry*>(set + s), empty_entry(), v)) return s;
+      continue;  // lost the race: re-read the same slot
+    }
+    if (e.key == key && (int32_t)e.row == tag) {
+      // first_pos only ever decreases: skip the atomic when the value just read is already
+      // lower (this removes the same-address atomic storm of hot keys in Zipf batches)
+      if ((int32_t)e.ts > pos) atomicMin(&set[s].first_pos, pos);
+      return s;
+    }
+    s = (s + 1) & mask;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // lane groups: G lanes (4, 8, 16 or 32) cooperate on one id / one pooled row.  All 32 lanes of a
 // warp stay converged (inactive groups run with `active == false`), so full-mask warp votes are legal.
 // ---------------------------------------------------------------------------------------------

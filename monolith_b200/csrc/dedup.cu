@@ -31,12 +31,6 @@ constexpr int64_t kMaxIds = (int64_t)1 << 30;       // the scratch set holds 2^3
 constexpr int kTileItems = 8;                       // ids per thread per tile
 constexpr int kTile = kThreads * kTileItems;        // ids per block tile
 
-struct DSet {  // 16-byte scratch-set entry, viewed as an Entry for the 128-bit CAS
-  int64_t key;
-  int32_t list;
-  int32_t first_pos;
-};
-
 __device__ __forceinline__ int shard_of(int64_t fid, int n_eff, int rank0_empty) {
   // ref: shard_func, fused_reorder_by_indices.cc:121-123 (unsigned so that negative FIDs stay in range)
   return (int)((uint64_t)fid % (uint64_t)n_eff) + rank0_empty;
@@ -53,31 +47,12 @@ __device__ __forceinline__ int list_of(const int64_t* __restrict__ split, int K,
 
 __global__ void __launch_bounds__(kThreads)
 dd_claim_kernel(const int64_t* __restrict__ ids, int64_t M, const int64_t* __restrict__ split, int K,
-                DSet* set, uint32_t mask, uint32_t* __restrict__ slot_of) {
+                FirstOcc* set, uint32_t mask, uint32_t* __restrict__ slot_of) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < M;
        i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t key = ids[i];
     const int m = K > 1 ? list_of(split, K, i) : 0;
-    uint32_t s = (uint32_t)(mix64((uint64_t)key * 0x9E3779B97F4A7C15ULL + (uint64_t)m) >> 20) & mask;
-    while (true) {
-      Entry e = ld_entry_cg(reinterpret_cast<Entry*>(set + s));
-      if ((int32_t)e.row == -1) {  // list == -1: empty
-        Entry v;
-        v.key = key;
-        v.row = (uint32_t)m;
-        v.ts = (uint32_t)i;
-        if (cas_entry(reinterpret_cast<Entry*>(set + s), empty_entry(), v)) break;
-        continue;
-      }
-      if (e.key == key && (int32_t)e.row == m) {
-        // first_pos only ever decreases: skip the atomic when the value just read is already
-        // lower (this removes the same-address atomic storm of hot keys in Zipf batches)
-        if ((int32_t)e.ts > (int32_t)i) atomicMin(&set[s].first_pos, (int32_t)i);
-        break;
-      }
-      s = (s + 1) & mask;
-    }
-    slot_of[i] = s;
+    slot_of[i] = claim_first_occ(set, mask, first_occ_slot(key, m, mask), key, m, (int32_t)i);
   }
 }
 
@@ -103,7 +78,7 @@ struct DDTables {
 template <int MODE>
 __global__ void __launch_bounds__(kThreads)
 dd_rank_kernel(const int64_t* __restrict__ ids, int64_t M, const int64_t* __restrict__ split, int K,
-               int N, int n_eff, int rank0_empty, const DSet* __restrict__ set,
+               int N, int n_eff, int rank0_empty, const FirstOcc* __restrict__ set,
                const uint32_t* __restrict__ slot_of, int32_t* __restrict__ blk_cnt, int nblk,
                DDTables tb, int64_t* __restrict__ output, int32_t* __restrict__ rank) {
   __shared__ int32_t wcnt[kThreads / 32][kMaxShards];   // per-warp counts, then per-warp bases
@@ -252,7 +227,7 @@ dd_scan_kernel(int32_t* blk_cnt, int nblk, int N, int K, const int32_t* __restri
 // ref: fused_reorder_by_indices.cc:101-112: ids_sets[m][val] + emb_offsets_cm[shard + m*N]
 __global__ void __launch_bounds__(kThreads)
 dd_offsets_kernel(const int64_t* __restrict__ ids, int64_t M, const int64_t* __restrict__ split, int K,
-                  int N, int n_eff, int rank0_empty, const DSet* __restrict__ set,
+                  int N, int n_eff, int rank0_empty, const FirstOcc* __restrict__ set,
                   const uint32_t* __restrict__ slot_of, const int32_t* __restrict__ rank,
                   const int32_t* __restrict__ dims, int dim0, DDTables tb,
                   int32_t* __restrict__ fused_emb_offset) {
@@ -267,7 +242,7 @@ dd_offsets_kernel(const int64_t* __restrict__ ids, int64_t M, const int64_t* __r
 
 // passes 2-5 over M > 0 ids, once slot_of and the scratch set's first positions are written
 static void rank_passes(const int64_t* ids_dev, int64_t M, const int64_t* split_dev, int K, int N, int n_eff,
-                        int rank0_empty, const DSet* set, const uint32_t* slot_of, int32_t* blk_cnt, int nblk,
+                        int rank0_empty, const FirstOcc* set, const uint32_t* slot_of, int32_t* blk_cnt, int nblk,
                         const int32_t* dims_dev, int dim0, DDTables tb, int64_t* output_dev, int32_t* rank,
                         int32_t* fused_emb_offset_dev, cudaStream_t s) {
   const int g = std::min(nblk, device_sms() * 8);
@@ -318,7 +293,7 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
   const size_t NK = (size_t)N * K;
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-  const size_t o_set = take(sizeof(DSet) * cap);
+  const size_t o_set = take(sizeof(FirstOcc) * cap);
   const size_t o_slot = take(sizeof(uint32_t) * (size_t)std::max<int64_t>(M, 1));
   const size_t o_rank = take(sizeof(int32_t) * (size_t)std::max<int64_t>(M, 1));
   const size_t o_blk = take(sizeof(int32_t) * (size_t)N * nblk);
@@ -327,7 +302,7 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
   const size_t o_small = take(sizeof(int32_t) * (4 * NK + N + 8));
   char* ws = nullptr;
   MONO_CUDA(cudaMallocAsync((void**)&ws, off, s));
-  DSet* set = reinterpret_cast<DSet*>(ws + o_set);
+  FirstOcc* set = reinterpret_cast<FirstOcc*>(ws + o_set);
   uint32_t* slot_of = reinterpret_cast<uint32_t*>(ws + o_slot);
   int32_t* rank = reinterpret_cast<int32_t*>(ws + o_rank);
   int32_t* blk_cnt = reinterpret_cast<int32_t*>(ws + o_blk);
@@ -348,7 +323,7 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
     MONO_CUDA(cudaMemcpyAsync(split_dev, id_split_host, sizeof(int64_t) * (K + 1), cudaMemcpyHostToDevice, s));
     MONO_CUDA(cudaMemcpyAsync(dims_dev, dims_host, sizeof(int32_t) * K, cudaMemcpyHostToDevice, s));
   }
-  MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(DSet) * cap, s));
+  MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(FirstOcc) * cap, s));
   MONO_CUDA(cudaMemsetAsync(small, 0, sizeof(int32_t) * (4 * NK + N + 8), s));
 
   if (M > 0) {
@@ -411,7 +386,7 @@ struct ShardStage {
 // list-order FIDs; unique = false also writes the identity grouping the rank passes read
 __global__ void __launch_bounds__(kThreads)
 sh_gather_kernel(const int64_t* __restrict__ fids, int64_t M, int F, ShardStage st, int identity,
-                 int64_t* __restrict__ ids_lo, DSet* __restrict__ set, uint32_t* __restrict__ slot_of) {
+                 int64_t* __restrict__ ids_lo, FirstOcc* __restrict__ set, uint32_t* __restrict__ slot_of) {
   for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < M; p += (int64_t)gridDim.x * blockDim.x) {
     const int j = F > 1 ? list_of(st.split_lo, F, p) : 0;
     ids_lo[p] = fids[st.split_in[st.feat_of_j[j]] + (p - st.split_lo[j])];
@@ -561,13 +536,13 @@ void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits
   const size_t NF = (size_t)N * F;
   off = 0;
   auto take256 = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-  const size_t o_set = take256(sizeof(DSet) * cap), o_slot = take256(sizeof(uint32_t) * M1),
+  const size_t o_set = take256(sizeof(FirstOcc) * cap), o_slot = take256(sizeof(uint32_t) * M1),
                o_rank = take256(sizeof(int32_t) * M1), o_blk = take256(sizeof(int32_t) * (size_t)N * nblk),
                o_ids = take256(sizeof(int64_t) * M1), o_offs = take256(sizeof(int32_t) * M1),
                o_small = take256(sizeof(int32_t) * (4 * NF + N + 8)), o_stage = take256(stage_bytes);
   char* ws = nullptr;
   MONO_CUDA(cudaMallocAsync((void**)&ws, off, s));
-  DSet* set = reinterpret_cast<DSet*>(ws + o_set);
+  FirstOcc* set = reinterpret_cast<FirstOcc*>(ws + o_set);
   uint32_t* slot_of = reinterpret_cast<uint32_t*>(ws + o_slot);
   int32_t* rank = reinterpret_cast<int32_t*>(ws + o_rank);
   int32_t* blk_cnt = reinterpret_cast<int32_t*>(ws + o_blk);
@@ -596,7 +571,7 @@ void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits
 
   // a pageable H2D copy is staged by the driver before the call returns: h may go out of scope after it
   MONO_CUDA(cudaMemcpyAsync(stage, h.data(), stage_bytes, cudaMemcpyHostToDevice, s));
-  if (unique) MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(DSet) * cap, s));
+  if (unique) MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(FirstOcc) * cap, s));
   MONO_CUDA(cudaMemsetAsync(small, 0, sizeof(int32_t) * (4 * NF + N + 8), s));
 
   if (M > 0) {

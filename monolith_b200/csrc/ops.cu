@@ -718,16 +718,16 @@ struct UpsertArgs {
   const CallSeg* segs;
   int nsegs;
   const int64_t* ids;
-  const uint32_t* idx_list;  // optional indirection: item j is ids[idx_list[j]]
-  int64_t n;                 // number of items to process
-  const uint32_t* n_dev;     // optional: item count on device (overrides n when non-null)
+  const uint32_t* idx_list = nullptr;  // optional indirection: item j is ids[idx_list[j]]
+  int64_t n;                           // number of items to process
+  const uint32_t* n_dev = nullptr;     // optional: item count on device (overrides n when non-null)
   const float* vals;
   const float* lr;           // device copy of the call's learning rates
   uint32_t update_ts;
   uint32_t* miss_ctr;        // global miss counter of the call
   uint32_t* miss_list;       // item indices j that missed
   uint32_t* rowidx;          // per item j: resolved row (bit 31 = freshly inserted)
-  int32_t* status;           // reinitialize only
+  int32_t* status = nullptr; // reinitialize only
   int64_t pos0 = 0;          // apply pass without idx_list: item j is position pos0 + j
   // admission filter (tables without one never filter): 0 = not consulted (reinitialize, restore); 1 = ids ABSENT
   // from the table consult it (optimize: tf_bridge.cc:296-326; assign: :181-185); 2 = every id does (AssignAdd2
@@ -866,57 +866,24 @@ __global__ void __launch_bounds__(kThreads) upsert_apply_kernel(UpsertArgs a) {
 }
 
 // ---- duplicate handling (ids not guaranteed unique) ------------------------------------------
-struct SetEntry {  // scratch open-addressing set keyed by (table, fid)
-  int64_t key;
-  int32_t table;
-  int32_t first_pos;
-};
-
-__device__ __forceinline__ bool cas_set(SetEntry* addr, const SetEntry& val) {
-  Entry cmp = empty_entry();
-  Entry v;
-  v.key = val.key;
-  v.row = (uint32_t)val.table;
-  v.ts = (uint32_t)val.first_pos;
-  return cas_entry(reinterpret_cast<Entry*>(addr), cmp, v);
-}
-
 // every pending position claims / joins the set slot of its (table, fid) and lowers first_pos
 __global__ void __launch_bounds__(kThreads)
 dup_claim_kernel(const CallSeg* __restrict__ segs, int nsegs, const int64_t* __restrict__ ids,
-                 const uint32_t* __restrict__ pending, int64_t n, SetEntry* set, uint32_t mask,
+                 const uint32_t* __restrict__ pending, int64_t n, FirstOcc* set, uint32_t mask,
                  uint32_t* __restrict__ slot_of, const uint32_t* __restrict__ n_dev = nullptr) {
   if (n_dev) n = (int64_t)*n_dev;
   for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n;
        j += (int64_t)gridDim.x * blockDim.x) {
     const int64_t i = pending ? (int64_t)pending[j] : j;
-    const int si = nsegs > 1 ? find_seg(segs, nsegs, i) : 0;
-    const int table = segs[si].table;
+    const int table = segs[nsegs > 1 ? find_seg(segs, nsegs, i) : 0].table;
     const int64_t key = ids[i];
-    uint32_t s = (uint32_t)(mix64((uint64_t)key * 31 + table) >> 20) & mask;
-    while (true) {
-      Entry e = ld_entry_cg(reinterpret_cast<Entry*>(set + s));
-      if (e.row == kEmptyRow && e.ts == 0xFFFFFFFFu && e.key == -1) {  // empty (table == -1)
-        SetEntry ne;
-        ne.key = key;
-        ne.table = table;
-        ne.first_pos = (int32_t)i;
-        if (cas_set(set + s, ne)) break;
-        continue;  // lost the race: re-read the same slot
-      }
-      if (e.key == key && (int32_t)e.row == table) {
-        if ((int32_t)e.ts > (int32_t)i) atomicMin(&set[s].first_pos, (int32_t)i);
-        break;
-      }
-      s = (s + 1) & mask;
-    }
-    slot_of[j] = s;
+    slot_of[j] = claim_first_occ(set, mask, first_occ_slot(key, table, mask), key, table, (int32_t)i);
   }
 }
 
 // split pending into leaders (lowest pending position of their key) and the rest
 __global__ void __launch_bounds__(kThreads)
-dup_split_kernel(const uint32_t* __restrict__ pending, int64_t n, const SetEntry* __restrict__ set,
+dup_split_kernel(const uint32_t* __restrict__ pending, int64_t n, const FirstOcc* __restrict__ set,
                  const uint32_t* __restrict__ slot_of, uint32_t* leaders, uint32_t* rest,
                  uint32_t* ctr /*[0]=leaders,[1]=rest*/, uint32_t* leader_of /*optional, by position*/) {
   for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n;
@@ -934,7 +901,7 @@ dup_split_kernel(const uint32_t* __restrict__ pending, int64_t n, const SetEntry
 // missing FID inserts it (leaders -> resolve_miss_kernel); the others take the leader's row, not fresh.
 __global__ void __launch_bounds__(kThreads)
 miss_split_kernel(const uint32_t* __restrict__ miss_list, const uint32_t* __restrict__ n_miss,
-                  const SetEntry* __restrict__ set, const uint32_t* __restrict__ slot_of,
+                  const FirstOcc* __restrict__ set, const uint32_t* __restrict__ slot_of,
                   uint32_t* __restrict__ leaders, uint32_t* __restrict__ followers,
                   uint32_t* __restrict__ fol_leader, uint32_t* ctr /*[1] = leaders, [2] = followers*/) {
   const int64_t n = *n_miss;
@@ -1378,6 +1345,53 @@ static void launch_upsert(UpsertOp op, int G, const UpsertArgs& a, int64_t n_upp
   }
 }
 
+// The fields every upsert launch fills alike; the caller sets idx_list, n_dev, pos0, wait_flag, filter_mode and status.
+static UpsertArgs upsert_args(const mono_mtable* mt, const CallBlob& cb, int nsegs, const int64_t* ids, int64_t n,
+                              const float* vals, uint32_t update_ts, uint32_t* miss_ctr, uint32_t* miss_list,
+                              uint32_t* rowidx) {
+  UpsertArgs a;
+  a.tables = mt->d_tables;
+  a.segs = cb.segs;
+  a.nsegs = nsegs;
+  a.ids = ids;
+  a.n = n;
+  a.vals = vals;
+  a.lr = cb.lr;
+  a.update_ts = update_ts;
+  a.miss_ctr = miss_ctr;
+  a.miss_list = miss_list;
+  a.rowidx = rowidx;
+  return a;
+}
+
+// The setup run_upsert and run_upsert_groups share: room for the call's ids in every table it touches (may rehash or
+// grow, so it precedes the descriptor upload), the staged segments and learning rates, the lane-group width of the
+// widest table and whether any of the tables has an admission filter.  issued() closes the call.
+struct UpsertCall {
+  std::vector<uint64_t> per_table;  // ids of the call per table
+  CallBlob cb;
+  int G;
+  bool any_filter = false;
+
+  UpsertCall(mono_mtable* mt, const CallSeg* h_segs, int nsegs, const float* lr_host, int n_lr, cudaStream_t s)
+      : per_table(mt->tables.size(), 0) {
+    for (int i = 0; i < nsegs; ++i)
+      per_table[h_segs[i].table] += (uint64_t)(h_segs[i].id_end - h_segs[i].id_begin);
+    for (size_t k = 0; k < per_table.size(); ++k)
+      if (per_table[k]) ensure_capacity(mt, (int)k, per_table[k], s);
+    upload_tables(mt, s);
+    cb = stage_call(mt, h_segs, nsegs, lr_host, n_lr, s);
+    G = pick_group(max_dim_of(mt, h_segs, nsegs));
+    for (size_t k = 0; k < per_table.size(); ++k)
+      if (per_table[k] && mt->tables[k].dev.flt_cells) any_filter = true;
+  }
+
+  void issued(mono_mtable* mt, int64_t update_time, cudaStream_t s) const {
+    for (size_t k = 0; k < per_table.size(); ++k)
+      if (per_table[k]) note_issued(mt, (int)k, per_table[k], update_time, s);
+  }
+};
+
 void run_upsert(mono_mtable* mt, UpsertOp op, const CallSeg* h_segs, int nsegs,
                 const int64_t* ids_dev, int64_t n_total, const float* vals_dev,
                 const float* lr_host, int n_lr, int64_t update_time, bool unique, bool dedup_sum,
@@ -1401,15 +1415,10 @@ void run_upsert(mono_mtable* mt, UpsertOp op, const CallSeg* h_segs, int nsegs,
     h_segs = rebased.data();
   }
   if (n_total >= (int64_t)1 << 31) throw ArgError("more than 2^31 ids in one call");
-  // capacity first (may rehash / grow and dirty the table descriptors)
-  std::vector<uint64_t> per_table(mt->tables.size(), 0);
-  for (int i = 0; i < nsegs; ++i)
-    per_table[h_segs[i].table] += (uint64_t)(h_segs[i].id_end - h_segs[i].id_begin);
-  for (size_t k = 0; k < per_table.size(); ++k)
-    if (per_table[k]) ensure_capacity(mt, (int)k, per_table[k], s);
-  upload_tables(mt, s);
-  CallBlob cb = stage_call(mt, h_segs, nsegs, lr_host, n_lr, s);
-  const int G = pick_group(max_dim_of(mt, h_segs, nsegs));
+  const UpsertCall call(mt, h_segs, nsegs, lr_host, n_lr, s);
+  const CallBlob& cb = call.cb;
+  const int G = call.G;
+  const bool any_filter = call.any_filter;
 
   // scratch: [miss_ctr (64 B) | miss_list u32[n_total] | rowidx u32[n_total]]
   char* ws = (char*)mt->ws_miss.get(64 + 2 * sizeof(uint32_t) * (size_t)n_total, s);
@@ -1418,24 +1427,9 @@ void run_upsert(mono_mtable* mt, UpsertOp op, const CallSeg* h_segs, int nsegs,
   uint32_t* rowidx = miss_list + n_total;
   MONO_CUDA(cudaMemsetAsync(miss_ctr, 0, 64, s));
 
-  UpsertArgs a;
-  a.tables = mt->d_tables;
-  a.segs = cb.segs;
-  a.nsegs = nsegs;
-  a.ids = ids_dev;
-  a.idx_list = nullptr;
-  a.n = n_total;
-  a.n_dev = nullptr;
-  a.vals = vals_dev;
-  a.lr = cb.lr;
-  a.update_ts = (uint32_t)update_time;
-  a.miss_ctr = miss_ctr;
-  a.miss_list = miss_list;
-  a.rowidx = rowidx;
+  UpsertArgs a = upsert_args(mt, cb, nsegs, ids_dev, n_total, vals_dev, (uint32_t)update_time, miss_ctr, miss_list,
+                             rowidx);
   a.status = status_dev;
-  bool any_filter = false;
-  for (size_t k = 0; k < per_table.size(); ++k)
-    if (per_table[k] && mt->tables[k].dev.flt_cells) any_filter = true;
   a.filter_mode = !any_filter ? 0 : (op == kOpOptimize || op == kOpAssign) ? 1 : (op == kOpAssignAdd ? 2 : 0);
   uint32_t* occ_extra = nullptr;
 
@@ -1447,7 +1441,7 @@ void run_upsert(mono_mtable* mt, UpsertOp op, const CallSeg* h_segs, int nsegs,
     // round r applies the r-th occurrence of every key; within a round keys are unique.
     if (n_total > ((int64_t)1 << 30)) throw ArgError("more than 2^30 non-unique ids in one call");
     const uint32_t cap = claim_set_slots(n_total);  // <= 2^31: n_total <= 2^30 checked above
-    SetEntry* set = (SetEntry*)mt->ws_a.get(sizeof(SetEntry) * (size_t)cap, s);
+    FirstOcc* set = (FirstOcc*)mt->ws_a.get(sizeof(FirstOcc) * (size_t)cap, s);
     uint32_t* slot_of = (uint32_t*)mt->ws_b.get(sizeof(uint32_t) * (size_t)n_total, s);
     uint32_t* lists = (uint32_t*)mt->ws_c.get(sizeof(uint32_t) * (size_t)n_total * 3 + 64, s);
     uint32_t* ctr = lists;  // [0] leaders [1] rest
@@ -1485,7 +1479,7 @@ void run_upsert(mono_mtable* mt, UpsertOp op, const CallSeg* h_segs, int nsegs,
     uint32_t* rest = bufA;
     int round = 0;
     while (n_pending > 0) {
-      MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(SetEntry) * (size_t)cap, s));
+      MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(FirstOcc) * (size_t)cap, s));
       MONO_CUDA(cudaMemsetAsync(ctr, 0, 64, s));
       dup_claim_kernel<<<grid_for(n_pending, kThreads), kThreads, 0, s>>>(
           cb.segs, nsegs, ids_dev, pending, n_pending, set, cap - 1, slot_of);
@@ -1531,8 +1525,7 @@ void run_upsert(mono_mtable* mt, UpsertOp op, const CallSeg* h_segs, int nsegs,
       launch_upsert_finalize(mt, cb, miss_ctr, (uint32_t)update_time, s);
     }
   }
-  for (size_t k = 0; k < per_table.size(); ++k)
-    if (per_table[k]) note_issued(mt, (int)k, per_table[k], update_time, s);
+  call.issued(mt, update_time, s);
 }
 
 
@@ -1551,14 +1544,8 @@ void run_upsert_groups(mono_mtable* mt, const CallSeg* h_segs, int nsegs, const 
   for (int i = 1; i < nsegs; ++i)
     if (h_segs[i].id_begin != h_segs[i - 1].id_end) throw ArgError("call segments must be contiguous");
   if (n_total >= (int64_t)1 << 31) throw ArgError("more than 2^31 ids in one call");
-  std::vector<uint64_t> per_table(mt->tables.size(), 0);
-  for (int i = 0; i < nsegs; ++i)
-    per_table[h_segs[i].table] += (uint64_t)(h_segs[i].id_end - h_segs[i].id_begin);
-  for (size_t k = 0; k < per_table.size(); ++k)
-    if (per_table[k]) ensure_capacity(mt, (int)k, per_table[k], s);
-  upload_tables(mt, s);
-  CallBlob cb = stage_call(mt, h_segs, nsegs, lr_host, n_lr, s);
-  const int G = pick_group(max_dim_of(mt, h_segs, nsegs));
+  const UpsertCall call(mt, h_segs, nsegs, lr_host, n_lr, s);
+  const CallBlob& cb = call.cb;
 
   if (n_total > ((int64_t)1 << 30)) throw ArgError("more than 2^30 ids in one grouped optimize call");
   const uint32_t cap = claim_set_slots(n_total);
@@ -1571,27 +1558,12 @@ void run_upsert_groups(mono_mtable* mt, const CallSeg* h_segs, int nsegs, const 
   uint32_t* followers = leaders + n_total;
   uint32_t* fol_leader = followers + n_total;
   uint32_t* slot_of = fol_leader + n_total;
-  SetEntry* set = (SetEntry*)mt->ws_a.get(sizeof(SetEntry) * (size_t)cap, s);
+  FirstOcc* set = (FirstOcc*)mt->ws_a.get(sizeof(FirstOcc) * (size_t)cap, s);
   MONO_CUDA(cudaMemsetAsync(ctr, 0, 64, s));
-  MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(SetEntry) * (size_t)cap, s));
+  MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(FirstOcc) * (size_t)cap, s));
 
-  UpsertArgs a;
-  a.tables = mt->d_tables;
-  a.segs = cb.segs;
-  a.nsegs = nsegs;
-  a.ids = ids_dev;
-  a.idx_list = nullptr;
-  a.n = n_total;
-  a.n_dev = nullptr;
-  a.vals = vals_dev;
-  a.lr = cb.lr;
-  a.update_ts = (uint32_t)update_time;
-  a.miss_ctr = ctr;
-  a.miss_list = miss_list;
-  a.rowidx = rowidx;
-  a.status = nullptr;
-  for (size_t k = 0; k < per_table.size(); ++k)
-    if (per_table[k] && mt->tables[k].dev.flt_cells) a.filter_mode = 1;
+  UpsertArgs a = upsert_args(mt, cb, nsegs, ids_dev, n_total, vals_dev, (uint32_t)update_time, ctr, miss_list, rowidx);
+  a.filter_mode = call.any_filter ? 1 : 0;
   resolve_hit_kernel<false><<<resident_grid(resolve_hit_kernel<false>, n_total, kThreads), kThreads, 0, s>>>(a);
   MONO_CHECK_LAUNCH();
   // misses are few in steady state: small grids, counts stay on the device
@@ -1615,10 +1587,9 @@ void run_upsert_groups(mono_mtable* mt, const CallSeg* h_segs, int nsegs, const 
     ag.pos0 = b;
     ag.n = e - b;
     ag.rowidx = rowidx + b;
-    launch_optimize_apply(G, ag, ag.n, s);
+    launch_optimize_apply(call.G, ag, ag.n, s);
   }
-  for (size_t k = 0; k < per_table.size(); ++k)
-    if (per_table[k]) note_issued(mt, (int)k, per_table[k], update_time, s);
+  call.issued(mt, update_time, s);
 }
 
 // Apply pass over one requester's segment of the owner-side window (device-driven sharded step): items are
@@ -1627,21 +1598,8 @@ void launch_apply_window(mono_mtable* mt, int k, const CallBlob& cb, const int64
                          int64_t pos0, const uint32_t* n_dev, int64_t n_upper, uint32_t* rowidx, uint32_t update_ts,
                          const uint64_t* wait_flag, uint64_t wait_seq, cudaStream_t s) {
   mt->note_insert(s);
-  UpsertArgs a;
-  a.tables = mt->d_tables;
-  a.segs = cb.segs;
-  a.nsegs = 1;
-  a.ids = ids_base;
-  a.idx_list = nullptr;
-  a.n = n_upper;
+  UpsertArgs a = upsert_args(mt, cb, 1, ids_base, n_upper, grads_base, update_ts, nullptr, nullptr, rowidx + pos0);
   a.n_dev = n_dev;
-  a.vals = grads_base;
-  a.lr = cb.lr;
-  a.update_ts = update_ts;
-  a.miss_ctr = nullptr;
-  a.miss_list = nullptr;
-  a.rowidx = rowidx + pos0;
-  a.status = nullptr;
   a.pos0 = pos0;
   a.wait_flag = wait_flag;
   a.wait_seq = wait_seq;
