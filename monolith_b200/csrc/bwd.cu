@@ -1121,9 +1121,8 @@ __global__ void __launch_bounds__(kThreads) runs_emit_kernel(BwdArgs a, int shif
 }
 
 
-// Claim set entry (16 B, viewed as Entry): key = FID, ts = epoch of the call that claimed it (any other value =
-// empty: the set is never cleared, engine.h ClaimSet), row = the FID's resolved table row (RESOLVE) or 0.
-// Claimed entries never change during the kernel, so every read may be served by L1 (plain ld.global): the hot
+// Claim set entry (epoch-versioned, common.cuh claim_epoch_slot): key = FID, row = the FID's resolved table row
+// (RESOLVE).  Claimed keys never change during the kernel, so every read may be served by L1 (plain ld.global): the hot
 // FIDs of a Zipf batch (8 % of the occurrences hit ONE slot) are answered per SM instead of serialising on one
 // L2 slice.  A stale L1 line can only show "empty" for a slot that has been claimed meanwhile; the CAS then
 // fails and returns the true entry.
@@ -1189,7 +1188,7 @@ fid_claim_kernel(const int64_t* __restrict__ fids, int64_t n, Entry* set, uint32
       key_next = __ldg(fids + i + stride);
       if (prefetch && !cr.regions) {
         const uint32_t o_n = N == 1 ? 0u : (uint32_t)((uint64_t)key_next % (uint64_t)N);
-        prefetch_l2(set + o_n * R + __umulhi((uint32_t)(mix64((uint64_t)key_next) >> 24), R));
+        prefetch_l2(set + o_n * R + epoch_slot(key_next, R));
         if (RESOLVE) {
           uint32_t b1, b2;
           bucket_pair(key_next, pf_nb, b1, b2);
@@ -1206,32 +1205,9 @@ fid_claim_kernel(const int64_t* __restrict__ fids, int64_t n, Entry* set, uint32
       R = rg.slots;
       tk = cr.t + rg.table;
     }
-    uint32_t idx = __umulhi((uint32_t)(mix64((uint64_t)key) >> 24), R);
-    uint32_t found = 0xFFFFFFFFu;
-    bool won = false;
-    for (uint32_t probes = 0; probes < R; ++probes) {
-      Entry* p = set + base + idx;
-      Entry e = ld_entry(p);  // L1-cacheable
-      while (e.ts != epoch) {  // empty as far as we can see: claim it (CAS against what we saw)
-        Entry ne;
-        ne.key = key;
-        ne.row = kEmptyRow;
-        ne.ts = epoch;
-        const Entry old = cas_entry_old(p, e, ne);
-        if (old.key == e.key && old.row == e.row && old.ts == e.ts) {
-          won = true;
-          e = ne;
-        } else {
-          e = old;  // somebody else changed it: the true entry (claimed this epoch, or a different stale one)
-        }
-      }
-      if (e.key == key) {
-        found = base + idx;
-        break;
-      }
-      idx = idx + 1 == R ? 0 : idx + 1;
-    }
-    if (found == 0xFFFFFFFFu) {  // region full (owner skew): the host retries with larger regions
+    bool won;
+    uint32_t found = claim_epoch_slot<ld_entry, true>(set, base, R, epoch_slot(key, R), key, epoch, &won);
+    if (found == kNoSlot) {  // region full (owner skew): the host retries with larger regions
       owner_cnt[256] = 1;
       found = base;
       won = false;
@@ -1256,8 +1232,8 @@ fid_claim_kernel(const int64_t* __restrict__ fids, int64_t n, Entry* set, uint32
     if (cnt[d]) atomicAdd(owner_cnt + d, cnt[d]);
 }
 
-// FIDs the claim found absent from the table (each exactly once): take a row (free list first, then the bump
-// allocator), publish {fid, row, ts} with the lock-free cuckoo insert and park row | fresh in the set entry.
+// FIDs the claim found absent from the table (each exactly once): take a row and publish {fid, row, ts}
+// (insert_new_row), and park row | fresh in the set entry.
 __global__ void __launch_bounds__(kThreads)
 claim_miss_kernel(const TableDev* __restrict__ tables, Entry* set, const uint32_t* __restrict__ miss_ctr,
                   const uint32_t* __restrict__ miss_slots, uint32_t update_ts,
@@ -1266,22 +1242,13 @@ claim_miss_kernel(const TableDev* __restrict__ tables, Entry* set, const uint32_
   for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x) {
     const uint32_t sl = miss_slots[q];
     const TableDev* t = regions ? tables + regions[call_table_of_slot(regions, n_regions, sl)].table : tables;
+    const int64_t key = ld_entry_cg(set + sl).key;
     // admission filter: the backward hands every distinct FID once per step (count 1), as the reference's
     // deduplicated optimize does; a FID below its slot's threshold gets no row (its run is skipped by the apply)
-    if (should_be_filtered(t, ld_entry_cg(set + sl).key, 1u)) continue;
-    const uint32_t ticket = atomicAdd(t->ctrs + kCtrMiss, 1u);
-    const uint32_t fc = t->ctrs[kCtrFree];  // stable during this kernel (finalize updates it)
-    const uint32_t row = ticket < fc ? t->free_list[fc - 1 - ticket] : t->ctrs[kCtrBump] + (ticket - fc);
-    if (row >= t->row_cap) {
-      atomicOr(t->ctrs + kCtrError, 2u);
-      continue;  // the set entry keeps kEmptyRow: the run is skipped by the apply pass
-    }
-    Entry e;
-    e.key = ld_entry_cg(set + sl).key;
-    e.row = row;
-    e.ts = update_ts;
-    cuckoo_insert(t, e);
-    set[sl].row = row | kFreshBit;
+    if (should_be_filtered(t, key, 1u)) continue;
+    const uint32_t row = insert_new_row(t, key, update_ts);
+    // row slab overflow: the set entry keeps kEmptyRow and the run is skipped by the apply pass
+    if (row != kEmptyRow) set[sl].row = row | kFreshBit;
   }
 }
 

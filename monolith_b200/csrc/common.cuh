@@ -494,6 +494,87 @@ __device__ __forceinline__ void cuckoo_insert(const TableDev* __restrict__ t, En
   placed();
 }
 
+// ---------------------------------------------------------------------------------------------
+// fresh rows: every inserter of an upsert call (resolve_miss_kernel, claim_miss_kernel, xmiss_insert_kernel) takes its
+// row here.  Ticket k of the call's kCtrMiss count takes the k-th row from the top of the free list, the tickets past
+// its end take the bump allocator's next rows in order.  kCtrFree and kCtrBump stay put during the call:
+// upsert_finalize_kernel (ops.cu), the other half of this protocol, folds the tickets into them after the call.
+// ---------------------------------------------------------------------------------------------
+// `key` is absent and admitted, and has exactly one inserter in the call.  Publishes {key, row, ts} with cuckoo_insert
+// and returns the row (kFreshBit clear), or kEmptyRow with error bit 2 when the row slab is full.
+__device__ __forceinline__ uint32_t insert_new_row(const TableDev* __restrict__ t, int64_t key, uint32_t ts) {
+  const uint32_t ticket = atomicAdd(t->ctrs + kCtrMiss, 1u);
+  const uint32_t fc = t->ctrs[kCtrFree];
+  const uint32_t row = ticket < fc ? t->free_list[fc - 1 - ticket] : t->ctrs[kCtrBump] + (ticket - fc);
+  if (row >= t->row_cap) {
+    atomicOr(t->ctrs + kCtrError, 2u);
+    return kEmptyRow;
+  }
+  Entry e;
+  e.key = key;
+  e.row = row;
+  e.ts = ts;
+  cuckoo_insert(t, e);
+  return row;
+}
+
+// ---------------------------------------------------------------------------------------------
+// epoch-versioned claim set (engine.h ClaimSet, which allocates it): entry key = FID, ts = epoch of the call that
+// claimed the slot (any other ts = empty, so the set is never cleared between calls), row = kEmptyRow at the claim,
+// then whatever the caller parks there.  A key's slot is found by linear probing from epoch_slot.
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t kNoSlot = 0xFFFFFFFFu;
+
+__device__ __forceinline__ uint32_t epoch_slot(int64_t key, uint32_t R) {
+  return __umulhi((uint32_t)(mix64((uint64_t)key) >> 24), R);
+}
+
+// Finds or claims the slot of `key` in the region set[base, base + R), probing linearly from set[base + start]; returns
+// its index in set.  BOUNDED gives up after R probes and returns kNoSlot; a caller whose region always has a free slot
+// passes false and keeps no probe count.  *won tells whether this thread's CAS claimed the slot (one thread per key and
+// call).  LOAD reads each slot first: a stale read only costs a failed CAS, which returns the true entry.
+template <Entry (*LOAD)(const Entry*), bool BOUNDED>
+__device__ __forceinline__ uint32_t claim_epoch_slot(Entry* set, uint32_t base, uint32_t R, uint32_t start, int64_t key,
+                                                     uint32_t epoch, bool* won) {
+  uint32_t idx = start;
+  *won = false;
+  for (uint32_t probes = 0; !BOUNDED || probes < R; ++probes) {
+    Entry* p = set + base + idx;
+    Entry e = LOAD(p);
+    while (e.ts != epoch) {  // empty as far as we can see: claim it (CAS against what we saw)
+      Entry ne;
+      ne.key = key;
+      ne.row = kEmptyRow;
+      ne.ts = epoch;
+      const Entry old = cas_entry_old(p, e, ne);
+      if (same_entry(old, e)) {
+        *won = true;
+        e = ne;
+      } else {
+        e = old;  // somebody else changed it: the true entry (claimed this epoch, or a different stale one)
+      }
+    }
+    if (e.key == key) return base + idx;
+    idx = idx + 1 == R ? 0 : idx + 1;
+  }
+  return kNoSlot;
+}
+
+// ---------------------------------------------------------------------------------------------
+// warp-aggregated append: every lane with `pred` set appends `value` to list, with one atomicAdd on *ctr per warp.
+// All 32 lanes of the warp must call it converged (full-mask ballot and shuffle).
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void warp_append(bool pred, uint32_t* ctr, uint32_t* list, uint32_t value) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t bal = __ballot_sync(0xffffffffu, pred);
+  if (bal) {
+    uint32_t base = 0;
+    if (lane == 0) base = atomicAdd(ctr, (uint32_t)__popc(bal));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (pred) list[base + __popc(bal & ((1u << lane) - 1u))] = value;
+  }
+}
+
 // Batched probe: U independent keys per lane group.  All U bucket loads are issued back to back
 // before the first ballot consumes one, so a group keeps U random 64-byte reads in flight instead
 // of one (the kernels are latency-bound on dependent HBM round trips, not on bytes).

@@ -155,6 +155,7 @@ struct DevBuf {
 // Scratch open-addressing set of the claim kernels, versioned by an epoch in every entry: an entry whose
 // epoch differs from the current call's is EMPTY, so the set is never cleared between calls (clearing 16 B
 // x 2 x occurrences is a full extra memset pass per step); it is zero-filled once per (re)allocation and when the epoch wraps.
+// The entry layout and the one claim loop: common.cuh claim_epoch_slot.
 struct ClaimSet {
   DevBuf buf;
   void* init_ptr = nullptr;

@@ -772,19 +772,12 @@ __global__ void __launch_bounds__(kThreads) resolve_hit_kernel(UpsertArgs a) {
         a.rowidx[j] = row;
       }
     }
-    const uint32_t mbal = __ballot_sync(0xffffffffu, miss);
-    if (mbal) {
-      uint32_t base = 0;
-      if (lane == 0) base = atomicAdd(a.miss_ctr, (uint32_t)__popc(mbal));
-      base = __shfl_sync(0xffffffffu, base, 0);
-      if (miss) a.miss_list[base + __popc(mbal & ((1u << lane) - 1u))] = (uint32_t)j;
-    }
+    warp_append(miss, a.miss_ctr, a.miss_list, (uint32_t)j);
   }
 }
 
-// Pass 2 — absent keys (unique within the call), thread per key: take a row (free list first, then
-// the bump allocator) and publish {fid, row, ts} with the lock-free cuckoo insert.  The row contents
-// are written by the apply pass (fresh bit set).
+// Pass 2 — absent keys (unique within the call), thread per key: take a row and publish {fid, row, ts}
+// (insert_new_row).  The row contents are written by the apply pass (fresh bit set).
 template <bool RESTORE>
 __global__ void __launch_bounds__(kThreads) resolve_miss_kernel(UpsertArgs a) {
   const int64_t n = (int64_t)*a.miss_ctr;
@@ -798,20 +791,8 @@ __global__ void __launch_bounds__(kThreads) resolve_miss_kernel(UpsertArgs a) {
       a.rowidx[j] = kEmptyRow;  // not admitted yet: no row, the apply pass skips it
       continue;
     }
-    const uint32_t ticket = atomicAdd(t->ctrs + kCtrMiss, 1u);
-    const uint32_t fc = t->ctrs[kCtrFree];  // stable during this kernel (finalize updates it)
-    const uint32_t row = ticket < fc ? t->free_list[fc - 1 - ticket] : t->ctrs[kCtrBump] + (ticket - fc);
-    if (row >= t->row_cap) {
-      atomicOr(t->ctrs + kCtrError, 2u);
-      a.rowidx[j] = kEmptyRow;
-      continue;
-    }
-    Entry e;
-    e.key = a.ids[i];
-    e.row = row;
-    e.ts = RESTORE ? restore_ts(a, sg, t, i) : a.update_ts;
-    cuckoo_insert(t, e);
-    a.rowidx[j] = row | kFreshBit;
+    const uint32_t row = insert_new_row(t, a.ids[i], RESTORE ? restore_ts(a, sg, t, i) : a.update_ts);
+    a.rowidx[j] = row == kEmptyRow ? row : row | kFreshBit;  // kEmptyRow: row slab overflow, the apply skips it
   }
 }
 

@@ -191,13 +191,7 @@ xowner_resolve_kernel(const TableDev* __restrict__ t, XWin w, int par, uint32_t 
           rowidx[src * w.C + i] = row;
         }
       }
-      const uint32_t mbal = __ballot_sync(0xffffffffu, miss);
-      if (mbal) {
-        uint32_t base = 0;
-        if (lane == 0) base = atomicAdd(miss_ctr, (uint32_t)__popc(mbal));
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (miss) miss_list[base + __popc(mbal & ((1u << lane) - 1u))] = (uint32_t)(src * w.C + i);
-      }
+      warp_append(miss, miss_ctr, miss_list, (uint32_t)(src * w.C + i));
     }
   }
 }
@@ -213,28 +207,17 @@ xmiss_claim_kernel(XWin w, int par, const uint32_t* __restrict__ miss_ctr, const
     const uint32_t pos = miss_list[q];
     const int src = (int)(pos / (uint64_t)w.C);
     const int64_t key = w.ids_in(w.me, par, src)[pos - (uint64_t)src * w.C];
-    uint32_t idx = __umulhi((uint32_t)(mix64((uint64_t)key) >> 24), cap);
-    while (true) {
-      Entry* p = set + idx;
-      Entry e = ld_entry_cg(p);
-      while (e.ts != epoch) {
-        Entry ne;
-        ne.key = key;
-        ne.row = kEmptyRow;
-        ne.ts = epoch;
-        const Entry old = cas_entry_old(p, e, ne);
-        if (old.key == e.key && old.row == e.row && old.ts == e.ts) e = ne; else e = old;
-      }
-      if (e.key == key) break;
-      idx = idx + 1 == cap ? 0 : idx + 1;
-    }
+    bool won;
+    // unbounded: cap = claim_set_slots(N * C) is at least twice the N * C items this owner can receive, so the probe
+    // always reaches the key's slot or a free one
+    const uint32_t idx = claim_epoch_slot<ld_entry_cg, false>(set, 0, cap, epoch_slot(key, cap), key, epoch, &won);
     slot_of[q] = idx;
     atomicMax(first + idx, ((unsigned long long)epoch << 32) | (unsigned long long)(~pos));
   }
 }
 
-// leaders (lowest position of a new FID = the first requester in rank order) insert: admission filter, row from the
-// free list / bump allocator, lock-free cuckoo insert; the row is parked in the set entry for the followers
+// leaders (lowest position of a new FID = the first requester in rank order) insert: admission filter, then
+// insert_new_row; the row is parked in the set entry for the followers
 __global__ void __launch_bounds__(kThreads)
 xmiss_insert_kernel(const TableDev* __restrict__ t, XWin w, int par, const uint32_t* __restrict__ miss_ctr,
                     const uint32_t* __restrict__ miss_list, Entry* set, const unsigned long long* __restrict__ first,
@@ -246,22 +229,7 @@ xmiss_insert_kernel(const TableDev* __restrict__ t, XWin w, int par, const uint3
     if ((uint32_t)(~first[sl]) != pos) continue;  // a follower
     const int src = (int)(pos / (uint64_t)w.C);
     const int64_t key = w.ids_in(w.me, par, src)[pos - (uint64_t)src * w.C];
-    uint32_t row = kEmptyRow;
-    if (!should_be_filtered(t, key, 1u)) {
-      const uint32_t ticket = atomicAdd(t->ctrs + kCtrMiss, 1u);
-      const uint32_t fc = t->ctrs[kCtrFree];
-      row = ticket < fc ? t->free_list[fc - 1 - ticket] : t->ctrs[kCtrBump] + (ticket - fc);
-      if (row >= t->row_cap) {
-        atomicOr(t->ctrs + kCtrError, 2u);
-        row = kEmptyRow;
-      } else {
-        Entry e;
-        e.key = key;
-        e.row = row;
-        e.ts = update_ts;
-        cuckoo_insert(t, e);
-      }
-    }
+    const uint32_t row = should_be_filtered(t, key, 1u) ? kEmptyRow : insert_new_row(t, key, update_ts);
     set[sl].row = row;
     rowidx[pos] = row == kEmptyRow ? row : (row | kFreshBit);
   }

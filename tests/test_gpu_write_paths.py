@@ -1,10 +1,11 @@
 """The table's write side against the CPU oracle, with the table's structure checked after every call.
 
-Every inserter (resolve_miss, claim_miss, xmiss_insert and rehash, all through common.cuh cuckoo_insert), growth,
-eviction, export and restore run on keys built (tests/cuckoo_place.py) to land where a case wants them: a free slot
-of the first bucket, the second bucket, a copy-first displacement that succeeds, closed bucket pairs of 9, 10 and 12
-keys written in one call (threads carry entries through the exchange chain and end in the stash), the keys -1, 0,
-INT64_MIN and INT64_MAX in full pairs, and stash keys hit again.  After every call `World.check` compares:
+Every inserter (resolve_miss, claim_miss and xmiss_insert, which take their rows from common.cuh insert_new_row, and
+rehash; all publish through common.cuh cuckoo_insert), growth, eviction, export and restore run on keys built
+(tests/cuckoo_place.py) to land where a case wants them: a free slot of the first bucket, the second bucket, a
+copy-first displacement that succeeds, closed bucket pairs of 9, 10 and 12 keys written in one call (threads carry
+entries through the exchange chain and end in the stash), the keys -1, 0, INT64_MIN and INT64_MAX in full pairs, and
+stash keys hit again.  After every call `World.check` compares:
   * lookup_entry of every key ever written, and of absent keys, with the oracle bit for bit (weights, state, found
     flag, timestamp);
   * the exported keys with the oracle's keys (no key twice), and each exported entry with its lookup_entry bits;

@@ -1,6 +1,7 @@
 """The rules tests/test_gpu_write_paths.py aims its cases at, pinned against the CUDA sources, and self-tests of the
 write-side key builders of tests/cuckoo_place.py.  A change to a constant, a counter, an error bit, the growth or
-eviction rule or the upsert kernel sequence fails here by name; the GPU cases then have to be re-aimed."""
+eviction rule, the row allocation, the scratch-set claim or the upsert kernel sequence fails here by name; the GPU
+cases then have to be re-aimed."""
 import os
 import re
 
@@ -29,6 +30,16 @@ def _body(src, head):
   raise AssertionError(f"unbalanced body after {head}")
 
 
+def _cu_sources():
+  return {f: _src(f) for f in sorted(os.listdir(CSRC)) if f.endswith(".cu")}
+
+
+# the three inserters of an upsert call, each of which takes its row from common.cuh insert_new_row
+INSERTERS = (("ops.cu", "resolve_miss_kernel("), ("bwd.cu", "claim_miss_kernel("), ("xstep.cu", "xmiss_insert_kernel("))
+# the two claims of the epoch-versioned scratch set (engine.h ClaimSet)
+EPOCH_CLAIMS = (("bwd.cu", "fid_claim_kernel("), ("xstep.cu", "xmiss_claim_kernel("))
+
+
 # counter words (common.cuh) as tests/test_gpu_write_paths.py and MultiHashTable.counters read them
 COUNTERS = {"bump": 0, "free": 1, "size": 2, "stash": 3, "error": 4, "moves": 8, "inflight": 9}
 ERROR_BITS = {1: "stash overflow", 2: "row slab overflow", 4: "lost a marked slot"}
@@ -44,7 +55,9 @@ def test_cuckoo_constants():
   assert "uint32_t s = (uint32_t)(mix64((uint64_t)e.key) >> 17) & mask;" in c and cp.STASH_SHIFT == 17
 
 
-def test_counter_words_and_error_bits():
+def test_counter_words_and_error_bits_with_one_row_allocator():
+  """The counter words and where each error bit is set; bit 2 (row slab overflow) is set in insert_new_row alone,
+  which every upsert inserter calls."""
   c = _src("common.cuh")
   for name, word in [("Bump", 0), ("Free", 1), ("Size", 2), ("Stash", 3), ("Error", 4), ("Moves", 8),
                      ("Inflight", 9)]:
@@ -55,8 +68,10 @@ def test_counter_words_and_error_bits():
   # where each bit is set: 1 when the stash is full, 2 when the row slab is, 4 when a marked slot was lost
   ins = _body(c, "__device__ __forceinline__ void cuckoo_insert(")
   assert "atomicOr(t->ctrs + kCtrError, 1u);" in ins and "if (copied) atomicOr(t->ctrs + kCtrError, 4u);" in ins
-  for f in ("ops.cu", "bwd.cu", "xstep.cu"):
-    assert "atomicOr(t->ctrs + kCtrError, 2u);" in _src(f), f
+  alloc = _body(c, "__device__ __forceinline__ uint32_t insert_new_row(")
+  assert "if (row >= t->row_cap) { atomicOr(t->ctrs + kCtrError, 2u); return kEmptyRow; }" in alloc
+  for f, head in INSERTERS:
+    assert "insert_new_row(t, " in _body(_src(f), head), f
   # the stash count rises before the entry is visible, and only on the stash path
   assert ins.count("atomicAdd(t->ctrs + kCtrStash, 1u);") == 1
 
@@ -124,9 +139,10 @@ def test_eviction_rule():
   assert "if (e.row >= kTombRow) continue;" in ex
 
 
-def test_upsert_ops_and_kernel_sequence():
+def test_upsert_ops_kernel_sequence_and_row_allocator():
   """The UpsertOp values are the second template argument of upsert_apply_kernel in the kernel names; one upsert
-  pass is resolve_hit, resolve_miss, upsert_apply (restore: the <true> resolves), then upsert_finalize."""
+  pass is resolve_hit, resolve_miss, upsert_apply (restore: the <true> resolves), then upsert_finalize; every
+  inserter takes its row from insert_new_row, whose tickets upsert_finalize folds."""
   e = _src("engine.h")
   assert "enum UpsertOp { kOpOptimize = 0, kOpAssign = 1, kOpAssignAdd = 2, kOpReinit = 3, kOpRestore = 4 };" in e
   ops = _src("ops.cu")
@@ -145,16 +161,39 @@ def test_upsert_ops_and_kernel_sequence():
   # finalize: both branches of the free-list fold
   fin = _body(ops, "__global__ void upsert_finalize_kernel(")
   assert "if (m <= fc) { t->ctrs[kCtrFree] = fc - m; } else { t->ctrs[kCtrFree] = 0; t->ctrs[kCtrBump] += m - fc; }" in fin
-  # a fresh row is taken from the top of the free list first, then from the bump allocator
-  for f, head in (("ops.cu", "resolve_miss_kernel("), ("bwd.cu", "claim_miss_kernel("),
-                  ("xstep.cu", "xmiss_insert_kernel(")):
-    b = _body(_src(f), head)
-    assert "ticket < fc ? t->free_list[fc - 1 - ticket] : t->ctrs[kCtrBump] + (ticket - fc)" in b, f
-    assert "cuckoo_insert(t, e);" in b, f
+  # a fresh row is taken from the top of the free list first, then from the bump allocator, in one place that every
+  # inserter calls; no other code takes a ticket that finalize folds
+  alloc = _body(_src("common.cuh"), "__device__ __forceinline__ uint32_t insert_new_row(")
+  assert "const uint32_t ticket = atomicAdd(t->ctrs + kCtrMiss, 1u);" in alloc
+  assert "ticket < fc ? t->free_list[fc - 1 - ticket] : t->ctrs[kCtrBump] + (ticket - fc)" in alloc
+  assert "cuckoo_insert(t, e);" in alloc
+  for f, head in INSERTERS:
+    assert "insert_new_row(t, " in _body(_src(f), head), f
+  for f, s in _cu_sources().items():
+    assert not re.search(r"atomicAdd\([^;]*kCtrMiss", s), f
   # the sharded step's insert pipeline
   xs = _src("xstep.cu")
   seq = re.findall(r"(xowner_resolve_kernel|xmiss_claim_kernel|xmiss_insert_kernel|xmiss_follow_kernel)<<<", xs)
   assert seq == ["xowner_resolve_kernel", "xmiss_claim_kernel", "xmiss_insert_kernel", "xmiss_follow_kernel"]
+
+
+def test_epoch_set_claim():
+  """Both claims of the epoch-versioned scratch set run common.cuh claim_epoch_slot from epoch_slot's start: a slot
+  whose epoch is not the call's is empty and is claimed with a CAS against what was read."""
+  c = _src("common.cuh")
+  assert "return __umulhi((uint32_t)(mix64((uint64_t)key) >> 24), R);" in _body(c, "uint32_t epoch_slot(")
+  claim = _body(c, "uint32_t claim_epoch_slot(")
+  assert "for (uint32_t probes = 0; !BOUNDED || probes < R; ++probes) {" in claim
+  assert "if (e.key == key) return base + idx;" in claim and claim.endswith("return kNoSlot; }")
+  assert "while (e.ts != epoch) {" in claim and "const Entry old = cas_entry_old(p, e, ne);" in claim
+  assert "if (same_entry(old, e)) { *won = true; e = ne; }" in claim
+  # the backward's claim reads through L1 and gives up on a full region; the sharded step's set always has room
+  for (f, head), targs in zip(EPOCH_CLAIMS, ("ld_entry, true", "ld_entry_cg, false")):
+    assert re.search(r"claim_epoch_slot<%s>\([^;]*epoch_slot\(key, " % targs, _body(_src(f), head)), f
+  # the claim kernel's prefetch aims at the same start slot
+  assert "prefetch_l2(set + o_n * R + epoch_slot(key_next, R));" in _body(_src("bwd.cu"), "fid_claim_kernel(")
+  for f, s in _cu_sources().items():
+    assert "cas_entry_old" not in s, f
 
 
 def test_pick_group():
