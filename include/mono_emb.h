@@ -357,6 +357,10 @@ int mono_mtable_evict(mono_mtable_t* t, int32_t k, int64_t max_update_time, void
 int mono_mtable_set_hash_filter(mono_mtable_t* t, int32_t k, int64_t capacity, uint32_t default_threshold,
                                 const uint32_t* slot_ids_host, const uint32_t* slot_thresholds_host,
                                 int32_t n_slots, void* stream);
+/* The filter's cells of table k, as they are: n = total + 64 uint16 cells (total = (uint64_t)(capacity * 1.5), at
+ * least 1; the 64 spill cells past total are where a probe window that starts near the end runs on), cell =
+ * 12-bit signature << 4 | 4-bit count, 0 = empty.  Errors when the table has no filter or n differs.  SYNC */
+int mono_mtable_hash_filter_cells(mono_mtable_t* t, int32_t k, uint16_t* out_host, int64_t n, void* stream);
 
 /* Full row access for checkpoint/restore and parity tests (ref: EntryDump,
  * embedding_hash_table.proto:45-50; LookupEntry, cuckoo_embedding_hash_table.cc:173-183).

@@ -97,6 +97,7 @@ SIGNATURES = {
     "mono_mtable_fused_offsets": (C.c_int, [_p, _p, _i32, _p, _p, _p]),
     "mono_mtable_fused_lookup": (C.c_int, [_p, _p, _p, _i32, _i64, _p, _p]),
     "mono_mtable_set_hash_filter": (C.c_int, [_p, _i32, _i64, _u32, _p, _p, _i32, _p]),
+    "mono_mtable_hash_filter_cells": (C.c_int, [_p, _i32, _p, _i64, _p]),
     "mono_mtable_contains": (C.c_int, [_p, _i32, _p, _i64, _p, _p]),
     "mono_mtable_lookup_pool": (C.c_int, [_p, _i32, _p, _p, _i64, _i32, _p, _i64, _i32, _p]),
     "mono_mtable_pool_backward": (C.c_int, [_p, _i32, _p, _i64, _p, _i64, _i32, _p, _i64, _i32, _p, _i64, _i64, _p]),

@@ -459,10 +459,17 @@ int mono_mtable_fused_optimize(mono_mtable_t* t, const int64_t* ids_dev,
               "id_offsets / grad_offsets do not match fused_slot_size");
     }
     int n_lr = 0;
-    for (auto& tb : t->tables) n_lr += tb.slices;
-    if ((flags & MONO_FLAG_IDS_UNIQUE) && !(flags & MONO_FLAG_DEDUP_SUM) && num_shards > 1) {
+    bool any_filter = false;
+    for (int k = 0; k < K; ++k) {
+      n_lr += t->tables[k].slices;
+      for (int s = 0; s < num_shards; ++s)
+        if (fused_slot_size_host[s * K + k] > 0 && t->tables[k].dev.flt_cells) any_filter = true;
+    }
+    if ((flags & MONO_FLAG_IDS_UNIQUE) && !(flags & MONO_FLAG_DEDUP_SUM) && num_shards > 1 && !any_filter) {
       // ids unique inside every shard: one resolve pass for the whole call, then the shards' rows are
-      // applied in shard order (same result as the loop below, without per-shard launch trains)
+      // applied in shard order, without per-shard launch trains.  The same rows and values as the loop below only
+      // without an admission filter: the loop hands a FID still absent at shard j to the filter once per shard (the
+      // reference's BatchOptimize per shard), the single resolve pass once per call.
       int64_t n_total = 0;
       auto segs = fused_segs(t, fused_slot_size_host, num_shards, 0, num_shards, &n_total);
       if (segs.empty()) return;
@@ -548,6 +555,19 @@ int mono_mtable_set_hash_filter(mono_mtable_t* t, int32_t k, int64_t capacity, u
     HandleGuard hg_(t);
     table_set_filter(t, k, (uint64_t)capacity, default_threshold, slot_ids_host, slot_thresholds_host, n_slots,
                      (cudaStream_t)stream);
+  });
+}
+
+int mono_mtable_hash_filter_cells(mono_mtable_t* t, int32_t k, uint16_t* out_host, int64_t n, void* stream) {
+  return guarded([&] {
+    require(t != nullptr && k >= 0 && k < (int)t->tables.size(), "bad table index");
+    HandleGuard hg_(t);
+    const TableDev& d = t->tables[k].dev;
+    require(d.flt_cells != nullptr, "hash_filter_cells: the table has no hash filter");
+    require(out_host != nullptr && n == (int64_t)d.flt_total + 64, "hash_filter_cells: n must be the filter's total + 64");
+    MONO_CUDA(cudaMemcpyAsync(out_host, d.flt_cells, sizeof(uint16_t) * (size_t)n, cudaMemcpyDeviceToHost,
+                              (cudaStream_t)stream));
+    MONO_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
   });
 }
 

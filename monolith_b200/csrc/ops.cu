@@ -734,6 +734,8 @@ struct UpsertArgs {
   // has no Contains check, tf_bridge.cc:224-232)
   int filter_mode = 0;
   const uint32_t* occ_extra = nullptr;  // dedup path: occurrences of id position i beyond the first (count = 1 + occ_extra[i])
+  // duplicate rounds with filter_mode 1: absent0[i] = id position i was absent from the table at call start
+  const uint8_t* absent0 = nullptr;
   // apply pass of the device-driven sharded step: do not start before *wait_flag >= wait_seq (the requester's
   // gradient rows have landed in this rank's window; acquire at system scope)
   const uint64_t* wait_flag = nullptr;
@@ -768,6 +770,9 @@ __global__ void __launch_bounds__(kThreads) resolve_hit_kernel(UpsertArgs a) {
       } else if (a.filter_mode == 2 && should_be_filtered(t, a.ids[i], 1)) {
         a.rowidx[j] = kEmptyRow;  // AssignAdd2: filtered although present — the op is skipped for this id
       } else {
+        // an id absent at call start adds 1 per occurrence, also once an earlier round has admitted it: the reference
+        // filters the whole id list before it writes a row (tf_bridge.cc:179-190, 312-326).  It stays admitted.
+        if (a.absent0 && a.absent0[i]) (void)should_be_filtered(t, a.ids[i], 1);
         slot->ts = RESTORE ? restore_ts(a, sg, t, i) : a.update_ts;
         a.rowidx[j] = row;
       }
@@ -793,6 +798,15 @@ __global__ void __launch_bounds__(kThreads) resolve_miss_kernel(UpsertArgs a) {
     }
     const uint32_t row = insert_new_row(t, a.ids[i], RESTORE ? restore_ts(a, sg, t, i) : a.update_ts);
     a.rowidx[j] = row == kEmptyRow ? row : row | kFreshBit;  // kEmptyRow: row slab overflow, the apply skips it
+  }
+}
+
+// Before the duplicate rounds of a filtered optimize / assign: which id positions are absent from the table.
+__global__ void __launch_bounds__(kThreads) absent_at_start_kernel(UpsertArgs a, uint8_t* __restrict__ absent0) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * blockDim.x) {
+    const CallSeg sg = a.segs[a.nsegs > 1 ? find_seg(a.segs, a.nsegs, i) : 0];
+    Entry* slot;
+    absent0[i] = probe_lane_slot(a.tables + sg.table, a.ids[i], &slot) == kEmptyRow;
   }
 }
 
@@ -1454,6 +1468,11 @@ void run_upsert(mono_mtable* mt, UpsertOp op, const CallSeg* h_segs, int nsegs,
         occ_extra = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(acc) + ((sizeof(float) * val_floats + 255) & ~(size_t)255));
         MONO_CUDA(cudaMemsetAsync(occ_extra, 0, 4 * (size_t)n_total, s));
       }
+    } else if (a.filter_mode == 1) {
+      uint8_t* absent0 = (uint8_t*)mt->ws_d.get((size_t)n_total, s);
+      absent_at_start_kernel<<<grid_for(n_total, kThreads), kThreads, 0, s>>>(a, absent0);
+      MONO_CHECK_LAUNCH();
+      a.absent0 = absent0;
     }
     const uint32_t* pending = nullptr;
     int64_t n_pending = n_total;

@@ -370,6 +370,11 @@ void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride
                     const int32_t* row_offsets, int pooling, const float* lr_host, int64_t update_time, cudaStream_t s) {
   MONO_CUDA(cudaSetDevice(x->mt->device));
   if (!x->fwd_done) throw ArgError("xstep_backward without a forward");
+  // the owner's insert hands a new FID to the filter once per step (its leader), where the reference counts it once
+  // per requesting rank; until each source gets its own ordered filter pass, a filtered table trains at world 1 only.
+  // Thrown before anything is pushed, on every rank alike (the tables are configured alike).
+  if (x->N > 1 && x->mt->tables[x->k].dev.flt_cells)
+    throw ArgError("xstep_backward: a table with a hash filter needs world 1 (per-rank filter counts are not kept)");
   x->fwd_done = false;
   mono_mtable* mt = x->mt;
   mt->note_insert(s);

@@ -90,6 +90,7 @@ class MultiHashTable:
     self._table_names: Tuple[str, ...] = tuple(sorted(configs.keys()))
     self._configs = {k: configs[k] for k in self._table_names}
     self._dims = tuple(self._configs[k].table_config.dim_size for k in self._table_names)
+    self._filter_cells: Dict[str, int] = {}  # cell count of each table's admission filter
     self._shared_name = "_".join([MultiHashTable.NAME_PREFIX, name_suffix])
     arr, keep = to_c_table_cfgs(self._configs)
     h = C.c_void_p()
@@ -502,7 +503,21 @@ class MultiHashTable:
     vs = (C.c_uint32 * max(len(st), 1))(*[int(x) for x in st.values()])
     _lib.check(self._lib.mono_mtable_set_hash_filter(self._h, k, int(capacity), int(default_threshold), ks, vs, len(st),
                                                      _stream(self._device)))
+    self._filter_cells[slot] = max(int(int(capacity) * 1.5), 1) + 64
     return self
+
+  def hash_filter_cells(self, slot: str):
+    """The admission filter's cells of table `slot` as a numpy uint16 array (mono_mtable_hash_filter_cells): total +
+    64 cells, total = int(capacity * 1.5) (at least 1), cell = 12-bit signature << 4 | 4-bit count.  Synchronises."""
+    import numpy as np
+    k = self._table_names.index(slot)
+    n = self._filter_cells.get(slot)
+    if n is None:
+      raise ValueError(f"table '{slot}' has no hash filter")
+    out = np.zeros(n, np.uint16)
+    _lib.check(self._lib.mono_mtable_hash_filter_cells(self._h, k, out.ctypes.data_as(C.c_void_p), n,
+                                                       _stream(self._device)))
+    return out
 
   def contains(self, slot: str, ids: torch.Tensor) -> torch.Tensor:
     ids = _ids(ids, self._device)

@@ -312,8 +312,11 @@ struct Table {
     const uint32_t slot = (uint32_t)(((uint64_t)fid >> 48) & 0x7FFF);
     auto it = slot_threshold.find(slot);
     const uint32_t thr = it == slot_threshold.end() ? default_threshold : it->second;
+    return FilterAtThreshold(filter.get(), fid, count, thr);
+  }
+  static bool FilterAtThreshold(HashFilter* f, int64_t fid, uint32_t count, uint32_t thr) {
     if (thr == 0) return false;
-    return filter->Add(fid, count) < thr;
+    return f->Add(fid, count) < thr;
   }
 
   // ref: EntryAccessor::Init (entry_accessor.cc:165-169): initializer then optimizer Init.
@@ -664,16 +667,43 @@ int orc_mtable_assign(orc_mtable* t, const int64_t* ids, const int64_t* id_split
   for (size_t k = 0; k < t->tables.size(); ++k) {
     Table& tb = t->tables[k];
     tb.BumpMaxTs(update_time);
-    for (int64_t i = id_split[k]; i < id_split[k + 1]; ++i) {
-      const float* v = values + voff;
-      voff += tb.dim;
-      if (!tb.m.count(ids[i]) && tb.ShouldBeFiltered(ids[i], 1)) continue;  // tf_bridge.cc:181-185
+    // tf_bridge.cc:179-190: the whole id list is filtered FIRST (Contains sees the table as it was before this call,
+    // each absent occurrence adds 1 to its counter), then the survivors are assigned in order
+    std::vector<int64_t> kept;
+    for (int64_t i = id_split[k]; i < id_split[k + 1]; ++i)
+      if (tb.m.count(ids[i]) || !tb.ShouldBeFiltered(ids[i], 1)) kept.push_back(i);
+    for (int64_t i : kept) {
+      const float* v = values + voff + (i - id_split[k]) * tb.dim;
       tb.Upsert(ids[i], [&](Row* r) {
         r->ts = (uint32_t)update_time;
         std::memcpy(r->data.data(), v, sizeof(float) * tb.dim);  // entry_accessor.cc:175-179
       });
     }
+    voff += (id_split[k + 1] - id_split[k]) * tb.dim;
   }
+  return 0;
+}
+
+// The [total + 64] cells of table k's filter (1 when the table has none or n is not its cell count).
+int orc_mtable_hash_filter_cells(const orc_mtable* t, int32_t k, uint16_t* out, int64_t n) {
+  if (k < 0 || k >= (int)t->tables.size()) return 1;
+  const auto& f = t->tables[k].filter;
+  if (!f || n != (int64_t)f->map.size()) return 1;
+  std::memcpy(out, f->map.data(), sizeof(uint16_t) * (size_t)n);
+  return 0;
+}
+
+// One HashFilter of `capacity` on its own, fed fids[i] in order: thresholds null -> out[i] = add(fids[i], counts[i])
+// (the count before the add); else out[i] = ShouldBeFiltered(fids[i], counts[i], thresholds[i]) (0 never adds).
+// cells [n_cells = total + 64] receive the final state.
+int orc_hash_filter_run(int64_t capacity, const int64_t* fids, const uint32_t* counts, const uint32_t* thresholds,
+                        int64_t n, uint32_t* out, uint16_t* cells, int64_t n_cells) {
+  HashFilter f((uint64_t)capacity);
+  if (n_cells != (int64_t)f.map.size()) return 1;
+  for (int64_t i = 0; i < n; ++i)
+    out[i] = thresholds ? (uint32_t)Table::FilterAtThreshold(&f, fids[i], counts[i], thresholds[i])
+                        : f.Add(fids[i], counts[i]);
+  std::memcpy(cells, f.map.data(), sizeof(uint16_t) * (size_t)n_cells);
   return 0;
 }
 

@@ -69,6 +69,14 @@ class OracleMultiHashTable:
     vs = np.ascontiguousarray(np.array(list(st.values()), np.uint32))
     assert lib().orc_mtable_set_hash_filter(self.h, self.names.index(slot), C.c_int64(capacity),
                                             C.c_uint32(default_threshold), p(ks), p(vs), len(st)) == 0
+    self.filter_cells = getattr(self, "filter_cells", {})
+    self.filter_cells[slot] = max(int(int(capacity) * 1.5), 1) + 64
+
+  def hash_filter_cells(self, slot):
+    """The [total + 64] uint16 cells of the filter of table `slot`."""
+    out = np.zeros(self.filter_cells[slot], np.uint16)
+    assert lib().orc_mtable_hash_filter_cells(self.h, self.names.index(slot), p(out), C.c_int64(out.size)) == 0
+    return out
 
   def lrs(self):
     out = []
@@ -190,6 +198,20 @@ class OracleMultiHashTable:
     lib().orc_mtable_lookup_pool(self.h, k, p(fids), p(ro), C.c_int64(n_rows), {"sum": 0, "mean": 1}[pooling],
                                  p(out), C.c_int64(self.dims[k]), 0)
     return out
+
+
+def hash_filter_run(capacity, fids, counts, thresholds=None):
+  """One oracle HashFilter of `capacity` fed fids[i] with counts[i] in order -> (per add: the count before it, or with
+  thresholds: 1 where ShouldBeFiltered said filtered; the final [total + 64] cells)."""
+  fids = i64(fids)
+  counts = np.ascontiguousarray(np.broadcast_to(np.asarray(counts, np.uint32), fids.shape))
+  thr = None if thresholds is None else np.ascontiguousarray(
+      np.broadcast_to(np.asarray(thresholds, np.uint32), fids.shape))
+  out = np.zeros(max(fids.size, 1), np.uint32)
+  cells = np.zeros(max(int(int(capacity) * 1.5), 1) + 64, np.uint16)
+  assert lib().orc_hash_filter_run(C.c_int64(capacity), p(fids), p(counts), p(thr), C.c_int64(fids.size), p(out),
+                                   p(cells), C.c_int64(cells.size)) == 0
+  return out[:fids.size], cells
 
 
 def reorder_by_indices(inputs, N, dims, rank0_empty=False):

@@ -119,7 +119,7 @@ def _fast_cfg():
   return {"t": table([(16, "adagrad", {})], [0.1])}
 
 
-def _fast_worker(rank, world, port, q, exchange="peer"):
+def _fast_worker(rank, world, port, q, exchange="peer", filtered=False):
   try:
     sys.path.insert(0, ROOT)
     import torch.distributed as dist
@@ -131,6 +131,8 @@ def _fast_worker(rank, world, port, q, exchange="peer"):
     from monolith_b200 import MultiHashTable
     from monolith_b200.distributed_ps import ShardedStep
     table = MultiHashTable(_fast_cfg(), device=dev)
+    if filtered:
+      table.set_hash_filter("t", 2_000_000, 2)
     if exchange.startswith("peer-"):
       os.environ["MONO_PEER_BULK"] = exchange.split("-")[1]
       exchange = "peer"
@@ -140,6 +142,18 @@ def _fast_worker(rank, world, port, q, exchange="peer"):
     for step in range(3):
       fids, g = _fast_batch(rank, step)
       out = torch.empty(fids.size, 16, device=dev)
+      if filtered and exchange == "direct":   # refused before anything is pushed, on both ranks
+        try:
+          st.step(devb[step], torch.from_numpy(g).to(dev), out, 20 + step)
+        except RuntimeError as e:
+          assert "hash filter needs world 1" in str(e), e
+          torch.cuda.synchronize()
+          q.put((rank, "REFUSED", None))
+          dist.barrier()
+          st.close_direct()
+          dist.destroy_process_group()
+          return
+        raise AssertionError("a filtered table's direct step at world 2 was not refused")
       st.step(devb[step], torch.from_numpy(g).to(dev), out, 20 + step)
       if exchange == "direct" and step + 1 < 3:
         st.prepare(devb[step + 1])          # next batch's grouping on a side stream, under this step's exchange
@@ -164,6 +178,18 @@ def _fast_worker(rank, world, port, q, exchange="peer"):
 def test_sharded_fast_step_two_gpus(exchange):
   """ShardedStep on 2 GPUs == one global oracle table; exchange over NVLink peer windows (bulk data pulled
   by the consumer, or pushed by the fused lookup+send / reduce+send kernels; flag barriers) and over NCCL."""
+  _fast_step_two_gpus(exchange, False)
+
+
+@pytest.mark.parametrize("exchange", ["direct", "peer-pull", "nccl"])
+def test_sharded_fast_step_two_gpus_filtered(exchange):
+  """The same with an admission filter of threshold 2 on every rank: the owners apply each requester's rows as one
+  optimize, so the filter counts a new FID once per requester, as the global table does; the direct exchange refuses
+  the backward (its owner insert would count a new FID once per step)."""
+  _fast_step_two_gpus(exchange, True)
+
+
+def _fast_step_two_gpus(exchange, filtered):
   if torch.cuda.device_count() < 2:
     pytest.skip("needs 2 GPUs")
   import torch.multiprocessing as mp
@@ -171,8 +197,8 @@ def test_sharded_fast_step_two_gpus(exchange):
   world = 2
   ctx = mp.get_context("spawn")
   q = ctx.Queue()
-  port = 29900 + (os.getpid() % 90) + {"peer-pull": 0, "peer-push": 3, "nccl": 7, "direct": 11}[exchange]
-  procs = [ctx.Process(target=_fast_worker, args=(r, world, port, q, exchange)) for r in range(world)]
+  port = 29900 + (os.getpid() % 90) + {"peer-pull": 0, "peer-push": 3, "nccl": 7, "direct": 11}[exchange] + 13 * filtered
+  procs = [ctx.Process(target=_fast_worker, args=(r, world, port, q, exchange, filtered)) for r in range(world)]
   for p in procs:
     p.start()
   got = [q.get(timeout=240) for _ in range(world)]
@@ -181,7 +207,12 @@ def test_sharded_fast_step_two_gpus(exchange):
   got = sorted(got, key=lambda x: x[0])
   for p in procs:
     p.join(timeout=60)
+  if filtered and exchange == "direct":
+    assert [g[1] for g in got] == ["REFUSED"] * world
+    return
   glob = orc.OracleMultiHashTable(_fast_cfg())
+  if filtered:
+    glob.set_hash_filter("t", 2_000_000, 2)
   for step in range(3):
     batches = [_fast_batch(r, step) for r in range(world)]
     for r, (fids, g) in enumerate(batches):
