@@ -28,18 +28,30 @@ namespace mono {
 
 // ==========================================================================================
 // Stable LSD radix sort of (key, position), 11 bits per pass.
-// Items travel as uint2 {key, position} (ONE 8-byte scattered store per item and pass); the first pass reads the
-// bare keys (position = index).  Per pass: tile histograms (shared-memory atomics) -> column scan over the tiles
-// -> stable scatter.  The scatter kernel ranks an item among the equal digits in front of it inside its tile
-// with ballots (11 votes give the lane mask of equal digits; lanes are consecutive positions, so the count of
-// lower lanes is the stable rank; one MATCH.ANY instead of the 11 votes measured slower over the two passes) and per-warp digit counters in shared memory; tiles are ordered by the scanned
-// histograms, so no atomic ever decides an output position.
+// Items travel as uint2 {key, position}; the first pass reads the bare keys (position = index).  Per pass: tile
+// histograms (shared-memory atomics) -> column scan over the tiles -> stable scatter.  The scatter kernel ranks an
+// item among the equal digits in front of it inside its tile with ballots (11 votes give the lane mask of equal
+// digits; lanes are consecutive positions, so the count of lower lanes is the stable rank; one MATCH.ANY instead of
+// the 11 votes measured slower over the two passes) and per-warp digit counters in shared memory; tiles are ordered
+// by the scanned histograms, so no atomic ever decides an output position.  The scatter copies its tile into shared
+// memory before ranking (kept in registers through the ranking rounds, ptxas issues the loads one per round), then
+// writes the tile in digit order into a second buffer and stores it from there: consecutive threads write consecutive
+// addresses of a digit's run (~4 items, 32 bytes, per digit and 8192-item tile) instead of one partly written sector
+// per item.
 // ==========================================================================================
 constexpr int kRadixBits = 11;
 constexpr int kRadixBins = 1 << kRadixBits;
-constexpr int kRadixIPT = 16;                         // items per thread
-constexpr int kRadixTile = kThreads * kRadixIPT;      // 4096 items per block iteration
-constexpr int kRadixWarps = kThreads / 32;
+constexpr int kRadixThreads = 512;                       // hist and scatter blocks
+constexpr int kRadixIPT = 16;                            // items per thread
+constexpr int kRadixTile = kRadixThreads * kRadixIPT;    // 8192 items per block iteration
+constexpr int kRadixWarps = kRadixThreads / 32;
+static_assert(kRadixBins == 4 * kRadixThreads, "a scatter thread scans the counters of 4 digits, one uint2");
+static_assert(kRadixTile < 65536, "tile-local positions live in the uint16 digit counters");
+// scatter shared memory: the tile in input order; the per-warp digit counters, whose bytes then take the tile in
+// digit order; per digit its global start and its output offset in the current tile; the warp sums of the block scans
+constexpr size_t kRadixStageBytes = sizeof(uint2) * kRadixTile;
+static_assert(sizeof(uint16_t) * kRadixWarps * kRadixBins <= kRadixStageBytes, "the counters fit the stage");
+constexpr size_t kRadixSmem = 2 * kRadixStageBytes + sizeof(uint32_t) * (2 * kRadixBins + kRadixWarps);
 
 template <bool FIRST>
 __device__ __forceinline__ uint2 radix_load(const void* __restrict__ in, int64_t i, int pre_shift) {
@@ -48,21 +60,21 @@ __device__ __forceinline__ uint2 radix_load(const void* __restrict__ in, int64_t
 }
 
 template <bool FIRST>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kRadixThreads)
 radix_hist_kernel(const void* __restrict__ in, int64_t n, int shift, int pre_shift, uint32_t* __restrict__ cnt /*[nblk][2048]*/,
                   int nblk) {
   __shared__ uint32_t h[kRadixBins];
   for (int blk = blockIdx.x; blk < nblk; blk += gridDim.x) {
-    for (int d = threadIdx.x; d < kRadixBins; d += kThreads) h[d] = 0;
+    for (int d = threadIdx.x; d < kRadixBins; d += kRadixThreads) h[d] = 0;
     __syncthreads();
     const int64_t base = (int64_t)blk * kRadixTile;
 #pragma unroll
     for (int r = 0; r < kRadixIPT; ++r) {
-      const int64_t i = base + r * kThreads + threadIdx.x;
+      const int64_t i = base + r * kRadixThreads + threadIdx.x;
       if (i < n) atomicAdd(&h[(radix_load<FIRST>(in, i, pre_shift).x >> shift) & (kRadixBins - 1)], 1u);
     }
     __syncthreads();
-    for (int d = threadIdx.x; d < kRadixBins; d += kThreads) cnt[(size_t)blk * kRadixBins + d] = h[d];
+    for (int d = threadIdx.x; d < kRadixBins; d += kRadixThreads) cnt[(size_t)blk * kRadixBins + d] = h[d];
     __syncthreads();
   }
 }
@@ -98,60 +110,74 @@ radix_colscan_kernel(uint32_t* __restrict__ cnt, int nblk, uint32_t* __restrict_
   }
 }
 
+// exclusive prefix of v over the scatter block's threads in thread order (wsum[kRadixWarps] is free again on return)
+__device__ __forceinline__ uint32_t radix_block_scan(uint32_t v, uint32_t* wsum) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  uint32_t x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) wsum[w] = x;
+  __syncthreads();
+  uint32_t off = 0;
+#pragma unroll
+  for (int ww = 0; ww < kRadixWarps; ++ww)
+    if (ww < w) off += wsum[ww];
+  __syncthreads();
+  return off + x - v;
+}
+
+// Thread t owns the digits 4t .. 4t+3 in the scans; their uint16 counters travel as one uint2 (two per word, every
+// sum below 65536: no carry crosses a half).
 template <bool FIRST>
-__global__ void __launch_bounds__(kThreads, 4)
+__global__ void __launch_bounds__(kRadixThreads, 1)
 radix_scatter_kernel(const void* __restrict__ in, int64_t n, int shift, int pre_shift,
                      const uint32_t* __restrict__ goff /*[nblk][2048] scanned*/, const uint32_t* __restrict__ dtot,
                      int nblk, uint2* __restrict__ out) {
-  __shared__ uint16_t wc[kRadixWarps][kRadixBins];   // per-warp digit counters, then exclusive warp offsets
-  __shared__ uint32_t bbase[kRadixBins];             // global offset of (tile, digit)
-  __shared__ uint32_t wsum[kRadixWarps];
+  extern __shared__ __align__(16) unsigned char radix_smem[];
+  uint2* items = reinterpret_cast<uint2*>(radix_smem);                                // the tile in input order
+  uint16_t(*wc)[kRadixBins] = reinterpret_cast<uint16_t(*)[kRadixBins]>(radix_smem + kRadixStageBytes);
+  uint2* wc4 = reinterpret_cast<uint2*>(wc);                                          // per-warp digit counters, 4 per uint2
+  uint2* stage = reinterpret_cast<uint2*>(wc);                                        // then the tile in digit order
+  uint4* dbase = reinterpret_cast<uint4*>(radix_smem + 2 * kRadixStageBytes);         // global start of digits 4t .. 4t+3
+  uint4* gdelta = dbase + kRadixThreads;                                              // output index - stage index, same
+  uint32_t* wsum = reinterpret_cast<uint32_t*>(gdelta + kRadixThreads);
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const uint32_t lt = (1u << lane) - 1u;
-  // exclusive scan of the 2048 digit totals; thread t keeps the bases of its digits q * 256 + t in registers
-  uint32_t dbase[kRadixBins / kThreads];
-  {
-    uint32_t carry = 0;
-#pragma unroll
-    for (int q = 0; q < kRadixBins / kThreads; ++q) {
-      const uint32_t v = dtot[q * kThreads + threadIdx.x];
-      uint32_t x = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-      }
-      if (lane == 31) wsum[w] = x;
-      __syncthreads();
-      uint32_t off = 0, tot = 0;
-#pragma unroll
-      for (int ww = 0; ww < kRadixWarps; ++ww) {
-        const uint32_t t = wsum[ww];
-        if (ww < w) off += t;
-        tot += t;
-      }
-      dbase[q] = carry + off + x - v;
-      carry += tot;
-      __syncthreads();
-    }
+  {  // exclusive scan of the digit totals
+    const uint4 v = reinterpret_cast<const uint4*>(dtot)[threadIdx.x];
+    const uint32_t off = radix_block_scan(v.x + v.y + v.z + v.w, wsum);
+    dbase[threadIdx.x] = make_uint4(off, off + v.x, off + v.x + v.y, off + v.x + v.y + v.z);
   }
   for (int blk = blockIdx.x; blk < nblk; blk += gridDim.x) {
-    uint32_t* wz = reinterpret_cast<uint32_t*>(&wc[0][0]);
-    for (int q = threadIdx.x; q < kRadixWarps * kRadixBins / 2; q += kThreads) wz[q] = 0;
+    const int64_t tbeg = (int64_t)blk * kRadixTile;
+    const int tn = (int)(n - tbeg < kRadixTile ? n - tbeg : kRadixTile);
+    // ---- the tile into shared memory (16 loads in flight per thread), the counters to zero ----
+    {
+      uint2 v[kRadixIPT];   // FIRST: the raw key (shifted once all loads are issued) and the index
+#pragma unroll
+      for (int r = 0; r < kRadixIPT; ++r) {
+        const int64_t i = tbeg + r * kRadixThreads + threadIdx.x;
+        if (FIRST) v[r] = make_uint2(i < n ? static_cast<const uint32_t*>(in)[i] : 0u, (uint32_t)i);
+        else v[r] = i < n ? static_cast<const uint2*>(in)[i] : make_uint2(0u, 0u);
+      }
+#pragma unroll
+      for (int r = 0; r < kRadixIPT; ++r)
+        items[r * kRadixThreads + threadIdx.x] = make_uint2(FIRST ? v[r].x >> pre_shift : v[r].x, v[r].y);
+    }
+    for (int q = threadIdx.x; q < kRadixWarps * kRadixBins / 4; q += kRadixThreads) wc4[q] = make_uint2(0u, 0u);
     __syncthreads();
-    // ---- phase 1: stable rank of every item among the equal digits of its warp's 512-item slice ----
-    const int64_t wbeg = (int64_t)blk * kRadixTile + (int64_t)w * (kRadixTile / kRadixWarps);
-    uint32_t dgv[kRadixIPT];   // all 16 digits first: 16 independent loads in flight (0xFFFFFFFF = past the end)
+    // ---- stable rank of every item among the equal digits of its warp's 512-item slice ----
+    const int wb = w * (kRadixTile / kRadixWarps);   // round r holds the slice's items wb + r * 32 + lane < tn
+    uint32_t rk[kRadixIPT];                          // digit | rank, then the item's index in the staged tile
 #pragma unroll
     for (int r = 0; r < kRadixIPT; ++r) {
-      const int64_t i = wbeg + r * 32 + lane;
-      dgv[r] = i < n ? (radix_load<FIRST>(in, i, pre_shift).x >> shift) & (kRadixBins - 1) : 0xFFFFFFFFu;
-    }
-#pragma unroll
-    for (int r = 0; r < kRadixIPT; ++r) {  // afterwards dgv[r] = digit | rank << 16 (rank < 1024)
-      const bool valid = dgv[r] != 0xFFFFFFFFu;
-      const uint32_t dg = valid ? dgv[r] : 0u;
-      uint32_t peers = __ballot_sync(0xffffffffu, valid);
+      const int m = tn - (wb + r * 32);   // the valid lanes of the round are its lowest m
+      const bool valid = lane < m;
+      const uint32_t dg = valid ? (items[wb + r * 32 + lane].x >> shift) & (kRadixBins - 1) : 0u;
+      uint32_t peers = m >= 32 ? 0xffffffffu : m > 0 ? (1u << m) - 1u : 0u;
 #pragma unroll
       for (int b = 0; b < kRadixBits; ++b) {
         const uint32_t bal = __ballot_sync(0xffffffffu, (dg >> b) & 1u);
@@ -164,41 +190,52 @@ radix_scatter_kernel(const void* __restrict__ in, int64_t n, int shift, int pre_
         wc[w][dg] = (uint16_t)(old + __popc(peers));
       }
       old = __shfl_sync(0xffffffffu, old, max(leader, 0));
-      if (valid) dgv[r] = dg | ((old + __popc(peers & lt)) << 16);
+      rk[r] = dg | (old + __popc(peers & lt)) << 16;   // rank < 512
       __syncwarp();
     }
     __syncthreads();
-    // ---- warp offsets per digit and the tile's global digit offsets ----
+    // ---- per digit: exclusive warp offsets, plus the digit's start in the staged tile; the output offsets ----
+    uint2 run = make_uint2(0u, 0u);
+#pragma unroll 4
+    for (int ww = 0; ww < kRadixWarps; ++ww) {
+      const uint2 v = wc4[ww * (kRadixBins / 4) + threadIdx.x];
+      wc4[ww * (kRadixBins / 4) + threadIdx.x] = run;
+      run.x += v.x;
+      run.y += v.y;
+    }
+    const uint32_t c0 = run.x & 0xffffu, c1 = run.x >> 16, c2 = run.y & 0xffffu;
+    uint32_t ts[4];
+    ts[0] = radix_block_scan(c0 + c1 + c2 + (run.y >> 16), wsum);
+    ts[1] = ts[0] + c0;
+    ts[2] = ts[1] + c1;
+    ts[3] = ts[2] + c2;
+    const uint2 tp = make_uint2(ts[0] | ts[1] << 16, ts[2] | ts[3] << 16);
+#pragma unroll 4
+    for (int ww = 0; ww < kRadixWarps; ++ww) {
+      uint2& v = wc4[ww * (kRadixBins / 4) + threadIdx.x];
+      v = make_uint2(v.x + tp.x, v.y + tp.y);
+    }
+    const uint4 g = reinterpret_cast<const uint4*>(goff + (size_t)blk * kRadixBins)[threadIdx.x];
+    const uint4 db = dbase[threadIdx.x];
+    gdelta[threadIdx.x] = make_uint4(g.x + db.x - ts[0], g.y + db.y - ts[1], g.z + db.z - ts[2], g.w + db.w - ts[3]);
+    __syncthreads();
 #pragma unroll
-    for (int q = 0; q < kRadixBins / kThreads; ++q) {
-      const int d = q * kThreads + threadIdx.x;
-      uint32_t run = 0;
+    for (int r = 0; r < kRadixIPT; ++r)
+      if (wb + r * 32 + lane < tn) rk[r] = (rk[r] >> 16) + wc[w][rk[r] & (kRadixBins - 1)];
+    __syncthreads();   // the counters are read: their bytes take the staged tile
 #pragma unroll
-      for (int ww = 0; ww < kRadixWarps; ++ww) {
-        const uint32_t v = wc[ww][d];
-        wc[ww][d] = (uint16_t)run;
-        run += v;
-      }
-      bbase[d] = goff[(size_t)blk * kRadixBins + d] + dbase[q];
+    for (int r = 0; r < kRadixIPT; ++r) {
+      const int j = wb + r * 32 + lane;
+      if (j < tn) stage[rk[r]] = items[j];
     }
     __syncthreads();
-    // ---- phase 2: scatter (digit and rank are in registers; the items are read again, 8 loads in flight) ----
+    // ---- store: consecutive threads take consecutive staged items, so a digit's run is written contiguously ----
 #pragma unroll
-    for (int h = 0; h < kRadixIPT; h += 8) {
-      uint2 itv[8];
-#pragma unroll
-      for (int r = 0; r < 8; ++r) {
-        const int64_t i = wbeg + (h + r) * 32 + lane;
-        itv[r] = make_uint2(0u, 0u);
-        if (dgv[h + r] != 0xFFFFFFFFu) itv[r] = radix_load<FIRST>(in, i, pre_shift);
-      }
-#pragma unroll
-      for (int r = 0; r < 8; ++r) {
-        const uint32_t v = dgv[h + r];
-        if (v != 0xFFFFFFFFu) {
-          const uint32_t dg = v & (kRadixBins - 1);
-          out[bbase[dg] + wc[w][dg] + (v >> 16)] = itv[r];
-        }
+    for (int r = 0; r < kRadixIPT; ++r) {
+      const int j = r * kRadixThreads + threadIdx.x;
+      if (j < tn) {
+        const uint2 v = stage[j];
+        out[reinterpret_cast<const uint32_t*>(gdelta)[(v.x >> shift) & (kRadixBins - 1)] + (uint32_t)j] = v;
       }
     }
     __syncthreads();
@@ -327,19 +364,25 @@ static const uint2* sort_and_runs(const SortWs& w, const uint32_t* keys, int64_t
     uint32_t* dt = w.dtot + kRadixBins * p;
     const int ps = p == 0 ? pre_shift : 0;
     if (p == 0) {
-      radix_hist_kernel<true><<<resident_grid(radix_hist_kernel<true>, nb, 1), kThreads, 0, s>>>(in, M, 0, ps, w.cnt, nb);
+      radix_hist_kernel<true><<<resident_grid(radix_hist_kernel<true>, nb, 1, kRadixThreads), kRadixThreads, 0, s>>>(
+          in, M, 0, ps, w.cnt, nb);
       MONO_CHECK_LAUNCH();
     } else {
-      radix_hist_kernel<false><<<resident_grid(radix_hist_kernel<false>, nb, 1), kThreads, 0, s>>>(in, M, kRadixBits * p, 0, w.cnt, nb);
+      radix_hist_kernel<false><<<resident_grid(radix_hist_kernel<false>, nb, 1, kRadixThreads), kRadixThreads, 0, s>>>(
+          in, M, kRadixBits * p, 0, w.cnt, nb);
       MONO_CHECK_LAUNCH();
     }
     radix_colscan_kernel<<<kRadixBins / 32, 1024, 0, s>>>(w.cnt, nb, dt);
     MONO_CHECK_LAUNCH();
     if (p == 0) {
-      radix_scatter_kernel<true><<<resident_grid(radix_scatter_kernel<true>, nb, 1), kThreads, 0, s>>>(in, M, 0, ps, w.cnt, dt, nb, out);
+      set_max_dynamic_smem<radix_scatter_kernel<true>>(kRadixSmem);
+      radix_scatter_kernel<true><<<resident_grid(radix_scatter_kernel<true>, nb, 1, kRadixThreads, kRadixSmem),
+                                   kRadixThreads, kRadixSmem, s>>>(in, M, 0, ps, w.cnt, dt, nb, out);
       MONO_CHECK_LAUNCH();
     } else {
-      radix_scatter_kernel<false><<<resident_grid(radix_scatter_kernel<false>, nb, 1), kThreads, 0, s>>>(in, M, kRadixBits * p, 0, w.cnt, dt, nb, out);
+      set_max_dynamic_smem<radix_scatter_kernel<false>>(kRadixSmem);
+      radix_scatter_kernel<false><<<resident_grid(radix_scatter_kernel<false>, nb, 1, kRadixThreads, kRadixSmem),
+                                    kRadixThreads, kRadixSmem, s>>>(in, M, kRadixBits * p, 0, w.cnt, dt, nb, out);
       MONO_CHECK_LAUNCH();
     }
     in = out;
