@@ -709,10 +709,11 @@ int mono_global_norm(int32_t device, const mono_norm_tensor* tensors_host, int32
                      float* norm_dev, float* scale_dev, void* stream);
 
 /* The _scaled backward calls: the arguments of the call they are named after, then grad_scale_dev (one device
- * float, read on the device), then the stream.  Semantics, for all eight:
+ * float, read on the device), then the stream.  Semantics, for every _scaled call (those below, and
+ * mono_grouping_reduce_push_scaled and mono_xstep_backward_scaled next to their twins further down):
  *   a scaled call is bit for bit the unscaled call on gradient rows pre-multiplied by s = *grad_scale_dev in fp32
  *   (g * s, round to nearest), which is what the reference computes, because it multiplies before the op:
- *   - MEAN divides the scaled term: (g * s) / n;
+ *   - MEAN divides the scaled term: (g * s) / n; ReduceMean's gradient multiplies it: (g * s) * factor;
  *   - FIRSTN positions at or beyond max_seq_len stay +0.0 (they are not part of the gradient rows);
  *   - bf16 rows are widened exactly and then multiplied in fp32, so a bf16 scaled call equals the fp32 scaled call
  *     on the widened rows (not the unscaled call on bf16 rows scaled and rounded to bf16);
@@ -759,6 +760,19 @@ int mono_scatter_grad_rows_bf16_scaled(int32_t device, const float* pooled_grad_
                                        const int32_t* row_offsets_dev, int64_t n_rows, int32_t dim, int32_t pooling,
                                        float* grad_fused_dev, int64_t total_floats, const float* grad_scale_dev,
                                        void* stream);
+int mono_mtable_pool_backward_scaled(mono_mtable_t* t, int32_t k, const int64_t* fids_dev, int64_t n_fids,
+                                     const int32_t* row_offsets_dev, int64_t n_rows, int32_t pooling,
+                                     const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                                     const float* learning_rate_host, int64_t update_time, int64_t global_step,
+                                     const float* grad_scale_dev, void* stream);
+int mono_reduce_and_split_grad_scaled(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                                      int32_t* bad_splits_dev, const float* grad_scale_dev, void* stream);
+int mono_reduce_and_split_grad_bf16_scaled(int32_t device, const mono_reduce_feature* features,
+                                           int32_t num_features, int32_t* bad_splits_dev,
+                                           const float* grad_scale_dev, void* stream);
+int mono_grouping_reduce_scaled(mono_grouping_t* g, const float* pooled_grad_dev, int64_t grad_stride,
+                                int32_t grad_col, const int32_t* row_offsets_dev, int64_t n_rows, int32_t pooling,
+                                float* out_rows_dev, const float* grad_scale_dev, void* stream);
 
 /* ---- NVLink peer window: the exchange steps of the sharded path as peer stores ---------------
  * ref: the all-to-alls of the reference's synchronous multi-GPU path (distributed_ps_sync.py:92-118
@@ -800,6 +814,12 @@ int mono_grouping_reduce_push(mono_grouping_t* g, const float* pooled_grad_dev, 
                               int32_t grad_col, const int32_t* row_offsets_dev, int64_t n_rows,
                               int32_t pooling, const int64_t* shard_counts, mono_peer_t* p,
                               int64_t region_off, const int64_t* dst_row_off, void* stream);
+/* reduce_push with the clip scale: see "The _scaled backward calls" above */
+int mono_grouping_reduce_push_scaled(mono_grouping_t* g, const float* pooled_grad_dev, int64_t grad_stride,
+                                     int32_t grad_col, const int32_t* row_offsets_dev, int64_t n_rows,
+                                     int32_t pooling, const int64_t* shard_counts, mono_peer_t* p,
+                                     int64_t region_off, const int64_t* dst_row_off, const float* grad_scale_dev,
+                                     void* stream);
 
 /* ---- host-buffer entry points (what a CPU-resident caller such as the reference's TF op shim
  *      would call: ids / grads in host memory, results back in host memory).  These stage through
@@ -883,6 +903,11 @@ int mono_xstep_forward(mono_xstep_t* x, const int64_t* fids_dev, int64_t n_fids,
 int mono_xstep_backward(mono_xstep_t* x, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
                         const int32_t* row_offsets_dev, int32_t pooling, const float* lr_host, int64_t update_time,
                         void* stream);
+/* backward with the clip scale (see "The _scaled backward calls" above): the requester's reduce multiplies, so the
+ * owners apply sums of scaled terms */
+int mono_xstep_backward_scaled(mono_xstep_t* x, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                               const int32_t* row_offsets_dev, int32_t pooling, const float* lr_host,
+                               int64_t update_time, const float* grad_scale_dev, void* stream);
 
 /* Number of kernel launches issued by this library since load (for bench.py's gpu_launches). */
 int64_t mono_kernel_launch_count(void);

@@ -166,6 +166,13 @@ SIGNATURES = {
                                                 _p]),
     "mono_scatter_grad_rows_bf16_scaled": (C.c_int, [_i32, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _i32, _p, _i64,
                                                      _p, _p]),
+    "mono_mtable_pool_backward_scaled": (C.c_int, [_p, _i32, _p, _i64, _p, _i64, _i32, _p, _i64, _i32, _p, _i64, _i64,
+                                                   _p, _p]),
+    "mono_reduce_and_split_grad_scaled": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p, _p]),
+    "mono_reduce_and_split_grad_bf16_scaled": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p, _p]),
+    "mono_grouping_reduce_scaled": (C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p, _p]),
+    "mono_grouping_reduce_push_scaled": (C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p, _i64, _p, _p, _p]),
+    "mono_xstep_backward_scaled": (C.c_int, [_p, _p, _i64, _i32, _p, _i32, _p, _i64, _p, _p]),
     "mono_ckpt_last_error": (C.c_char_p, []),
     "mono_ckpt_writer_open": (C.c_int, [C.c_char_p, C.c_char_p, _i32, C.POINTER(_p)]),
     "mono_ckpt_writer_begin_table": (C.c_int, [_p, C.c_char_p, C.POINTER(SegmentCfg), _i32]),

@@ -5,10 +5,14 @@ The norm is one call of mono_global_norm: fp64 sums of exact squares in a fixed 
 sizes only (include/mono_emb.h states it), so its bits do not change from run to run.  The reference sums fp32
 squares with float atomics.  Nothing here synchronises with the host: the norm and the scale stay on the device.
 
-The sparse side takes the scale where the gradient rows are loaded (`grad_scale=` of
-MultiHashTable.pool_backward_parts and PartitionedHashTable.apply_gradients, `layout_tensors_grad_scale=` of
-distribution_ops.fused_embedding_to_layout_grad, `scale=` of gather_pool_grad / scatter_grad_rows); the dense side
-multiplies with torch.
+The sparse side takes the scale where the gradient rows are loaded; the dense side multiplies with torch:
+- `grad_scale=` of MultiHashTable.pool_backward and pool_backward_parts, PartitionedHashTable.apply_gradients and
+  ShardedStep.step (every exchange);
+- `grad_scale=` of distribution_ops.reduce_sum_gradient, reduce_mean_gradient, fused_reduce_sum_and_split_gradient
+  and fused_reduce_and_split_gpu_grad, and of Grouping.reduce / reduce_push;
+- `layout_tensors_grad_scale=` of distribution_ops.fused_embedding_to_layout_grad, `scale=` of gather_pool_grad /
+  scatter_grad_rows.
+Each is bit for bit the call without the scale on the gradients multiplied by it in float32 first.
 """
 import ctypes as C
 from typing import List, Optional, Sequence, Tuple

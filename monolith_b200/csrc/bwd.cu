@@ -1595,7 +1595,7 @@ static void reduce_and_apply(mono_mtable* mt, int k, const BwdScratch& w, SegLau
 void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t n_fids,
                        const int32_t* row_offsets, int64_t n_rows, int pooling,
                        const float* pooled_grad, int64_t grad_stride, int grad_col,
-                       const float* lr_host, int64_t update_time, cudaStream_t s) {
+                       const float* lr_host, int64_t update_time, cudaStream_t s, const float* grad_scale) {
   mt->note_insert(s);
   if (n_fids <= 0) return;
   if (n_fids > ((int64_t)1 << 30)) throw ArgError("more than 2^30 fids in one call");
@@ -1621,7 +1621,9 @@ void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t 
   ClaimResolve cr{};
   cr.t = mt->d_tables + k;
   claim_insert_sort(mt, cb, &w, fids_dev, M, set, cap, epoch, cr, update_time, s);
-  const SegArgs sa = seg_args(w, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, w.ugrad, s);
+  const GradScale gsc{grad_scale, nullptr};
+  const SegLaunch sa(seg_args(w, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, w.ugrad, s),
+                     grad_scale ? &gsc : nullptr);
   reduce_and_apply(mt, k, w, sa, fids_dev, cb.lr, M, update_time, s, false);
 }
 
@@ -1978,7 +1980,7 @@ void grouping_build(mono_grouping* g, const int64_t* fids_dev, int64_t M, int N,
 
 static void grouping_reduce_impl(mono_grouping* g, const float* pooled_grad, int64_t grad_stride, int grad_col,
                                  const int32_t* row_offsets, int64_t n_rows, int pooling, float* out_rows,
-                                 const PeerOut& po, cudaStream_t s) {
+                                 const PeerOut& po, cudaStream_t s, const float* grad_scale) {
   MONO_CUDA(cudaSetDevice(g->device));
   const int64_t M = g->M;
   const int D = g->dim;
@@ -1989,13 +1991,16 @@ static void grouping_reduce_impl(mono_grouping* g, const float* pooled_grad, int
   // runs are already in the bucketed order: the sums are written in place
   const SegArgs sa = seg_args(g->plan, M, D, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling,
                               out_rows, s);
-  launch_reduce(sa, pick_group(D), po, false, s);
+  const GradScale gsc{grad_scale, nullptr};
+  launch_reduce(SegLaunch(sa, grad_scale ? &gsc : nullptr), pick_group(D), po, false, s);
 }
 
 // out_rows[u] = summed gradient of the u-th distinct FID of the bucketed list (ref: ScatterGrad)
 void grouping_reduce(mono_grouping* g, const float* pooled_grad, int64_t grad_stride, int grad_col,
-                     const int32_t* row_offsets, int64_t n_rows, int pooling, float* out_rows, cudaStream_t s) {
-  grouping_reduce_impl(g, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, out_rows, no_peer, s);
+                     const int32_t* row_offsets, int64_t n_rows, int pooling, float* out_rows, cudaStream_t s,
+                     const float* grad_scale) {
+  grouping_reduce_impl(g, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, out_rows, no_peer, s,
+                       grad_scale);
 }
 
 // same, fused with the gradient exchange of the sharded backward: the row of the u-th distinct FID is stored
@@ -2003,9 +2008,10 @@ void grouping_reduce(mono_grouping* g, const float* pooled_grad, int64_t grad_st
 // distributed_ps_sync.py:531-573); the NVLink stores overlap the reduction, run by run.
 void grouping_reduce_push(mono_grouping* g, const float* pooled_grad, int64_t grad_stride, int grad_col,
                           const int32_t* row_offsets, int64_t n_rows, int pooling, const PeerOut& po,
-                          cudaStream_t s) {
+                          cudaStream_t s, const float* grad_scale) {
   if (po.n <= 0) throw ArgError("grouping_reduce_push without a peer window");
-  grouping_reduce_impl(g, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, nullptr, po, s);
+  grouping_reduce_impl(g, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, nullptr, po, s,
+                       grad_scale);
 }
 
 }  // namespace mono

@@ -158,11 +158,60 @@ int layout_entry(bool backward, int32_t device, float* const* emb_ptrs_dev, cons
 
 template <typename T>
 int reduce_split_entry(bool backward, int32_t device, const mono_reduce_feature* features, int32_t num_features,
-                       int32_t* bad_splits_dev, void* stream) {
+                       int32_t* bad_splits_dev, void* stream, const float* grad_scale = nullptr) {
   return guarded([&] {
     check_reduce_split(features, num_features);
     MONO_CUDA(cudaSetDevice(device));
-    launch_reduce_split<T>(backward, features, num_features, bad_splits_dev, (cudaStream_t)stream);
+    launch_reduce_split<T>(backward, features, num_features, bad_splits_dev, (cudaStream_t)stream, grad_scale);
+  });
+}
+
+// The bodies of the entry points that have a _scaled twin (grad_scale: null for the unscaled call)
+int pool_backward_entry(mono_mtable_t* t, int32_t k, const int64_t* fids_dev, int64_t n_fids,
+                        const int32_t* row_offsets_dev, int64_t n_rows, int32_t pooling, const float* pooled_grad_dev,
+                        int64_t grad_stride, int32_t grad_col, const float* learning_rate_host, int64_t update_time,
+                        void* stream, const float* grad_scale = nullptr) {
+  return guarded([&] {
+    require(k >= 0 && k < (int)t->tables.size(), "bad table index");
+    require(fids_dev && pooled_grad_dev && learning_rate_host, "pool_backward: null argument");
+    require(row_offsets_dev != nullptr || n_rows == n_fids, "pool_backward: n_rows must equal n_fids without offsets");
+    HandleGuard hg_(t);
+    run_pool_backward(t, k, fids_dev, n_fids, row_offsets_dev, n_rows, pooling, pooled_grad_dev, grad_stride,
+                      grad_col, learning_rate_host, update_time, (cudaStream_t)stream, grad_scale);
+  });
+}
+
+int grouping_reduce_entry(mono_grouping_t* g, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                          const int32_t* row_offsets_dev, int64_t n_rows, int32_t pooling, float* out_rows_dev,
+                          void* stream, const float* grad_scale = nullptr) {
+  return guarded([&] {
+    require(g && pooled_grad_dev && out_rows_dev, "grouping_reduce: null argument");
+    grouping_reduce(g, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, n_rows, pooling, out_rows_dev,
+                    (cudaStream_t)stream, grad_scale);
+  });
+}
+
+int grouping_reduce_push_entry(mono_grouping_t* g, const float* pooled_grad_dev, int64_t grad_stride,
+                               int32_t grad_col, const int32_t* row_offsets_dev, int64_t n_rows, int32_t pooling,
+                               const int64_t* shard_counts, mono_peer_t* p, int64_t region_off,
+                               const int64_t* dst_row_off, void* stream, const float* grad_scale = nullptr) {
+  return guarded([&] {
+    require(g && pooled_grad_dev && shard_counts && p && dst_row_off, "grouping_reduce_push: null argument");
+    require(p->device == g->device, "grouping_reduce_push: window and grouping on different devices");
+    PeerOut po = peer_out(p, region_off, dst_row_off, shard_counts, (int64_t)g->dim * 4);
+    grouping_reduce_push(g, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, n_rows, pooling, po,
+                         (cudaStream_t)stream, grad_scale);
+  });
+}
+
+int xstep_backward_entry(mono_xstep_t* x, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                         const int32_t* row_offsets_dev, int32_t pooling, const float* lr_host, int64_t update_time,
+                         void* stream, const float* grad_scale = nullptr) {
+  return guarded([&] {
+    require(x && pooled_grad_dev && lr_host, "xstep_backward: null argument");
+    HandleGuard hg_(x->mt);
+    xstep_backward(x, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, pooling, lr_host, update_time,
+                   (cudaStream_t)stream, grad_scale);
   });
 }
 }  // namespace
@@ -381,14 +430,8 @@ int mono_mtable_pool_backward(mono_mtable_t* t, int32_t k, const int64_t* fids_d
                               const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
                               const float* learning_rate_host, int64_t update_time,
                               int64_t /*global_step*/, void* stream) {
-  return guarded([&] {
-    require(k >= 0 && k < (int)t->tables.size(), "bad table index");
-    require(fids_dev && pooled_grad_dev && learning_rate_host, "pool_backward: null argument");
-    require(row_offsets_dev != nullptr || n_rows == n_fids, "pool_backward: n_rows must equal n_fids without offsets");
-    HandleGuard hg_(t);
-    run_pool_backward(t, k, fids_dev, n_fids, row_offsets_dev, n_rows, pooling, pooled_grad_dev, grad_stride,
-                      grad_col, learning_rate_host, update_time, (cudaStream_t)stream);
-  });
+  return pool_backward_entry(t, k, fids_dev, n_fids, row_offsets_dev, n_rows, pooling, pooled_grad_dev, grad_stride,
+                             grad_col, learning_rate_host, update_time, stream);
 }
 
 int mono_mtable_lookup_pool_parts(mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
@@ -683,11 +726,8 @@ int mono_grouping_build(mono_grouping_t* g, const int64_t* fids_dev, int64_t n_f
 int mono_grouping_reduce(mono_grouping_t* g, const float* pooled_grad_dev, int64_t grad_stride,
                          int32_t grad_col, const int32_t* row_offsets_dev, int64_t n_rows,
                          int32_t pooling, float* out_rows_dev, void* stream) {
-  return guarded([&] {
-    require(g && pooled_grad_dev && out_rows_dev, "grouping_reduce: null argument");
-    grouping_reduce(g, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, n_rows, pooling, out_rows_dev,
-                    (cudaStream_t)stream);
-  });
+  return grouping_reduce_entry(g, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, n_rows, pooling,
+                               out_rows_dev, stream);
 }
 
 int mono_peer_create(int32_t device, int32_t world, int32_t rank, int64_t bytes, mono_peer_t** out) {
@@ -772,13 +812,8 @@ int mono_grouping_reduce_push(mono_grouping_t* g, const float* pooled_grad_dev, 
                               int32_t grad_col, const int32_t* row_offsets_dev, int64_t n_rows,
                               int32_t pooling, const int64_t* shard_counts, mono_peer_t* p,
                               int64_t region_off, const int64_t* dst_row_off, void* stream) {
-  return guarded([&] {
-    require(g && pooled_grad_dev && shard_counts && p && dst_row_off, "grouping_reduce_push: null argument");
-    require(p->device == g->device, "grouping_reduce_push: window and grouping on different devices");
-    PeerOut po = peer_out(p, region_off, dst_row_off, shard_counts, (int64_t)g->dim * 4);
-    grouping_reduce_push(g, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, n_rows, pooling, po,
-                         (cudaStream_t)stream);
-  });
+  return grouping_reduce_push_entry(g, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, n_rows, pooling,
+                                    shard_counts, p, region_off, dst_row_off, stream);
 }
 
 int64_t mono_xstep_window_bytes(int32_t world, int64_t cap_pair, int32_t dim) {
@@ -820,12 +855,8 @@ int mono_xstep_forward(mono_xstep_t* x, const int64_t* fids_dev, int64_t n_fids,
 int mono_xstep_backward(mono_xstep_t* x, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
                         const int32_t* row_offsets_dev, int32_t pooling, const float* lr_host, int64_t update_time,
                         void* stream) {
-  return guarded([&] {
-    require(x && pooled_grad_dev && lr_host, "xstep_backward: null argument");
-    HandleGuard hg_(x->mt);
-    xstep_backward(x, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, pooling, lr_host, update_time,
-                   (cudaStream_t)stream);
-  });
+  return xstep_backward_entry(x, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, pooling, lr_host,
+                              update_time, stream);
 }
 
 int mono_gather_pool(int32_t device, const float* fused_emb_dev, const int32_t* emb_offset_dev,
@@ -1025,6 +1056,50 @@ int mono_embedding_to_layout_grad_bf16_scaled(int32_t device, float* const* emb_
   return layout_entry(true, device, emb_grad_ptrs_dev, emb_strides_dev, n_emb, fid_offset_dev, total_fid,
                       feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host, n_tasks,
                       const_cast<float* const*>(out_grad_ptrs_dev), stream, true, grad_scale_dev);
+}
+
+int mono_mtable_pool_backward_scaled(mono_mtable_t* t, int32_t k, const int64_t* fids_dev, int64_t n_fids,
+                                     const int32_t* row_offsets_dev, int64_t n_rows, int32_t pooling,
+                                     const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                                     const float* learning_rate_host, int64_t update_time, int64_t /*global_step*/,
+                                     const float* grad_scale_dev, void* stream) {
+  return pool_backward_entry(t, k, fids_dev, n_fids, row_offsets_dev, n_rows, pooling, pooled_grad_dev, grad_stride,
+                             grad_col, learning_rate_host, update_time, stream, grad_scale_dev);
+}
+
+int mono_reduce_and_split_grad_scaled(int32_t device, const mono_reduce_feature* features, int32_t num_features,
+                                      int32_t* bad_splits_dev, const float* grad_scale_dev, void* stream) {
+  return reduce_split_entry<float>(true, device, features, num_features, bad_splits_dev, stream, grad_scale_dev);
+}
+
+int mono_reduce_and_split_grad_bf16_scaled(int32_t device, const mono_reduce_feature* features,
+                                           int32_t num_features, int32_t* bad_splits_dev,
+                                           const float* grad_scale_dev, void* stream) {
+  return reduce_split_entry<__nv_bfloat16>(true, device, features, num_features, bad_splits_dev, stream,
+                                           grad_scale_dev);
+}
+
+int mono_grouping_reduce_scaled(mono_grouping_t* g, const float* pooled_grad_dev, int64_t grad_stride,
+                                int32_t grad_col, const int32_t* row_offsets_dev, int64_t n_rows, int32_t pooling,
+                                float* out_rows_dev, const float* grad_scale_dev, void* stream) {
+  return grouping_reduce_entry(g, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, n_rows, pooling,
+                               out_rows_dev, stream, grad_scale_dev);
+}
+
+int mono_grouping_reduce_push_scaled(mono_grouping_t* g, const float* pooled_grad_dev, int64_t grad_stride,
+                                     int32_t grad_col, const int32_t* row_offsets_dev, int64_t n_rows,
+                                     int32_t pooling, const int64_t* shard_counts, mono_peer_t* p,
+                                     int64_t region_off, const int64_t* dst_row_off, const float* grad_scale_dev,
+                                     void* stream) {
+  return grouping_reduce_push_entry(g, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, n_rows, pooling,
+                                    shard_counts, p, region_off, dst_row_off, stream, grad_scale_dev);
+}
+
+int mono_xstep_backward_scaled(mono_xstep_t* x, const float* pooled_grad_dev, int64_t grad_stride, int32_t grad_col,
+                               const int32_t* row_offsets_dev, int32_t pooling, const float* lr_host,
+                               int64_t update_time, const float* grad_scale_dev, void* stream) {
+  return xstep_backward_entry(x, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, pooling, lr_host,
+                              update_time, stream, grad_scale_dev);
 }
 
 // ---- global norm + clip scale ----------------------------------------------------------------

@@ -420,9 +420,11 @@ PeerOut peer_out(mono_peer* p, int64_t region_off, const int64_t* dst_item_off, 
                  int64_t item_bytes);
 void launch_lookup_push(mono_mtable* mt, int k, const int64_t* ids_dev, int64_t n_total, const PeerOut& po,
                         cudaStream_t s);
+// grad_scale (here and in grouping_reduce, xstep_backward): device float, or null; every pooled gradient element is
+// multiplied by it in fp32 where the reduce loads it (the scaled_ reduce kernels)
 void grouping_reduce_push(mono_grouping* g, const float* pooled_grad, int64_t grad_stride, int grad_col,
                           const int32_t* row_offsets, int64_t n_rows, int pooling, const PeerOut& po,
-                          cudaStream_t s);
+                          cudaStream_t s, const float* grad_scale = nullptr);
 
 mono_grouping* grouping_create(int device);
 void grouping_destroy(mono_grouping* g);  // synchronises the device first
@@ -430,7 +432,8 @@ void grouping_build(mono_grouping* g, const int64_t* fids_dev, int64_t M, int N,
                     int64_t* uniq_out, int32_t* occ_offset_out, int32_t* shard_counts_host,
                     int64_t* n_unique_host, cudaStream_t s);
 void grouping_reduce(mono_grouping* g, const float* pooled_grad, int64_t grad_stride, int grad_col,
-                     const int32_t* row_offsets, int64_t n_rows, int pooling, float* out_rows, cudaStream_t s);
+                     const int32_t* row_offsets, int64_t n_rows, int pooling, float* out_rows, cudaStream_t s,
+                     const float* grad_scale = nullptr);
 
 // xstep.cu
 int64_t xstep_window_bytes(int N, int64_t C, int D);
@@ -440,7 +443,8 @@ void xstep_prepare(mono_xstep* x, const int64_t* fids_next_dev, int64_t M, cudaS
 void xstep_forward(mono_xstep* x, const int64_t* fids_dev, int64_t M, const int32_t* row_offsets, int64_t n_rows,
                    int pooling, float* out, int64_t out_stride, int out_col, cudaStream_t s);
 void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride, int grad_col,
-                    const int32_t* row_offsets, int pooling, const float* lr_host, int64_t update_time, cudaStream_t s);
+                    const int32_t* row_offsets, int pooling, const float* lr_host, int64_t update_time, cudaStream_t s,
+                    const float* grad_scale = nullptr);
 
 // table.cu
 void table_init(mono_mtable* mt, HostTable& t, const mono_table_cfg& cfg, cudaStream_t s);
@@ -480,10 +484,12 @@ void run_upsert_groups(mono_mtable* mt, const CallSeg* h_segs, int nsegs, const 
                        int ngroups, const int64_t* ids_dev, const float* vals_dev, const float* lr_host,
                        int n_lr, int64_t update_time, cudaStream_t s);
 
+// grad_scale: as run_pool_backward_parts' (the one table has no FIRSTN rows)
 void run_pool_backward(mono_mtable* mt, int k, const int64_t* fids_dev, int64_t n_fids,
                        const int32_t* row_offsets, int64_t n_rows, int pooling,
                        const float* pooled_grad, int64_t grad_stride, int grad_col,
-                       const float* lr_host, int64_t update_time, cudaStream_t s);
+                       const float* lr_host, int64_t update_time, cudaStream_t s,
+                       const float* grad_scale = nullptr);
 
 // A FIRSTN part's sequence length (max_seq_len is read for FIRSTN parts only): L >= 1 and n_rows * L <= 2^31
 inline void check_firstn(const char* who, const mono_pool_part& p) {
@@ -531,11 +537,12 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,
                    int total_nfl, int batch_size, const mono_slice_task* tasks_host, int n_tasks,
                    float* const* out_ptrs_dev, cudaStream_t s, bool bf16 = false, const float* grad_scale = nullptr);
-// mono_reduce_and_split[_grad]; T: element type of the slice rows
+// mono_reduce_and_split[_grad]; T: element type of the slice rows.  grad_scale (backward only; device float, or
+// null): every slice gradient element is multiplied by it in fp32 where it is loaded (the scaled_ kernels)
 void check_reduce_split(const mono_reduce_feature* feats, int n_features);
 template <typename T>
 void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int n_features, int32_t* bad_splits_dev,
-                         cudaStream_t s);
+                         cudaStream_t s, const float* grad_scale = nullptr);
 
 // clip.cu
 void check_global_norm(const mono_norm_tensor* tensors, int n_tensors, float clip_norm, const float* norm_dev,

@@ -673,8 +673,9 @@ __device__ __forceinline__ void reduce_split_fwd(const RsArgs& a) {
 }
 
 // Every occurrence row of sample b gets b's slice gradients: copied (SUM) or times the forward's factor (MEAN).
-template <typename T, int G>
-__device__ __forceinline__ void reduce_split_bwd(const RsArgs& a) {
+// SCALED (scaled_ kernels): each gradient element times *scale in fp32 where it is loaded, before the MEAN factor.
+template <typename T, int G, bool SCALED = false>
+__device__ __forceinline__ void reduce_split_bwd(const RsArgs& a, const float* scale = nullptr) {
   const int64_t u = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
   if (u >= a.units) return;
   const RsFeat f = a.feats[a.order[u / a.batch]];
@@ -684,6 +685,7 @@ __device__ __forceinline__ void reduce_split_bwd(const RsArgs& a) {
   if (n == 0) return;
   const float mult = rs_mean_factor(n);
   const bool mean = f.pooling == MONO_POOL_MEAN;
+  const float gscale = SCALED ? *scale : 1.f;
   const int gl = Group<G>::gl();
   float* occ = f.rows + (int64_t)lo * f.row_stride;
   for (int s = f.slice0; s < f.slice0 + f.n_slices; ++s) {
@@ -694,6 +696,10 @@ __device__ __forceinline__ void reduce_split_bwd(const RsArgs& a) {
       float* dst = occ + sl.col + c;
       if (vec) {
         float4 x = rs_load4(g + c);
+        if (SCALED) {
+          x.x = __fmul_rn(x.x, gscale); x.y = __fmul_rn(x.y, gscale);
+          x.z = __fmul_rn(x.z, gscale); x.w = __fmul_rn(x.w, gscale);
+        }
         if (mean) {
           x.x = __fmul_rn(x.x, mult); x.y = __fmul_rn(x.y, mult);
           x.z = __fmul_rn(x.z, mult); x.w = __fmul_rn(x.w, mult);
@@ -704,6 +710,7 @@ __device__ __forceinline__ void reduce_split_bwd(const RsArgs& a) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           x[i] = c + i * G < sl.dim ? row_elem_f32(g[c + i * G]) : 0.f;
+          if (SCALED) x[i] = __fmul_rn(x[i], gscale);
           if (mean) x[i] = __fmul_rn(x[i], mult);
         }
         for (int j = 0; j < n; ++j) {
@@ -734,6 +741,17 @@ __global__ void __launch_bounds__(kThreads) reduce_split_bwd_kernel(RsArgs a) {
 template <int G>
 __global__ void __launch_bounds__(kThreads) bf16_reduce_split_bwd_kernel(RsArgs a) {
   reduce_split_bwd<__nv_bfloat16, G>(a);
+}
+
+// the two above with every gradient element multiplied by *scale (the _scaled calls' grad_scale_dev)
+template <int G>
+__global__ void __launch_bounds__(kThreads) scaled_reduce_split_bwd_kernel(RsArgs a, const float* scale) {
+  reduce_split_bwd<float, G, true>(a, scale);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads) scaled_bf16_reduce_split_bwd_kernel(RsArgs a, const float* scale) {
+  reduce_split_bwd<__nv_bfloat16, G, true>(a, scale);
 }
 
 // Host-side checks of the records: the kernels index with every field unchecked.
@@ -768,7 +786,8 @@ void check_reduce_split(const mono_reduce_feature* feats, int F) {
 }
 
 template <typename T>
-void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int F, int32_t* bad_dev, cudaStream_t s) {
+void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int F, int32_t* bad_dev, cudaStream_t s,
+                         const float* grad_scale) {
   if (bad_dev) MONO_CUDA(cudaMemsetAsync(bad_dev, 0, sizeof(int32_t), s));
   const int64_t B = F > 0 ? feats[0].batch_size : 0;
   if (F == 0 || B == 0) return;
@@ -818,6 +837,8 @@ void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int F,
       const int64_t grid = (a.units + kThreads / GG - 1) / (kThreads / GG);
       if (!backward) by_elem<T>(reduce_split_fwd_kernel<GG>, bf16_reduce_split_fwd_kernel<GG>)
                          <<<(unsigned)grid, kThreads, 0, s>>>(a);
+      else if (grad_scale) by_elem<T>(scaled_reduce_split_bwd_kernel<GG>, scaled_bf16_reduce_split_bwd_kernel<GG>)
+                               <<<(unsigned)grid, kThreads, 0, s>>>(a, grad_scale);
       else by_elem<T>(reduce_split_bwd_kernel<GG>, bf16_reduce_split_bwd_kernel<GG>)
                <<<(unsigned)grid, kThreads, 0, s>>>(a);
     });
@@ -826,7 +847,9 @@ void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int F,
   MONO_CUDA(cudaFreeAsync(ws, s));
 }
 
-template void launch_reduce_split<float>(bool, const mono_reduce_feature*, int, int32_t*, cudaStream_t);
-template void launch_reduce_split<__nv_bfloat16>(bool, const mono_reduce_feature*, int, int32_t*, cudaStream_t);
+template void launch_reduce_split<float>(bool, const mono_reduce_feature*, int, int32_t*, cudaStream_t,
+                                         const float*);
+template void launch_reduce_split<__nv_bfloat16>(bool, const mono_reduce_feature*, int, int32_t*, cudaStream_t,
+                                                 const float*);
 
 }  // namespace mono

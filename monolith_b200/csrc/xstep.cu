@@ -367,7 +367,8 @@ void xstep_forward(mono_xstep* x, const int64_t* fids_dev, int64_t M, const int3
 // backward of the step started by the last forward: per-FID gradient sums pushed to the owners, then this rank, as
 // an owner, resolves what it received and applies the sources in rank order.
 void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride, int grad_col,
-                    const int32_t* row_offsets, int pooling, const float* lr_host, int64_t update_time, cudaStream_t s) {
+                    const int32_t* row_offsets, int pooling, const float* lr_host, int64_t update_time, cudaStream_t s,
+                    const float* grad_scale) {
   MONO_CUDA(cudaSetDevice(x->mt->device));
   if (!x->fwd_done) throw ArgError("xstep_backward without a forward");
   // the owner's insert hands a new FID to the filter once per step (its leader), where the reference counts it once
@@ -382,7 +383,7 @@ void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride
   const XWin& w = x->w;
   const uint64_t seq = x->step;
   const int par = (int)(seq & 1);
-  // requester: reduce + push
+  // requester: reduce + push (grad_scale: the pushed sums are of scaled terms, so the owner's apply below is as is)
   PeerOut po;
   std::memset(&po, 0, sizeof(po));
   po.n = x->N;
@@ -390,7 +391,7 @@ void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride
     po.base[r] = x->win->base[r] + kPeerFlagBytes + w.off_grads + (int64_t)x->me * x->C * x->D * 4;
   mono_grouping* g = x->grouping[par];
   po.cnt_dev = g->plan.ctr + kCtrOwners;
-  grouping_reduce_push(g, pooled_grad, grad_stride, grad_col, row_offsets, x->last_rows, pooling, po, s);
+  grouping_reduce_push(g, pooled_grad, grad_stride, grad_col, row_offsets, x->last_rows, pooling, po, s, grad_scale);
   xsignal_kernel<<<1, 32, 0, s>>>(w, kPhaseGrads, seq, nullptr);
   MONO_CHECK_LAUNCH();
   // owner: resolve (+ insert) everything received, then apply source by source

@@ -384,7 +384,7 @@ class ShardedStep:
     total = self.off_grads_out + al(self.cap_rows * D * 4)
     self.window = self.dops.PeerWindow(self.device, self.N, self.rank, total, self.group)
 
-  def _step_peer(self, fids, pooled_grad, out, req_time, row_offsets, pooling):
+  def _step_peer(self, fids, pooled_grad, out, req_time, row_offsets, pooling, grad_scale):
     import numpy as np
     N, D, me, ph = self.N, self.dim, self.rank, self.phases
     ph.mark("start")
@@ -425,13 +425,14 @@ class ShardedStep:
     if callable(pooled_grad):   # forward enqueued: the caller's dense tower / host round trip goes here
       pooled_grad = pooled_grad()
     if self.bulk == "push":
-      self.grouping.reduce_push(pooled_grad, cnt[me], self.window, self.off_grads, my_seg, row_offsets, pooling)  # 7+8
+      self.grouping.reduce_push(pooled_grad, cnt[me], self.window, self.off_grads, my_seg, row_offsets, pooling,  # 7+8
+                                grad_scale=grad_scale)
       ph.fine("b8a_reduce_push_kernels")
       self.window.barrier()
       ph.mark("b8_reduce_push")
     else:
       grads_out = self.window.view(self.off_grads_out, uniq.numel() * D, torch.float32)
-      self.grouping.reduce(pooled_grad, grads_out, row_offsets, pooling)              # 7 requester: bucketed by owner
+      self.grouping.reduce(pooled_grad, grads_out, row_offsets, pooling, grad_scale=grad_scale)  # 7 requester: bucketed by owner
       ph.fine("b8a_reduce")
       self.window.barrier()
       ph.fine("b8b_barrier")
@@ -494,7 +495,7 @@ class ShardedStep:
       self.window.close(self.group)
       self.window = None
 
-  def _step_direct(self, fids, pooled_grad, out, req_time, row_offsets, pooling):
+  def _step_direct(self, fids, pooled_grad, out, req_time, row_offsets, pooling, grad_scale):
     import ctypes as C
     from . import _lib
     lib = _lib.load()
@@ -521,10 +522,13 @@ class ShardedStep:
     lr = self.table.configs[self.name].call_learning_rate_fns()
     lr_arr = (C.c_float * len(lr))(*lr)
     stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-    _lib.check(lib.mono_xstep_backward(self.xstep, C.c_void_p(pooled_grad.data_ptr()),
-                                       pooled_grad.stride(0) if pooled_grad.dim() == 2 else self.dim, 0, ro, pool, lr_arr,
-                                       int(req_time), stream))
-    self._keep = (fids, pooled_grad, row_offsets)   # alive until the kernels have consumed them
+    args = (self.xstep, C.c_void_p(pooled_grad.data_ptr()), pooled_grad.stride(0) if pooled_grad.dim() == 2 else self.dim,
+            0, ro, pool, lr_arr, int(req_time))
+    if grad_scale is None:
+      _lib.check(lib.mono_xstep_backward(*args, stream))
+    else:
+      _lib.check(lib.mono_xstep_backward_scaled(*args, C.c_void_p(grad_scale.data_ptr()), stream))
+    self._keep = (fids, pooled_grad, row_offsets, grad_scale)   # alive until the kernels have consumed them
     self.direct_steps += 1
     return 0
 
@@ -536,14 +540,26 @@ class ShardedStep:
     return out
 
   def step(self, fids: torch.Tensor, pooled_grad, out: torch.Tensor, req_time: int,
-           row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum"):
+           row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum",
+           grad_scale: Optional[torch.Tensor] = None):
     """One sparse train step.  `pooled_grad` is the gradient w.r.t. the pooled rows written to `out`, or a
     callable returning it: the callable runs once the forward has been enqueued (what produces the gradient —
-    the dense tower, or a round trip of `out` to the host — belongs there)."""
+    the dense tower, or a round trip of `out` to the host — belongs there).
+
+    grad_scale (clip by global norm, ref: the deferred sparse scale of feature_utils.py:245-265): a one-element
+    float32 tensor on the step's device.  The step is then bit for bit the step on pooled_grad multiplied by it in
+    float32 first, in every exchange: the backward's per-FID reduce multiplies each term where it loads it
+    (mono_xstep_backward_scaled, mono_grouping_reduce[_push]_scaled), so the owners apply sums of scaled terms.
+    The value is read on the device when that reduce runs, not when step() is entered: a callable `pooled_grad`
+    may fill the tensor on the current stream, e.g.
+    `scale_buf.copy_(clip_ops.global_norm_scale(dense_grads + [g], clip_norm)[0])` before it returns g."""
+    if grad_scale is not None:
+      from .clip_ops import scale_ptr
+      scale_ptr(grad_scale, self.device, "grad_scale")
     if self.exchange == "direct":
-      return self._step_direct(fids, pooled_grad, out, req_time, row_offsets, pooling)
+      return self._step_direct(fids, pooled_grad, out, req_time, row_offsets, pooling, grad_scale)
     if self.exchange == "peer":
-      return self._step_peer(fids, pooled_grad, out, req_time, row_offsets, pooling)
+      return self._step_peer(fids, pooled_grad, out, req_time, row_offsets, pooling, grad_scale)
     N, D, dev, ph = self.N, self.dim, fids.device, self.phases
     self.nccl_steps += 1
     ph.mark("start")
@@ -567,7 +583,7 @@ class ShardedStep:
     if callable(pooled_grad):
       pooled_grad = pooled_grad()
     grad_rows = torch.empty(uniq.numel() * D, dtype=torch.float32, device=dev)        # 7
-    self.grouping.reduce(pooled_grad, grad_rows, row_offsets, pooling)
+    self.grouping.reduce(pooled_grad, grad_rows, row_offsets, pooling, grad_scale=grad_scale)
     ph.mark("b7_reduce_grads")
     owner_grads = torch.empty(sum(recv_sizes) * D, dtype=torch.float32, device=dev)   # 8
     _a2a(owner_grads, grad_rows, [s * D for s in recv_sizes], [s * D for s in shard_sizes], self.group)

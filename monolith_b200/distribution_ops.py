@@ -327,9 +327,10 @@ def _rows2d(t, what):
   return t
 
 
-def _reduce_split_call(backward, splits, rows, slices, poolings, bad_splits):
+def _reduce_split_call(backward, splits, rows, slices, poolings, bad_splits, scale=None):
   """splits[f]: int32 [B + 1]; rows[f]: [n_f, D_f] float32 (read forward, written backward); slices[f]: the 2-D
-  tensors of feature f's slices (written forward, read backward), all float32 or all bfloat16."""
+  tensors of feature f's slices (written forward, read backward), all float32 or all bfloat16.  scale (backward
+  only): the clip_ops.scale_ptr of the gradient scale, or None for the unscaled call."""
   lib = _lib.load()
   F = len(splits)
   flat = [t for s in slices for t in s]
@@ -350,6 +351,10 @@ def _reduce_split_call(backward, splits, rows, slices, poolings, bad_splits):
     recs[f].dim, recs[f].pooling = r.size(1), _POOLINGS[poolings[f]]
     recs[f].slices, recs[f].n_slices = sl, len(slices[f])
   bf16 = dtype == torch.bfloat16
+  if scale is not None:
+    fn = lib.mono_reduce_and_split_grad_bf16_scaled if bf16 else lib.mono_reduce_and_split_grad_scaled
+    _lib.check(fn(dev.index, recs, F, _ptr(bad_splits), scale, _stream(dev)))
+    return
   fn = {(False, False): lib.mono_reduce_and_split, (True, False): lib.mono_reduce_and_split_grad,
         (False, True): lib.mono_reduce_and_split_bf16, (True, True): lib.mono_reduce_and_split_grad_bf16}[backward, bf16]
   _lib.check(fn(dev.index, recs, F, _ptr(bad_splits), _stream(dev)))
@@ -383,12 +388,18 @@ def fused_reduce_and_split_gpu(splits: Sequence[torch.Tensor], embeddings: Seque
 def fused_reduce_and_split_gpu_grad(splits: Sequence[torch.Tensor], embeddings: Sequence[torch.Tensor],
                                     grads: Sequence[torch.Tensor], slice_dims: Sequence[Sequence[int]], *,
                                     pooling="sum", out: Optional[Sequence[torch.Tensor]] = None,
-                                    bad_splits: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
+                                    bad_splits: Optional[torch.Tensor] = None,
+                                    grad_scale: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
   """ref: MonolithFusedReduceAndSplitGPUGrad (reduce_op.cu.cc:478-680).  grads is the flat list of slice gradients
   (all float32 or all bfloat16, widened exactly).  Returns feature f's occurrence-row gradients [n_f, D_f] float32:
   sample b's slice gradients copied (SUM) or times ReduceMean's factor (MEAN) into each of b's rows.  out[f], when
   given, is written instead (a [n_f, D_f] view, e.g. of the flat gradient buffer raw_apply_gradients takes); rows
-  no sample covers are left as they are.  embeddings only give the shapes (as in the reference gradient)."""
+  no sample covers are left as they are.  embeddings only give the shapes (as in the reference gradient).
+
+  grad_scale: a one-element float32 tensor on the splits' device (clip_ops.global_norm_scale's scale), read on the
+  device: the result is bit for bit this call on every slice gradient multiplied by it in float32 first (a bfloat16
+  gradient is widened before the multiply; MEAN's factor comes after it).  mono_reduce_and_split_grad[_bf16]_scaled."""
+  sc = _grad_scale_ptr(grad_scale, splits[0].device if len(splits) else None)
   F = len(splits)
   sp = [_splits32(s) for s in splits]
   shapes = [(e.size(0), e.size(1)) for e in embeddings]
@@ -401,7 +412,7 @@ def fused_reduce_and_split_gpu_grad(splits: Sequence[torch.Tensor], embeddings: 
   per = [[next(it) for _ in dims] for dims in slice_dims]
   if sum(len(d) for d in slice_dims) != len(grads):
     raise ValueError("grads must hold one tensor per slice")
-  _reduce_split_call(True, sp, rows, per, _poolings(pooling, F), bad_splits)
+  _reduce_split_call(True, sp, rows, per, _poolings(pooling, F), bad_splits, sc)
   return list(rows)
 
 
@@ -433,11 +444,21 @@ def _reduce(id_indices, id_values, B, split_dims, pooling, dtype, sync):
   return fused_reduce_and_split_gpu([splits], [id_values], [split_dims], pooling=pooling, dtype=dtype)
 
 
-def _reduce_grad(id_indices, grads, split_dims, pooling, sync, B=None):
+def _grad_scale_ptr(grad_scale, dev):
+  """grad_scale checked before any device work (clip_ops.scale_ptr; dev None: the current CUDA device)."""
+  if grad_scale is None:
+    return None
+  from .clip_ops import scale_ptr
+  return scale_ptr(grad_scale, dev if dev is not None else torch.device("cuda", torch.cuda.current_device()))
+
+
+def _reduce_grad(id_indices, grads, split_dims, pooling, sync, B=None, grad_scale=None):
+  _grad_scale_ptr(grad_scale, id_indices.device)
   B = grads[0].size(0) if B is None else B
   splits = _splits_from_indices(id_indices, B, sync)
   out = torch.empty(id_indices.size(0), sum(split_dims), dtype=torch.float32, device=splits.device)
-  return fused_reduce_and_split_gpu_grad([splits], [out], grads, [split_dims], pooling=pooling, out=[out])[0]
+  return fused_reduce_and_split_gpu_grad([splits], [out], grads, [split_dims], pooling=pooling, out=[out],
+                                         grad_scale=grad_scale)[0]
 
 
 def reduce_sum(id_indices: torch.Tensor, id_values: torch.Tensor, id_dense_shape, *,
@@ -454,15 +475,19 @@ def reduce_mean(id_indices: torch.Tensor, id_values: torch.Tensor, id_dense_shap
   return _reduce(id_indices, id_values, _batch_size(id_dense_shape), [id_values.size(1)], "mean", dtype, sync)[0]
 
 
-def reduce_sum_gradient(id_indices: torch.Tensor, grads: torch.Tensor, *, sync: bool = True) -> torch.Tensor:
-  """ref: MonolithReduceSumGradient (reduce_op.cc:124-148): row i is grads[id_indices[i]] ([n, D] float32)."""
-  return _reduce_grad(id_indices, [grads], [grads.size(1)], "sum", sync)
+def reduce_sum_gradient(id_indices: torch.Tensor, grads: torch.Tensor, *, sync: bool = True,
+                        grad_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+  """ref: MonolithReduceSumGradient (reduce_op.cc:124-148): row i is grads[id_indices[i]] ([n, D] float32).
+  grad_scale: as fused_reduce_and_split_gpu_grad's, on id_indices' device: row i is grads[id_indices[i]] * scale."""
+  return _reduce_grad(id_indices, [grads], [grads.size(1)], "sum", sync, grad_scale=grad_scale)
 
 
-def reduce_mean_gradient(id_indices: torch.Tensor, grads: torch.Tensor, *, sync: bool = True) -> torch.Tensor:
+def reduce_mean_gradient(id_indices: torch.Tensor, grads: torch.Tensor, *, sync: bool = True,
+                         grad_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
   """ref: MonolithReduceMeanGradient (reduce_op.cc:150-180): row i is grads[b] times the forward's factor for
-  b = id_indices[i], counted per sample (the reference sizes its counter by the dim, reduce_op.cc:166)."""
-  return _reduce_grad(id_indices, [grads], [grads.size(1)], "mean", sync)
+  b = id_indices[i], counted per sample (the reference sizes its counter by the dim, reduce_op.cc:166).
+  grad_scale: as reduce_sum_gradient's; row i is (grads[b] * scale) * factor."""
+  return _reduce_grad(id_indices, [grads], [grads.size(1)], "mean", sync, grad_scale=grad_scale)
 
 
 def fused_reduce_sum_and_split(id_indices: torch.Tensor, id_values: torch.Tensor, id_length, split_dims: Sequence[int],
@@ -475,12 +500,13 @@ def fused_reduce_sum_and_split(id_indices: torch.Tensor, id_values: torch.Tensor
 
 
 def fused_reduce_sum_and_split_gradient(id_indices: torch.Tensor, grads: Sequence[torch.Tensor],
-                                        split_dims: Sequence[int], *, sync: bool = True) -> torch.Tensor:
+                                        split_dims: Sequence[int], *, sync: bool = True,
+                                        grad_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
   """ref: MonolithFusedReduceSumAndSplitGradient (reduce_op.cc:282-330): [n, sum(split_dims)] float32, row i the
-  concatenated slice gradients of sample id_indices[i]."""
+  concatenated slice gradients of sample id_indices[i].  grad_scale: as reduce_sum_gradient's."""
   if [g.size(1) for g in grads] != list(split_dims):
     raise ValueError("grads must have the split_dims widths")
-  return _reduce_grad(id_indices, list(grads), list(split_dims), "sum", sync)
+  return _reduce_grad(id_indices, list(grads), list(split_dims), "sum", sync, grad_scale=grad_scale)
 
 
 class Grouping:
@@ -519,28 +545,39 @@ class Grouping:
     return uniq[:n_u.value], offs[:M], list(counts)
 
   def reduce(self, pooled_grad: torch.Tensor, out_rows: torch.Tensor, row_offsets: Optional[torch.Tensor] = None,
-             pooling: str = "sum", grad_col: int = 0):
+             pooling: str = "sum", grad_col: int = 0, grad_scale: Optional[torch.Tensor] = None):
+    """grad_scale: a one-element float32 tensor on the grouping's device, read on the device when the reduce runs:
+    the rows are bit for bit this call's on pooled_grad multiplied by it in float32 (mono_grouping_reduce_scaled)."""
+    sp = _grad_scale_ptr(grad_scale, self.device)
     n_rows = self._keep.numel() if row_offsets is None else row_offsets.numel() - 1
     if row_offsets is not None:
       row_offsets = row_offsets.to(torch.int32).contiguous()
     pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-    _lib.check(self._lib.mono_grouping_reduce(self._h, _ptr(pooled_grad), pooled_grad.stride(0), grad_col,
-                                              _ptr(row_offsets), n_rows, pool, _ptr(out_rows), _stream(self.device)))
+    args = (self._h, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(row_offsets), n_rows, pool, _ptr(out_rows))
+    if sp is None:
+      _lib.check(self._lib.mono_grouping_reduce(*args, _stream(self.device)))
+    else:
+      _lib.check(self._lib.mono_grouping_reduce_scaled(*args, sp, _stream(self.device)))
     return out_rows
 
   def reduce_push(self, pooled_grad: torch.Tensor, shard_sizes: Sequence[int], window: "PeerWindow", region_off: int,
                   dst_row_off: Sequence[int], row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum",
-                  grad_col: int = 0):
-    """reduce() whose output rows are stored into the owners' windows (fused gradient exchange)."""
+                  grad_col: int = 0, grad_scale: Optional[torch.Tensor] = None):
+    """reduce() whose output rows are stored into the owners' windows (fused gradient exchange).  grad_scale: as
+    reduce()'s (mono_grouping_reduce_push_scaled)."""
+    sp = _grad_scale_ptr(grad_scale, self.device)
     n_rows = self._keep.numel() if row_offsets is None else row_offsets.numel() - 1
     if row_offsets is not None:
       row_offsets = row_offsets.to(torch.int32).contiguous()
     pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
     n = window.world
-    _lib.check(self._lib.mono_grouping_reduce_push(
-        self._h, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(row_offsets), n_rows, pool,
-        (C.c_int64 * n)(*[int(x) for x in shard_sizes]), window._h, int(region_off),
-        (C.c_int64 * n)(*[int(x) for x in dst_row_off]), _stream(self.device)))
+    args = (self._h, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(row_offsets), n_rows, pool,
+            (C.c_int64 * n)(*[int(x) for x in shard_sizes]), window._h, int(region_off),
+            (C.c_int64 * n)(*[int(x) for x in dst_row_off]))
+    if sp is None:
+      _lib.check(self._lib.mono_grouping_reduce_push(*args, _stream(self.device)))
+    else:
+      _lib.check(self._lib.mono_grouping_reduce_push_scaled(*args, sp, _stream(self.device)))
 
 
 class _RawCuda:

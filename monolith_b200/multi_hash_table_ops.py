@@ -372,11 +372,18 @@ class MultiHashTable:
 
   def pool_backward(self, slot: str, fids: torch.Tensor, pooled_grad: torch.Tensor,
                     row_offsets: Optional[torch.Tensor] = None, pooling: str = "sum", req_time: int = 0,
-                    global_step: int = 0, grad_col: int = 0):
+                    global_step: int = 0, grad_col: int = 0, grad_scale: Optional[torch.Tensor] = None):
     """Fused backward of lookup_pool: scatters the pooled-row gradients to the unique FIDs, applies one
     sparse optimizer step per FID and bumps the expiry timestamp (upsert), deterministically and without
     a per-unique gradient buffer.  Equivalent to fused_embedding_to_layout_grad / ScatterGrad followed by
-    apply_gradients on the deduplicated ids (ref: distributed_ps.py:1321-1332,1390-1395)."""
+    apply_gradients on the deduplicated ids (ref: distributed_ps.py:1321-1332,1390-1395).
+
+    grad_scale: as pool_backward_parts' (mono_mtable_pool_backward_scaled): the call is bit for bit this call on
+    pooled_grad multiplied by it in float32 first."""
+    sp = None
+    if grad_scale is not None:
+      from .clip_ops import scale_ptr
+      sp = scale_ptr(grad_scale, self._device, "grad_scale")
     k = self._table_names.index(slot)
     fids = _ids(fids, self._device)
     pooled_grad = _f32(pooled_grad, self._device)
@@ -389,9 +396,15 @@ class MultiHashTable:
     lr = self._configs[slot].call_learning_rate_fns()
     lr_arr = (C.c_float * len(lr))(*lr)
     pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-    _lib.check(self._lib.mono_mtable_pool_backward(self._h, k, _ptr(fids), fids.numel(), _ptr(row_offsets), n_rows,
-                                                   pool, _ptr(pooled_grad), stride, grad_col, lr_arr, int(req_time),
-                                                   int(global_step), _stream(self._device)))
+    if sp is None:
+      _lib.check(self._lib.mono_mtable_pool_backward(self._h, k, _ptr(fids), fids.numel(), _ptr(row_offsets), n_rows,
+                                                     pool, _ptr(pooled_grad), stride, grad_col, lr_arr, int(req_time),
+                                                     int(global_step), _stream(self._device)))
+    else:
+      _lib.check(self._lib.mono_mtable_pool_backward_scaled(self._h, k, _ptr(fids), fids.numel(), _ptr(row_offsets),
+                                                            n_rows, pool, _ptr(pooled_grad), stride, grad_col, lr_arr,
+                                                            int(req_time), int(global_step), sp,
+                                                            _stream(self._device)))
     return self
 
   @staticmethod
