@@ -462,6 +462,79 @@ int mono_sharding_sparse_fids(int32_t device, const int64_t* fids_dev, const int
                               int32_t* emb_row_length_dev, int32_t* bad_row_splits_dev,
                               int32_t* table_row_length_host, void* stream);
 
+/* ---- async parameter-server worker path ------------------------------------------------------------------------
+ * ref: DistributedMultiTypeHashTable.lookup / apply_gradients on the raw API, NT/distributed_ps.py:266-337, 481-516:
+ * dedup the K tables' keys (unique_key_with_value_and_offset), split the unique keys over S servers by
+ * floormod(key, S) (ragged_split_by_indices), look up / apply on each server with its row splits, then copy every
+ * server's rows to all occurrences of their keys (fill_with_offset_map) or sum the occurrence gradients per unique key
+ * (fill_with_offset_map_grad).  Keys are int64 and equal when their bits are equal; offsets are int64 floats. */
+
+/* ref: UniqueKeyWitValueAndOffsetOp, RT/ops/unique_mapping_ops.cc:51-124.  key_dev[M] holds K tables' keys,
+ * table k = key_dev[key_split_host[k] : key_split_host[k + 1]], with dims_host[k] floats per row.  Outputs:
+ *   unique_key_dev           int64[max(M, 1)]  every table's distinct keys in first-occurrence order, table after table;
+ *                                              the first U entries are written
+ *   unique_key_split_dev     int64[K + 1]      row splits of unique_key (U = unique_key_split[K])
+ *   value_offset_dev         int64[M]          for every unique key in order, the float offsets of all its occurrences in
+ *                                              occurrence order: occurrence i of table k sits at
+ *                                              base_k + (i - key_split[k]) * dims[k], base_k = sum_{k' < k} count_k' dims_k'
+ *   value_offset_split_dev   int64[M + 1]      row splits of value_offset over the unique keys; the first U + 1 are written
+ *   value_len_host           int64, optional   the value buffer's length sum_k count_k * dims[k] (from the host arguments)
+ *   unique_key_split_host    int64[K + 1], optional: a host copy of unique_key_split, the only output that synchronises
+ *                            (SYNC); without it the call makes no host round trip.
+ * Limits, checked on the host before the device is selected (MONO_ERR_INVALID_ARGUMENT, nothing launched):
+ * 1 <= K <= 2^25, key_split[0] == 0 and non-decreasing, M = key_split[K] <= 2^30, every dims[k] >= 1.
+ * Kernel launches do not grow with K. */
+int mono_unique_key_with_value_and_offset(int32_t device, const int64_t* key_dev, const int64_t* key_split_host,
+                                          int32_t num_tables, const int32_t* dims_host, int64_t* unique_key_dev,
+                                          int64_t* unique_key_split_dev, int64_t* value_offset_dev,
+                                          int64_t* value_offset_split_dev, int64_t* value_len_host,
+                                          int64_t* unique_key_split_host, void* stream);
+
+/* ref: RaggedSplitByIndicesOp, RT/ops/split_by_indices_op.cc:188-243.  A stable split of a ragged tensor of K rows
+ * (values_dev, with row splits num_split_dev[K + 1] on the device) by indices_dev[t] in [0, S).  values_dev and
+ * indices_dev have `capacity` entries, of which the first n = num_split[K] are the tensor.  Outputs, the S ragged
+ * tensors concatenated split after split, each in input order:
+ *   values_out_dev      int64[capacity]   split s's values at [split_offsets[s], split_offsets[s + 1])
+ *   pos_out_dev         int64[capacity]   the input index of every value, same layout
+ *   row_splits_out_dev  int64[S * (K + 1)]  split s's own row splits (starting at 0) at s * (K + 1)
+ *   split_offsets_dev   int64[S + 1]
+ *   bad_dev             int32[1], optional: 1 when an index lies outside [0, S) (that value goes to split 0; the
+ *                       reference writes out of bounds) or num_split does not start at 0, decreases or ends beyond
+ *                       `capacity`; else 0
+ *   row_splits_host     int64[S * (K + 1)], optional: a host copy of row_splits_out, the only output that synchronises
+ *                       (SYNC); the call then also returns MONO_ERR_INVALID_ARGUMENT when bad would be set.
+ * Limits, checked on the host before the device is selected (MONO_ERR_INVALID_ARGUMENT, nothing launched): K >= 1,
+ * S >= 1, S * K <= 2^31, 0 <= capacity <= 2^30. */
+int mono_ragged_split_by_indices(int32_t device, const int64_t* indices_dev, const int64_t* values_dev,
+                                 int64_t capacity, const int64_t* num_split_dev, int32_t num_tables,
+                                 int32_t num_splits, int64_t* values_out_dev, int64_t* pos_out_dev,
+                                 int64_t* row_splits_out_dev, int64_t* split_offsets_dev, int32_t* bad_dev,
+                                 int64_t* row_splits_host, void* stream);
+
+/* ref: FillWithOffsetMapOp, RT/ops/unique_mapping_ops.cc:204-268.  One server's n = pos_split_host[K] rows: row t
+ * belongs to table k (pos_split_host) and is dims_host[k] floats of value_dev, rows packed in row order; pos_dev[t] is
+ * the unique ordinal of its key.  The row is copied to every offset value_offset[value_offset_split[pos[t]] ..
+ * value_offset_split[pos[t] + 1]) of buffer_dev (the unique op's outputs; num_unique = U).  Across
+ * the S servers' calls every float of the buffer is written once.  bad_dev (int32[1], optional): 1 when a pos lies
+ * outside [0, num_unique) (that row is not copied), else 0.  No host round trip.
+ * MONO_ERR_INVALID_ARGUMENT, before the device is selected: K >= 1, pos_split[0] == 0 and non-decreasing, n <= 2^30,
+ * every dims[k] >= 1, num_unique in [0, 2^30], and value_len >= sum_k count_k * dims[k]
+ * (a longer value is accepted, as in the reference). */
+int mono_fill_with_offset_map(int32_t device, const int64_t* pos_dev, const int64_t* pos_split_host,
+                              int32_t num_tables, const int32_t* dims_host, const float* value_dev, int64_t value_len,
+                              const int64_t* value_offset_dev, const int64_t* value_offset_split_dev,
+                              int64_t num_unique, float* buffer_dev, int32_t* bad_dev, void* stream);
+
+/* ref: FillWithOffsetMapGradientOp, RT/ops/unique_mapping_ops.cc:284-329.  The same rows: out_dev row t
+ * (sum_k count_k * dims[k] floats, packed in row order) = +0.0f + grad[o_1 ..] + grad[o_2 ..] + ... in fp32 over the
+ * offsets of pos[t]'s occurrences, in occurrence order: the reference's setZero followed by sequential +=, bit for bit
+ * at every run length.  A key's occurrences are summed by one lane group, so a run costs time linear in its length.
+ * bad_dev as above (that row is +0.0).  No host round trip.  MONO_ERR_INVALID_ARGUMENT as above, without value_len. */
+int mono_fill_with_offset_map_grad(int32_t device, const int64_t* pos_dev, const int64_t* pos_split_host,
+                                   int32_t num_tables, const int32_t* dims_host, const float* grad_dev,
+                                   const int64_t* value_offset_dev, const int64_t* value_offset_split_dev,
+                                   int64_t num_unique, float* out_dev, int32_t* bad_dev, void* stream);
+
 /* ---- owner grouping: one grouping per batch shared by the sharded forward and backward -------
  * Replaces FusedReorderByIndices (ref: RT/ops/fused_reorder_by_indices.cc:38-123) + the float-atomic
  * FusedGatherGrad scatter (ref: RT/ops/map_id_to_embedding.cu.cc:75-118) for ONE id list on the

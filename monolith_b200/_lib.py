@@ -118,6 +118,10 @@ SIGNATURES = {
     "mono_dedup": (C.c_int, [_i32, _p, _i64, _p, _p, _p, _p, _p]),
     "mono_sharding_sparse_fids": (C.c_int, [_i32, _p, _p, C.POINTER(ShardingFeature), _i32, _i32, _i32, _i32, _p, _p,
                                             _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "mono_unique_key_with_value_and_offset": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "mono_ragged_split_by_indices": (C.c_int, [_i32, _p, _p, _i64, _p, _i32, _i32, _p, _p, _p, _p, _p, _p, _p]),
+    "mono_fill_with_offset_map": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _i64, _p, _p, _p]),
+    "mono_fill_with_offset_map_grad": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _p, _p]),
     "mono_grouping_create": (C.c_int, [_i32, C.POINTER(_p)]),
     "mono_grouping_destroy": (C.c_int, [_p]),
     "mono_grouping_build": (C.c_int, [_p, _p, _i64, _i32, _i32, _p, _p, _p, C.POINTER(_i64), _p]),

@@ -354,8 +354,8 @@ static int sort_passes(int bits) { return std::max(1, (bits + kRadixBits - 1) / 
 // stable LSD radix sort of (keys[i] >> pre_shift, i) over `bits` key bits, then the ordered run list (one run per
 // distinct key; claim_set != null: the keys are its slots and each run's resolved row is gathered into w.rowidx).
 // Everything stays on the stream; counts stay on the device.
-static const uint2* sort_and_runs(const SortWs& w, const uint32_t* keys, int64_t M, int bits, int pre_shift,
-                                  const Entry* claim_set, cudaStream_t s) {
+static const uint2* sort_pairs(const SortWs& w, const uint32_t* keys, int64_t M, int bits, int pre_shift,
+                               cudaStream_t s) {
   const int passes = sort_passes(bits);
   const int nb = radix_blocks(M);
   const void* in = keys;
@@ -388,7 +388,12 @@ static const uint2* sort_and_runs(const SortWs& w, const uint32_t* keys, int64_t
     in = out;
     out = (out == w.a) ? w.b : w.a;
   }
-  const uint2* sorted = static_cast<const uint2*>(in);
+  return static_cast<const uint2*>(in);
+}
+
+static const uint2* sort_and_runs(const SortWs& w, const uint32_t* keys, int64_t M, int bits, int pre_shift,
+                                  const Entry* claim_set, cudaStream_t s) {
+  const uint2* sorted = sort_pairs(w, keys, M, bits, pre_shift, s);
   const int nr = run_blocks(M);
   runs_count_kernel<<<resident_grid(runs_count_kernel, nr, 1), kThreads, 0, s>>>(sorted, M, nr, w.blk_runs);
   MONO_CHECK_LAUNCH();
@@ -1344,6 +1349,15 @@ static BwdScratch scratch_plan(int64_t M, int D, int bits, unsigned parts, char*
   w.sorted = nullptr;
   w.bytes = off;
   return w;
+}
+
+size_t key_sort_bytes(int64_t M, int bits) { return scratch_plan(M, 1, bits, 0, nullptr).bytes; }
+
+SortWs key_sort(char* ws, const uint32_t* keys, int64_t M, int bits, bool runs, const uint2** sorted,
+                cudaStream_t s) {
+  const BwdScratch w = scratch_plan(M, 1, bits, 0, ws);
+  *sorted = runs ? sort_and_runs(w.sort, keys, M, bits, 0, nullptr, s) : sort_pairs(w.sort, keys, M, bits, 0, s);
+  return w.sort;
 }
 
 // The reduce reads and writes gradient rows as 4-element vectors (16 bytes; 8 of bf16 rows, elem_bytes = 2), one

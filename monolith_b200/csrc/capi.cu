@@ -698,6 +698,58 @@ int mono_dedup(int32_t device, const int64_t* ids_dev, int64_t n, int64_t* uniqu
   });
 }
 
+int mono_unique_key_with_value_and_offset(int32_t device, const int64_t* key_dev, const int64_t* key_split_host,
+                                          int32_t num_tables, const int32_t* dims_host, int64_t* unique_key_dev,
+                                          int64_t* unique_key_split_dev, int64_t* value_offset_dev,
+                                          int64_t* value_offset_split_dev, int64_t* value_len_host,
+                                          int64_t* unique_key_split_host, void* stream) {
+  return guarded([&] {
+    require(key_split_host && dims_host && unique_key_dev && unique_key_split_dev && value_offset_dev &&
+                value_offset_split_dev,
+            "unique_key_with_value_and_offset: null argument");
+    run_unique_offset(device, key_dev, key_split_host, num_tables, dims_host, unique_key_dev, unique_key_split_dev,
+                      value_offset_dev, value_offset_split_dev, value_len_host, unique_key_split_host,
+                      (cudaStream_t)stream);
+  });
+}
+
+int mono_ragged_split_by_indices(int32_t device, const int64_t* indices_dev, const int64_t* values_dev,
+                                 int64_t capacity, const int64_t* num_split_dev, int32_t num_tables,
+                                 int32_t num_splits, int64_t* values_out_dev, int64_t* pos_out_dev,
+                                 int64_t* row_splits_out_dev, int64_t* split_offsets_dev, int32_t* bad_dev,
+                                 int64_t* row_splits_host, void* stream) {
+  return guarded([&] {
+    require(num_split_dev && values_out_dev && pos_out_dev && row_splits_out_dev && split_offsets_dev &&
+                (capacity == 0 || (indices_dev && values_dev)),
+            "ragged_split_by_indices: null argument");
+    run_ragged_split(device, indices_dev, values_dev, capacity, num_split_dev, num_tables, num_splits, values_out_dev,
+                     pos_out_dev, row_splits_out_dev, split_offsets_dev, bad_dev, row_splits_host,
+                     (cudaStream_t)stream);
+  });
+}
+
+int mono_fill_with_offset_map(int32_t device, const int64_t* pos_dev, const int64_t* pos_split_host,
+                              int32_t num_tables, const int32_t* dims_host, const float* value_dev, int64_t value_len,
+                              const int64_t* value_offset_dev, const int64_t* value_offset_split_dev,
+                              int64_t num_unique, float* buffer_dev, int32_t* bad_dev, void* stream) {
+  return guarded([&] {
+    require(pos_split_host && dims_host, "fill_with_offset_map: null argument");
+    run_fill_offset_map(false, device, pos_dev, pos_split_host, num_tables, dims_host, value_dev, value_len,
+                        value_offset_dev, value_offset_split_dev, num_unique, buffer_dev, bad_dev, (cudaStream_t)stream);
+  });
+}
+
+int mono_fill_with_offset_map_grad(int32_t device, const int64_t* pos_dev, const int64_t* pos_split_host,
+                                   int32_t num_tables, const int32_t* dims_host, const float* grad_dev,
+                                   const int64_t* value_offset_dev, const int64_t* value_offset_split_dev,
+                                   int64_t num_unique, float* out_dev, int32_t* bad_dev, void* stream) {
+  return guarded([&] {
+    require(pos_split_host && dims_host, "fill_with_offset_map_gradient: null argument");
+    run_fill_offset_map(true, device, pos_dev, pos_split_host, num_tables, dims_host, grad_dev, 0, value_offset_dev,
+                        value_offset_split_dev, num_unique, out_dev, bad_dev, (cudaStream_t)stream);
+  });
+}
+
 int mono_grouping_create(int32_t device, mono_grouping_t** out) {
   return guarded([&] {
     require(out != nullptr, "grouping_create: null out");

@@ -240,11 +240,12 @@ dd_offsets_kernel(const int64_t* __restrict__ ids, int64_t M, const int64_t* __r
   }
 }
 
-// passes 2-5 over M > 0 ids, once slot_of and the scratch set's first positions are written
-static void rank_passes(const int64_t* ids_dev, int64_t M, const int64_t* split_dev, int K, int N, int n_eff,
-                        int rank0_empty, const FirstOcc* set, const uint32_t* slot_of, int32_t* blk_cnt, int nblk,
-                        const int32_t* dims_dev, int dim0, DDTables tb, int64_t* output_dev, int32_t* rank,
-                        int32_t* fused_emb_offset_dev, cudaStream_t s) {
+// passes 2-4 over M > 0 ids, once slot_of and the scratch set's first positions are written: the small tables, the
+// unique ids in output[] and every first occurrence's ordinal inside its (shard, list) in rank[]
+static void rank_scan_passes(const int64_t* ids_dev, int64_t M, const int64_t* split_dev, int K, int N, int n_eff,
+                             int rank0_empty, const FirstOcc* set, const uint32_t* slot_of, int32_t* blk_cnt, int nblk,
+                             const int32_t* dims_dev, int dim0, DDTables tb, int64_t* output_dev, int32_t* rank,
+                             cudaStream_t s) {
   const int g = std::min(nblk, device_sms() * 8);
   dd_rank_kernel<0><<<g, kThreads, 0, s>>>(ids_dev, M, split_dev, K, N, n_eff, rank0_empty, set, slot_of, blk_cnt,
                                           nblk, tb, output_dev, rank);
@@ -254,6 +255,15 @@ static void rank_passes(const int64_t* ids_dev, int64_t M, const int64_t* split_
   dd_rank_kernel<1><<<g, kThreads, 0, s>>>(ids_dev, M, split_dev, K, N, n_eff, rank0_empty, set, slot_of, blk_cnt,
                                           nblk, tb, output_dev, rank);
   MONO_CHECK_LAUNCH();
+}
+
+// passes 2-5: the above, then every occurrence's float offset
+static void rank_passes(const int64_t* ids_dev, int64_t M, const int64_t* split_dev, int K, int N, int n_eff,
+                        int rank0_empty, const FirstOcc* set, const uint32_t* slot_of, int32_t* blk_cnt, int nblk,
+                        const int32_t* dims_dev, int dim0, DDTables tb, int64_t* output_dev, int32_t* rank,
+                        int32_t* fused_emb_offset_dev, cudaStream_t s) {
+  rank_scan_passes(ids_dev, M, split_dev, K, N, n_eff, rank0_empty, set, slot_of, blk_cnt, nblk, dims_dev, dim0, tb,
+                   output_dev, rank, s);
   dd_offsets_kernel<<<grid_for(M, kThreads), kThreads, 0, s>>>(ids_dev, M, split_dev, K, N, n_eff, rank0_empty, set,
                                                               slot_of, rank, dims_dev, dim0, tb, fused_emb_offset_dev);
   MONO_CHECK_LAUNCH();
@@ -608,6 +618,298 @@ void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits
     MONO_CUDA(cudaStreamSynchronize(s));
     if (back[(size_t)N * K]) throw ArgError("row splits must start at 0, not decrease and end at the feature's n_fids");
     std::memcpy(table_len_host, back.data(), sizeof(int32_t) * N * K);
+  }
+}
+
+// ---- UniqueKeyWithValueAndOffset (ref: unique_mapping_ops.cc:51-124) ---------------------------------------------
+//
+// The distinct keys of every table in first-occurrence order are the reorder's claim and rank passes with one shard
+// and one list per table: the rank scatter writes them table after table, and out_base[k] + rank is every key's
+// unique ordinal.  The occurrences are then grouped by ordinal with the backward's stable radix sort of (ordinal,
+// position): sorted entry q is an occurrence of ordinal run(q), runs in ordinal order and occurrences in position
+// order, which is the reference's value_offset order; the run starts are value_offset_split.
+
+// Per-call tables staged from the host (one H2D copy)
+struct UoStage {
+  int64_t* split;  // [K + 1] key_split
+  int64_t* base;   // [K]     float offset of table k's first occurrence in the value buffer
+  int32_t* dims;   // [K]
+  int32_t* ones;   // [K]     the rank passes' row widths: their float offsets are not used
+};
+
+// every occurrence: its unique ordinal (the sort key); the first K + 1 threads write unique_key_split
+__global__ void __launch_bounds__(kThreads)
+uo_ordinal_kernel(int64_t M, int K, UoStage st, const FirstOcc* __restrict__ set, const uint32_t* __restrict__ slot_of,
+                  const int32_t* __restrict__ rank, DDTables tb, uint32_t* __restrict__ ord,
+                  int64_t* __restrict__ unique_key_split) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < M || i <= K;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    if (i <= K) unique_key_split[i] = i < K ? tb.out_base[i] : *tb.n_unique;
+    if (i >= M) continue;
+    const int m = K > 1 ? list_of(st.split, K, i) : 0;
+    ord[i] = (uint32_t)(tb.out_base[m] + rank[set[slot_of[i]].first_pos]);
+  }
+}
+
+// sorted entry q -> value_offset[q]; run j -> value_offset_split[j] (run_start[U] = M)
+__global__ void __launch_bounds__(kThreads)
+uo_emit_kernel(int64_t M, int K, UoStage st, const uint2* __restrict__ sorted, const uint32_t* __restrict__ run_start,
+               const uint32_t* __restrict__ n_runs, int64_t* __restrict__ value_offset,
+               int64_t* __restrict__ value_offset_split) {
+  const int64_t U = *n_runs;
+  for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < M || q <= U;
+       q += (int64_t)gridDim.x * blockDim.x) {
+    if (q <= U) value_offset_split[q] = run_start[q];
+    if (q >= M) continue;
+    const int64_t i = sorted[q].y;
+    const int m = K > 1 ? list_of(st.split, K, i) : 0;
+    value_offset[q] = st.base[m] + (i - st.split[m]) * st.dims[m];
+  }
+}
+
+static int key_bits(int64_t n) {  // bits of a key in [0, n)
+  int bits = 1;
+  while (((int64_t)1 << bits) < n) ++bits;
+  return bits;
+}
+
+void run_unique_offset(int device, const int64_t* key_dev, const int64_t* key_split_host, int K,
+                       const int32_t* dims_host, int64_t* unique_key_dev, int64_t* unique_key_split_dev,
+                       int64_t* value_offset_dev, int64_t* value_offset_split_dev, int64_t* value_len_host,
+                       int64_t* unique_key_split_host, cudaStream_t s) {
+  // every argument check runs before the device is touched
+  if (K <= 0) throw ArgError("unique_key_with_value_and_offset: num_tables must be positive");
+  if (K > kMaxLists) throw ArgError("unique_key_with_value_and_offset: num_tables > 2^25 is not supported");
+  if (key_split_host[0] != 0) throw ArgError("unique_key_with_value_and_offset: key_split must start at 0");
+  for (int k = 0; k < K; ++k) {
+    if (key_split_host[k + 1] < key_split_host[k])
+      throw ArgError("unique_key_with_value_and_offset: key_split must not decrease");
+    if (dims_host[k] <= 0) throw ArgError("unique_key_with_value_and_offset: dims must be positive");
+  }
+  const int64_t M = key_split_host[K];
+  if (M > kMaxIds) throw ArgError("unique_key_with_value_and_offset: more than 2^30 keys in one call");
+  MONO_CUDA(cudaSetDevice(device));
+
+  size_t off = 0;
+  auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 15) & ~(size_t)15; return o; };
+  const size_t o_split = take(sizeof(int64_t) * (K + 1)), o_base = take(sizeof(int64_t) * K),
+               o_dims = take(sizeof(int32_t) * K), o_ones = take(sizeof(int32_t) * K);
+  const size_t stage_bytes = off;
+  std::vector<char> h(stage_bytes);
+  int64_t* hbase = reinterpret_cast<int64_t*>(h.data() + o_base);
+  int32_t* hones = reinterpret_cast<int32_t*>(h.data() + o_ones);
+  std::memcpy(h.data() + o_split, key_split_host, sizeof(int64_t) * (K + 1));
+  std::memcpy(h.data() + o_dims, dims_host, sizeof(int32_t) * K);
+  int64_t floats = 0;
+  for (int k = 0; k < K; ++k) {
+    hbase[k] = floats;
+    hones[k] = 1;
+    floats += (key_split_host[k + 1] - key_split_host[k]) * dims_host[k];
+  }
+  if (value_len_host) *value_len_host = floats;
+
+  const int nblk = (int)std::max<int64_t>(1, (M + kTile - 1) / kTile);
+  const size_t M1 = (size_t)std::max<int64_t>(M, 1);
+  const uint32_t cap = claim_set_slots((int64_t)M1);
+  const int bits = key_bits((int64_t)M1);
+  off = 0;
+  auto take256 = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_set = take256(sizeof(FirstOcc) * cap), o_slot = take256(sizeof(uint32_t) * M1),
+               o_rank = take256(sizeof(int32_t) * M1), o_ord = take256(sizeof(uint32_t) * M1),
+               o_blk = take256(sizeof(int32_t) * nblk), o_small = take256(sizeof(int32_t) * (4 * (size_t)K + 9)),
+               o_stage = take256(stage_bytes), o_sort = take256(key_sort_bytes((int64_t)M1, bits));
+  char* ws = nullptr;
+  MONO_CUDA(cudaMallocAsync((void**)&ws, off, s));
+  FirstOcc* set = reinterpret_cast<FirstOcc*>(ws + o_set);
+  uint32_t* slot_of = reinterpret_cast<uint32_t*>(ws + o_slot);
+  int32_t* rank = reinterpret_cast<int32_t*>(ws + o_rank);
+  uint32_t* ord = reinterpret_cast<uint32_t*>(ws + o_ord);
+  int32_t* blk_cnt = reinterpret_cast<int32_t*>(ws + o_blk);
+  int32_t* small = reinterpret_cast<int32_t*>(ws + o_small);
+  char* stage = ws + o_stage;
+  DDTables tb;
+  tb.sizes = small;
+  tb.shard_sz = small + K;
+  tb.out_base = tb.shard_sz + 1;
+  tb.emb_base = tb.out_base + K;
+  tb.list_rank0 = tb.emb_base + K;
+  tb.n_unique = tb.list_rank0 + K;
+  UoStage st;
+  st.split = reinterpret_cast<int64_t*>(stage + o_split);
+  st.base = reinterpret_cast<int64_t*>(stage + o_base);
+  st.dims = reinterpret_cast<int32_t*>(stage + o_dims);
+  st.ones = reinterpret_cast<int32_t*>(stage + o_ones);
+
+  // a pageable H2D copy is staged by the driver before the call returns: h may go out of scope after it
+  MONO_CUDA(cudaMemcpyAsync(stage, h.data(), stage_bytes, cudaMemcpyHostToDevice, s));
+  MONO_CUDA(cudaMemsetAsync(small, 0, sizeof(int32_t) * (4 * (size_t)K + 9), s));
+  if (M > 0) {
+    MONO_CUDA(cudaMemsetAsync(set, 0xFF, sizeof(FirstOcc) * cap, s));
+    dd_claim_kernel<<<grid_for(M, kThreads), kThreads, 0, s>>>(key_dev, M, st.split, K, set, cap - 1, slot_of);
+    MONO_CHECK_LAUNCH();
+    rank_scan_passes(key_dev, M, st.split, K, 1, 1, 0, set, slot_of, blk_cnt, nblk, st.ones, 1, tb, unique_key_dev,
+                     rank, s);
+  }
+  uo_ordinal_kernel<<<grid_for(std::max<int64_t>(M, K + 1), kThreads), kThreads, 0, s>>>(
+      M, K, st, set, slot_of, rank, tb, ord, unique_key_split_dev);
+  MONO_CHECK_LAUNCH();
+  if (M > 0) {
+    const uint2* sorted = nullptr;
+    const SortWs sw = key_sort(ws + o_sort, ord, M, bits, true, &sorted, s);
+    uo_emit_kernel<<<grid_for(M + 1, kThreads), kThreads, 0, s>>>(M, K, st, sorted, sw.run_start, sw.n_runs,
+                                                                  value_offset_dev, value_offset_split_dev);
+    MONO_CHECK_LAUNCH();
+  } else {
+    MONO_CUDA(cudaMemsetAsync(value_offset_split_dev, 0, sizeof(int64_t), s));
+  }
+  if (unique_key_split_host)
+    MONO_CUDA(cudaMemcpyAsync(unique_key_split_host, unique_key_split_dev, sizeof(int64_t) * (K + 1),
+                              cudaMemcpyDeviceToHost, s));
+  MONO_CUDA(cudaFreeAsync(ws, s));
+  if (unique_key_split_host) MONO_CUDA(cudaStreamSynchronize(s));
+}
+
+// ---- RaggedSplitByIndices (ref: split_by_indices_op.cc:188-243) -------------------------------------------------
+//
+// A counting partition of the n (<= capacity) values by index, stable: (index, position) pairs through the backward's
+// radix sort, the (split, table) counts by a count pass and one scan block.  The outputs are the S ragged tensors
+// concatenated split after split: split s owns [split_offsets[s], split_offsets[s + 1]) of values_out and pos_out,
+// and its own K + 1 row splits at row_splits_out[s * (K + 1)].  The value count n is num_split[K], read on the
+// device; entries from n to the capacity sort behind every split (key S) and are not written.
+
+// every entry: its sort key, and the (split, table) counts; bad = 1 for an index outside [0, S) (sorted and counted
+// as split 0, as a defined stand-in) or a num_split that does not start at 0, decreases or exceeds the capacity
+__global__ void __launch_bounds__(kThreads)
+rsi_count_kernel(const int64_t* __restrict__ indices, int64_t cap, const int64_t* __restrict__ num_split, int K, int S,
+                 uint32_t* __restrict__ keys, uint32_t* __restrict__ cnt, int32_t* __restrict__ bad) {
+  const int64_t n = num_split[K];
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < cap || t < K;
+       t += (int64_t)gridDim.x * blockDim.x) {
+    if (t < K && (num_split[t + 1] < num_split[t] || (t == 0 && num_split[0] != 0) || (t == K - 1 && n > cap)))
+      *bad = 1;
+    int64_t cell = -1;  // the (split, table) counter of a counted entry
+    if (t < cap) {
+      int64_t sp = S;
+      if (t < n && n <= cap) {
+        sp = indices[t];
+        if (sp < 0 || sp >= S) {
+          *bad = 1;
+          sp = 0;
+        }
+        cell = sp * K + (K > 1 ? list_of(num_split, K, t) : 0);
+      }
+      keys[t] = (uint32_t)sp;
+    }
+    // one atomic per distinct counter of the warp (few counters take all of a batch: S * K is small)
+    const uint32_t peers = __match_any_sync(__activemask(), cell);
+    if (cell >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(cnt + cell, (uint32_t)__popc(peers));
+  }
+}
+
+// one block: every split's row splits from its table counts, then the split offsets (exclusive scan over splits)
+__global__ void __launch_bounds__(1024)
+rsi_scan_kernel(const uint32_t* __restrict__ cnt, int K, int S, int64_t* __restrict__ row_splits,
+                int64_t* __restrict__ split_offsets) {
+  __shared__ int64_t wsum[32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int per = (S + 1023) / 1024;
+  const int b = min(S, (int)threadIdx.x * per), e = min(S, b + per);
+  int64_t sum = 0;
+  for (int s = b; s < e; ++s) {
+    int64_t run = 0;
+    int64_t* rs = row_splits + (size_t)s * (K + 1);
+    rs[0] = 0;
+    for (int k = 0; k < K; ++k) {
+      run += cnt[(size_t)s * K + k];
+      rs[k + 1] = run;
+    }
+    sum += run;
+  }
+  int64_t x = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int64_t y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) wsum[w] = x;
+  __syncthreads();
+  if (w == 0) {
+    int64_t t = wsum[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int64_t y = __shfl_up_sync(0xffffffffu, t, o);
+      if (lane >= o) t += y;
+    }
+    wsum[lane] = t;
+  }
+  __syncthreads();
+  int64_t run = (w ? wsum[w - 1] : 0) + x - sum;
+  for (int s = b; s < e; ++s) {
+    split_offsets[s] = run;
+    run += row_splits[(size_t)s * (K + 1) + K];
+  }
+  if (threadIdx.x == 1023) split_offsets[S] = wsum[31];
+}
+
+__global__ void __launch_bounds__(kThreads)
+rsi_scatter_kernel(const int64_t* __restrict__ values, const uint2* __restrict__ sorted, int64_t cap,
+                   const int64_t* __restrict__ split_offsets, int S, int64_t* __restrict__ values_out,
+                   int64_t* __restrict__ pos_out) {
+  const int64_t n = split_offsets[S];
+  for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < n && q < cap;
+       q += (int64_t)gridDim.x * blockDim.x) {
+    const uint32_t t = sorted[q].y;
+    values_out[q] = values[t];
+    pos_out[q] = t;
+  }
+}
+
+void run_ragged_split(int device, const int64_t* indices_dev, const int64_t* values_dev, int64_t cap,
+                      const int64_t* num_split_dev, int K, int S, int64_t* values_out_dev, int64_t* pos_out_dev,
+                      int64_t* row_splits_out_dev, int64_t* split_offsets_dev, int32_t* bad_dev,
+                      int64_t* row_splits_host, cudaStream_t s) {
+  if (K <= 0) throw ArgError("ragged_split_by_indices: num_tables must be positive");
+  if (S <= 0) throw ArgError("ragged_split_by_indices: num_splits must be positive");
+  if (cap < 0 || cap > kMaxIds) throw ArgError("ragged_split_by_indices: capacity outside [0, 2^30]");
+  if ((int64_t)S * K > ((int64_t)1 << 31)) throw ArgError("ragged_split_by_indices: num_splits x num_tables > 2^31");
+  MONO_CUDA(cudaSetDevice(device));
+  const size_t C1 = (size_t)std::max<int64_t>(cap, 1);
+  const int bits = key_bits((int64_t)S + 1);  // keys 0 .. S
+  size_t off = 0;
+  auto take256 = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_keys = take256(sizeof(uint32_t) * C1), o_cnt = take256(sizeof(uint32_t) * (size_t)S * K),
+               o_bad = take256(sizeof(int32_t)), o_sort = take256(key_sort_bytes((int64_t)C1, bits));
+  char* ws = nullptr;
+  MONO_CUDA(cudaMallocAsync((void**)&ws, off, s));
+  uint32_t* keys = reinterpret_cast<uint32_t*>(ws + o_keys);
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(ws + o_cnt);
+  int32_t* bad = reinterpret_cast<int32_t*>(ws + o_bad);
+  MONO_CUDA(cudaMemsetAsync(ws + o_cnt, 0, o_sort - o_cnt, s));  // the counters and the flag
+  rsi_count_kernel<<<grid_for(std::max<int64_t>(cap, K), kThreads), kThreads, 0, s>>>(indices_dev, cap, num_split_dev,
+                                                                                      K, S, keys, cnt, bad);
+  MONO_CHECK_LAUNCH();
+  rsi_scan_kernel<<<1, 1024, 0, s>>>(cnt, K, S, row_splits_out_dev, split_offsets_dev);
+  MONO_CHECK_LAUNCH();
+  if (cap > 0) {
+    const uint2* sorted = nullptr;
+    key_sort(ws + o_sort, keys, cap, bits, false, &sorted, s);
+    rsi_scatter_kernel<<<grid_for(cap, kThreads), kThreads, 0, s>>>(values_dev, sorted, cap, split_offsets_dev, S,
+                                                                    values_out_dev, pos_out_dev);
+    MONO_CHECK_LAUNCH();
+  }
+  if (bad_dev) MONO_CUDA(cudaMemcpyAsync(bad_dev, bad, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+  int32_t bad_host = 0;
+  if (row_splits_host) {
+    MONO_CUDA(cudaMemcpyAsync(row_splits_host, row_splits_out_dev, sizeof(int64_t) * (size_t)S * (K + 1),
+                              cudaMemcpyDeviceToHost, s));
+    MONO_CUDA(cudaMemcpyAsync(&bad_host, bad, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  }
+  MONO_CUDA(cudaFreeAsync(ws, s));
+  if (row_splits_host) {
+    MONO_CUDA(cudaStreamSynchronize(s));
+    if (bad_host)
+      throw ArgError("ragged_split_by_indices: an index outside [0, num_splits), or num_split does not start at 0, "
+                     "decreases or exceeds the capacity");
   }
 }
 

@@ -510,6 +510,12 @@ void run_scatter_rows(int device, const int32_t* offs_dev, int64_t M, int dim, c
                       int grad_col, float* out_rows, int64_t total_floats, cudaStream_t s, bool bf16 = false,
                       const float* grad_scale = nullptr);
 
+// bwd.cu: the backward's stable LSD radix sort of (keys[i], i) over `bits` key bits (keys < 2^bits), stand-alone in
+// key_sort_bytes(M, bits) bytes of scratch at ws; runs: also the ordered run list (the returned regions' run_start
+// [n_runs + 1] and *n_runs).  *sorted receives the sorted {key, position} pairs.
+size_t key_sort_bytes(int64_t M, int bits);
+SortWs key_sort(char* ws, const uint32_t* keys, int64_t M, int bits, bool runs, const uint2** sorted, cudaStream_t s);
+
 // dedup.cu
 void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_host, int K, int N,
                  const int32_t* dims_host, int rank0_empty, int64_t* output_dev, int32_t* sizes_dev,
@@ -521,6 +527,16 @@ void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits
                   uint64_t* fid_offset_dev, int32_t* feature_offset_dev, uint32_t* nfl_offset_dev,
                   int64_t* row_splits_out_dev, int32_t* table_len_dev, int32_t* shard_len_dev, int32_t* emb_len_dev,
                   int32_t* bad_row_splits_dev, int32_t* table_len_host, cudaStream_t s);
+
+// the async parameter-server worker path (mono_unique_key_with_value_and_offset, mono_ragged_split_by_indices)
+void run_unique_offset(int device, const int64_t* key_dev, const int64_t* key_split_host, int K,
+                       const int32_t* dims_host, int64_t* unique_key_dev, int64_t* unique_key_split_dev,
+                       int64_t* value_offset_dev, int64_t* value_offset_split_dev, int64_t* value_len_host,
+                       int64_t* unique_key_split_host, cudaStream_t s);
+void run_ragged_split(int device, const int64_t* indices_dev, const int64_t* values_dev, int64_t cap,
+                      const int64_t* num_split_dev, int K, int S, int64_t* values_out_dev, int64_t* pos_out_dev,
+                      int64_t* row_splits_out_dev, int64_t* split_offsets_dev, int32_t* bad_dev,
+                      int64_t* row_splits_host, cudaStream_t s);
 
 // layout.cu; T: element type of the pooled rows, float or __nv_bfloat16
 template <typename T>
@@ -543,6 +559,13 @@ void check_reduce_split(const mono_reduce_feature* feats, int n_features);
 template <typename T>
 void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int n_features, int32_t* bad_splits_dev,
                          cudaStream_t s, const float* grad_scale = nullptr);
+
+// mono_fill_with_offset_map (grad = false: src = the server's rows, dst = the value buffer) and
+// mono_fill_with_offset_map_grad (grad = true: src = the value buffer's gradient, dst = the server's row gradients)
+void run_fill_offset_map(bool grad, int device, const int64_t* pos_dev, const int64_t* pos_split_host, int K,
+                         const int32_t* dims_host, const float* src_dev, int64_t src_len,
+                         const int64_t* value_offset_dev, const int64_t* value_offset_split_dev, int64_t num_unique,
+                         float* dst_dev, int32_t* bad_dev, cudaStream_t s);
 
 // clip.cu
 void check_global_norm(const mono_norm_tensor* tensors, int n_tensors, float clip_norm, const float* norm_dev,

@@ -615,6 +615,49 @@ __device__ __forceinline__ bool rs_vec(const RsFeat& f, const RsSlice& sl, const
          (sl.stride & 3) == 0 && (reinterpret_cast<uintptr_t>(tower_row) & (4 * sizeof(T) - 1)) == 0;
 }
 
+// The occurrence rows of one sum: get() is the address of the current occurrence's column c, advance() moves on
+struct RsStridedRows {  // rows row_stride floats apart (ReduceSum)
+  const float* p;
+  int64_t stride;
+  __device__ __forceinline__ const float* get() const { return p; }
+  __device__ __forceinline__ void advance() { p += stride; }
+};
+struct RsOffsetRows {  // rows at float offsets (FillWithOffsetMapGradient)
+  const float* base;   // the gradient buffer plus column c
+  const int64_t* off;  // the occurrences' float offsets, in occurrence order
+  __device__ __forceinline__ const float* get() const { return base + *off; }
+  __device__ __forceinline__ void advance() { ++off; }
+};
+
+// +0.0 + row_0 + row_1 + ... + row_{n-1}, strictly in that order, for the 4 columns a lane owns (c .. c + 3 when vec,
+// else c, c + G, c + 2G, c + 3G below dim), the rows staged kRsStage at a time through the lane's slot of `stage`
+template <int G, class Rows>
+__device__ __forceinline__ float4 rs_sum_rows(float4 (*stage)[kThreads], float* slot, Rows rows, int n, int c, int dim,
+                                              bool vec) {
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);  // ReduceSumOp's zero-filled output (reduce_op.cc:44)
+  for (int j0 = 0; j0 < n; j0 += kRsStage) {
+    const int m = min(kRsStage, n - j0);
+    for (int k = 0; k < m; ++k, rows.advance()) {
+      const float* p = rows.get();
+      if (vec) {
+        rs_cp_async16(slot + k * kThreads * 4, p);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          if (c + i * G < dim) rs_cp_async4(slot + k * kThreads * 4 + i, p + i * G);
+      }
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    for (int k = 0; k < m; ++k) {
+      const float4 x = stage[k][threadIdx.x];
+      acc.x = __fadd_rn(acc.x, x.x); acc.y = __fadd_rn(acc.y, x.y);
+      acc.z = __fadd_rn(acc.z, x.z); acc.w = __fadd_rn(acc.w, x.w);
+    }
+  }
+  return acc;
+}
+
 template <typename T, int G>
 __device__ __forceinline__ void reduce_split_fwd(const RsArgs& a) {
   __shared__ float4 stage[kRsStage][kThreads];
@@ -634,27 +677,7 @@ __device__ __forceinline__ void reduce_split_fwd(const RsArgs& a) {
     const int step = vec ? 1 : G;
     float* slot = reinterpret_cast<float*>(&stage[0][threadIdx.x]);
     for (int c = vec ? gl * 4 : gl; c < sl.dim; c += 4 * G) {
-      const float* p = occ + sl.col + c;
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);  // ReduceSumOp's zero-filled output (reduce_op.cc:44)
-      for (int j0 = 0; j0 < n; j0 += kRsStage) {
-        const int m = min(kRsStage, n - j0);
-        for (int k = 0; k < m; ++k, p += rstride) {
-          if (vec) {
-            rs_cp_async16(slot + k * kThreads * 4, p);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              if (c + i * G < sl.dim) rs_cp_async4(slot + k * kThreads * 4 + i, p + i * G);
-          }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        for (int k = 0; k < m; ++k) {
-          const float4 x = stage[k][threadIdx.x];
-          acc.x = __fadd_rn(acc.x, x.x); acc.y = __fadd_rn(acc.y, x.y);
-          acc.z = __fadd_rn(acc.z, x.z); acc.w = __fadd_rn(acc.w, x.w);
-        }
-      }
+      float4 acc = rs_sum_rows<G>(stage, slot, RsStridedRows{occ + sl.col + c, rstride}, n, c, sl.dim, vec);
       if (f.pooling == MONO_POOL_MEAN) {
         const float mult = rs_mean_factor(n);
         acc.x = __fmul_rn(acc.x, mult); acc.y = __fmul_rn(acc.y, mult);
@@ -851,5 +874,304 @@ template void launch_reduce_split<float>(bool, const mono_reduce_feature*, int, 
                                          const float*);
 template void launch_reduce_split<__nv_bfloat16>(bool, const mono_reduce_feature*, int, int32_t*, cudaStream_t,
                                                  const float*);
+
+// ------------------------------------------------------------------------------------------
+// FillWithOffsetMap and its gradient (ref: RT/ops/unique_mapping_ops.cc:204-329): the n rows of one parameter server,
+// row t of table k(t) (pos_split) with dims[k] floats, packed in row order, and each row's unique key pos[t], whose
+// occurrences sit at value_offset[value_offset_split[pos[t]] ..].  The forward is the ReduceSum gradient's broadcast
+// copy and the gradient the ReduceSum forward's sequential sum (rs_sum_rows), with occurrence rows addressed through
+// value_offset instead of a row stride.  The forward runs over occurrences so that a hot key's copies spread over
+// the grid; the gradient keeps one lane group per row, its adds in occurrence order.
+// ------------------------------------------------------------------------------------------
+struct FoStage {
+  int64_t* split;  // [K + 1] pos_split
+  int64_t* base;   // [K]     float offset of table k's first row in the packed rows
+  int32_t* dims;   // [K]
+};
+
+struct FoArgs {
+  const int64_t* pos;
+  int64_t n;                  // rows
+  int K;
+  FoStage st;
+  const int64_t* value_offset;
+  const int64_t* value_offset_split;
+  int64_t num_unique;
+  int32_t* bad;
+};
+
+// table of row t: the last k with split[k] <= t
+__device__ __forceinline__ int fo_table(const int64_t* __restrict__ split, int K, int64_t t) {
+  int lo = 0, hi = K - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (split[mid] <= t) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// row t: its table, dim and first float in the packed rows; false (and bad = 1) for a pos outside [0, num_unique)
+__device__ __forceinline__ bool fo_row(const FoArgs& a, int64_t t, int* dim, int64_t* row, int64_t* occ_lo,
+                                       int64_t* occ_n) {
+  const int k = a.K > 1 ? fo_table(a.st.split, a.K, t) : 0;
+  *dim = a.st.dims[k];
+  *row = a.st.base[k] + (t - a.st.split[k]) * *dim;
+  const int64_t p = a.pos[t];
+  if (p < 0 || p >= a.num_unique) {
+    *a.bad = 1;
+    *occ_lo = *occ_n = 0;
+    return false;
+  }
+  *occ_lo = a.value_offset_split[p];
+  *occ_n = a.value_offset_split[p + 1] - *occ_lo;
+  return true;
+}
+
+// The forward's occurrences are spread over the whole grid, so that a hot key's copies run in parallel: a three-pass
+// scan of the rows' occurrence counts (tile sums of kFillRows rows, one block over the tile sums, the rows' starts),
+// then one lane group per occurrence, which finds its row by binary search over the starts.
+constexpr int kFillRows = 4 * kThreads;
+
+// tile_occ[b] = occurrences of tile b's rows
+__global__ void __launch_bounds__(kThreads) fill_count_kernel(FoArgs a, int64_t n_tiles, int64_t* __restrict__ tile_occ) {
+  __shared__ int64_t wsum[kThreads / 32];
+  for (int64_t b = blockIdx.x; b < n_tiles; b += gridDim.x) {
+    int64_t sum = 0;
+    for (int i = threadIdx.x; i < kFillRows; i += kThreads) {
+      const int64_t t = b * kFillRows + i;
+      if (t >= a.n) break;
+      int dim;
+      int64_t row, lo, n;
+      fo_row(a, t, &dim, &row, &lo, &n);
+      sum += n;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_down_sync(0xffffffffu, sum, o);
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = sum;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int64_t tot = 0;
+      for (int w = 0; w < kThreads / 32; ++w) tot += wsum[w];
+      tile_occ[b] = tot;
+    }
+    __syncthreads();
+  }
+}
+
+// one block: in-place exclusive scan of v[0, n), v[n] = the total
+__global__ void __launch_bounds__(1024) fill_scan_kernel(int64_t* __restrict__ v, int64_t n) {
+  __shared__ int64_t wsum[32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t per = (n + 1023) / 1024;
+  const int64_t b = min(n, (int64_t)threadIdx.x * per), e = min(n, b + per);
+  int64_t sum = 0;
+  for (int64_t i = b; i < e; ++i) sum += v[i];
+  int64_t x = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int64_t y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) wsum[w] = x;
+  __syncthreads();
+  if (w == 0) {
+    int64_t t = wsum[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int64_t y = __shfl_up_sync(0xffffffffu, t, o);
+      if (lane >= o) t += y;
+    }
+    wsum[lane] = t;
+  }
+  __syncthreads();
+  int64_t run = (w ? wsum[w - 1] : 0) + x - sum;
+  for (int64_t i = b; i < e; ++i) {
+    const int64_t c = v[i];
+    v[i] = run;
+    run += c;
+  }
+  if (threadIdx.x == 1023) v[n] = wsum[31];
+}
+
+// occ_start[t] = tile_off[tile of t] + occurrences of the rows before t in its tile; occ_start[n] = the total
+__global__ void __launch_bounds__(kThreads)
+fill_rows_kernel(FoArgs a, int64_t n_tiles, const int64_t* __restrict__ tile_off, int64_t* __restrict__ occ_start) {
+  constexpr int R = kFillRows / kThreads;  // rows per thread: thread i owns rows R i .. R i + R - 1 of the tile
+  __shared__ int64_t wsum[kThreads / 32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int64_t b = blockIdx.x; b < n_tiles; b += gridDim.x) {
+    const int64_t t0 = b * kFillRows;
+    int64_t cnt[R], sum = 0;
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const int64_t t = t0 + threadIdx.x * R + r;
+      cnt[r] = 0;
+      if (t < a.n) {
+        int dim;
+        int64_t row, lo;
+        fo_row(a, t, &dim, &row, &lo, &cnt[r]);
+      }
+      sum += cnt[r];
+    }
+    int64_t x = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int64_t y = __shfl_up_sync(0xffffffffu, x, o);
+      if (lane >= o) x += y;
+    }
+    if (lane == 31) wsum[w] = x;
+    __syncthreads();
+    int64_t run = tile_off[b] + x - sum;
+    for (int ww = 0; ww < w; ++ww) run += wsum[ww];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const int64_t t = t0 + threadIdx.x * R + r;
+      if (t < a.n) occ_start[t] = run;
+      run += cnt[r];
+    }
+    if (b == n_tiles - 1 && threadIdx.x == 0) occ_start[a.n] = tile_off[n_tiles];
+    __syncthreads();
+  }
+}
+
+// one lane group per occurrence q: the row t whose occurrences hold q (the last t with occ_start[t] <= q), copied
+// to the occurrence's offset
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+fill_copy_kernel(FoArgs a, const int64_t* __restrict__ occ_start, const float* __restrict__ value,
+                 float* __restrict__ buffer) {
+  const int gl = Group<G>::gl();
+  const int64_t total = occ_start[a.n];
+  const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
+  for (int64_t q = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G; q < total; q += gstride) {
+    int64_t lo = 0, hi = a.n - 1;
+    while (lo < hi) {
+      const int64_t mid = (lo + hi + 1) >> 1;
+      if (occ_start[mid] <= q) lo = mid; else hi = mid - 1;
+    }
+    const int k = a.K > 1 ? fo_table(a.st.split, a.K, lo) : 0;
+    const int dim = a.st.dims[k];
+    const float* src = value + a.st.base[k] + (lo - a.st.split[k]) * dim;
+    float* dst = buffer + a.value_offset[a.value_offset_split[a.pos[lo]] + (q - occ_start[lo])];
+    for (int c = gl; c < dim; c += G) dst[c] = __ldg(src + c);
+  }
+}
+
+// one lane group per row: out row t = +0.0 + g[o_1 ..] + g[o_2 ..] + ... over its key's occurrences, in order
+template <int G>
+__global__ void __launch_bounds__(kThreads, 4)
+fill_grad_kernel(FoArgs a, const float* __restrict__ grad, float* __restrict__ out) {
+  __shared__ float4 stage[kRsStage][kThreads];
+  const int64_t t = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
+  if (t >= a.n) return;
+  int dim;
+  int64_t row, lo, n;
+  fo_row(a, t, &dim, &row, &lo, &n);
+  const int gl = Group<G>::gl();
+  float* slot = reinterpret_cast<float*>(&stage[0][threadIdx.x]);
+  for (int c = gl; c < dim; c += 4 * G) {
+    const float4 acc = rs_sum_rows<G>(stage, slot, RsOffsetRows{grad + c, a.value_offset + lo}, (int)n, c, dim, false);
+    float* dst = out + row + c;
+    dst[0] = acc.x;
+    if (c + G < dim) dst[G] = acc.y;
+    if (c + 2 * G < dim) dst[2 * G] = acc.z;
+    if (c + 3 * G < dim) dst[3 * G] = acc.w;
+  }
+}
+
+// Host-side checks and the staged tables; returns the packed rows' float count
+static int64_t fill_setup(const int64_t* pos_split_host, int K, const int32_t* dims_host, std::vector<char>* h,
+                          size_t* o_base, size_t* o_dims, int* max_dim) {
+  if (K <= 0) throw ArgError("fill_with_offset_map: num_tables must be positive");
+  if (pos_split_host[0] != 0) throw ArgError("fill_with_offset_map: pos_split must start at 0");
+  int64_t floats = 0;
+  *max_dim = 1;
+  const size_t o_split = 0;
+  *o_base = (sizeof(int64_t) * (K + 1) + 15) & ~(size_t)15;
+  *o_dims = *o_base + sizeof(int64_t) * K;
+  h->assign(*o_dims + sizeof(int32_t) * K, 0);
+  int64_t* split = reinterpret_cast<int64_t*>(h->data() + o_split);
+  int64_t* base = reinterpret_cast<int64_t*>(h->data() + *o_base);
+  int32_t* dims = reinterpret_cast<int32_t*>(h->data() + *o_dims);
+  for (int k = 0; k < K; ++k) {
+    if (pos_split_host[k + 1] < pos_split_host[k]) throw ArgError("fill_with_offset_map: pos_split must not decrease");
+    if (dims_host[k] <= 0) throw ArgError("fill_with_offset_map: dims must be positive");
+    base[k] = floats;
+    floats += (pos_split_host[k + 1] - pos_split_host[k]) * dims_host[k];
+    *max_dim = std::max(*max_dim, dims_host[k]);
+  }
+  std::memcpy(split, pos_split_host, sizeof(int64_t) * (K + 1));
+  std::memcpy(dims, dims_host, sizeof(int32_t) * K);
+  if (pos_split_host[K] > ((int64_t)1 << 30)) throw ArgError("fill_with_offset_map: more than 2^30 rows in one call");
+  return floats;
+}
+
+void run_fill_offset_map(bool grad, int device, const int64_t* pos_dev, const int64_t* pos_split_host, int K,
+                         const int32_t* dims_host, const float* src_dev, int64_t src_len,
+                         const int64_t* value_offset_dev, const int64_t* value_offset_split_dev, int64_t num_unique,
+                         float* dst_dev, int32_t* bad_dev, cudaStream_t s) {
+  std::vector<char> h;
+  size_t o_base, o_dims;
+  int max_dim;
+  const int64_t floats = fill_setup(pos_split_host, K, dims_host, &h, &o_base, &o_dims, &max_dim);
+  const char* who = grad ? "fill_with_offset_map_gradient" : "fill_with_offset_map";
+  if (num_unique < 0 || num_unique > ((int64_t)1 << 30))
+    throw ArgError(std::string(who) + ": num_unique must be in [0, 2^30]");
+  // ref: FillWithOffsetMapOp's value size check, unique_mapping_ops.cc:233-235 (a longer value is accepted)
+  if (!grad && src_len < floats)
+    throw ArgError("fill_with_offset_map: Value size doesn't match expected size. expected: " + std::to_string(floats) +
+                   ", actual: " + std::to_string(src_len));
+  const int64_t n = pos_split_host[K];
+  if (n > 0 && !(pos_dev && src_dev && value_offset_dev && value_offset_split_dev && dst_dev))
+    throw ArgError(std::string(who) + ": null argument");
+  MONO_CUDA(cudaSetDevice(device));
+  const size_t o_bad = (h.size() + 15) & ~(size_t)15, o_occ = o_bad + 16;
+  const int64_t n_tiles = (n + kFillRows - 1) / kFillRows;
+  const size_t bytes = o_occ + (grad ? 0 : sizeof(int64_t) * (n_tiles + 1 + n + 1));
+  char* ws = nullptr;
+  MONO_CUDA(cudaMallocAsync((void**)&ws, bytes, s));
+  // a pageable H2D copy is staged by the driver before the call returns: h may go out of scope after it
+  MONO_CUDA(cudaMemcpyAsync(ws, h.data(), h.size(), cudaMemcpyHostToDevice, s));
+  MONO_CUDA(cudaMemsetAsync(ws + o_bad, 0, 16, s));
+  FoArgs a;
+  a.pos = pos_dev;
+  a.n = n;
+  a.K = K;
+  a.st.split = reinterpret_cast<int64_t*>(ws);
+  a.st.base = reinterpret_cast<int64_t*>(ws + o_base);
+  a.st.dims = reinterpret_cast<int32_t*>(ws + o_dims);
+  a.value_offset = value_offset_dev;
+  a.value_offset_split = value_offset_split_dev;
+  a.num_unique = num_unique;
+  a.bad = reinterpret_cast<int32_t*>(ws + o_bad);
+  if (n > 0) {
+    if (grad) {
+      by_group(pick_group(max_dim), [&](auto g) {
+        constexpr int GG = decltype(g)::value;
+        fill_grad_kernel<GG><<<(unsigned)((n + kThreads / GG - 1) / (kThreads / GG)), kThreads, 0, s>>>(a, src_dev,
+                                                                                                     dst_dev);
+      });
+      MONO_CHECK_LAUNCH();
+    } else {
+      int64_t* tile_off = reinterpret_cast<int64_t*>(ws + o_occ);
+      int64_t* occ_start = tile_off + n_tiles + 1;
+      fill_count_kernel<<<grid_for(n_tiles, 1), kThreads, 0, s>>>(a, n_tiles, tile_off);
+      MONO_CHECK_LAUNCH();
+      fill_scan_kernel<<<1, 1024, 0, s>>>(tile_off, n_tiles);
+      MONO_CHECK_LAUNCH();
+      fill_rows_kernel<<<grid_for(n_tiles, 1), kThreads, 0, s>>>(a, n_tiles, tile_off, occ_start);
+      MONO_CHECK_LAUNCH();
+      // the occurrence count is on the device: one resident wave, grid-stride
+      by_group(pick_group(max_dim * 4), [&](auto g) {  // one float per lane
+        constexpr int GG = decltype(g)::value;
+        fill_copy_kernel<GG><<<resident_grid(fill_copy_kernel<GG>, INT32_MAX, 1), kThreads, 0, s>>>(a, occ_start,
+                                                                                                    src_dev, dst_dev);
+      });
+      MONO_CHECK_LAUNCH();
+    }
+  }
+  if (bad_dev) MONO_CUDA(cudaMemcpyAsync(bad_dev, a.bad, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+  MONO_CUDA(cudaFreeAsync(ws, s));
+}
 
 }  // namespace mono

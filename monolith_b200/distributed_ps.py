@@ -594,3 +594,120 @@ class ShardedStep:
     ph.mark("b9_owner_apply")
     ph.flush()
     return uniq.numel()
+
+
+class DistributedMultiTypeHashTable:
+  """The async parameter-server (PS) table on the raw API — ref: DistributedMultiTypeHashTable, NT/distributed_ps.py
+  :192-516, the table distributed_ps_factory.create_native_multi_hash_table builds for num_ps > 0.
+
+  table_factory(i, slot_to_config) -> MultiHashTable makes PS i's table; the PS tables may sit on any CUDA devices and
+  every table must hold the same tables with the same dims.  A unique key k lives on PS floormod(k, num_ps)
+  (tf.math.floormod, so key -1 with 3 PS goes to PS 2).  The worker side runs on the device of PS 0's table: dedup
+  of the keys with their occurrence offsets (unique_key_with_value_and_offset), the split by PS
+  (ragged_split_by_indices), and the fill of every PS's rows into the occurrences (fill_with_offset_map) or the sum of
+  the occurrence gradients per unique key (fill_with_offset_map_gradient).  Ids, rows and gradients cross devices
+  with plain torch copies.
+
+  lookup and apply_gradients make one host synchronisation each on the worker side: the split's per-PS row splits,
+  which the PS tables' raw calls take on the host."""
+
+  def __init__(self, num_ps: int, slot_to_config: Dict, table_factory):
+    if num_ps < 1:
+      raise ValueError("num_ps must be >= 1")
+    self._num_ps = int(num_ps)
+    self._slot_to_config = slot_to_config
+    self._tables = [table_factory(i, slot_to_config) for i in range(self._num_ps)]
+    t0 = self._tables[0]
+    for t in self._tables[1:]:
+      if tuple(t.table_names) != tuple(t0.table_names) or tuple(t.get_table_dim_sizes()) != tuple(
+          t0.get_table_dim_sizes()):
+        raise ValueError("every PS table must hold the same tables with the same dims")
+
+  @property
+  def tables(self):
+    return self._tables
+
+  def get_table_dim_sizes(self):
+    """ref: distributed_ps.py get_table_dim_sizes: PS 0's table's dims, tables in sorted-name order."""
+    return self._tables[0].get_table_dim_sizes()
+
+  def as_op(self, *args, **kwargs):
+    return self
+
+  def _unique_split(self, slot_to_id, generate_buffer):
+    from . import distribution_ops as dops
+    t0 = self._tables[0]
+    ids, splits = t0.get_ragged_id(slot_to_id)
+    dims = t0.get_table_dim_sizes()
+    res = dops.unique_key_with_value_and_offset(ids, splits, dims, generate_buffer, sync=False)
+    uniq, uniq_split = res.unique_key
+    index = torch.remainder(uniq, self._num_ps)  # tf.math.floormod; the entries past U are ignored by the split
+    sp = dops.ragged_split_by_indices(index, uniq, uniq_split, self._num_ps, sync=True)  # the one synchronisation
+    U = sum(r[-1] for r in sp.row_splits_host)
+    return splits, dims, res, sp, U
+
+  def lookup(self, slot_to_id: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """ref: distributed_ps.py:282-338 (raw API path): every slot's embeddings [n, dim], misses as the tables give them."""
+    from . import distribution_ops as dops
+    splits, dims, res, sp, U = self._unique_split(slot_to_id, True)
+    buf = res.value_buffer
+    for i, table in enumerate(self._tables):
+      (vals, _), rs = sp.splits[i], sp.row_splits_host[i]
+      flat = table.raw_lookup(vals.to(table.device), rs)
+      dops.fill_with_offset_map(sp.pos[i], rs, flat.to(buf.device), res.value_offset, buf, dims, num_unique=U,
+                                sync=False)
+    emb = self._tables[0].get_embeddings(splits, buf)
+    return {k: v for k, v in emb.items() if k in slot_to_id}
+
+  def apply_gradients(self, slot_to_id_and_grad: Dict[str, Tuple[torch.Tensor, torch.Tensor]], global_step: int = 0,
+                      req_time: int = 0) -> "DistributedMultiTypeHashTable":
+    """ref: distributed_ps.py:481-514 (raw API path): the occurrence gradients summed per unique key in occurrence
+    order, then each PS's raw_apply_gradients on its keys."""
+    from . import distribution_ops as dops
+    slot_to_id = {k: v[0] for k, v in slot_to_id_and_grad.items()}
+    splits, dims, res, sp, U = self._unique_split(slot_to_id, False)
+    flat_grad = self._tables[0].get_flat_value({k: v[1] for k, v in slot_to_id_and_grad.items()})
+    for i, table in enumerate(self._tables):
+      (vals, _), rs = sp.splits[i], sp.row_splits_host[i]
+      g = dops.fill_with_offset_map_gradient(sp.pos[i], rs, flat_grad, res.value_offset, dims, num_unique=U,
+                                             sync=False)
+      table.raw_apply_gradients(vals.to(table.device), rs, g.to(table.device), global_step=global_step,
+                                req_time=req_time)
+    return self
+
+  def _update(self, method_name: str, slot_to_id_and_value):
+    """ref: distributed_ps.py:430-451: every slot's ids and values split by floormod(id, num_ps)."""
+    from . import distribution_ops as dops
+    per_ps = [dict() for _ in range(self._num_ps)]
+    for slot, (ids, value) in slot_to_id_and_value.items():
+      ids = ids.reshape(-1).to(torch.int64)
+      index = torch.remainder(ids, self._num_ps)
+      split_ids = dops.split_by_indices(index, ids, self._num_ps)
+      split_values = dops.split_by_indices(index, value.to(ids.device), self._num_ps)
+      for i in range(self._num_ps):
+        per_ps[i][slot] = (split_ids[i], split_values[i])
+    for i, table in enumerate(self._tables):
+      dev = table.device
+      getattr(table, method_name)({k: (a.to(dev), b.to(dev)) for k, (a, b) in per_ps[i].items()})
+    return self
+
+  def assign(self, slot_to_id_and_value: Dict[str, Tuple[torch.Tensor, torch.Tensor]]):
+    """ref: distributed_ps.py:453-456."""
+    return self._update("assign", slot_to_id_and_value)
+
+  def assign_add(self, slot_to_id_and_value: Dict[str, Tuple[torch.Tensor, torch.Tensor]]):
+    """ref: distributed_ps.py:458-461."""
+    return self._update("assign_add", slot_to_id_and_value)
+
+  def reinitialize(self, slot: str, ids: torch.Tensor):
+    """ref: distributed_ps.py:463-476: the ids split by PS, each PS's status concatenated in PS order (so the status
+    follows the split, not the input order)."""
+    from . import distribution_ops as dops
+    ids = ids.reshape(-1).to(torch.int64)
+    index = torch.remainder(ids, self._num_ps)
+    split_ids = dops.split_by_indices(index, ids, self._num_ps)
+    status = []
+    for i, table in enumerate(self._tables):
+      _, st = table.reinitialize(slot, split_ids[i].to(table.device))
+      status.append(st.to(ids.device))
+    return self, torch.cat(status)

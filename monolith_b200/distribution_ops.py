@@ -753,3 +753,183 @@ def fused_embedding_to_layout_grad(emb_sizes: Sequence[int], emb_strides: Sequen
           lib.mono_embedding_to_layout_grad_scaled)
     _lib.check(fn(*args, sp, _stream(dev)))
   return grads
+
+
+# ---- async parameter-server worker path (ref: NT/distributed_ps.py:266-337, 430-516) --------------------------------
+def _host_splits(splits, what):
+  s = [int(x) for x in (splits.tolist() if isinstance(splits, torch.Tensor) else splits)]
+  if not s or s[0] != 0 or any(b < a for a, b in zip(s, s[1:])):
+    raise ValueError(f"{what} must start at 0 and not decrease")
+  return s
+
+
+@dataclasses.dataclass
+class UniqueKeyWithValueAndOffset:
+  """unique_key_with_value_and_offset's outputs.  unique_key = (values, row_splits): every table's distinct keys in
+  first-occurrence order, row splits int64[K + 1] on the device.  value_offset = (values, row_splits): for every unique
+  key the float offsets of all its occurrences in the value buffer, in occurrence order, and its int64 row splits over
+  the unique keys.  value_buffer: float32[value_len], uninitialised (None without generate_buffer).  num_unique: U, or
+  None with sync=False, when unique_key's values and value_offset's row splits are allocated for every key (M and
+  M + 1 entries) and only the first U and U + 1 are written."""
+  unique_key: Tuple[torch.Tensor, torch.Tensor]
+  value_offset: Tuple[torch.Tensor, torch.Tensor]
+  value_buffer: Optional[torch.Tensor]
+  value_len: int
+  num_unique: Optional[int]
+
+
+def unique_key_with_value_and_offset(ids: torch.Tensor, key_split: Sequence[int], dims: Sequence[int],
+                                     generate_buffer: bool = True, *, sync: bool = True) -> UniqueKeyWithValueAndOffset:
+  """ref: distribution_ops.unique_key_with_value_and_offset / UniqueKeyWitValueAndOffsetOp (RT/ops/unique_mapping_ops.cc
+  :51-124).  ids: int64 keys of K tables (CUDA), table k = ids[key_split[k]:key_split[k + 1]] (host row splits, as
+  MultiHashTable.get_ragged_id gives them) with dims[k] floats per row.  Occurrence i of table k sits at float
+  base_k + (i - key_split[k]) * dims[k] of the value buffer, base_k = sum of count_k' * dims[k'] over k' < k.
+  sync=True reads the K + 1 unique row splits back (one synchronisation) to trim the outputs; sync=False makes no host
+  round trip."""
+  lib = _lib.load()
+  splits = _host_splits(key_split, "key_split")
+  K = len(splits) - 1
+  if len(dims) != K:
+    raise ValueError(f"dims has {len(dims)} entries for {K} tables")
+  ids = ids.reshape(-1).to(torch.int64).contiguous()
+  if splits[-1] != ids.numel():
+    raise ValueError("key_split does not cover ids")
+  M, dev = ids.numel(), ids.device
+  i64 = dict(dtype=torch.int64, device=dev)
+  uniq, uniq_split = torch.empty(max(M, 1), **i64), torch.empty(K + 1, **i64)
+  off, off_split = torch.empty(max(M, 1), **i64), torch.empty(M + 1, **i64)
+  value_len = C.c_int64(0)
+  host = (C.c_int64 * (K + 1))() if sync else None
+  _lib.check(lib.mono_unique_key_with_value_and_offset(
+      dev.index, _ptr(ids), (C.c_int64 * (K + 1))(*splits), K, (C.c_int32 * K)(*[int(d) for d in dims]), _ptr(uniq),
+      _ptr(uniq_split), _ptr(off), _ptr(off_split), C.byref(value_len), host, _stream(dev)))
+  buf = torch.empty(value_len.value, dtype=torch.float32, device=dev) if generate_buffer else None
+  U = host[K] if sync else None
+  if sync:
+    uniq, off_split = uniq[:U], off_split[:U + 1]
+  else:
+    uniq = uniq[:M]
+  return UniqueKeyWithValueAndOffset((uniq, uniq_split), (off[:M], off_split), buf, value_len.value, U)
+
+
+@dataclasses.dataclass
+class RaggedSplit:
+  """ragged_split_by_indices' outputs.  splits[s] = (values, row_splits) of split s (row splits int64[K + 1] on the
+  device, starting at 0) and pos[s] the input index of each of its values; row_splits_host[s] the same row splits as
+  Python ints.  All three are None with sync=False.  The flat fields hold the S splits concatenated split after
+  split: values, positions, row_splits [S, K + 1], offsets [S + 1] (split s at offsets[s] .. offsets[s + 1]) and bad
+  (int32[1], 1 for an index outside [0, S) or malformed row splits)."""
+  splits: Optional[List[Tuple[torch.Tensor, torch.Tensor]]]
+  pos: Optional[List[torch.Tensor]]
+  row_splits_host: Optional[List[List[int]]]
+  values: torch.Tensor
+  positions: torch.Tensor
+  row_splits: torch.Tensor
+  offsets: torch.Tensor
+  bad: torch.Tensor
+
+
+def ragged_split_by_indices(indices: torch.Tensor, values: torch.Tensor, row_splits: torch.Tensor, num_splits: int, *,
+                            sync: bool = True) -> RaggedSplit:
+  """ref: distribution_ops.ragged_split_by_indices / RaggedSplitByIndicesOp (RT/ops/split_by_indices_op.cc:188-243):
+  the ragged tensor (values, row_splits int64[K + 1], CUDA) split by indices[t] in [0, num_splits), stably.  values
+  and indices may be longer than row_splits[K] (sync=False outputs of unique_key_with_value_and_offset); the rest is
+  ignored.  sync=True reads every split's row splits back (one synchronisation), raises ValueError for an index outside
+  [0, num_splits) or malformed row splits, and slices the splits; sync=False makes no host round trip."""
+  lib = _lib.load()
+  S = int(num_splits)
+  dev = values.device
+  values = values.reshape(-1).to(torch.int64).contiguous()
+  indices = indices.reshape(-1).to(device=dev, dtype=torch.int64).contiguous()
+  row_splits = row_splits.reshape(-1).to(device=dev, dtype=torch.int64).contiguous()
+  if indices.numel() != values.numel():
+    raise ValueError(f"Ragged tensor values size must match indices size. Got {values.numel()} v.s. {indices.numel()}")
+  K, cap = row_splits.numel() - 1, values.numel()
+  i64 = dict(dtype=torch.int64, device=dev)
+  v_out, p_out = torch.empty(max(cap, 1), **i64), torch.empty(max(cap, 1), **i64)
+  rs_out, offs = torch.empty(max(S, 0) * max(K + 1, 0), **i64), torch.empty(max(S, 0) + 1, **i64)
+  bad = torch.zeros(1, dtype=torch.int32, device=dev)
+  host = (C.c_int64 * (S * (K + 1)))() if sync and S > 0 and K > 0 else None
+  status = lib.mono_ragged_split_by_indices(dev.index, _ptr(indices), _ptr(values), cap, _ptr(row_splits), K, S,
+                                            _ptr(v_out), _ptr(p_out), _ptr(rs_out), _ptr(offs), _ptr(bad), host,
+                                            _stream(dev))
+  if status == -1:
+    raise ValueError(_lib.load().mono_last_error().decode())
+  _lib.check(status)
+  rs2 = rs_out.view(S, K + 1)
+  out = RaggedSplit(None, None, None, v_out[:cap], p_out[:cap], rs2, offs, bad)
+  if sync:
+    h = [list(host[s * (K + 1):(s + 1) * (K + 1)]) for s in range(S)]
+    starts = [0]
+    for r in h:
+      starts.append(starts[-1] + r[-1])
+    out.row_splits_host = h
+    out.splits = [(v_out[starts[s]:starts[s + 1]], rs2[s]) for s in range(S)]
+    out.pos = [p_out[starts[s]:starts[s + 1]] for s in range(S)]
+  return out
+
+
+def split_by_indices(indices: torch.Tensor, tensor: torch.Tensor, num_splits: int) -> List[torch.Tensor]:
+  """ref: distribution_ops.split_by_indices: the rows of `tensor` split by indices[i] in [0, num_splits), each split in
+  input order.  One ragged split of the positions (a single list), then index_select by them.  Synchronises once."""
+  n = indices.numel()
+  dev = tensor.device
+  positions = torch.arange(n, dtype=torch.int64, device=dev)
+  r = ragged_split_by_indices(indices, positions, torch.tensor([0, n], dtype=torch.int64, device=dev), num_splits)
+  return [tensor.index_select(0, p) for p in r.pos]
+
+
+def _fill_call(grad, pos, pos_split, src, value_offset, dims, num_unique, dst, sync):
+  lib = _lib.load()
+  splits = _host_splits(pos_split, "pos_split")
+  K = len(splits) - 1
+  if len(dims) != K:
+    raise ValueError(f"dims has {len(dims)} entries for {K} tables")
+  dev = src.device
+  pos = pos.reshape(-1).to(device=dev, dtype=torch.int64).contiguous()
+  if pos.numel() != splits[-1]:
+    raise ValueError("pos_split does not cover pos")
+  offs, offs_split = (t.reshape(-1).to(device=dev, dtype=torch.int64).contiguous() for t in value_offset)
+  U = offs_split.numel() - 1 if num_unique is None else int(num_unique)
+  src = src.reshape(-1).to(torch.float32).contiguous()
+  bad = torch.zeros(1, dtype=torch.int32, device=dev)
+  c_split, c_dims = (C.c_int64 * (K + 1))(*splits), (C.c_int32 * K)(*[int(d) for d in dims])
+  if grad:
+    status = lib.mono_fill_with_offset_map_grad(dev.index, _ptr(pos), c_split, K, c_dims, _ptr(src), _ptr(offs),
+                                                _ptr(offs_split), U, _ptr(dst), _ptr(bad), _stream(dev))
+  else:
+    status = lib.mono_fill_with_offset_map(dev.index, _ptr(pos), c_split, K, c_dims, _ptr(src), src.numel(),
+                                           _ptr(offs), _ptr(offs_split), U, _ptr(dst), _ptr(bad), _stream(dev))
+  if status == -1:
+    raise ValueError(lib.mono_last_error().decode())
+  _lib.check(status)
+  if sync and int(bad.item()):
+    raise ValueError(f"pos is bigger than offset size: a pos outside [0, {U})")
+  return dst
+
+
+def fill_with_offset_map(pos: torch.Tensor, pos_split: Sequence[int], value: torch.Tensor,
+                         value_offset: Tuple[torch.Tensor, torch.Tensor], value_buffer: torch.Tensor,
+                         dims: Sequence[int], *, num_unique: Optional[int] = None, sync: bool = True) -> torch.Tensor:
+  """ref: distribution_ops.fill_with_offset_map / FillWithOffsetMapOp (RT/ops/unique_mapping_ops.cc:204-268): one
+  server's rows `value` (row t of table k = pos_split row t, dims[k] floats, packed in row order) copied to every
+  occurrence offset of the unique key pos[t] (value_offset = the unique op's (offsets, row splits)) in value_buffer,
+  which is returned.  pos_split: host row splits.  num_unique defaults to value_offset's row splits length - 1.
+  Raises ValueError when value is shorter than the rows need (a longer one is accepted); sync=True also checks that
+  every pos lies in [0, num_unique) (one synchronisation); sync=False makes no host round trip."""
+  if value_buffer.dtype != torch.float32 or not value_buffer.is_contiguous():
+    raise ValueError("value_buffer must be a contiguous float32 tensor")
+  return _fill_call(False, pos, pos_split, value, value_offset, dims, num_unique, value_buffer, sync)
+
+
+def fill_with_offset_map_gradient(pos: torch.Tensor, pos_split: Sequence[int], grad: torch.Tensor,
+                                  value_offset: Tuple[torch.Tensor, torch.Tensor], dims: Sequence[int], *,
+                                  num_unique: Optional[int] = None, sync: bool = True) -> torch.Tensor:
+  """ref: distribution_ops.fill_with_offset_map_gradient / FillWithOffsetMapGradientOp (unique_mapping_ops.cc:284-329):
+  row t of the result (packed like fill_with_offset_map's value) is +0.0 + grad[o_1 ..] + grad[o_2 ..] + ... in fp32
+  over pos[t]'s occurrence offsets in occurrence order: the reference's bits at every run length.  sync as in
+  fill_with_offset_map."""
+  splits = _host_splits(pos_split, "pos_split")
+  n_floats = sum((splits[k + 1] - splits[k]) * int(dims[k]) for k in range(len(splits) - 1))
+  out = torch.empty(n_floats, dtype=torch.float32, device=grad.device)
+  return _fill_call(True, pos, splits, grad, value_offset, dims, num_unique, out, sync)
