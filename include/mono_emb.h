@@ -143,6 +143,13 @@ int64_t mono_mtable_max_update_ts(const mono_mtable_t* t, int32_t k);
  * (ref: cuckoo_embedding_hash_table.cc:161-171). */
 int mono_mtable_lookup(mono_mtable_t* t, const int64_t* ids_dev, const int64_t* id_split_host,
                        float* emb_out_dev, void* stream);
+/* mono_mtable_lookup with fp16 rows (the async parameter-server table's transfer_float16, ref: distributed_ps.py
+ * :392-396): emb_out_dev points at fp16 storage (a cast pointer) of sum_k n_k x D_k elements.  Bit for bit the
+ * twin's fp32 result rounded once to fp16 (__float2half_rn: nearest even, beyond the fp16 range to +-inf, below half
+ * the smallest fp16 subnormal to +-0, the sign of zero kept); a miss is +0.0.  NaN stays NaN; the engine writes
+ * 0x7FFF for every NaN (payload not kept).  Always the register-path kernel, one launch. */
+int mono_mtable_lookup_f16(mono_mtable_t* t, const int64_t* ids_dev, const int64_t* id_split_host,
+                           float* emb_out_dev, void* stream);
 
 /* ref: MonolithMultiHashTableFusedLookup, multi_hash_table_lookup_op.cc:143-197,229-255 and
  * ComputeFusedOffsets, RT/hash_table/utils.h:28-61.  ids are laid out shard-major / table-minor
@@ -534,6 +541,24 @@ int mono_fill_with_offset_map_grad(int32_t device, const int64_t* pos_dev, const
                                    int32_t num_tables, const int32_t* dims_host, const float* grad_dev,
                                    const int64_t* value_offset_dev, const int64_t* value_offset_split_dev,
                                    int64_t num_unique, float* out_dev, int32_t* bad_dev, void* stream);
+
+/* The fp16 forms, for rows and gradients sent between the servers and the worker as fp16 (transfer_float16, ref:
+ * distributed_ps.py:392-410,539-549).  Each takes its twin's arguments and checks; the 16-bit rows pass through the
+ * same float pointer (cast pointers):
+ *   mono_fill_with_offset_map_f16: value_dev holds fp16 rows and value_len counts fp16 elements.  The buffer (fp32) is
+ *     bit for bit the twin's result on the rows widened exactly to fp32.
+ *   mono_fill_with_offset_map_grad_f16: out_dev receives fp16 rows.  Bit for bit the twin's fp32 result (the same
+ *     +0.0-started sequential sum) rounded once to fp16 (__float2half_rn, as mono_mtable_lookup_f16; sums beyond the
+ *     fp16 range become +-inf).  NaN stays NaN; the engine writes 0x7FFF for every NaN. */
+int mono_fill_with_offset_map_f16(int32_t device, const int64_t* pos_dev, const int64_t* pos_split_host,
+                                  int32_t num_tables, const int32_t* dims_host, const float* value_dev,
+                                  int64_t value_len, const int64_t* value_offset_dev,
+                                  const int64_t* value_offset_split_dev, int64_t num_unique, float* buffer_dev,
+                                  int32_t* bad_dev, void* stream);
+int mono_fill_with_offset_map_grad_f16(int32_t device, const int64_t* pos_dev, const int64_t* pos_split_host,
+                                       int32_t num_tables, const int32_t* dims_host, const float* grad_dev,
+                                       const int64_t* value_offset_dev, const int64_t* value_offset_split_dev,
+                                       int64_t num_unique, float* out_dev, int32_t* bad_dev, void* stream);
 
 /* ---- owner grouping: one grouping per batch shared by the sharded forward and backward -------
  * Replaces FusedReorderByIndices (ref: RT/ops/fused_reorder_by_indices.cc:38-123) + the float-atomic

@@ -122,6 +122,9 @@ SIGNATURES = {
     "mono_ragged_split_by_indices": (C.c_int, [_i32, _p, _p, _i64, _p, _i32, _i32, _p, _p, _p, _p, _p, _p, _p]),
     "mono_fill_with_offset_map": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _i64, _p, _p, _p]),
     "mono_fill_with_offset_map_grad": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _p, _p]),
+    "mono_mtable_lookup_f16": (C.c_int, [_p, _p, _p, _p, _p]),
+    "mono_fill_with_offset_map_f16": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _i64, _p, _p, _p]),
+    "mono_fill_with_offset_map_grad_f16": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _p, _p]),
     "mono_grouping_create": (C.c_int, [_i32, C.POINTER(_p)]),
     "mono_grouping_destroy": (C.c_int, [_p]),
     "mono_grouping_build": (C.c_int, [_p, _p, _i64, _i32, _i32, _p, _p, _p, C.POINTER(_i64), _p]),

@@ -356,6 +356,18 @@ int mono_mtable_lookup(mono_mtable_t* t, const int64_t* ids_dev, const int64_t* 
   });
 }
 
+int mono_mtable_lookup_f16(mono_mtable_t* t, const int64_t* ids_dev, const int64_t* id_split_host, float* emb_out_dev,
+                           void* stream) {
+  return guarded([&] {
+    HandleGuard hg_(t);
+    int64_t n_total = 0;
+    auto segs = table_segs(t, id_split_host, 0, &n_total, nullptr);
+    if (segs.empty()) return;
+    launch_lookup(t, segs.data(), (int)segs.size(), ids_dev, n_total, reinterpret_cast<__half*>(emb_out_dev),
+                  (cudaStream_t)stream);
+  });
+}
+
 int mono_mtable_fused_offsets(const mono_mtable_t* t, const int32_t* fused_slot_size_host,
                               int32_t num_shards, int32_t* emb_splits_host,
                               int32_t* id_offsets_host, int32_t* emb_offsets_host) {
@@ -747,6 +759,30 @@ int mono_fill_with_offset_map_grad(int32_t device, const int64_t* pos_dev, const
     require(pos_split_host && dims_host, "fill_with_offset_map_gradient: null argument");
     run_fill_offset_map(true, device, pos_dev, pos_split_host, num_tables, dims_host, grad_dev, 0, value_offset_dev,
                         value_offset_split_dev, num_unique, out_dev, bad_dev, (cudaStream_t)stream);
+  });
+}
+
+int mono_fill_with_offset_map_f16(int32_t device, const int64_t* pos_dev, const int64_t* pos_split_host,
+                                  int32_t num_tables, const int32_t* dims_host, const float* value_dev,
+                                  int64_t value_len, const int64_t* value_offset_dev,
+                                  const int64_t* value_offset_split_dev, int64_t num_unique, float* buffer_dev,
+                                  int32_t* bad_dev, void* stream) {
+  return guarded([&] {
+    require(pos_split_host && dims_host, "fill_with_offset_map: null argument");
+    run_fill_offset_map(false, device, pos_dev, pos_split_host, num_tables, dims_host, value_dev, value_len,
+                        value_offset_dev, value_offset_split_dev, num_unique, buffer_dev, bad_dev, (cudaStream_t)stream,
+                        true);
+  });
+}
+
+int mono_fill_with_offset_map_grad_f16(int32_t device, const int64_t* pos_dev, const int64_t* pos_split_host,
+                                       int32_t num_tables, const int32_t* dims_host, const float* grad_dev,
+                                       const int64_t* value_offset_dev, const int64_t* value_offset_split_dev,
+                                       int64_t num_unique, float* out_dev, int32_t* bad_dev, void* stream) {
+  return guarded([&] {
+    require(pos_split_host && dims_host, "fill_with_offset_map_gradient: null argument");
+    run_fill_offset_map(true, device, pos_dev, pos_split_host, num_tables, dims_host, grad_dev, 0, value_offset_dev,
+                        value_offset_split_dev, num_unique, out_dev, bad_dev, (cudaStream_t)stream, true);
   });
 }
 

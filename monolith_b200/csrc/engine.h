@@ -2,6 +2,7 @@
 #pragma once
 
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -464,8 +465,10 @@ int64_t export_rows(mono_mtable* mt, int k, int64_t* cursor, int64_t max_n, int6
 
 // ops.cu
 enum UpsertOp { kOpOptimize = 0, kOpAssign = 1, kOpAssignAdd = 2, kOpReinit = 3, kOpRestore = 4 };
+// T: element type of the output rows, float or __half (mono_mtable_lookup_f16: each element rounded once to fp16)
+template <typename T>
 void launch_lookup(mono_mtable* mt, const CallSeg* h_segs, int nsegs, const int64_t* ids_dev,
-                   int64_t n_total, float* out_dev, cudaStream_t s);
+                   int64_t n_total, T* out_dev, cudaStream_t s);
 void launch_lookup_pool(mono_mtable* mt, int k, const int64_t* fids_dev, const int32_t* row_offsets,
                         int64_t n_rows, int pooling, float* out, int64_t out_stride, int out_col,
                         cudaStream_t s);
@@ -561,11 +564,13 @@ void launch_reduce_split(bool backward, const mono_reduce_feature* feats, int n_
                          cudaStream_t s, const float* grad_scale = nullptr);
 
 // mono_fill_with_offset_map (grad = false: src = the server's rows, dst = the value buffer) and
-// mono_fill_with_offset_map_grad (grad = true: src = the value buffer's gradient, dst = the server's row gradients)
+// mono_fill_with_offset_map_grad (grad = true: src = the value buffer's gradient, dst = the server's row gradients).
+// f16: the server's rows (src, or dst with grad) are __half behind the float pointer (the _f16 calls); src_len then
+// counts fp16 elements.
 void run_fill_offset_map(bool grad, int device, const int64_t* pos_dev, const int64_t* pos_split_host, int K,
                          const int32_t* dims_host, const float* src_dev, int64_t src_len,
                          const int64_t* value_offset_dev, const int64_t* value_offset_split_dev, int64_t num_unique,
-                         float* dst_dev, int32_t* bad_dev, cudaStream_t s);
+                         float* dst_dev, int32_t* bad_dev, cudaStream_t s, bool f16 = false);
 
 // clip.cu
 void check_global_norm(const mono_norm_tensor* tensors, int n_tensors, float clip_norm, const float* norm_dev,

@@ -1035,11 +1035,10 @@ fill_rows_kernel(FoArgs a, int64_t n_tiles, const int64_t* __restrict__ tile_off
 }
 
 // one lane group per occurrence q: the row t whose occurrences hold q (the last t with occ_start[t] <= q), copied
-// to the occurrence's offset
-template <int G>
-__global__ void __launch_bounds__(kThreads)
-fill_copy_kernel(FoArgs a, const int64_t* __restrict__ occ_start, const float* __restrict__ value,
-                 float* __restrict__ buffer) {
+// to the occurrence's offset.  T: element type of the server's rows, float or __half (widened exactly where loaded).
+template <typename T, int G>
+__device__ __forceinline__ void fill_copy(const FoArgs& a, const int64_t* __restrict__ occ_start,
+                                          const T* __restrict__ value, float* __restrict__ buffer) {
   const int gl = Group<G>::gl();
   const int64_t total = occ_start[a.n];
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
@@ -1051,16 +1050,31 @@ fill_copy_kernel(FoArgs a, const int64_t* __restrict__ occ_start, const float* _
     }
     const int k = a.K > 1 ? fo_table(a.st.split, a.K, lo) : 0;
     const int dim = a.st.dims[k];
-    const float* src = value + a.st.base[k] + (lo - a.st.split[k]) * dim;
+    const T* src = value + a.st.base[k] + (lo - a.st.split[k]) * dim;
     float* dst = buffer + a.value_offset[a.value_offset_split[a.pos[lo]] + (q - occ_start[lo])];
-    for (int c = gl; c < dim; c += G) dst[c] = __ldg(src + c);
+    for (int c = gl; c < dim; c += G) dst[c] = row_elem_f32(__ldg(src + c));
   }
 }
 
-// one lane group per row: out row t = +0.0 + g[o_1 ..] + g[o_2 ..] + ... over its key's occurrences, in order
 template <int G>
-__global__ void __launch_bounds__(kThreads, 4)
-fill_grad_kernel(FoArgs a, const float* __restrict__ grad, float* __restrict__ out) {
+__global__ void __launch_bounds__(kThreads)
+fill_copy_kernel(FoArgs a, const int64_t* __restrict__ occ_start, const float* __restrict__ value,
+                 float* __restrict__ buffer) {
+  fill_copy<float, G>(a, occ_start, value, buffer);
+}
+
+// mono_fill_with_offset_map_f16: fp16 server rows
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+f16_fill_copy_kernel(FoArgs a, const int64_t* __restrict__ occ_start, const __half* __restrict__ value,
+                     float* __restrict__ buffer) {
+  fill_copy<__half, G>(a, occ_start, value, buffer);
+}
+
+// one lane group per row: out row t = +0.0 + g[o_1 ..] + g[o_2 ..] + ... over its key's occurrences, in order.
+// T: element type of the output rows, float or __half (the fp32 sum rounded once where it is stored).
+template <typename T, int G>
+__device__ __forceinline__ void fill_grad(const FoArgs& a, const float* __restrict__ grad, T* __restrict__ out) {
   __shared__ float4 stage[kRsStage][kThreads];
   const int64_t t = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
   if (t >= a.n) return;
@@ -1071,12 +1085,25 @@ fill_grad_kernel(FoArgs a, const float* __restrict__ grad, float* __restrict__ o
   float* slot = reinterpret_cast<float*>(&stage[0][threadIdx.x]);
   for (int c = gl; c < dim; c += 4 * G) {
     const float4 acc = rs_sum_rows<G>(stage, slot, RsOffsetRows{grad + c, a.value_offset + lo}, (int)n, c, dim, false);
-    float* dst = out + row + c;
-    dst[0] = acc.x;
-    if (c + G < dim) dst[G] = acc.y;
-    if (c + 2 * G < dim) dst[2 * G] = acc.z;
-    if (c + 3 * G < dim) dst[3 * G] = acc.w;
+    T* dst = out + row + c;
+    dst[0] = to_row_elem(acc.x, dst);
+    if (c + G < dim) dst[G] = to_row_elem(acc.y, dst);
+    if (c + 2 * G < dim) dst[2 * G] = to_row_elem(acc.z, dst);
+    if (c + 3 * G < dim) dst[3 * G] = to_row_elem(acc.w, dst);
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads, 4)
+fill_grad_kernel(FoArgs a, const float* __restrict__ grad, float* __restrict__ out) {
+  fill_grad<float, G>(a, grad, out);
+}
+
+// mono_fill_with_offset_map_grad_f16: fp16 output rows
+template <int G>
+__global__ void __launch_bounds__(kThreads, 4)
+f16_fill_grad_kernel(FoArgs a, const float* __restrict__ grad, __half* __restrict__ out) {
+  fill_grad<__half, G>(a, grad, out);
 }
 
 // Host-side checks and the staged tables; returns the packed rows' float count
@@ -1109,7 +1136,7 @@ static int64_t fill_setup(const int64_t* pos_split_host, int K, const int32_t* d
 void run_fill_offset_map(bool grad, int device, const int64_t* pos_dev, const int64_t* pos_split_host, int K,
                          const int32_t* dims_host, const float* src_dev, int64_t src_len,
                          const int64_t* value_offset_dev, const int64_t* value_offset_split_dev, int64_t num_unique,
-                         float* dst_dev, int32_t* bad_dev, cudaStream_t s) {
+                         float* dst_dev, int32_t* bad_dev, cudaStream_t s, bool f16) {
   std::vector<char> h;
   size_t o_base, o_dims;
   int max_dim;
@@ -1148,8 +1175,11 @@ void run_fill_offset_map(bool grad, int device, const int64_t* pos_dev, const in
     if (grad) {
       by_group(pick_group(max_dim), [&](auto g) {
         constexpr int GG = decltype(g)::value;
-        fill_grad_kernel<GG><<<(unsigned)((n + kThreads / GG - 1) / (kThreads / GG)), kThreads, 0, s>>>(a, src_dev,
-                                                                                                     dst_dev);
+        const unsigned grid = (unsigned)((n + kThreads / GG - 1) / (kThreads / GG));
+        if (f16)
+          f16_fill_grad_kernel<GG><<<grid, kThreads, 0, s>>>(a, src_dev, reinterpret_cast<__half*>(dst_dev));
+        else
+          fill_grad_kernel<GG><<<grid, kThreads, 0, s>>>(a, src_dev, dst_dev);
       });
       MONO_CHECK_LAUNCH();
     } else {
@@ -1162,10 +1192,14 @@ void run_fill_offset_map(bool grad, int device, const int64_t* pos_dev, const in
       fill_rows_kernel<<<grid_for(n_tiles, 1), kThreads, 0, s>>>(a, n_tiles, tile_off, occ_start);
       MONO_CHECK_LAUNCH();
       // the occurrence count is on the device: one resident wave, grid-stride
-      by_group(pick_group(max_dim * 4), [&](auto g) {  // one float per lane
+      by_group(pick_group(max_dim * 4), [&](auto g) {  // one element per lane
         constexpr int GG = decltype(g)::value;
-        fill_copy_kernel<GG><<<resident_grid(fill_copy_kernel<GG>, INT32_MAX, 1), kThreads, 0, s>>>(a, occ_start,
-                                                                                                    src_dev, dst_dev);
+        if (f16)
+          f16_fill_copy_kernel<GG><<<resident_grid(f16_fill_copy_kernel<GG>, INT32_MAX, 1), kThreads, 0, s>>>(
+              a, occ_start, reinterpret_cast<const __half*>(src_dev), dst_dev);
+        else
+          fill_copy_kernel<GG><<<resident_grid(fill_copy_kernel<GG>, INT32_MAX, 1), kThreads, 0, s>>>(a, occ_start,
+                                                                                                      src_dev, dst_dev);
       });
       MONO_CHECK_LAUNCH();
     }

@@ -166,6 +166,17 @@ lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ s
                                                parts);
 }
 
+// mono_mtable_lookup_f16: lookup_kernel with fp16 output rows, each element rounded once where it is stored (a miss
+// stores +0.0).  The same arguments as lookup_kernel; parts is always null here.
+template <int G, bool SINGLE, bool DUAL = false, bool CONFIRM = true>
+__global__ void __launch_bounds__(kThreads, SINGLE && !DUAL ? 6 : 4)
+f16_lookup_kernel(const TableDev* __restrict__ tables, const CallSeg* __restrict__ segs, int nsegs,
+                  const int64_t* __restrict__ ids, int64_t n_total, __half* __restrict__ out, int64_t out_stride,
+                  int out_col, int prefetch, const FwdPart* __restrict__ parts = nullptr) {
+  lookup_rows<__half, G, SINGLE, DUAL, CONFIRM>(tables, segs, nsegs, ids, n_total, out, out_stride, out_col, prefetch,
+                                                parts);
+}
+
 // one-FID parts of lookup_pool_parts_bf16 (lookup_kernel<G, true, false, CONFIRM> with bf16 rows)
 template <int G, bool CONFIRM>
 __global__ void __launch_bounds__(kThreads, 6)
@@ -988,7 +999,8 @@ static int max_dim_of(mono_mtable* mt, const CallSeg* h_segs, int nsegs) {
   return m;
 }
 
-// whether the TMA variant serves a one-FID-per-row lookup of table k into out_dev
+// whether the TMA variant serves a one-FID-per-row lookup of table k into out_dev.  fp32 rows only: it copies rows
+// unchanged, so fp16 output rows (mono_mtable_lookup_f16) always take the register path (f16_lookup_kernel).
 static bool tma_applies(mono_mtable* mt, int k, const float* out_dev, int64_t out_stride, int out_col) {
   static const int env_mode = [] {  // MONO_LOOKUP_TMA=0/1 presets mono_set_option("lookup_tma")
     const char* e = std::getenv("MONO_LOOKUP_TMA");
@@ -1048,8 +1060,26 @@ static void launch_lookup_staged(mono_mtable* mt, const CallSeg* d_segs, int nse
   MONO_CHECK_LAUNCH();
 }
 
+// fp16 output rows: the same selection over f16_lookup_kernel
+static void launch_lookup_staged(mono_mtable* mt, const CallSeg* d_segs, int nsegs, int G,
+                                 const int64_t* ids_dev, int64_t n_total, __half* out_dev,
+                                 int64_t out_stride, int out_col, cudaStream_t s) {
+  const int pf = knob(KNOB_LOOKUP_PF);
+  by_group(G, [&](auto g) {
+    constexpr int GG = decltype(g)::value;
+    const auto kern = nsegs == 1 && knob(KNOB_LOOKUP_DUAL) ? f16_lookup_kernel<GG, true, true>
+                      : nsegs == 1 && !mt->lookup_must_confirm(s) ? f16_lookup_kernel<GG, true, false, false>
+                      : nsegs == 1 ? f16_lookup_kernel<GG, true>
+                      : f16_lookup_kernel<GG, false>;
+    kern<<<resident_grid(kern, n_total, kThreads), kThreads, 0, s>>>(mt->d_tables, d_segs, nsegs, ids_dev, n_total,
+                                                                     out_dev, out_stride, out_col, pf, nullptr);
+  });
+  MONO_CHECK_LAUNCH();
+}
+
+template <typename T>
 void launch_lookup(mono_mtable* mt, const CallSeg* h_segs, int nsegs, const int64_t* ids_dev,
-                   int64_t n_total, float* out_dev, cudaStream_t s) {
+                   int64_t n_total, T* out_dev, cudaStream_t s) {
   if (n_total <= 0) return;
   upload_tables(mt, s);
   // merge adjacent segments of the same table whose ids and output rows are contiguous (fused_lookup
@@ -1069,13 +1099,17 @@ void launch_lookup(mono_mtable* mt, const CallSeg* h_segs, int nsegs, const int6
   }
   h_segs = merged.data();
   nsegs = (int)merged.size();
-  if (nsegs == 1 && h_segs[0].id_begin == 0 &&
-      try_lookup_tma(mt, h_segs[0].table, ids_dev, n_total, out_dev + h_segs[0].val_off, 0, 0, s))
-    return;
+  if constexpr (std::is_same_v<T, float>) {
+    if (nsegs == 1 && h_segs[0].id_begin == 0 &&
+        try_lookup_tma(mt, h_segs[0].table, ids_dev, n_total, out_dev + h_segs[0].val_off, 0, 0, s))
+      return;
+  }
   CallBlob cb = stage_call(mt, h_segs, nsegs, nullptr, 0, s);
   launch_lookup_staged(mt, cb.segs, nsegs, pick_group(max_dim_of(mt, h_segs, nsegs)), ids_dev, n_total,
                        out_dev, 0, 0, s);
 }
+template void launch_lookup<float>(mono_mtable*, const CallSeg*, int, const int64_t*, int64_t, float*, cudaStream_t);
+template void launch_lookup<__half>(mono_mtable*, const CallSeg*, int, const int64_t*, int64_t, __half*, cudaStream_t);
 
 void launch_lookup_push(mono_mtable* mt, int k, const int64_t* ids_dev, int64_t n_total, const PeerOut& po,
                         cudaStream_t s) {

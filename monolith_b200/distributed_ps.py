@@ -609,12 +609,19 @@ class DistributedMultiTypeHashTable:
   with plain torch copies.
 
   lookup and apply_gradients make one host synchronisation each on the worker side: the split's per-PS row splits,
-  which the PS tables' raw calls take on the host."""
+  which the PS tables' raw calls take on the host.
 
-  def __init__(self, num_ps: int, slot_to_config: Dict, table_factory):
+  transfer_float16 (ref: distributed_ps.py:201,207,392-410,539-549): rows and gradients cross between the servers and
+  the worker as fp16.  Each server's lookup writes its rows rounded to fp16 and the worker's fill widens them; the
+  worker's gradient sums are rounded to fp16 and each server widens them (exactly) before its apply.  So a looked-up
+  value is f32(f16(row)) and a server applies f32(f16(sum)), which is what the reference's per-slot path with the
+  casts computes.  assign, assign_add and reinitialize send fp32, as in the reference."""
+
+  def __init__(self, num_ps: int, slot_to_config: Dict, table_factory, transfer_float16: bool = False):
     if num_ps < 1:
       raise ValueError("num_ps must be >= 1")
     self._num_ps = int(num_ps)
+    self._transfer_dtype = torch.float16 if transfer_float16 else torch.float32
     self._slot_to_config = slot_to_config
     self._tables = [table_factory(i, slot_to_config) for i in range(self._num_ps)]
     t0 = self._tables[0]
@@ -630,6 +637,10 @@ class DistributedMultiTypeHashTable:
   def get_table_dim_sizes(self):
     """ref: distributed_ps.py get_table_dim_sizes: PS 0's table's dims, tables in sorted-name order."""
     return self._tables[0].get_table_dim_sizes()
+
+  @property
+  def transfer_float16(self) -> bool:
+    return self._transfer_dtype == torch.float16
 
   def as_op(self, *args, **kwargs):
     return self
@@ -653,7 +664,7 @@ class DistributedMultiTypeHashTable:
     buf = res.value_buffer
     for i, table in enumerate(self._tables):
       (vals, _), rs = sp.splits[i], sp.row_splits_host[i]
-      flat = table.raw_lookup(vals.to(table.device), rs)
+      flat = table.raw_lookup(vals.to(table.device), rs, dtype=self._transfer_dtype)
       dops.fill_with_offset_map(sp.pos[i], rs, flat.to(buf.device), res.value_offset, buf, dims, num_unique=U,
                                 sync=False)
     emb = self._tables[0].get_embeddings(splits, buf)
@@ -670,9 +681,11 @@ class DistributedMultiTypeHashTable:
     for i, table in enumerate(self._tables):
       (vals, _), rs = sp.splits[i], sp.row_splits_host[i]
       g = dops.fill_with_offset_map_gradient(sp.pos[i], rs, flat_grad, res.value_offset, dims, num_unique=U,
-                                             sync=False)
-      table.raw_apply_gradients(vals.to(table.device), rs, g.to(table.device), global_step=global_step,
-                                req_time=req_time)
+                                             sync=False, dtype=self._transfer_dtype)
+      g = g.to(table.device)
+      if self.transfer_float16:
+        g = g.float()  # the server's exact widening (the reference's CastToFloat32 on the PS)
+      table.raw_apply_gradients(vals.to(table.device), rs, g, global_step=global_step, req_time=req_time)
     return self
 
   def _update(self, method_name: str, slot_to_id_and_value):

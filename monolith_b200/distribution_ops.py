@@ -891,15 +891,19 @@ def _fill_call(grad, pos, pos_split, src, value_offset, dims, num_unique, dst, s
     raise ValueError("pos_split does not cover pos")
   offs, offs_split = (t.reshape(-1).to(device=dev, dtype=torch.int64).contiguous() for t in value_offset)
   U = offs_split.numel() - 1 if num_unique is None else int(num_unique)
-  src = src.reshape(-1).to(torch.float32).contiguous()
+  # fp16 server rows are read as they are (the _f16 fill widens them exactly); anything else is widened here
+  f16_src = not grad and src.dtype == torch.float16
+  src = src.reshape(-1).to(torch.float16 if f16_src else torch.float32).contiguous()
   bad = torch.zeros(1, dtype=torch.int32, device=dev)
   c_split, c_dims = (C.c_int64 * (K + 1))(*splits), (C.c_int32 * K)(*[int(d) for d in dims])
   if grad:
-    status = lib.mono_fill_with_offset_map_grad(dev.index, _ptr(pos), c_split, K, c_dims, _ptr(src), _ptr(offs),
-                                                _ptr(offs_split), U, _ptr(dst), _ptr(bad), _stream(dev))
+    fn = lib.mono_fill_with_offset_map_grad_f16 if dst.dtype == torch.float16 else lib.mono_fill_with_offset_map_grad
+    status = fn(dev.index, _ptr(pos), c_split, K, c_dims, _ptr(src), _ptr(offs), _ptr(offs_split), U, _ptr(dst),
+                _ptr(bad), _stream(dev))
   else:
-    status = lib.mono_fill_with_offset_map(dev.index, _ptr(pos), c_split, K, c_dims, _ptr(src), src.numel(),
-                                           _ptr(offs), _ptr(offs_split), U, _ptr(dst), _ptr(bad), _stream(dev))
+    fn = lib.mono_fill_with_offset_map_f16 if f16_src else lib.mono_fill_with_offset_map
+    status = fn(dev.index, _ptr(pos), c_split, K, c_dims, _ptr(src), src.numel(), _ptr(offs), _ptr(offs_split), U,
+                _ptr(dst), _ptr(bad), _stream(dev))
   if status == -1:
     raise ValueError(lib.mono_last_error().decode())
   _lib.check(status)
@@ -916,7 +920,9 @@ def fill_with_offset_map(pos: torch.Tensor, pos_split: Sequence[int], value: tor
   occurrence offset of the unique key pos[t] (value_offset = the unique op's (offsets, row splits)) in value_buffer,
   which is returned.  pos_split: host row splits.  num_unique defaults to value_offset's row splits length - 1.
   Raises ValueError when value is shorter than the rows need (a longer one is accepted); sync=True also checks that
-  every pos lies in [0, num_unique) (one synchronisation); sync=False makes no host round trip."""
+  every pos lies in [0, num_unique) (one synchronisation); sync=False makes no host round trip.  A float16 value (rows
+  sent as fp16, transfer_float16) is read as fp16 and widened exactly in the copy; another dtype is converted to
+  float32 first."""
   if value_buffer.dtype != torch.float32 or not value_buffer.is_contiguous():
     raise ValueError("value_buffer must be a contiguous float32 tensor")
   return _fill_call(False, pos, pos_split, value, value_offset, dims, num_unique, value_buffer, sync)
@@ -924,12 +930,16 @@ def fill_with_offset_map(pos: torch.Tensor, pos_split: Sequence[int], value: tor
 
 def fill_with_offset_map_gradient(pos: torch.Tensor, pos_split: Sequence[int], grad: torch.Tensor,
                                   value_offset: Tuple[torch.Tensor, torch.Tensor], dims: Sequence[int], *,
-                                  num_unique: Optional[int] = None, sync: bool = True) -> torch.Tensor:
+                                  num_unique: Optional[int] = None, sync: bool = True,
+                                  dtype: torch.dtype = torch.float32) -> torch.Tensor:
   """ref: distribution_ops.fill_with_offset_map_gradient / FillWithOffsetMapGradientOp (unique_mapping_ops.cc:284-329):
   row t of the result (packed like fill_with_offset_map's value) is +0.0 + grad[o_1 ..] + grad[o_2 ..] + ... in fp32
   over pos[t]'s occurrence offsets in occurrence order: the reference's bits at every run length.  sync as in
-  fill_with_offset_map."""
+  fill_with_offset_map.  dtype=torch.float16 returns the same sums, each rounded once to fp16 (the gradients a
+  transfer_float16 worker sends to its servers)."""
+  if dtype not in (torch.float32, torch.float16):
+    raise ValueError(f"fill_with_offset_map_gradient: dtype must be torch.float32 or torch.float16, not {dtype}")
   splits = _host_splits(pos_split, "pos_split")
   n_floats = sum((splits[k + 1] - splits[k]) * int(dims[k]) for k in range(len(splits) - 1))
-  out = torch.empty(n_floats, dtype=torch.float32, device=grad.device)
+  out = torch.empty(n_floats, dtype=dtype, device=grad.device)
   return _fill_call(True, pos, splits, grad, value_offset, dims, num_unique, out, sync)

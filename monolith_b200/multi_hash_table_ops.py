@@ -250,14 +250,19 @@ class MultiHashTable:
     return self
 
   # ---- RawMultiTypeHashTable API (ref: multi_hash_table_ops.py:492-526) ------------------------
-  def raw_lookup(self, ids: torch.Tensor, id_split: Sequence[int]) -> torch.Tensor:
+  def raw_lookup(self, ids: torch.Tensor, id_split: Sequence[int], dtype: torch.dtype = torch.float32) -> torch.Tensor:
+    """The rows of ids (table k = ids[id_split[k]:id_split[k + 1]]) packed table after table, misses as +0.0.
+    dtype=torch.float16: the same rows, each element rounded once to fp16 (the async parameter-server table's
+    transfer_float16)."""
+    if dtype not in (torch.float32, torch.float16):
+      raise ValueError(f"raw_lookup: dtype must be torch.float32 or torch.float16, not {dtype}")
     ids = _ids(ids, self._device)
     total = sum((id_split[k + 1] - id_split[k]) * self._dims[k] for k in range(len(self._dims)))
-    out = torch.empty(total, dtype=torch.float32, device=self._device)
+    out = torch.empty(total, dtype=dtype, device=self._device)
     if id_split[-1] != ids.numel():
       raise ValueError("id_split does not cover ids")
-    _lib.check(self._lib.mono_mtable_lookup(self._h, _ptr(ids), self._split_arr(id_split), _ptr(out),
-                                            _stream(self._device)))
+    fn = self._lib.mono_mtable_lookup_f16 if dtype == torch.float16 else self._lib.mono_mtable_lookup
+    _lib.check(fn(self._h, _ptr(ids), self._split_arr(id_split), _ptr(out), _stream(self._device)))
     return out
 
   def _check_values(self, ids, id_split, flat):

@@ -16,7 +16,13 @@ clock around a synchronised step.  The card's name and power limit are read in t
 Workloads: c3, Criteo-shaped: 26 tables of dim 16, B one key per sample per table, per-table Zipf(1.1) keys; c2,
 MovieLens-shaped: 2 tables (uid, movie) of dim 32, Zipf(1.05) over 5 M ranks each.
 
+--transfer-float16: the table's transfer_float16 path.  The servers' lookup writes fp16 rows, the fill reads them, the
+fill gradient writes fp16 sums and the apply phase includes each server's widening of them to fp32.  Rows and
+gradients between servers and worker then count 2 bytes per element in the algorithmic bytes.  --host-steps 0 skips
+the host comparison step.
+
   python scripts/bench_async_ps.py [--workload c3 c2] [--num-ps 1 4] [--batch 65536] [--steps 20] [--warmup 5]
+                                   [--host-steps 2] [--transfer-float16]
 """
 import argparse
 import json
@@ -66,13 +72,14 @@ def timed(fn, times, key):
   return out
 
 
-def phase_bytes(M, U, rows_floats, occ_floats):
-  """M occurrences, U unique keys, rows_floats = sum over unique keys of their dim, occ_floats = the value buffer"""
+def phase_bytes(M, U, rows_floats, occ_floats, row_bytes=4):
+  """M occurrences, U unique keys, rows_floats = sum over unique keys of their dim, occ_floats = the value buffer;
+  row_bytes: bytes per element of the rows and row gradients between servers and worker (2 with transfer_float16)"""
   return {
       "unique": 8 * M + 8 * U + 8 * M + 8 * (U + 1),          # keys in; unique keys, offsets, offset splits out
       "split": 8 * U + 8 * U + 8 * U + 8 * U,                  # indices and keys in; keys and positions out
-      "fill": 8 * U + 16 * U + 8 * M + 4 * rows_floats + 4 * occ_floats,   # pos, splits, offsets, rows in; buffer out
-      "fill_grad": 8 * U + 16 * U + 8 * M + 4 * occ_floats + 4 * rows_floats,
+      "fill": 8 * U + 16 * U + 8 * M + row_bytes * rows_floats + 4 * occ_floats,   # pos, splits, offsets, rows in
+      "fill_grad": 8 * U + 16 * U + 8 * M + 4 * occ_floats + row_bytes * rows_floats,
   }
 
 
@@ -81,7 +88,10 @@ def run(name, S, B, args, dev, power):
   shape = workload(name, B, rng)
   names = sorted(shape)
   dims = [shape[s][0] for s in names]
-  dmt = DistributedMultiTypeHashTable(S, configs(shape), lambda i, c: MultiHashTable(configs(shape), device=dev))
+  f16 = args.transfer_float16
+  row_dtype = torch.float16 if f16 else torch.float32
+  dmt = DistributedMultiTypeHashTable(S, configs(shape), lambda i, c: MultiHashTable(configs(shape), device=dev),
+                                      transfer_float16=f16)
   ids = {s: torch.from_numpy(shape[s][1]).to(dev) for s in names}
   grads = {s: torch.randn(shape[s][1].size, shape[s][0], device=dev) for s in names}
   dmt.apply_gradients({s: (ids[s], grads[s]) for s in names}, req_time=1)   # populate the servers
@@ -107,7 +117,8 @@ def run(name, S, B, args, dev, power):
                                         sync=False)
 
   def ph_lookup():
-    lrs["rows"] = [t.raw_lookup(sp.splits[i][0], sp.row_splits_host[i]) for i, t in enumerate(dmt.tables)]
+    lrs["rows"] = [t.raw_lookup(sp.splits[i][0], sp.row_splits_host[i], dtype=row_dtype) for i, t in
+                   enumerate(dmt.tables)]
 
   def ph_fill():
     for i in range(S):
@@ -116,11 +127,11 @@ def run(name, S, B, args, dev, power):
 
   def ph_fill_grad():
     lrs["g"] = [dops.fill_with_offset_map_gradient(sp.pos[i], sp.row_splits_host[i], flat_grad, res.value_offset, dims,
-                                                   num_unique=U, sync=False) for i in range(S)]
+                                                   num_unique=U, sync=False, dtype=row_dtype) for i in range(S)]
 
   def ph_apply():
     for i, t in enumerate(dmt.tables):
-      t.raw_apply_gradients(sp.splits[i][0], sp.row_splits_host[i], lrs["g"][i], req_time=2)
+      t.raw_apply_gradients(sp.splits[i][0], sp.row_splits_host[i], lrs["g"][i].float(), req_time=2)
 
   # the hot key's row alone: its server, its table and its place in that server's rows
   hot_ps = int(np.mod(res.unique_key[0][hot].item(), S))
@@ -131,7 +142,7 @@ def run(name, S, B, args, dev, power):
 
   def ph_hot_grad():
     dops.fill_with_offset_map_gradient(sp.pos[hot_ps][hot_row:hot_row + 1], one_split, flat_grad, res.value_offset,
-                                       dims, num_unique=U, sync=False)
+                                       dims, num_unique=U, sync=False, dtype=row_dtype)
 
   phases = [("unique", ph_unique), ("split", ph_split), ("lookup", ph_lookup), ("fill", ph_fill),
             ("fill_grad", ph_fill_grad), ("apply", ph_apply), ("hot_row_grad", ph_hot_grad)]
@@ -168,8 +179,10 @@ def run(name, S, B, args, dev, power):
     torch.cuda.synchronize()
 
   steps = {}
-  for it in range(1 + args.host_steps):
+  for it in range(1 + max(args.host_steps, 2)):
     for key, fn in (("step_device", step_device), ("step_host", step_host)):
+      if key == "step_host" and (not args.host_steps or it > args.host_steps):
+        continue
       torch.cuda.synchronize()
       t1 = time.perf_counter()
       fn()
@@ -182,9 +195,16 @@ def run(name, S, B, args, dev, power):
   msp, mpos = om.ragged_split_by_indices(np.mod(uk, S), uk, uks_h, S)
   for i in range(S):
     want = om.fill_with_offset_map_gradient(mpos[i], msp[i][1], g_np, vo, vos_h, dims)
-    same = same and np.array_equal(lrs["g"][i].cpu().numpy().view(np.uint32), want.view(np.uint32))
-  nbytes = phase_bytes(M, U, rows_floats, res.value_len)
-  out = {"workload": name, "num_ps": S, "batch": B, "tables": len(dims), "dims": sorted(set(dims)),
+    got = lrs["g"][i].cpu().numpy()
+    if f16:
+      with np.errstate(over="ignore"):
+        want = want.astype(np.float16)
+      same = same and np.array_equal(got.view(np.uint16), want.view(np.uint16))
+    else:
+      same = same and np.array_equal(got.view(np.uint32), want.view(np.uint32))
+  nbytes = phase_bytes(M, U, rows_floats, res.value_len, 2 if f16 else 4)
+  out = {"workload": name, "num_ps": S, "transfer_float16": f16, "batch": B, "tables": len(dims),
+         "dims": sorted(set(dims)),
          "occurrences": M, "unique": U, "longest_run": int(runs[hot]), "steps": args.steps,
          "device_ms": {k: round(v, 4) for k, v in med.items() if k != "hot_row_grad"},
          "spread_ms": {k: [round(float(np.min(v)), 4), round(float(np.max(v)), 4)] for k, v in times.items()},
@@ -194,7 +214,7 @@ def run(name, S, B, args, dev, power):
          "longest_run_grad_ms": round(med["hot_row_grad"], 4),
          "longest_run_share_of_fill_grad": round(med["hot_row_grad"] / med["fill_grad"], 4),
          "step_device_ms": round(float(np.median(steps["step_device"])), 3),
-         "step_host_ops_ms": round(float(np.median(steps["step_host"])), 3),
+         "step_host_ops_ms": round(float(np.median(steps["step_host"])), 3) if "step_host" in steps else None,
          "host_ops_label": "unique, split, fill and fill gradient in numpy on the host (tests/offset_map_model.py)",
          "device_equals_host_bits": bool(same),
          "gpu": torch.cuda.get_device_properties(dev).name, "power_limit": power}
@@ -211,6 +231,7 @@ def main():
   ap.add_argument("--steps", type=int, default=20)
   ap.add_argument("--warmup", type=int, default=5)
   ap.add_argument("--host-steps", type=int, default=2)
+  ap.add_argument("--transfer-float16", action="store_true")
   args = ap.parse_args()
   assert torch.cuda.is_available(), "bench_async_ps.py measures on a GPU"
   dev = torch.device("cuda", 0)
