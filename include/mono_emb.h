@@ -469,6 +469,43 @@ int mono_sharding_sparse_fids(int32_t device, const int64_t* fids_dev, const int
                               int32_t* emb_row_length_dev, int32_t* bad_row_splits_dev,
                               int32_t* table_row_length_host, void* stream);
 
+/* ShardingSparseFids version 5 (ref: parse_sparse_feature.cc:287-301, 329-336, 390-404, parse_sparse_feature.h:
+ * 837-893): the arguments and outputs of mono_sharding_sparse_fids, bit for bit, then batch_size (>= 0, echoed
+ * back) and three more device outputs, written by one more kernel on the same stream after the v3/v4 outputs:
+ *   fid_list_row_splits_size_dev int32[K * N]  features of table k + 1 at k * N + n (list (table k, shard n)'s
+ *                                              row-splits length)
+ *   emb_size_dev                 int32[K * N]  floats of list (table k, shard n) at k * N + n: emb_row_length's
+ *                                              (n, k) entry, table-major
+ *   sizes_dev                    int32[4]      nfl_size = F + 1, feature_size = R + 1, fid_size = M, batch_size
+ * Synchronises exactly when mono_sharding_sparse_fids does (table_row_length_host given). */
+int mono_sharding_sparse_fids_v5(int32_t device, const int64_t* fids_dev, const int64_t* row_splits_dev,
+                                 const mono_sharding_feature* features, int32_t num_features, int32_t num_tables,
+                                 int32_t num_shards, int32_t unique, int64_t* fid_list_dev, uint64_t* fid_offset_dev,
+                                 int32_t* feature_offset_dev, uint32_t* nfl_offset_dev,
+                                 int64_t* fid_list_row_splits_dev, int32_t* table_row_length_dev,
+                                 int32_t* shard_row_length_dev, int32_t* emb_row_length_dev,
+                                 int32_t* bad_row_splits_dev, int32_t* table_row_length_host, int32_t batch_size,
+                                 int32_t* fid_list_row_splits_size_dev, int32_t* emb_size_dev, int32_t* sizes_dev,
+                                 void* stream);
+
+/* NormalizeMergedSplit (ref: RT/ops/normalize_merged_split_op.cc:33-90).  row_split_dev holds merge_num row splits
+ * end to end (split_num entries), split i being row_split_size_dev[i] entries that start at 0.  Writes
+ * normed_row_split_dev[split_num + 1 - merge_num]: split 0 as it is, then every later split's entries after its
+ * first, each shifted by the sum of the last entries of the splits before it.  E.g. row_split 0 2 5 5 9 0 0 3 4 with
+ * sizes 5 4 gives 0 2 5 5 9 9 12 13.  *bad_dev is set to 1 (never cleared) for a size below 1 (negative sizes
+ * included) or sizes that do not add up to split_num, the reference's undefined cases; no entry outside row_split is
+ * read and none outside the output is written.  One single-block
+ * launch, no host round trip.  merge_num == 0 with split_num == 0 launches nothing; merge_num > split_num and
+ * negative sizes return MONO_ERR_INVALID_ARGUMENT before the device is touched. */
+int mono_normalize_merged_split(int32_t device, const int64_t* row_split_dev, int64_t split_num,
+                                const int32_t* row_split_size_dev, int64_t merge_num, int64_t* normed_row_split_dev,
+                                int32_t* bad_dev, void* stream);
+
+/* dst_f16_dev[i] = src_dev[i] rounded once to fp16, nearest even (beyond the fp16 range +-inf, NaN stays NaN):
+ * the fp32 layout gradient a transfer_float16 worker sends to its parameter servers.  One launch; n == 0 launches
+ * nothing. */
+int mono_round_to_f16(int32_t device, const float* src_dev, int64_t n, void* dst_f16_dev, void* stream);
+
 /* ---- async parameter-server worker path ------------------------------------------------------------------------
  * ref: DistributedMultiTypeHashTable.lookup / apply_gradients on the raw API, NT/distributed_ps.py:266-337, 481-516:
  * dedup the K tables' keys (unique_key_with_value_and_offset), split the unique keys over S servers by
@@ -709,6 +746,25 @@ int mono_embedding_to_layout_bf16(int32_t device, const float* const* emb_ptrs_d
                                   const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
                                   const mono_slice_task* tasks_host, int32_t n_tasks,
                                   float* const* out_ptrs_dev, void* stream);
+/* The layout forward on fp16 embedding lists (rows a transfer_float16 parameter server sent): the arguments of
+ * mono_embedding_to_layout (_f16in) / mono_embedding_to_layout_bf16 (_f16in_bf16), but emb_ptrs_dev point at fp16
+ * lists and the row offsets and strides count fp16 elements.  Each element is widened exactly where it is loaded,
+ * so the result is bit for bit the fp32-input call on the lists widened to fp32, with no cast pass.  The same task
+ * validation, error codes and one launch as the twins.  The gradient stays the fp32 calls'. */
+int mono_embedding_to_layout_f16in(int32_t device, const void* const* emb_ptrs_dev,
+                                   const int32_t* emb_strides_dev, int32_t n_emb,
+                                   const uint64_t* fid_offset_dev, int64_t total_fid,
+                                   const int32_t* feature_offset_dev, int32_t total_feature,
+                                   const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                   const mono_slice_task* tasks_host, int32_t n_tasks,
+                                   float* const* out_ptrs_dev, void* stream);
+int mono_embedding_to_layout_f16in_bf16(int32_t device, const void* const* emb_ptrs_dev,
+                                        const int32_t* emb_strides_dev, int32_t n_emb,
+                                        const uint64_t* fid_offset_dev, int64_t total_fid,
+                                        const int32_t* feature_offset_dev, int32_t total_feature,
+                                        const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                        const mono_slice_task* tasks_host, int32_t n_tasks,
+                                        float* const* out_ptrs_dev, void* stream);
 int mono_embedding_to_layout_grad_bf16(int32_t device, float* const* emb_grad_ptrs_dev,
                                        const int32_t* emb_strides_dev, int32_t n_emb,
                                        const uint64_t* fid_offset_dev, int64_t total_fid,

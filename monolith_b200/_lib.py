@@ -123,6 +123,14 @@ SIGNATURES = {
     "mono_fill_with_offset_map": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _i64, _p, _p, _p]),
     "mono_fill_with_offset_map_grad": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _p, _p]),
     "mono_mtable_lookup_f16": (C.c_int, [_p, _p, _p, _p, _p]),
+    "mono_sharding_sparse_fids_v5": (C.c_int, [_i32, _p, _p, C.POINTER(ShardingFeature), _i32, _i32, _i32, _i32, _p,
+                                               _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _p, _p, _p]),
+    "mono_normalize_merged_split": (C.c_int, [_i32, _p, _i64, _p, _i64, _p, _p, _p]),
+    "mono_round_to_f16": (C.c_int, [_i32, _p, _i64, _p, _p]),
+    "mono_embedding_to_layout_f16in": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
+                                                 C.POINTER(SliceTask), _i32, _p, _p]),
+    "mono_embedding_to_layout_f16in_bf16": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
+                                                      C.POINTER(SliceTask), _i32, _p, _p]),
     "mono_fill_with_offset_map_f16": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _i64, _p, _p, _p]),
     "mono_fill_with_offset_map_grad_f16": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _p, _p]),
     "mono_grouping_create": (C.c_int, [_i32, C.POINTER(_p)]),

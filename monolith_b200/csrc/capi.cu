@@ -146,13 +146,13 @@ int layout_entry(bool backward, int32_t device, float* const* emb_ptrs_dev, cons
                  int32_t n_emb, const uint64_t* fid_offset_dev, int64_t total_fid, const int32_t* feature_offset_dev,
                  int32_t total_feature, const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
                  const mono_slice_task* tasks_host, int32_t n_tasks, float* const* out_ptrs_dev, void* stream,
-                 bool bf16, const float* grad_scale = nullptr) {
+                 bool bf16, const float* grad_scale = nullptr, bool f16_in = false) {
   return guarded([&] {
     check_layout_tasks(tasks_host, n_tasks, total_nfl);
     MONO_CUDA(cudaSetDevice(device));
     launch_layout(backward, emb_ptrs_dev, emb_strides_dev, n_emb, fid_offset_dev, total_fid, feature_offset_dev,
                   total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host, n_tasks, out_ptrs_dev,
-                  (cudaStream_t)stream, bf16, grad_scale);
+                  (cudaStream_t)stream, bf16, grad_scale, f16_in);
   });
 }
 
@@ -699,6 +699,50 @@ int mono_sharding_sparse_fids(int32_t device, const int64_t* fids_dev, const int
   });
 }
 
+int mono_sharding_sparse_fids_v5(int32_t device, const int64_t* fids_dev, const int64_t* row_splits_dev,
+                                 const mono_sharding_feature* features, int32_t num_features, int32_t num_tables,
+                                 int32_t num_shards, int32_t unique, int64_t* fid_list_dev, uint64_t* fid_offset_dev,
+                                 int32_t* feature_offset_dev, uint32_t* nfl_offset_dev,
+                                 int64_t* fid_list_row_splits_dev, int32_t* table_row_length_dev,
+                                 int32_t* shard_row_length_dev, int32_t* emb_row_length_dev,
+                                 int32_t* bad_row_splits_dev, int32_t* table_row_length_host, int32_t batch_size,
+                                 int32_t* fid_list_row_splits_size_dev, int32_t* emb_size_dev, int32_t* sizes_dev,
+                                 void* stream) {
+  return guarded([&] {
+    require(features && row_splits_dev && fid_list_dev && fid_offset_dev && feature_offset_dev && nfl_offset_dev &&
+                fid_list_row_splits_dev && table_row_length_dev && shard_row_length_dev && emb_row_length_dev &&
+                fid_list_row_splits_size_dev && emb_size_dev && sizes_dev,
+            "sharding_sparse_fids_v5: null argument");
+    require(batch_size >= 0, "sharding_sparse_fids_v5: negative batch_size");
+    const ShardingV5 v5{batch_size, fid_list_row_splits_size_dev, emb_size_dev, sizes_dev};
+    run_sharding(device, fids_dev, row_splits_dev, features, num_features, num_tables, num_shards, unique,
+                 fid_list_dev, fid_offset_dev, feature_offset_dev, nfl_offset_dev, fid_list_row_splits_dev,
+                 table_row_length_dev, shard_row_length_dev, emb_row_length_dev, bad_row_splits_dev,
+                 table_row_length_host, (cudaStream_t)stream, &v5);
+  });
+}
+
+int mono_normalize_merged_split(int32_t device, const int64_t* row_split_dev, int64_t split_num,
+                                const int32_t* row_split_size_dev, int64_t merge_num, int64_t* normed_row_split_dev,
+                                int32_t* bad_dev, void* stream) {
+  return guarded([&] {
+    require(merge_num == 0 || (row_split_dev && row_split_size_dev && normed_row_split_dev && bad_dev),
+            "normalize_merged_split: null argument");
+    run_normalize_merged_split(device, row_split_dev, split_num, row_split_size_dev, merge_num, normed_row_split_dev,
+                               bad_dev, (cudaStream_t)stream);
+  });
+}
+
+int mono_round_to_f16(int32_t device, const float* src_dev, int64_t n, void* dst_f16_dev, void* stream) {
+  return guarded([&] {
+    require(n >= 0, "round_to_f16: negative n");
+    if (n == 0) return;
+    require(src_dev && dst_f16_dev, "round_to_f16: null argument");
+    MONO_CUDA(cudaSetDevice(device));
+    launch_round_to_f16(src_dev, n, reinterpret_cast<__half*>(dst_f16_dev), (cudaStream_t)stream);
+  });
+}
+
 int mono_dedup(int32_t device, const int64_t* ids_dev, int64_t n, int64_t* unique_out_dev,
                int32_t* inverse_out_dev, int32_t* n_unique_dev, int64_t* n_unique_host, void* stream) {
   return guarded([&] {
@@ -1048,6 +1092,32 @@ int mono_embedding_to_layout_bf16(int32_t device, const float* const* emb_ptrs_d
   return layout_entry(false, device, const_cast<float* const*>(emb_ptrs_dev), emb_strides_dev, n_emb, fid_offset_dev,
                       total_fid, feature_offset_dev, total_feature, nfl_offset_dev, total_nfl, batch_size, tasks_host,
                       n_tasks, out_ptrs_dev, stream, true);
+}
+
+int mono_embedding_to_layout_f16in(int32_t device, const void* const* emb_ptrs_dev,
+                                   const int32_t* emb_strides_dev, int32_t n_emb,
+                                   const uint64_t* fid_offset_dev, int64_t total_fid,
+                                   const int32_t* feature_offset_dev, int32_t total_feature,
+                                   const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                   const mono_slice_task* tasks_host, int32_t n_tasks,
+                                   float* const* out_ptrs_dev, void* stream) {
+  return layout_entry(false, device, const_cast<float* const*>(reinterpret_cast<const float* const*>(emb_ptrs_dev)),
+                      emb_strides_dev, n_emb, fid_offset_dev, total_fid, feature_offset_dev, total_feature,
+                      nfl_offset_dev, total_nfl, batch_size, tasks_host, n_tasks, out_ptrs_dev, stream, false, nullptr,
+                      true);
+}
+
+int mono_embedding_to_layout_f16in_bf16(int32_t device, const void* const* emb_ptrs_dev,
+                                        const int32_t* emb_strides_dev, int32_t n_emb,
+                                        const uint64_t* fid_offset_dev, int64_t total_fid,
+                                        const int32_t* feature_offset_dev, int32_t total_feature,
+                                        const uint32_t* nfl_offset_dev, int32_t total_nfl, int32_t batch_size,
+                                        const mono_slice_task* tasks_host, int32_t n_tasks,
+                                        float* const* out_ptrs_dev, void* stream) {
+  return layout_entry(false, device, const_cast<float* const*>(reinterpret_cast<const float* const*>(emb_ptrs_dev)),
+                      emb_strides_dev, n_emb, fid_offset_dev, total_fid, feature_offset_dev, total_feature,
+                      nfl_offset_dev, total_nfl, batch_size, tasks_host, n_tasks, out_ptrs_dev, stream, true, nullptr,
+                      true);
 }
 
 int mono_embedding_to_layout_grad_bf16(int32_t device, float* const* emb_grad_ptrs_dev,

@@ -475,11 +475,31 @@ sh_feature_offset_kernel(const int64_t* __restrict__ rs_in, int64_t R, int F, Sh
   }
 }
 
+// version 5 (ref: parse_sparse_feature.cc:287-301,329-336,390-404, parse_sparse_feature.h:837-893): one thread per
+// list (table k, shard n) writes fid_list_row_splits_size (features of table k + 1) and emb_size (the list's floats:
+// the version-4 emb_row_length of (n, k), transposed to table-major); thread 0 also writes nfl_size = F + 1,
+// feature_size = R + 1, fid_size = M and batch_size
+__global__ void __launch_bounds__(kThreads)
+sh_v5_sizes_kernel(int N, int K, int F, int64_t R, int64_t M, ShardStage st, const int32_t* __restrict__ emb_len,
+                   ShardingV5 v5) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx == 0) {
+    v5.sizes[0] = F + 1;
+    v5.sizes[1] = (int32_t)(R + 1);
+    v5.sizes[2] = (int32_t)M;
+    v5.sizes[3] = v5.batch_size;
+  }
+  if (idx >= N * K) return;
+  const int k = idx / N, n = idx % N;
+  v5.row_splits_size[idx] = st.first_j[k + 1] - st.first_j[k] + 1;
+  v5.emb_size[idx] = emb_len[(size_t)n * K + k];
+}
+
 void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits_dev,
                   const mono_sharding_feature* feats, int F, int K, int N, int unique, int64_t* fid_list_dev,
                   uint64_t* fid_offset_dev, int32_t* feature_offset_dev, uint32_t* nfl_offset_dev,
                   int64_t* row_splits_out_dev, int32_t* table_len_dev, int32_t* shard_len_dev, int32_t* emb_len_dev,
-                  int32_t* bad_row_splits_dev, int32_t* table_len_host, cudaStream_t s) {
+                  int32_t* bad_row_splits_dev, int32_t* table_len_host, cudaStream_t s, const ShardingV5* v5) {
   // every argument check runs before the device is touched
   if (F <= 0 || K <= 0 || N <= 0) throw ArgError("num_features, num_tables and num_shards must be positive");
   if (F > kMaxLists) throw ArgError("num_features > 2^25 is not supported");
@@ -598,6 +618,10 @@ void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits
   sh_tables_kernel<<<(N * K + kThreads - 1) / kThreads, kThreads, 0, s>>>(N, K, F, st, tb, row_splits_out_dev,
                                                                          table_len_dev, shard_len_dev, emb_len_dev);
   MONO_CHECK_LAUNCH();
+  if (v5) {
+    sh_v5_sizes_kernel<<<(N * K + kThreads - 1) / kThreads, kThreads, 0, s>>>(N, K, F, R, M, st, emb_len_dev, *v5);
+    MONO_CHECK_LAUNCH();
+  }
   if (M > 0) {
     sh_fid_offset_kernel<<<grid_for(M, kThreads), kThreads, 0, s>>>(fids_dev, M, N, F, st, tb, offs_lo,
                                                                    fid_offset_dev);
@@ -619,6 +643,81 @@ void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits
     if (back[(size_t)N * K]) throw ArgError("row splits must start at 0, not decrease and end at the feature's n_fids");
     std::memcpy(table_len_host, back.data(), sizeof(int32_t) * N * K);
   }
+}
+
+// ---- NormalizeMergedSplit (ref: RT/ops/normalize_merged_split_op.cc:33-90) ---------------------------------------
+//
+// row_split holds merge_num row splits end to end, split i being row_split_size[i] entries that start at 0.  The
+// output joins them: split i's entries after its first, shifted by the sum of the last entries of splits 0 .. i - 1
+// (split 0 keeps its first entry).  One block: the sizes and the last entries are scanned 1024 groups at a time,
+// then each thread writes its group's entries.  bad = 1 for a size below 1 or sizes that do not add up to split_num.
+constexpr int kNmsThreads = 1024;
+
+__global__ void __launch_bounds__(kNmsThreads)
+normalize_merged_split_kernel(const int64_t* __restrict__ rs, int64_t split_num, const int32_t* __restrict__ sizes,
+                              int64_t merge_num, int64_t* __restrict__ out, int32_t* __restrict__ bad) {
+  __shared__ int64_t sc[kNmsThreads];
+  __shared__ int64_t carry_off, carry_pre;
+  __shared__ int any_bad;
+  if (threadIdx.x == 0) carry_off = carry_pre = 0, any_bad = 0;
+  __syncthreads();
+  for (int64_t base = 0; base < merge_num; base += kNmsThreads) {
+    const int64_t i = base + threadIdx.x;
+    const bool live = i < merge_num;
+    const int64_t sz = live ? (int64_t)sizes[i] : 0;
+    if (live && sz < 1) any_bad = 1;
+    // inclusive scan of the sizes -> this group's first entry
+    sc[threadIdx.x] = sz;
+    __syncthreads();
+    for (int d = 1; d < kNmsThreads; d <<= 1) {
+      const int64_t v = threadIdx.x >= d ? sc[threadIdx.x - d] : 0;
+      __syncthreads();
+      sc[threadIdx.x] += v;
+      __syncthreads();
+    }
+    const int64_t end = carry_off + sc[threadIdx.x], start = end - sz;
+    const int64_t chunk_sizes = sc[kNmsThreads - 1];
+    __syncthreads();
+    // start >= 0: after a negative size a later split can end at or below 0; every read stays in [0, split_num)
+    const bool ok = live && sz >= 1 && start >= 0 && end <= split_num;
+    if (live && end > split_num) any_bad = 1;
+    const int64_t last = ok ? rs[end - 1] : 0;
+    // inclusive scan of the last entries -> the shift of this group (the exclusive prefix)
+    sc[threadIdx.x] = last;
+    __syncthreads();
+    for (int d = 1; d < kNmsThreads; d <<= 1) {
+      const int64_t v = threadIdx.x >= d ? sc[threadIdx.x - d] : 0;
+      __syncthreads();
+      sc[threadIdx.x] += v;
+      __syncthreads();
+    }
+    const int64_t pre = carry_pre + sc[threadIdx.x] - last;
+    const int64_t chunk_last = sc[kNmsThreads - 1];
+    if (ok) {
+      const int64_t n_out = split_num + 1 - merge_num;  // malformed sizes must not write outside the output
+      for (int64_t j = (i == 0 ? start : start + 1); j < end; ++j)
+        if (j - i >= 0 && j - i < n_out) out[j - i] = pre + rs[j];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) carry_off += chunk_sizes, carry_pre += chunk_last;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0 && (any_bad || carry_off != split_num)) *bad = 1;
+}
+
+void run_normalize_merged_split(int device, const int64_t* row_split_dev, int64_t split_num,
+                                const int32_t* row_split_size_dev, int64_t merge_num, int64_t* out_dev,
+                                int32_t* bad_dev, cudaStream_t s) {
+  if (split_num < 0 || merge_num < 0) throw ArgError("normalize_merged_split: negative size");
+  if (merge_num > split_num) throw ArgError("normalize_merged_split: more merged splits than entries");
+  if (merge_num == 0) {
+    if (split_num != 0) throw ArgError("normalize_merged_split: entries without a merged split");
+    return;
+  }
+  MONO_CUDA(cudaSetDevice(device));
+  normalize_merged_split_kernel<<<1, kNmsThreads, 0, s>>>(row_split_dev, split_num, row_split_size_dev, merge_num,
+                                                          out_dev, bad_dev);
+  MONO_CHECK_LAUNCH();
 }
 
 // ---- UniqueKeyWithValueAndOffset (ref: unique_mapping_ops.cc:51-124) ---------------------------------------------

@@ -525,11 +525,25 @@ void run_reorder(int device, const int64_t* ids_dev, const int64_t* id_split_hos
                  int32_t* fused_emb_offset_dev, int32_t* shard_sizes_host,
                  int32_t* sharded_slot_sizes_host, int64_t* n_unique_host, int32_t* n_unique_dev,
                  cudaStream_t s);
+// The version-5 outputs of mono_sharding_sparse_fids_v5, written on the device after the v3/v4 outputs:
+// row_splits_size[k * N + n] = features of table k + 1, emb_size[k * N + n] = floats of list (table k, shard n) and
+// sizes = {nfl_size, feature_size, fid_size, batch_size}.
+struct ShardingV5 {
+  int32_t batch_size;
+  int32_t* row_splits_size;
+  int32_t* emb_size;
+  int32_t* sizes;
+};
 void run_sharding(int device, const int64_t* fids_dev, const int64_t* row_splits_dev,
                   const mono_sharding_feature* feats, int F, int K, int N, int unique, int64_t* fid_list_dev,
                   uint64_t* fid_offset_dev, int32_t* feature_offset_dev, uint32_t* nfl_offset_dev,
                   int64_t* row_splits_out_dev, int32_t* table_len_dev, int32_t* shard_len_dev, int32_t* emb_len_dev,
-                  int32_t* bad_row_splits_dev, int32_t* table_len_host, cudaStream_t s);
+                  int32_t* bad_row_splits_dev, int32_t* table_len_host, cudaStream_t s,
+                  const ShardingV5* v5 = nullptr);
+// mono_normalize_merged_split: merge_num row splits laid end to end, each restarting at 0, joined into one
+void run_normalize_merged_split(int device, const int64_t* row_split_dev, int64_t split_num,
+                                const int32_t* row_split_size_dev, int64_t merge_num, int64_t* out_dev,
+                                int32_t* bad_dev, cudaStream_t s);
 
 // the async parameter-server worker path (mono_unique_key_with_value_and_offset, mono_ragged_split_by_indices)
 void run_unique_offset(int device, const int64_t* key_dev, const int64_t* key_split_host, int K,
@@ -555,7 +569,11 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
                    int n_emb, const uint64_t* fid_offset, int64_t total_fid,
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,
                    int total_nfl, int batch_size, const mono_slice_task* tasks_host, int n_tasks,
-                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16 = false, const float* grad_scale = nullptr);
+                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16 = false, const float* grad_scale = nullptr,
+                   bool f16_in = false);
+// f16_in (forward only): emb_ptrs_dev point at __half rows, widened exactly where they are loaded (the f16in_ kernels)
+// mono_round_to_f16: dst[i] = fp16 round-to-nearest-even of src[i]
+void launch_round_to_f16(const float* src, int64_t n, __half* dst, cudaStream_t s);
 // mono_reduce_and_split[_grad]; T: element type of the slice rows.  grad_scale (backward only; device float, or
 // null): every slice gradient element is multiplied by it in fp32 where it is loaded (the scaled_ kernels)
 void check_reduce_split(const mono_reduce_feature* feats, int n_features);

@@ -317,8 +317,10 @@ __device__ __forceinline__ void fid_range(const LayoutArgs& a, int feature_idx, 
 // for ADDN outputs, where the reference sums the slices in config order:
 // ForwardTaskRunImpl, fused_embedding_to_layout.cc:468-540).
 // T: element type of the outputs (a.out_ptrs point at T storage; out_row_stride and out_col count T elements).
-template <typename T, int G>
+// S: element type of the embedding lists (float, or __half for the f16in_ kernels, widened exactly at the load).
+template <typename T, int G, typename S = float>
 __device__ __forceinline__ void layout_fwd(const LayoutArgs& a) {
+  const S* const* emb = reinterpret_cast<const S* const*>(a.emb_ptrs);
   const int gl = Group<G>::gl();
   const int64_t total = (int64_t)a.n_chains * a.batch_size;
   const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
@@ -336,13 +338,14 @@ __device__ __forceinline__ void layout_fwd(const LayoutArgs& a) {
       int start = 0, fnum = 0;
       if (num) fid_range(a, shared ? off : off + b, &start, &fnum);
       for (int q = 0; q < first.max_seq_len; ++q) {
-        const float* src = nullptr;
+        const S* src = nullptr;
         if (q < fnum) {
           const uint64_t fo = a.fid_offset[start + q];
           const int i1 = (int)(fo >> 32), i2 = (int)(fo & 0xffffffffu);
-          src = a.emb_ptrs[i1] + (int64_t)i2 * a.emb_strides[i1] + first.slice_start;
+          src = emb[i1] + (int64_t)i2 * a.emb_strides[i1] + first.slice_start;
         }
-        for (int c = gl; c < first.dim; c += G) dst[q * first.dim + c] = to_row_elem(src ? src[c] : 0.0f, dst);
+        for (int c = gl; c < first.dim; c += G)
+          dst[q * first.dim + c] = to_row_elem(src ? row_elem_f32(src[c]) : 0.0f, dst);
       }
       continue;
     }
@@ -364,7 +367,7 @@ __device__ __forceinline__ void layout_fwd(const LayoutArgs& a) {
         for (int f = 0; f < fnum; ++f) {
           const uint64_t fo = a.fid_offset[start + f];
           const int i1 = (int)(fo >> 32), i2 = (int)(fo & 0xffffffffu);
-          float x = a.emb_ptrs[i1][(int64_t)i2 * a.emb_strides[i1] + tk.slice_start + c];
+          float x = row_elem_f32(emb[i1][(int64_t)i2 * a.emb_strides[i1] + tk.slice_start + c]);
           if (tk.pooling == MONO_POOL_MEAN) x = __fdiv_rn(x, fn);
           if (via_tmp) {
             tmp = tinit ? x : __fadd_rn(tmp, x);
@@ -391,6 +394,17 @@ __global__ void __launch_bounds__(kThreads) layout_fwd_kernel(LayoutArgs a) {
 template <int G>
 __global__ void __launch_bounds__(kThreads) bf16_layout_fwd_kernel(LayoutArgs a) {
   layout_fwd<__nv_bfloat16, G>(a);
+}
+
+// fp16 embedding lists (rows a transfer_float16 server sent), fp32 or bf16 outputs
+template <int G>
+__global__ void __launch_bounds__(kThreads) f16in_layout_fwd_kernel(LayoutArgs a) {
+  layout_fwd<float, G, __half>(a);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads) f16in_bf16_layout_fwd_kernel(LayoutArgs a) {
+  layout_fwd<__nv_bfloat16, G, __half>(a);
 }
 
 // Backward: ScatterGrad (ref: fused_embedding_to_layout.h:286-347) with float atomics, as the
@@ -478,7 +492,7 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
                    int n_emb, const uint64_t* fid_offset, int64_t total_fid,
                    const int32_t* feature_offset, int total_feature, const uint32_t* nfl_offset,
                    int total_nfl, int batch_size, const mono_slice_task* tasks_host, int n_tasks,
-                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16, const float* grad_scale) {
+                   float* const* out_ptrs_dev, cudaStream_t s, bool bf16, const float* grad_scale, bool f16_in) {
   (void)n_emb;
   if (n_tasks <= 0 || batch_size <= 0) return;
   // chains: consecutive grouping of tasks by destination (accumulate tasks with equal destination)
@@ -534,7 +548,9 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
   const int grid = grid_for(units, kThreads / G);
   by_group(G, [&](auto g) {
     constexpr int GG = decltype(g)::value;
-    if (!backward && !bf16) layout_fwd_kernel<GG><<<grid, kThreads, 0, s>>>(a);
+    if (!backward && f16_in && !bf16) f16in_layout_fwd_kernel<GG><<<grid, kThreads, 0, s>>>(a);
+    else if (!backward && f16_in) f16in_bf16_layout_fwd_kernel<GG><<<grid, kThreads, 0, s>>>(a);
+    else if (!backward && !bf16) layout_fwd_kernel<GG><<<grid, kThreads, 0, s>>>(a);
     else if (!backward) bf16_layout_fwd_kernel<GG><<<grid, kThreads, 0, s>>>(a);
     else if (grad_scale && !bf16) scaled_layout_bwd_kernel<GG><<<grid, kThreads, 0, s>>>(a, nt, grad_scale);
     else if (grad_scale) scaled_bf16_layout_bwd_kernel<GG><<<grid, kThreads, 0, s>>>(a, nt, grad_scale);
@@ -545,6 +561,29 @@ void launch_layout(bool backward, float* const* emb_ptrs_dev, const int32_t* emb
   MONO_CUDA(cudaFreeAsync(ws, s));
   // `ordered` / `chain_start` are pageable sources of async copies: wait for them
   MONO_CUDA(cudaStreamSynchronize(s));
+}
+
+// One rounding of fp32 values to fp16 (nearest even): the layout gradient a transfer_float16 worker sends to its
+// servers.  4 elements per thread where the pointers allow 16-byte loads, else one.
+__global__ void __launch_bounds__(kThreads) round_to_f16_kernel(const float* __restrict__ src, int64_t n,
+                                                                 __half* __restrict__ dst, int vec) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t t0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (vec) {
+    const int64_t n4 = n / 4;
+    for (int64_t t = t0; t < n4; t += stride)
+      store_row4(dst + 4 * t, reinterpret_cast<const float4*>(src)[t]);
+    for (int64_t i = 4 * n4 + t0; i < n; i += stride) dst[i] = __float2half_rn(src[i]);
+  } else {
+    for (int64_t i = t0; i < n; i += stride) dst[i] = __float2half_rn(src[i]);
+  }
+}
+
+void launch_round_to_f16(const float* src, int64_t n, __half* dst, cudaStream_t s) {
+  if (n <= 0) return;
+  const int vec = ((uintptr_t)src % 16 == 0 && (uintptr_t)dst % 8 == 0) ? 1 : 0;
+  round_to_f16_kernel<<<grid_for(vec ? (n + 3) / 4 : n, kThreads), kThreads, 0, s>>>(src, n, dst, vec);
+  MONO_CHECK_LAUNCH();
 }
 
 // ------------------------------------------------------------------------------------------

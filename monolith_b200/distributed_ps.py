@@ -724,3 +724,155 @@ class DistributedMultiTypeHashTable:
       _, st = table.reinitialize(slot, split_ids[i].to(table.device))
       status.append(st.to(ids.device))
     return self, torch.cat(status)
+
+
+class PSLayoutContext:
+  """What PartitionedHashTablePS.apply_gradients needs from its lookup (ref: the `__sharding_sparse_fids__*` entries
+  of the auxiliary bundle): the version-5 sharding outputs, every server's ids and host row splits over its tables,
+  the float size of every (table, server) list and the batch size."""
+  __slots__ = ("sharding", "server_ids", "server_splits", "emb_sizes", "batch_size")
+
+
+class PartitionedHashTablePS:
+  """PartitionedHashTable's parameter-server mode with the fused layout — ref: NT/distributed_ps.py:581-2001 without
+  enable_gpu_emb, the table a job with enable_fused_layout=True and num_ps > 0 builds (NT/cpu_training.py:713-741).
+  The GPU all-to-all mode is PartitionedHashTable above; the two share no step logic.
+
+  table_factory(i, slot_to_config) -> MultiHashTable makes server i's table (any CUDA device; every server holds the
+  same tables, named like the features' tables).  feature_table / feature_dims_sum / shared_features describe the
+  features as sharding_sparse_fids takes them, and every feature's dims_sum must be its table's dim.  tasks are
+  fused_embedding_to_layout's (nfl_idx = the feature's index in sorted-name order) and out_shapes the layout tensors'
+  shapes per sample: each lookup allocates [batch_size, *shape].  Every task's out_row_stride must fit in its tensor's
+  per-sample elements.  A FID lives on server (uint64)fid % num_ps, the sharding's shard.
+
+  lookup: sharding_sparse_fids(version=5), one raw_lookup per server over its (table, server) lists, then
+  fused_embedding_to_layout over the K*N lists (index table_index * num_ps + server).  apply_gradients: the layout
+  gradient into one zeroed buffer laid out server after server, then one raw_apply_gradients per server on its slab.
+  Both calls synchronise with the host: lookup reads the sharding's list lengths back (the servers' raw calls take
+  them on the host), the layout forward and gradient launchers wait for their staged task tables, and the servers'
+  raw table calls may wait as well (e.g. for rounds of duplicate ids in an apply).
+  unique: the sharding's (each (feature, server) list keeps its distinct FIDs, or every occurrence).
+
+  transfer_float16 (ref: distributed_ps.py:912-927, 1425-1440): each server's lookup writes its rows rounded to fp16
+  and the layout forward reads them as they are, widening where it loads (no cast pass on the worker); the fp32 layout
+  gradient is rounded once to fp16 after its atomics have completed, and each server widens its slab exactly before
+  its apply.  So a looked-up element is f32(f16(row)) and a server applies f32(f16(sum)).  Rows and gradients cross
+  devices with plain torch copies."""
+
+  def __init__(self, num_ps: int, slot_to_config: Dict, table_factory, feature_table: Dict[str, str],
+               feature_dims_sum: Dict[str, int], tasks, out_shapes, shared_features: Sequence[str] = (), *,
+               unique: bool = True, transfer_float16: bool = False):
+    if num_ps < 1:
+      raise ValueError("num_ps must be >= 1")
+    self._num_ps = int(num_ps)
+    self._transfer_dtype = torch.float16 if transfer_float16 else torch.float32
+    self._tables = [table_factory(i, slot_to_config) for i in range(self._num_ps)]
+    t0 = self._tables[0]
+    for t in self._tables[1:]:
+      if tuple(t.table_names) != tuple(t0.table_names) or tuple(t.get_table_dim_sizes()) != tuple(
+          t0.get_table_dim_sizes()):
+        raise ValueError("every PS table must hold the same tables with the same dims")
+    dims = dict(zip(t0.table_names, t0.get_table_dim_sizes()))
+    for f, t in feature_table.items():
+      if t not in dims:
+        raise ValueError(f"feature {f}'s table {t} is not a table of the servers")
+      if int(feature_dims_sum[f]) != dims[t]:
+        raise ValueError(f"feature {f}: dims_sum {feature_dims_sum[f]} is not table {t}'s dim {dims[t]}")
+    self._feature_table = dict(feature_table)
+    self._dims_sum = {f: int(feature_dims_sum[f]) for f in feature_table}
+    self._shared = tuple(shared_features)
+    self._tasks = list(tasks)
+    self._out_shapes = [tuple(int(x) for x in s) for s in out_shapes]
+    for t in self._tasks:
+      if not 0 <= t.out_tensor < len(self._out_shapes):
+        raise ValueError(f"task out_tensor {t.out_tensor} outside the {len(self._out_shapes)} layout tensors")
+      per_sample = 1
+      for x in self._out_shapes[t.out_tensor]:
+        per_sample *= x
+      if t.out_row_stride > per_sample:
+        raise ValueError(f"task out_row_stride {t.out_row_stride} exceeds layout tensor {t.out_tensor}'s "
+                         f"{per_sample} elements per sample")
+    self._unique = bool(unique)
+    self._dims = dims
+
+  @property
+  def tables(self):
+    return self._tables
+
+  @property
+  def transfer_float16(self) -> bool:
+    return self._transfer_dtype == torch.float16
+
+  def lookup(self, features: Dict[str, Tuple[torch.Tensor, torch.Tensor]], dtype: torch.dtype = torch.float32,
+             batch_size: Optional[int] = None):
+    """features[name] = (fids int64, row_splits int64[rows + 1]) on the worker's CUDA device, every configured
+    feature present.  Returns (the layout tensors, float32 or bfloat16, ctx)."""
+    from . import distribution_ops as dops
+    if set(features) != set(self._feature_table):
+      raise ValueError(f"features must be exactly {sorted(self._feature_table)}, not {sorted(features)}")
+    if dtype not in (torch.float32, torch.bfloat16):
+      raise ValueError(f"dtype must be torch.float32 or torch.bfloat16, not {dtype}")
+    N = self._num_ps
+    names = sorted(features)
+    B = dops._v5_batch_size(features, names, set(self._shared), batch_size)
+    sh = dops.sharding_sparse_fids(features, self._feature_table, self._dims_sum, N, self._shared, unique=self._unique,
+                                   sync=True, version=5, batch_size=B)   # the one synchronisation
+    dev = sh["fid_offset"].device
+    k_of = {t: k for k, t in enumerate(sh["table_names"])}
+    lens = [t.numel() for t in sh["fid_list"]]                          # [k * N + i], host ints
+    fused = sh["fid_list_fused"]                                         # server-major, table-minor
+    embs = [None] * (len(k_of) * N)
+    server_ids, server_splits, emb_sizes = [], [], [0] * (len(k_of) * N)
+    start = 0
+    for i, table in enumerate(self._tables):
+      split = [0]
+      for name in table.table_names:
+        split.append(split[-1] + (lens[k_of[name] * N + i] if name in k_of else 0))
+      ids = fused[start:start + split[-1]].to(table.device)
+      start += split[-1]
+      flat = table.raw_lookup(ids, split, dtype=self._transfer_dtype).to(dev)
+      off = 0
+      for name in table.table_names:
+        if name in k_of:
+          k = k_of[name]
+          n = lens[k * N + i] * self._dims[name]
+          embs[k * N + i], emb_sizes[k * N + i] = flat[off:off + n], n
+          off += n
+      server_ids.append(ids)
+      server_splits.append(split)
+    layouts = dops.fused_embedding_to_layout(embs, [1] * len(embs), sh["fid_offset"], sh["feature_offset"],
+                                             sh["nfl_offset"], B, self._tasks,
+                                             [(B,) + s for s in self._out_shapes], dtype=dtype)
+    ctx = PSLayoutContext()
+    ctx.sharding, ctx.server_ids, ctx.server_splits, ctx.emb_sizes, ctx.batch_size = (sh, server_ids, server_splits,
+                                                                                       emb_sizes, B)
+    return layouts, ctx
+
+  def apply_gradients(self, ctx: PSLayoutContext, layout_grads: Sequence[torch.Tensor], global_step: int = 0,
+                      req_time: int = 0, layout_tensors_grad_scale: Optional[torch.Tensor] = None):
+    """layout_grads: the gradients of lookup's layout tensors (all float32 or all bfloat16).
+    layout_tensors_grad_scale: as fused_embedding_to_layout_grad's (e.g. clip_ops.global_norm_scale's scale)."""
+    from . import distribution_ops as dops
+    sh, N = ctx.sharding, self._num_ps
+    dev = sh["fid_offset"].device
+    K = len(ctx.emb_sizes) // N
+    buf = torch.zeros(sum(ctx.emb_sizes), dtype=torch.float32, device=dev)
+    views, bounds, off = [None] * (K * N), [], 0
+    for i in range(N):                                                    # server-major: one slab per server
+      lo = off
+      for k in range(K):
+        views[k * N + i] = buf[off:off + ctx.emb_sizes[k * N + i]]
+        off += ctx.emb_sizes[k * N + i]
+      bounds.append((lo, off))
+    dops.fused_embedding_to_layout_grad(ctx.emb_sizes, [1] * (K * N), sh["fid_offset"], sh["feature_offset"],
+                                        sh["nfl_offset"], ctx.batch_size, self._tasks, layout_grads,
+                                        layout_tensors_grad_scale, out=views)
+    send = dops.round_to_f16(buf) if self.transfer_float16 else buf
+    for i, table in enumerate(self._tables):
+      lo, hi = bounds[i]
+      g = send[lo:hi].to(table.device)
+      if self.transfer_float16:
+        g = g.float()  # the server's exact widening (the reference's CastToFloat32 on the PS)
+      table.raw_apply_gradients(ctx.server_ids[i], ctx.server_splits[i], g, global_step=global_step,
+                                req_time=req_time)
+    return self

@@ -82,7 +82,8 @@ def unique_with_inverse(ids: torch.Tensor, sync: bool = True):
 
 def sharding_sparse_fids(features: Dict[str, Tuple[torch.Tensor, torch.Tensor]], feature_table: Dict[str, str],
                          feature_dims_sum: Dict[str, int], num_of_shards: int, shared_features: Sequence[str] = (),
-                         reorder_fn=None, *, unique: bool = True, sync: bool = True):
+                         reorder_fn=None, *, unique: bool = True, sync: bool = True, version: int = 4,
+                         batch_size: Optional[int] = None):
   """Outputs of the reference's ShardingSparseFids (versions 3 and 4) from per-feature FID lists —
   ref: ShardingSparseFidsOp::FillFidList / CreateOffsetTensor, NT/data/kernels/parse_sparse_feature.cc:187-330,
   version 4: parse_sparse_feature.h:714-920; Python model: NT/data/parse_sparse_feature_test.py:87-301 (SURVEY §8
@@ -109,11 +110,26 @@ def sharding_sparse_fids(features: Dict[str, Tuple[torch.Tensor, torch.Tensor]],
   sync=True reads the N*K list lengths back to slice fid_list (one synchronisation); sync=False makes no host round
   trip.  reorder_fn (the CPU twin: lists, N, dims -> fused_reorder_by_indices' outputs) keeps the version-3
   unique outputs only and the adapter's own index arithmetic.
+  version=5 (the reference's default without GPU embeddings, parse_sparse_feature.cc:287-404; CUDA inputs, one
+  mono_sharding_sparse_fids_v5 call) adds, all int32 on the device and written there:
+    fid_list_row_splits_size   K*N one-element tensors: the table's feature count + 1
+    nfl_size, feature_size, fid_size, batch_size   one-element tensors: F + 1, #(feature, row) + 1, M, batch size
+    emb_size                   int32[K*N], table-major (index table_index * N + shard): floats of each list
+  batch_size defaults to the row count the non-shared features share (ValueError if they differ, or if every
+  feature is shared).
   (The reference dedups per (feature, shard); FIDs carry their slot, so features never share a FID.)"""
   N = int(num_of_shards)
   names = sorted(features)
+  if version not in (3, 4, 5):
+    raise ValueError(f"version must be 3, 4 or 5, not {version!r}")
   if reorder_fn is None and names and features[names[0]][0].is_cuda:
-    return _sharding_sparse_fids_device(features, feature_table, feature_dims_sum, N, shared_features, unique, sync)
+    v5 = None
+    if version == 5:
+      v5 = _v5_batch_size(features, names, set(shared_features), batch_size)
+    return _sharding_sparse_fids_device(features, feature_table, feature_dims_sum, N, shared_features, unique, sync,
+                                        v5)
+  if version == 5:
+    raise ValueError("version=5 needs CUDA inputs and no reorder_fn")
   if not unique or not sync:
     raise ValueError("unique=False and sync=False need CUDA inputs and no reorder_fn")
   if reorder_fn is None:
@@ -173,7 +189,20 @@ def sharding_sparse_fids(features: Dict[str, Tuple[torch.Tensor, torch.Tensor]],
           "table_names": tables, "feature_names": names}
 
 
-def _sharding_sparse_fids_device(features, feature_table, feature_dims_sum, N, shared_features, unique, sync):
+def _v5_batch_size(features, names, shared, batch_size):
+  if batch_size is not None:
+    if int(batch_size) < 0:
+      raise ValueError("batch_size must not be negative")
+    return int(batch_size)
+  rows = {features[n][1].numel() - 1 for n in names if n not in shared}
+  if len(rows) != 1:
+    raise ValueError("batch_size is needed: the non-shared features do not give one row count "
+                     f"({sorted(rows) if rows else 'every feature is shared'})")
+  return rows.pop()
+
+
+def _sharding_sparse_fids_device(features, feature_table, feature_dims_sum, N, shared_features, unique, sync,
+                                 v5_batch_size=None):
   lib = _lib.load()
   names = sorted(features)
   tables = sorted({feature_table[n] for n in names})
@@ -196,10 +225,15 @@ def _sharding_sparse_fids_device(features, feature_table, feature_dims_sum, N, s
   row_splits = torch.empty(N * (F + K), dtype=torch.int64, device=device)
   table_len, shard_len, emb_len = torch.empty(N * K, **i32), torch.empty(N, **i32), torch.empty(N * K, **i32)
   host_len = (C.c_int32 * (N * K))() if sync else None
-  _lib.check(lib.mono_sharding_sparse_fids(device.index, _ptr(fids), _ptr(splits), recs, F, K, N, 1 if unique else 0,
-                                           _ptr(fused), _ptr(fid_offset), _ptr(feature_offset), _ptr(nfl_offset),
-                                           _ptr(row_splits), _ptr(table_len), _ptr(shard_len), _ptr(emb_len), None,
-                                           host_len, _stream(device)))
+  args = (device.index, _ptr(fids), _ptr(splits), recs, F, K, N, 1 if unique else 0, _ptr(fused), _ptr(fid_offset),
+          _ptr(feature_offset), _ptr(nfl_offset), _ptr(row_splits), _ptr(table_len), _ptr(shard_len), _ptr(emb_len),
+          None, host_len)
+  if v5_batch_size is None:
+    _lib.check(lib.mono_sharding_sparse_fids(*args, _stream(device)))
+  else:
+    rs_size, emb_size, sizes = torch.empty(K * N, **i32), torch.empty(K * N, **i32), torch.empty(4, **i32)
+    _lib.check(lib.mono_sharding_sparse_fids_v5(*args, v5_batch_size, _ptr(rs_size), _ptr(emb_size), _ptr(sizes),
+                                                _stream(device)))
   # lists of table k: features first[k] .. first[k + 1] - 1 in table-major order; row splits block of (n, k) at
   # n * (F + K) + first[k] + k
   per_table = [sum(1 for n in names if t_idx[feature_table[n]] == k) for k in range(K)]
@@ -218,10 +252,48 @@ def _sharding_sparse_fids_device(features, feature_table, feature_dims_sum, N, s
     fused = fused[:starts[-1]]
   else:
     fused = fused[:M]
-  return {"fid_list": fid_list, "fid_offset": fid_offset[:M], "feature_offset": feature_offset, "nfl_offset": nfl_offset,
-          "table_names": tables, "feature_names": names, "fid_list_row_splits": rs_list, "fid_list_fused": fused,
-          "fid_list_table_row_length": table_len, "fid_list_shard_row_length": shard_len,
-          "fid_list_emb_row_length": emb_len}
+  out = {"fid_list": fid_list, "fid_offset": fid_offset[:M], "feature_offset": feature_offset, "nfl_offset": nfl_offset,
+         "table_names": tables, "feature_names": names, "fid_list_row_splits": rs_list, "fid_list_fused": fused,
+         "fid_list_table_row_length": table_len, "fid_list_shard_row_length": shard_len,
+         "fid_list_emb_row_length": emb_len}
+  if v5_batch_size is not None:
+    out.update({"fid_list_row_splits_size": [rs_size[i:i + 1] for i in range(K * N)], "nfl_size": sizes[0:1],
+                "feature_size": sizes[1:2], "fid_size": sizes[2:3], "batch_size": sizes[3:4], "emb_size": emb_size})
+  return out
+
+
+def normalize_merged_split(row_split: torch.Tensor, row_split_size: torch.Tensor, *, sync: bool = True) -> torch.Tensor:
+  """ref: distribution_ops.normalize_merged_split / MonolithNormalizeMergedSplit (RT/ops/normalize_merged_split_op.cc
+  :33-90): row_split (int64, CUDA) holds len(row_split_size) row splits end to end, split i being row_split_size[i]
+  entries that start at 0; the result (int64[len(row_split) + 1 - len(row_split_size)]) joins them, every later
+  split's entries after its first shifted by the sum of the last entries of the splits before it.  E.g. [0, 2, 5, 5,
+  9, 0, 0, 3, 4] with sizes [5, 4] gives [0, 2, 5, 5, 9, 9, 12, 13].  One device kernel (mono_normalize_merged_split).
+  sync=True checks on the device that every size is >= 1 and that they add up to len(row_split), and raises
+  ValueError otherwise (one synchronisation); sync=False makes no host round trip."""
+  lib = _lib.load()
+  dev = row_split.device
+  rs = row_split.reshape(-1).to(torch.int64).contiguous()
+  sz = row_split_size.reshape(-1).to(device=dev, dtype=torch.int32).contiguous()
+  n, m = rs.numel(), sz.numel()
+  if m > n or (m == 0 and n > 0):
+    raise ValueError(f"normalize_merged_split: {m} merged splits for {n} entries")
+  out = torch.empty(n + 1 - m if m else 0, dtype=torch.int64, device=dev)
+  bad = torch.zeros(1, dtype=torch.int32, device=dev)
+  _lib.check(lib.mono_normalize_merged_split(dev.index, _ptr(rs), n, _ptr(sz), m, _ptr(out), _ptr(bad), _stream(dev)))
+  if sync and int(bad.item()):
+    raise ValueError("normalize_merged_split: every row_split_size must be >= 1 and they must add up to row_split's "
+                     "length")
+  return out
+
+
+def round_to_f16(x: torch.Tensor) -> torch.Tensor:
+  """x (float32, CUDA) rounded once to fp16, nearest even, by one kernel (mono_round_to_f16)."""
+  if x.dtype != torch.float32 or x.device.type != "cuda":
+    raise ValueError(f"round_to_f16 takes a CUDA float32 tensor, not {x.dtype} on {x.device}")
+  x = x.contiguous()
+  out = torch.empty(x.shape, dtype=torch.float16, device=x.device)
+  _lib.check(_lib.load().mono_round_to_f16(x.device.index, _ptr(x), x.numel(), _ptr(out), _stream(x.device)))
+  return out
 
 
 def gather_pool(fused_embeddings: torch.Tensor, fused_embedding_offsets: torch.Tensor, dim: int,
@@ -707,15 +779,23 @@ def fused_embedding_to_layout(embeddings_list: Sequence[torch.Tensor], emb_strid
   fid_offset: uint64 viewed as int64 tensor; nfl_offset: uint32 viewed as int32 tensor (sharding_sparse_fids'
   outputs as they are).  Raises ValueError for any other dtype, a non-CUDA or non-contiguous index tensor, or
   embeddings that are not float32 on the same device.  dtype: of the outputs, float32 or bfloat16 (the float32
-  results rounded once to nearest even; the tasks' strides and columns then count bfloat16 elements)."""
+  results rounded once to nearest even; the tasks' strides and columns then count bfloat16 elements).
+  embeddings_list may also be all float16 (rows a transfer_float16 parameter server sent): the f16in kernels then
+  widen every element exactly where they load it, so the outputs are bit for bit this call on the lists widened to
+  float32 (mono_embedding_to_layout_f16in[_bf16])."""
   bf16 = _tower_dtype(dtype, "dtype") == torch.bfloat16
-  dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, embeddings_list, "embeddings_list")
+  f16_in = len(embeddings_list) > 0 and embeddings_list[0].dtype == torch.float16
+  dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, embeddings_list, "embeddings_list",
+                             torch.float16 if f16_in else torch.float32)
   lib = _lib.load()
   outs = [torch.zeros(*s, dtype=dtype, device=dev) for s in out_shapes]
   embs = [e.contiguous() for e in embeddings_list]
   ep, op = _ptr_table(embs, dev), _ptr_table(outs, dev)
   st = torch.tensor(list(emb_strides), dtype=torch.int32, device=dev)
-  fn = lib.mono_embedding_to_layout_bf16 if bf16 else lib.mono_embedding_to_layout
+  if f16_in:
+    fn = lib.mono_embedding_to_layout_f16in_bf16 if bf16 else lib.mono_embedding_to_layout_f16in
+  else:
+    fn = lib.mono_embedding_to_layout_bf16 if bf16 else lib.mono_embedding_to_layout
   _lib.check(fn(dev.index, _ptr(ep), _ptr(st), len(embs), _ptr(fid_offset), fid_offset.numel(), _ptr(feature_offset),
                 feature_offset.numel(), _ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks), len(tasks),
                 _ptr(op), _stream(dev)))
@@ -725,12 +805,15 @@ def fused_embedding_to_layout(embeddings_list: Sequence[torch.Tensor], emb_strid
 def fused_embedding_to_layout_grad(emb_sizes: Sequence[int], emb_strides: Sequence[int], fid_offset: torch.Tensor,
                                    feature_offset: torch.Tensor, nfl_offset: torch.Tensor, batch_size: int,
                                    tasks: Sequence[SliceTask], out_grads: Sequence[torch.Tensor],
-                                   layout_tensors_grad_scale: Optional[torch.Tensor] = None):
+                                   layout_tensors_grad_scale: Optional[torch.Tensor] = None,
+                                   out: Optional[Sequence[torch.Tensor]] = None):
   """ref: MonolithEmbeddingToLayoutGradV* (fused_embedding_to_layout.cc:697-948).  The index tensors as in
   fused_embedding_to_layout; out_grads all float32 or all bfloat16 (widened exactly) on their device.  The
   returned embedding gradients are float32.  layout_tensors_grad_scale: a one-element float32 tensor on that device
   (the reference's `layout_tensors_grad_scale * grad`, distribution_ops.py:544-550): every gradient element is
-  multiplied by it in float32 before the MEAN division (mono_embedding_to_layout_grad[_bf16]_scaled)."""
+  multiplied by it in float32 before the MEAN division (mono_embedding_to_layout_grad[_bf16]_scaled).
+  out: zero-filled contiguous float32 tensors of emb_sizes elements on that device (e.g. views of one buffer) that
+  receive the gradients and are returned, in place of fresh ones."""
   from .clip_ops import scale_ptr
   dtype = _tower_dtype(out_grads[0].dtype if len(out_grads) else torch.float32, "out_grads")
   if any(g.dtype != dtype for g in out_grads):
@@ -738,7 +821,13 @@ def fused_embedding_to_layout_grad(emb_sizes: Sequence[int], emb_strides: Sequen
   dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, out_grads, "out_grads", dtype)
   sp = scale_ptr(layout_tensors_grad_scale, dev, "layout_tensors_grad_scale")
   lib = _lib.load()
-  grads = [torch.zeros(n, dtype=torch.float32, device=dev) for n in emb_sizes]
+  if out is None:
+    grads = [torch.zeros(n, dtype=torch.float32, device=dev) for n in emb_sizes]
+  else:
+    grads = list(out)
+    if len(grads) != len(emb_sizes) or any(g.dtype != torch.float32 or g.device != dev or not g.is_contiguous() or
+                                           g.numel() != int(n) for g, n in zip(grads, emb_sizes)):
+      raise ValueError(f"out must be {len(emb_sizes)} contiguous float32 tensors on {dev} of emb_sizes elements")
   og = [g.contiguous() for g in out_grads]
   gp, op = _ptr_table(grads, dev), _ptr_table(og, dev)
   st = torch.tensor(list(emb_strides), dtype=torch.int32, device=dev)
