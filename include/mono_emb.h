@@ -1063,6 +1063,84 @@ int mono_xstep_backward_scaled(mono_xstep_t* x, const float* pooled_grad_dev, in
                                const int32_t* row_offsets_dev, int32_t pooling, const float* lr_host,
                                int64_t update_time, const float* grad_scale_dev, void* stream);
 
+/* ---- the sharded step over parts: several features of ONE table in one exchange --------------------------------
+ * The parts (mono_pool_part, as for mono_mtable_lookup_pool_parts) of one sharded step.  Every part must name the
+ * step's table (the xstep's; for the grouping and gather calls the table of parts_host[0], which every other part must
+ * name too).  The occurrences of all parts are ONE batch, part order then occurrence order: the grouping is built over
+ * their concatenated FIDs, so the results are those of mono_mtable_lookup_pool_parts and
+ * mono_mtable_pool_backward_parts on the global table:
+ *   forward : every SUM / MEAN part's rows are bit for bit mono_mtable_lookup_pool_parts' (the same pooling order and
+ *             MEAN division, absent FIDs give zero rows); a FIRSTN part's position j < min(n_r, L) is the row of the
+ *             row's j-th FID and positions n_r <= j < L are +0.0.  rows_dev / stride / col are the output rows.
+ *   backward: rows_dev / stride / col are the gradient rows (the forward's FIDs, offsets and poolings).  Each distinct
+ *             FID gets one upsert, one timestamp bump, one admission-filter count and one optimizer step, with the sum
+ *             of its terms over all parts (a CSR MEAN term divided by its row's n; a FIRSTN occurrence at j >= L a +0.0
+ *             term), associated as mono_grouping_reduce associates the terms of one list.  With one SUM or MEAN part
+ *             the step is bit for bit the step of mono_xstep_forward / mono_xstep_backward (or the grouping calls) on
+ *             that part's FIDs, offsets and rows.
+ * _bf16: every part's rows are bfloat16 (stride and col in bf16 elements): outputs are the fp32 results rounded once
+ * to nearest even; gradients are widened exactly first, so the table equals the fp32 call's on the widened rows.
+ * _scaled: see "The _scaled backward calls" (FIRSTN positions at or past L stay +0.0).
+ * MONO_ERR_INVALID_ARGUMENT, before any device work (no table change): n_parts outside [1, MONO_MAX_POOL_PARTS], a part
+ * naming another table, pooling other than SUM, MEAN or FIRSTN, a FIRSTN part with max_seq_len < 1 or
+ * n_rows * max_seq_len > 2^31, n_rows != n_fids without offsets, a null pointer, 2^29 occurrences or more, a table dim
+ * that is not a multiple of 4 or above 128; for gradient rows also stride % 4 != 0, col % 4 != 0 or rows that are not
+ * 16-byte (bf16: 8-byte) aligned; for a backward or reduce, parts whose occurrence count is not the forward's / the
+ * grouping's.  Output rows take any stride and column.
+ *   mono_xstep_forward_parts[_bf16]: mono_xstep_forward's exchange over the concatenated FIDs, then the pooling of the
+ *     received rows.  Launches: those of mono_xstep_forward without its pooling kernel, + 1 (the concatenated FID list
+ *     on the device; none with one part), + 1 per distinct pooling kernel among the parts (the row copy of aligned
+ *     one-FID parts, the pooling kernel of CSR or unaligned parts, the FIRSTN kernel), not one per part.
+ *   mono_xstep_backward_parts[_bf16][_scaled]: mono_xstep_backward's launches without the CSR occurrence map, + 1 (the
+ *     parts occurrence map: every occurrence's gradient row and MEAN divisor).  Nothing returns to the host.
+ *   mono_grouping_build_parts: mono_grouping_build over the concatenated FIDs (+ 1 launch with more than one part).
+ *   mono_gather_pool_parts[_bf16]: the forward's pooling from a row buffer (rows_in_dev, 16-byte aligned) with the
+ *     build's occurrence offsets: 1 launch per distinct pooling kernel.
+ *   mono_grouping_reduce[_push]_parts[_bf16][_scaled]: mono_grouping_reduce[_push] with the parts' gradient rows:
+ *     its launches without the CSR occurrence map, + 1 (the parts occurrence map). */
+int mono_xstep_forward_parts(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts, void* stream);
+int mono_xstep_forward_parts_bf16(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts, void* stream);
+int mono_xstep_backward_parts(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts, const float* lr_host,
+                              int64_t update_time, void* stream);
+int mono_xstep_backward_parts_bf16(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts,
+                                   const float* lr_host, int64_t update_time, void* stream);
+int mono_xstep_backward_parts_scaled(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts,
+                                     const float* lr_host, int64_t update_time, const float* grad_scale_dev,
+                                     void* stream);
+int mono_xstep_backward_parts_bf16_scaled(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts,
+                                          const float* lr_host, int64_t update_time, const float* grad_scale_dev,
+                                          void* stream);
+int mono_grouping_build_parts(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                              int32_t num_shards, int64_t* uniq_out_dev, int32_t* occ_offset_out_dev,
+                              int32_t* shard_counts_host, int64_t* n_unique_host, void* stream);
+int mono_gather_pool_parts(mono_mtable_t* t, const float* rows_in_dev, const int32_t* occ_offset_dev,
+                           const mono_pool_part* parts_host, int32_t n_parts, void* stream);
+int mono_gather_pool_parts_bf16(mono_mtable_t* t, const float* rows_in_dev, const int32_t* occ_offset_dev,
+                                const mono_pool_part* parts_host, int32_t n_parts, void* stream);
+int mono_grouping_reduce_parts(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                               int32_t n_parts, float* out_rows_dev, void* stream);
+int mono_grouping_reduce_parts_bf16(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                    int32_t n_parts, float* out_rows_dev, void* stream);
+int mono_grouping_reduce_parts_scaled(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                      int32_t n_parts, float* out_rows_dev, const float* grad_scale_dev, void* stream);
+int mono_grouping_reduce_parts_bf16_scaled(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                           int32_t n_parts, float* out_rows_dev, const float* grad_scale_dev,
+                                           void* stream);
+int mono_grouping_reduce_push_parts(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                    int32_t n_parts, const int64_t* shard_counts, mono_peer_t* p, int64_t region_off,
+                                    const int64_t* dst_row_off, void* stream);
+int mono_grouping_reduce_push_parts_bf16(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                         int32_t n_parts, const int64_t* shard_counts, mono_peer_t* p,
+                                         int64_t region_off, const int64_t* dst_row_off, void* stream);
+int mono_grouping_reduce_push_parts_scaled(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                           int32_t n_parts, const int64_t* shard_counts, mono_peer_t* p,
+                                           int64_t region_off, const int64_t* dst_row_off,
+                                           const float* grad_scale_dev, void* stream);
+int mono_grouping_reduce_push_parts_bf16_scaled(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                                int32_t n_parts, const int64_t* shard_counts, mono_peer_t* p,
+                                                int64_t region_off, const int64_t* dst_row_off,
+                                                const float* grad_scale_dev, void* stream);
+
 /* Number of kernel launches issued by this library since load (for bench.py's gpu_launches). */
 int64_t mono_kernel_launch_count(void);
 

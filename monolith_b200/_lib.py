@@ -188,6 +188,26 @@ SIGNATURES = {
     "mono_grouping_reduce_scaled": (C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p, _p]),
     "mono_grouping_reduce_push_scaled": (C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p, _i64, _p, _p, _p]),
     "mono_xstep_backward_scaled": (C.c_int, [_p, _p, _i64, _i32, _p, _i32, _p, _i64, _p, _p]),
+    "mono_xstep_forward_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p]),
+    "mono_xstep_forward_parts_bf16": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p]),
+    "mono_xstep_backward_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _p]),
+    "mono_xstep_backward_parts_bf16": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _p]),
+    "mono_xstep_backward_parts_scaled": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _p, _p]),
+    "mono_xstep_backward_parts_bf16_scaled": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _p, _p]),
+    "mono_grouping_build_parts": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _i32, _p, _p, _p, C.POINTER(_i64),
+                                            _p]),
+    "mono_gather_pool_parts": (C.c_int, [_p, _p, _p, C.POINTER(PoolPartC), _i32, _p]),
+    "mono_gather_pool_parts_bf16": (C.c_int, [_p, _p, _p, C.POINTER(PoolPartC), _i32, _p]),
+    "mono_grouping_reduce_parts": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p]),
+    "mono_grouping_reduce_parts_bf16": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p]),
+    "mono_grouping_reduce_parts_scaled": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _p]),
+    "mono_grouping_reduce_parts_bf16_scaled": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _p]),
+    "mono_grouping_reduce_push_parts": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _i64, _p, _p]),
+    "mono_grouping_reduce_push_parts_bf16": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _i64, _p, _p]),
+    "mono_grouping_reduce_push_parts_scaled": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _i64, _p, _p,
+                                                         _p]),
+    "mono_grouping_reduce_push_parts_bf16_scaled": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _i64, _p,
+                                                              _p, _p]),
     "mono_ckpt_last_error": (C.c_char_p, []),
     "mono_ckpt_writer_open": (C.c_int, [C.c_char_p, C.c_char_p, _i32, C.POINTER(_p)]),
     "mono_ckpt_writer_begin_table": (C.c_int, [_p, C.c_char_p, C.POINTER(SegmentCfg), _i32]),

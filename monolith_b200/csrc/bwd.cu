@@ -1658,6 +1658,8 @@ struct PartDev {
 // One thread per row of the concatenated parts: the row's occurrences get their FID, gradient row and MEAN divisor.
 // Occurrence j of a FIRSTN row reads position j of the row for j < L and zero_row (128 floats of +0.0) beyond it,
 // as ScatterGrad's FIRSTN branch leaves such a FID's gradient at its zero fill (fused_embedding_to_layout.h:334-340).
+// fids_out == null: the gradient rows and divisors only (the sharded backward); src_out == null: the FIDs only (the
+// sharded forward's concatenated FID list, before any gradient exists).
 __global__ void __launch_bounds__(kThreads)
 parts_occ_kernel(const PartDev* __restrict__ parts, int n_parts, int64_t n_rows, int64_t* __restrict__ fids_out,
                  const float** __restrict__ src_out, float* __restrict__ div_out, const float* __restrict__ zero_row) {
@@ -1678,12 +1680,36 @@ parts_occ_kernel(const PartDev* __restrict__ parts, int n_parts, int64_t n_rows,
     const float* src = p.rows + lr * p.stride;
     const float dv = p.mean ? (float)(e - b) : 0.f;
     for (int64_t m = b; m < e; ++m) {
-      fids_out[p.occ_begin + m] = p.fids[m];
+      if (fids_out) fids_out[p.occ_begin + m] = p.fids[m];
+      if (!src_out) continue;
       const int64_t j = m - b;
       src_out[p.occ_begin + m] = !p.seq_len ? src : j < p.seq_len ? src + j * p.dim : zero_row;
       div_out[p.occ_begin + m] = dv;
     }
   }
+}
+
+// A part as parts_occ_kernel reads it: its occurrences from occ_begin, its rows from row_begin of the concatenation; D
+// is the table's dim.  bf16: the kernel steps in floats, so a bf16 row's stride and position step are halved (stride
+// and dim % 4 == 0).
+static PartDev part_dev(const mono_pool_part& p, int D, bool bf16, int64_t occ_begin, int64_t row_begin) {
+  PartDev d;
+  d.fids = p.fids_dev;
+  d.row_offsets = p.row_offsets_dev;
+  d.rows = p.rows_dev + p.col;
+  d.stride = p.stride;
+  d.occ_begin = occ_begin;
+  d.row_begin = row_begin;
+  d.mean = p.pooling == MONO_POOL_MEAN && p.row_offsets_dev ? 1 : 0;
+  d.seq_len = p.pooling == MONO_POOL_FIRSTN ? p.max_seq_len : 0;
+  d.dim = D;
+  if (bf16) {
+    d.rows = reinterpret_cast<const float*>(reinterpret_cast<const __nv_bfloat16*>(p.rows_dev) + p.col);
+    d.stride = p.stride / 2;
+    d.dim = D / 2;
+  }
+  d.pad = 0;
+  return d;
 }
 
 // The occurrences of all parts of one table are one batch (part order, then occurrence order): the claim set gets one
@@ -1772,23 +1798,7 @@ void run_pool_backward_parts(mono_mtable* mt, const mono_pool_part* parts, int n
     for (int i = 0; i < n_parts; ++i) {
       const mono_pool_part& p = parts[i];
       if (p.table != k || p.n_fids == 0) continue;
-      PartDev d;
-      d.fids = p.fids_dev;
-      d.row_offsets = p.row_offsets_dev;
-      d.rows = p.rows_dev + p.col;
-      d.stride = p.stride;
-      d.occ_begin = occ_at[k];
-      d.row_begin = row_at[k];
-      d.mean = p.pooling == MONO_POOL_MEAN && p.row_offsets_dev ? 1 : 0;
-      d.seq_len = p.pooling == MONO_POOL_FIRSTN ? p.max_seq_len : 0;
-      d.dim = mt->tables[k].dim;
-      if (bf16) {  // parts_occ_kernel steps in floats: half as many floats as bf16 elements (stride, dim % 4 == 0)
-        d.rows = reinterpret_cast<const float*>(reinterpret_cast<const __nv_bfloat16*>(p.rows_dev) + p.col);
-        d.stride = p.stride / 2;
-        d.dim = d.dim / 2;
-      }
-      d.pad = 0;
-      pd.push_back(d);
+      pd.push_back(part_dev(p, mt->tables[k].dim, bf16, occ_at[k], row_at[k]));
       occ_at[k] += p.n_fids;
       row_at[k] += p.n_rows;
     }
@@ -1916,6 +1926,8 @@ void grouping_destroy(mono_grouping* g) {
   cudaDeviceSynchronize();
   g->ws.release();
   g->claim_set.release();
+  g->fids_cat.release();
+  g->occ_map.release();
   if (g->h_counts) cudaFreeHost(g->h_counts);
   if (g->ev_claimed) cudaEventDestroy(g->ev_claimed);
   if (g->ev_copied) cudaEventDestroy(g->ev_copied);
@@ -2026,6 +2038,114 @@ void grouping_reduce_push(mono_grouping* g, const float* pooled_grad, int64_t gr
   if (po.n <= 0) throw ArgError("grouping_reduce_push without a peer window");
   grouping_reduce_impl(g, pooled_grad, grad_stride, grad_col, row_offsets, n_rows, pooling, nullptr, po, s,
                        grad_scale);
+}
+
+// ---- the sharded step over parts: several features of ONE table as one grouping -------------------------------
+// The occurrences of all parts are one batch, part order then occurrence order: the grouping is built over their
+// concatenated FIDs, and the reduce reads every occurrence's gradient row and MEAN divisor from the parts occurrence
+// map (parts_occ_kernel) instead of one (pooled_grad, stride, col, row_offsets) source.
+int64_t check_shard_parts(const char* who, mono_mtable* mt, int k, const mono_pool_part* parts, int n_parts,
+                          bool grads, bool bf16) {
+  const std::string w(who);
+  if (n_parts < 1 || n_parts > MONO_MAX_POOL_PARTS) throw ArgError(w + ": bad part count");
+  if (!parts) throw ArgError(w + ": null argument");
+  const int D = mt->tables[k].dim;
+  check_grad_rows(who, D);
+  int64_t M = 0;
+  for (int i = 0; i < n_parts; ++i) {
+    const mono_pool_part& p = parts[i];
+    if (p.table != k) throw ArgError(w + ": every part must name the step's table");
+    if (p.pooling != MONO_POOL_SUM && p.pooling != MONO_POOL_MEAN && p.pooling != MONO_POOL_FIRSTN)
+      throw ArgError(w + ": SUM, MEAN or FIRSTN");
+    if (p.n_fids < 0 || p.n_rows < 0) throw ArgError(w + ": negative count");
+    check_firstn(who, p);
+    if (!p.row_offsets_dev && p.n_rows != p.n_fids) throw ArgError(w + ": n_rows must equal n_fids without offsets");
+    if ((p.n_fids > 0 && !p.fids_dev) || (p.n_rows > 0 && !p.rows_dev)) throw ArgError(w + ": null argument");
+    if (grads) check_grad_rows(who, D, p.rows_dev, p.stride, p.col, nullptr, bf16 ? 2 : 4);
+    M += p.n_fids;
+    if (M >= ((int64_t)1 << 29)) throw ArgError(w + ": 2^29 occurrences or more in one step");
+  }
+  return M;
+}
+
+// The parts with occurrences, staged on the device for parts_occ_kernel (n == 0: none)
+struct StagedParts {
+  const PartDev* d;
+  int n;
+  int64_t n_rows;  // rows of the parts with occurrences
+  bool mean;       // some part pools by CSR MEAN
+};
+static StagedParts stage_shard_parts(mono_mtable* mt, int k, const mono_pool_part* parts, int n_parts, bool bf16,
+                                     cudaStream_t s) {
+  std::vector<PartDev> pd;
+  StagedParts sp{nullptr, 0, 0, false};
+  int64_t occ = 0;
+  for (int i = 0; i < n_parts; ++i) {
+    const mono_pool_part& p = parts[i];
+    if (p.n_fids == 0) continue;
+    pd.push_back(part_dev(p, mt->tables[k].dim, bf16, occ, sp.n_rows));
+    occ += p.n_fids;
+    sp.n_rows += p.n_rows;
+    sp.mean |= pd.back().mean != 0;
+  }
+  if (pd.empty()) return sp;
+  static_assert(sizeof(PartDev) * MONO_MAX_POOL_PARTS <= StageRing::kBlockBytes, "the parts fit one staged block");
+  const int rb = mt->ring.acquire();
+  std::memcpy(mt->ring.h(rb), pd.data(), sizeof(PartDev) * pd.size());
+  mt->ring.commit(rb, sizeof(PartDev) * pd.size(), s);
+  sp.d = reinterpret_cast<const PartDev*>(mt->ring.d(rb));
+  sp.n = (int)pd.size();
+  return sp;
+}
+
+const int64_t* shard_parts_fids(mono_mtable* mt, int k, const mono_pool_part* parts, int n_parts, int64_t M,
+                                DevBuf& buf, cudaStream_t s) {
+  if (n_parts == 1 || M == 0) return parts[0].fids_dev;
+  const StagedParts sp = stage_shard_parts(mt, k, parts, n_parts, false, s);
+  int64_t* out = (int64_t*)buf.get(8 * (size_t)M, s);
+  parts_occ_kernel<<<resident_grid(parts_occ_kernel, sp.n_rows, kThreads), kThreads, 0, s>>>(
+      sp.d, sp.n, sp.n_rows, out, nullptr, nullptr, nullptr);
+  MONO_CHECK_LAUNCH();
+  return out;
+}
+
+void grouping_build_parts(mono_grouping* g, mono_mtable* mt, int k, const mono_pool_part* parts, int n_parts, int N,
+                          int64_t* uniq_out, int32_t* occ_offset_out, int32_t* shard_counts_host,
+                          int64_t* n_unique_host, cudaStream_t s) {
+  const int64_t M = check_shard_parts("grouping_build_parts", mt, k, parts, n_parts, false, false);
+  if (N <= 0 || N > 256) throw ArgError("grouping: num_shards must be in [1, 256]");
+  if (g->device != mt->device) throw ArgError("grouping_build_parts: grouping and table on different devices");
+  MONO_CUDA(cudaSetDevice(g->device));
+  const int64_t* fids = shard_parts_fids(mt, k, parts, n_parts, M, g->fids_cat, s);
+  grouping_build(g, fids, M, N, mt->tables[k].dim, uniq_out, occ_offset_out, shard_counts_host, n_unique_host, s);
+}
+
+void grouping_reduce_parts(mono_grouping* g, mono_mtable* mt, int k, const mono_pool_part* parts, int n_parts,
+                           bool bf16, float* out_rows, const PeerOut& po, cudaStream_t s, const float* grad_scale) {
+  const std::string who = po.n ? "grouping_reduce_push_parts" : "grouping_reduce_parts";
+  const int64_t M = check_shard_parts(who.c_str(), mt, k, parts, n_parts, true, bf16);
+  const int D = g->dim;
+  if (g->device != mt->device) throw ArgError(who + ": grouping and table on different devices");
+  if (M != g->M || (M > 0 && !g->plan.sorted))
+    throw ArgError(who + ": the parts are not the batch of the grouping's last build");
+  if (mt->tables[k].dim != D) throw ArgError(who + ": the table's dim is not the grouping's");
+  if (po.n == 0) check_grad_rows(who.c_str(), D, nullptr, 0, 0, out_rows);
+  MONO_CUDA(cudaSetDevice(g->device));
+  if (M == 0) return;
+  const StagedParts sp = stage_shard_parts(mt, k, parts, n_parts, bf16, s);
+  const size_t src_bytes = ((sizeof(float*) * (size_t)M) + 255) & ~(size_t)255;
+  char* map = (char*)g->occ_map.get(src_bytes + 4 * (size_t)M, s);
+  BwdScratch w = g->plan;
+  w.occ_src = (const float**)map;
+  w.occ_div = (float*)(map + src_bytes);
+  parts_occ_kernel<<<resident_grid(parts_occ_kernel, sp.n_rows, kThreads), kThreads, 0, s>>>(
+      sp.d, sp.n, sp.n_rows, nullptr, w.occ_src, w.occ_div, mt->zero_row);
+  MONO_CHECK_LAUNCH();
+  // the whole sorted list is the range; its runs are already in the bucketed order: the sums are written in place
+  const SortedRange rg = {0, M, sp.mean};
+  const SegArgs sa = seg_args(w, M, D, nullptr, 0, 0, nullptr, 0, MONO_POOL_SUM, out_rows, s, &rg);
+  const GradScale gsc{grad_scale, mt->zero_row};
+  launch_reduce(SegLaunch(sa, grad_scale ? &gsc : nullptr), pick_group(D), po, false, s, bf16);
 }
 
 }  // namespace mono

@@ -214,6 +214,70 @@ int xstep_backward_entry(mono_xstep_t* x, const float* pooled_grad_dev, int64_t 
                    (cudaStream_t)stream, grad_scale);
   });
 }
+
+// The bodies of the sharded step's parts calls (bf16: the parts' rows are bf16; grad_scale: the _scaled twins)
+int xstep_forward_parts_entry(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts, void* stream,
+                              bool bf16) {
+  return guarded([&] {
+    require(x, "xstep_forward_parts: null argument");
+    HandleGuard hg_(x->mt);
+    xstep_forward_parts(x, parts_host, n_parts, bf16, (cudaStream_t)stream);
+  });
+}
+
+int xstep_backward_parts_entry(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts,
+                               const float* lr_host, int64_t update_time, void* stream, bool bf16,
+                               const float* grad_scale) {
+  return guarded([&] {
+    require(x && lr_host, "xstep_backward_parts: null argument");
+    HandleGuard hg_(x->mt);
+    xstep_backward_parts(x, parts_host, n_parts, bf16, lr_host, update_time, (cudaStream_t)stream, grad_scale);
+  });
+}
+
+// the table of a parts call on one table: the first part's (check_shard_parts holds every other part to it)
+int parts_table(const mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts, const char* who) {
+  if (n_parts < 1 || !parts_host) throw ArgError(std::string(who) + ": bad part count");
+  if (parts_host[0].table < 0 || parts_host[0].table >= (int)t->tables.size())
+    throw ArgError(std::string(who) + ": bad table index");
+  return parts_host[0].table;
+}
+
+int gather_pool_parts_entry(mono_mtable_t* t, const float* rows_in_dev, const int32_t* occ_offset_dev,
+                            const mono_pool_part* parts_host, int32_t n_parts, void* stream, bool bf16) {
+  return guarded([&] {
+    require(t && rows_in_dev && occ_offset_dev, "gather_pool_parts: null argument");
+    HandleGuard hg_(t);
+    const int k = parts_table(t, parts_host, n_parts, "gather_pool_parts");
+    check_shard_parts("gather_pool_parts", t, k, parts_host, n_parts, false, bf16);
+    MONO_CUDA(cudaSetDevice(t->device));
+    if (bf16) launch_gather_pool_parts<__nv_bfloat16>(t, k, rows_in_dev, occ_offset_dev, parts_host, n_parts,
+                                                      (cudaStream_t)stream);
+    else launch_gather_pool_parts<float>(t, k, rows_in_dev, occ_offset_dev, parts_host, n_parts, (cudaStream_t)stream);
+  });
+}
+
+// p == null: grouping_reduce_parts into out_rows_dev; else reduce_push_parts into the windows of p
+int grouping_reduce_parts_entry(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                int32_t n_parts, float* out_rows_dev, const int64_t* shard_counts, int64_t region_off,
+                                mono_peer_t* p, const int64_t* dst_row_off, void* stream, bool bf16,
+                                const float* grad_scale) {
+  return guarded([&] {
+    require(g && t, "grouping_reduce_parts: null argument");
+    HandleGuard hg_(t);
+    const int k = parts_table(t, parts_host, n_parts, "grouping_reduce_parts");
+    PeerOut po;
+    std::memset(&po, 0, sizeof(po));
+    if (p) {
+      require(shard_counts && dst_row_off, "grouping_reduce_push_parts: null argument");
+      require(p->device == g->device, "grouping_reduce_push_parts: window and grouping on different devices");
+      po = peer_out(p, region_off, dst_row_off, shard_counts, (int64_t)g->dim * 4);
+    } else {
+      require(out_rows_dev, "grouping_reduce_parts: null argument");
+    }
+    grouping_reduce_parts(g, t, k, parts_host, n_parts, bf16, out_rows_dev, po, (cudaStream_t)stream, grad_scale);
+  });
+}
 }  // namespace
 
 extern "C" {
@@ -1258,6 +1322,101 @@ int mono_xstep_backward_scaled(mono_xstep_t* x, const float* pooled_grad_dev, in
                                int64_t update_time, const float* grad_scale_dev, void* stream) {
   return xstep_backward_entry(x, pooled_grad_dev, grad_stride, grad_col, row_offsets_dev, pooling, lr_host,
                               update_time, stream, grad_scale_dev);
+}
+
+// ---- the sharded step over parts of one table ---------------------------------------------------------------
+int mono_xstep_forward_parts(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts, void* stream) {
+  return xstep_forward_parts_entry(x, parts_host, n_parts, stream, false);
+}
+int mono_xstep_forward_parts_bf16(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts, void* stream) {
+  return xstep_forward_parts_entry(x, parts_host, n_parts, stream, true);
+}
+int mono_xstep_backward_parts(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts, const float* lr_host,
+                              int64_t update_time, void* stream) {
+  return xstep_backward_parts_entry(x, parts_host, n_parts, lr_host, update_time, stream, false, nullptr);
+}
+int mono_xstep_backward_parts_bf16(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts,
+                                   const float* lr_host, int64_t update_time, void* stream) {
+  return xstep_backward_parts_entry(x, parts_host, n_parts, lr_host, update_time, stream, true, nullptr);
+}
+int mono_xstep_backward_parts_scaled(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts,
+                                     const float* lr_host, int64_t update_time, const float* grad_scale_dev,
+                                     void* stream) {
+  return xstep_backward_parts_entry(x, parts_host, n_parts, lr_host, update_time, stream, false, grad_scale_dev);
+}
+int mono_xstep_backward_parts_bf16_scaled(mono_xstep_t* x, const mono_pool_part* parts_host, int32_t n_parts,
+                                          const float* lr_host, int64_t update_time, const float* grad_scale_dev,
+                                          void* stream) {
+  return xstep_backward_parts_entry(x, parts_host, n_parts, lr_host, update_time, stream, true, grad_scale_dev);
+}
+
+int mono_grouping_build_parts(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host, int32_t n_parts,
+                              int32_t num_shards, int64_t* uniq_out_dev, int32_t* occ_offset_out_dev,
+                              int32_t* shard_counts_host, int64_t* n_unique_host, void* stream) {
+  return guarded([&] {
+    require(g && t && uniq_out_dev && occ_offset_out_dev && shard_counts_host, "grouping_build_parts: null argument");
+    HandleGuard hg_(t);
+    const int k = parts_table(t, parts_host, n_parts, "grouping_build_parts");
+    grouping_build_parts(g, t, k, parts_host, n_parts, num_shards, uniq_out_dev, occ_offset_out_dev,
+                         shard_counts_host, n_unique_host, (cudaStream_t)stream);
+  });
+}
+
+int mono_gather_pool_parts(mono_mtable_t* t, const float* rows_in_dev, const int32_t* occ_offset_dev,
+                           const mono_pool_part* parts_host, int32_t n_parts, void* stream) {
+  return gather_pool_parts_entry(t, rows_in_dev, occ_offset_dev, parts_host, n_parts, stream, false);
+}
+int mono_gather_pool_parts_bf16(mono_mtable_t* t, const float* rows_in_dev, const int32_t* occ_offset_dev,
+                                const mono_pool_part* parts_host, int32_t n_parts, void* stream) {
+  return gather_pool_parts_entry(t, rows_in_dev, occ_offset_dev, parts_host, n_parts, stream, true);
+}
+
+int mono_grouping_reduce_parts(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                               int32_t n_parts, float* out_rows_dev, void* stream) {
+  return grouping_reduce_parts_entry(g, t, parts_host, n_parts, out_rows_dev, nullptr, 0, nullptr, nullptr, stream,
+                                     false, nullptr);
+}
+int mono_grouping_reduce_parts_bf16(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                    int32_t n_parts, float* out_rows_dev, void* stream) {
+  return grouping_reduce_parts_entry(g, t, parts_host, n_parts, out_rows_dev, nullptr, 0, nullptr, nullptr, stream,
+                                     true, nullptr);
+}
+int mono_grouping_reduce_parts_scaled(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                      int32_t n_parts, float* out_rows_dev, const float* grad_scale_dev, void* stream) {
+  return grouping_reduce_parts_entry(g, t, parts_host, n_parts, out_rows_dev, nullptr, 0, nullptr, nullptr, stream,
+                                     false, grad_scale_dev);
+}
+int mono_grouping_reduce_parts_bf16_scaled(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                           int32_t n_parts, float* out_rows_dev, const float* grad_scale_dev,
+                                           void* stream) {
+  return grouping_reduce_parts_entry(g, t, parts_host, n_parts, out_rows_dev, nullptr, 0, nullptr, nullptr, stream,
+                                     true, grad_scale_dev);
+}
+int mono_grouping_reduce_push_parts(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                    int32_t n_parts, const int64_t* shard_counts, mono_peer_t* p, int64_t region_off,
+                                    const int64_t* dst_row_off, void* stream) {
+  return grouping_reduce_parts_entry(g, t, parts_host, n_parts, nullptr, shard_counts, region_off, p, dst_row_off,
+                                     stream, false, nullptr);
+}
+int mono_grouping_reduce_push_parts_bf16(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                         int32_t n_parts, const int64_t* shard_counts, mono_peer_t* p,
+                                         int64_t region_off, const int64_t* dst_row_off, void* stream) {
+  return grouping_reduce_parts_entry(g, t, parts_host, n_parts, nullptr, shard_counts, region_off, p, dst_row_off,
+                                     stream, true, nullptr);
+}
+int mono_grouping_reduce_push_parts_scaled(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                           int32_t n_parts, const int64_t* shard_counts, mono_peer_t* p,
+                                           int64_t region_off, const int64_t* dst_row_off,
+                                           const float* grad_scale_dev, void* stream) {
+  return grouping_reduce_parts_entry(g, t, parts_host, n_parts, nullptr, shard_counts, region_off, p, dst_row_off,
+                                     stream, false, grad_scale_dev);
+}
+int mono_grouping_reduce_push_parts_bf16_scaled(mono_grouping_t* g, mono_mtable_t* t, const mono_pool_part* parts_host,
+                                                int32_t n_parts, const int64_t* shard_counts, mono_peer_t* p,
+                                                int64_t region_off, const int64_t* dst_row_off,
+                                                const float* grad_scale_dev, void* stream) {
+  return grouping_reduce_parts_entry(g, t, parts_host, n_parts, nullptr, shard_counts, region_off, p, dst_row_off,
+                                     stream, true, grad_scale_dev);
 }
 
 // ---- global norm + clip scale ----------------------------------------------------------------

@@ -308,6 +308,8 @@ struct mono_grouping {
   uint32_t* h_counts = nullptr;  // pinned: per-owner distinct counts [256] + overflow flag
   cudaStream_t side = nullptr;   // carries the early counts copy while the sort runs on the caller's stream
   cudaEvent_t ev_claimed = nullptr, ev_copied = nullptr;
+  // the sharded step over parts: the concatenated FIDs of the parts, and the occurrence map of their gradient rows
+  mono::DevBuf fids_cat, occ_map;
 };
 
 // ---- NVLink peer window (peer.cu) ----------------------------------------------------------------
@@ -387,6 +389,7 @@ struct mono_xstep {
   // (mono_xstep_prepare) — it does not depend on the table
   mono_grouping* grouping[2] = {nullptr, nullptr};  // owned
   mono::DevBuf uniq[2], offs[2];                     // bucketed unique list, per-occurrence row offsets
+  mono::DevBuf fids_cat;                             // forward over parts: the parts' concatenated FIDs
   cudaEvent_t ev_prep[2] = {nullptr, nullptr};       // grouping [slot] built (recorded on the prepare stream)
   cudaEvent_t ev_bwd[2] = {nullptr, nullptr};        // backward of the step that used grouping [slot] enqueued
   bool bwd_recorded[2] = {false, false};
@@ -436,6 +439,24 @@ void grouping_reduce(mono_grouping* g, const float* pooled_grad, int64_t grad_st
                      const int32_t* row_offsets, int64_t n_rows, int pooling, float* out_rows, cudaStream_t s,
                      const float* grad_scale = nullptr);
 
+// The sharded step over parts of ONE table k (bwd.cu): the occurrences of all parts are one batch, part order then
+// occurrence order.  check_shard_parts checks the parts before any device work (grads: their rows are gradient rows
+// the reduce reads, bf16 ones when bf16) and returns the occurrence count.
+int64_t check_shard_parts(const char* who, mono_mtable* mt, int k, const mono_pool_part* parts, int n_parts,
+                          bool grads, bool bf16);
+// the concatenated FIDs of the parts: one part's FIDs as they are, else written into buf (one launch)
+const int64_t* shard_parts_fids(mono_mtable* mt, int k, const mono_pool_part* parts, int n_parts, int64_t M,
+                                DevBuf& buf, cudaStream_t s);
+// grouping_build over the concatenated FIDs of the parts
+void grouping_build_parts(mono_grouping* g, mono_mtable* mt, int k, const mono_pool_part* parts, int n_parts, int N,
+                          int64_t* uniq_out, int32_t* occ_offset_out, int32_t* shard_counts_host,
+                          int64_t* n_unique_host, cudaStream_t s);
+// grouping_reduce (po.n == 0: into out_rows) or grouping_reduce_push (po.n > 0) with the parts' rows as the gradient
+// source (bf16: bf16 rows), through the parts occurrence map: one more launch than the reduce itself
+void grouping_reduce_parts(mono_grouping* g, mono_mtable* mt, int k, const mono_pool_part* parts, int n_parts,
+                           bool bf16, float* out_rows, const PeerOut& po, cudaStream_t s,
+                           const float* grad_scale = nullptr);
+
 // xstep.cu
 int64_t xstep_window_bytes(int N, int64_t C, int D);
 mono_xstep* xstep_create(mono_mtable* mt, int k, mono_peer* win, int64_t cap_pair);
@@ -446,6 +467,10 @@ void xstep_forward(mono_xstep* x, const int64_t* fids_dev, int64_t M, const int3
 void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride, int grad_col,
                     const int32_t* row_offsets, int pooling, const float* lr_host, int64_t update_time, cudaStream_t s,
                     const float* grad_scale = nullptr);
+// the step over parts of the xstep's table (bf16: the parts' rows are bf16; forward: output rows, backward: gradients)
+void xstep_forward_parts(mono_xstep* x, const mono_pool_part* parts, int n_parts, bool bf16, cudaStream_t s);
+void xstep_backward_parts(mono_xstep* x, const mono_pool_part* parts, int n_parts, bool bf16, const float* lr_host,
+                          int64_t update_time, cudaStream_t s, const float* grad_scale = nullptr);
 
 // table.cu
 void table_init(mono_mtable* mt, HostTable& t, const mono_table_cfg& cfg, cudaStream_t s);
@@ -560,6 +585,11 @@ template <typename T>
 void launch_gather_pool(const float* fused_emb, const int32_t* emb_offset, const int32_t* row_offsets,
                         int64_t n_rows, int dim, int pooling, T* out, int64_t out_stride, int out_col,
                         cudaStream_t s);
+// the pooling of received rows over the parts of table k of a sharded step (occ_offset: the grouping's row offset of
+// every occurrence of the concatenated parts): one launch per distinct kernel among the parts
+template <typename T>
+void launch_gather_pool_parts(mono_mtable* mt, int k, const float* rows_in, const int32_t* occ_offset,
+                              const mono_pool_part* parts, int n_parts, cudaStream_t s);
 template <typename T>
 void launch_gather_pool_grad(const T* pooled_grad, int64_t grad_stride, int grad_col, const int32_t* emb_offset,
                              const int32_t* row_offsets, int64_t n_rows, int dim, int pooling, float* grad_fused,

@@ -268,6 +268,146 @@ void launch_gather_pool_grad(const T* pooled_grad, int64_t grad_stride, int grad
   MONO_CHECK_LAUNCH();
 }
 
+// ---- pooling of received rows over the parts of a sharded step (ShardedStep.step_parts) ----
+// A part as the kernels below see it: blockIdx.y serves one part; offs points at the grouping's row offset of the
+// part's first occurrence, so offs[m] is the row of the part's occurrence m (row_offsets index the part's own FIDs).
+struct GatherPart {
+  const int32_t* offs;
+  const int32_t* row_offsets;  // null: one occurrence per row
+  int64_t n_rows;
+  void* out;                   // T rows of the launch
+  int64_t out_stride;
+  int32_t out_col, pooling;    // pooling: SUM or MEAN (gather_pool_parts_kernel)
+  int32_t seq_len, pad;        // FIRSTN: L (gather_seq_parts_kernel)
+};
+
+template <typename T, int G>
+__global__ void __launch_bounds__(kThreads, 4)
+gather_rows_parts_kernel(const float* __restrict__ rows_in, int dim, const GatherPart* __restrict__ parts) {
+  const GatherPart& p = parts[blockIdx.y];
+  gather_rows<T, G>(rows_in, p.offs, p.n_rows, dim, reinterpret_cast<T*>(p.out), p.out_stride, p.out_col);
+}
+
+template <typename T, int G>
+__global__ void __launch_bounds__(kThreads)
+gather_pool_parts_kernel(const float* __restrict__ rows_in, int dim, const GatherPart* __restrict__ parts) {
+  const GatherPart& p = parts[blockIdx.y];
+  gather_pool<T, G>(rows_in, p.offs, p.row_offsets, p.n_rows, dim, p.pooling, reinterpret_cast<T*>(p.out),
+                    p.out_stride, p.out_col);
+}
+
+// FIRSTN: one lane group per position slot q = r * L + j; position j < n_r is the row of the row's j-th occurrence,
+// the rest are +0.0 (as lookup_seq_kernel writes them).  rows_in is 16-byte aligned and dim % 4 == 0.
+template <typename T, int G>
+__global__ void __launch_bounds__(kThreads)
+gather_seq_parts_kernel(const float* __restrict__ rows_in, int dim, const GatherPart* __restrict__ parts) {
+  const GatherPart& p = parts[blockIdx.y];
+  const int gl = Group<G>::gl();
+  const int64_t L = p.seq_len, n_slots = p.n_rows * L;
+  const int64_t gstride = (int64_t)gridDim.x * (kThreads / G);
+  T* const out = reinterpret_cast<T*>(p.out) + p.out_col;
+  for (int64_t q = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G; q < n_slots; q += gstride) {
+    const int64_t r = q / L, j = q - r * L;
+    int64_t b = r, e = r + 1;
+    if (p.row_offsets) {
+      b = p.row_offsets[r];
+      e = p.row_offsets[r + 1];
+    }
+    const float* src = j < e - b ? rows_in + p.offs[b + j] : nullptr;
+    T* dst = out + r * p.out_stride + j * dim;
+    const bool vec = (reinterpret_cast<uintptr_t>(dst) & (4 * sizeof(T) - 1)) == 0;
+    for (int c = gl * 4; c < dim; c += G * 4) {
+      const float4 x = src ? __ldg(reinterpret_cast<const float4*>(src + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      if (vec) {
+        stcs_row4(dst + c, x);
+      } else {
+        const float a[4] = {x.x, x.y, x.z, x.w};
+        for (int w = 0; w < 4; ++w) dst[c + w] = to_row_elem(a[w], dst);
+      }
+    }
+  }
+}
+
+// The kernels of the parts pooling: the row copy (aligned one-FID parts), the pooling kernel, the FirstN kernel
+enum GatherKind { kGatherRows, kGatherPool, kGatherSeq, kGatherKinds };
+
+// One launch of a parts pooling kernel over ny parts
+template <typename T, int G>
+static void launch_gather_parts_kind(int kind, int64_t work, unsigned ny, const float* rows_in, int D,
+                                     const GatherPart* parts, cudaStream_t s) {
+  if (kind == kGatherRows) {
+    const auto kern = gather_rows_parts_kernel<T, G>;
+    kern<<<dim3(resident_grid(kern, work, kThreads), ny), kThreads, 0, s>>>(rows_in, D, parts);
+  } else if (kind == kGatherPool) {
+    const auto kern = gather_pool_parts_kernel<T, G>;
+    kern<<<dim3(grid_for(work, kThreads / G), ny), kThreads, 0, s>>>(rows_in, D, parts);
+  } else {
+    const auto kern = gather_seq_parts_kernel<T, G>;
+    kern<<<dim3(resident_grid(kern, work, kThreads / G), ny), kThreads, 0, s>>>(rows_in, D, parts);
+  }
+  MONO_CHECK_LAUNCH();
+}
+
+// Every SUM / MEAN part pooled exactly as launch_gather_pool pools it alone (the row copy for an aligned one-FID part,
+// the pooling kernel otherwise), every FIRSTN part by gather_seq_parts_kernel; the parts served by the same kernel share
+// one launch, one grid row per part, their arguments in one staged array.
+template <typename T>
+void launch_gather_pool_parts(mono_mtable* mt, int k, const float* rows_in, const int32_t* occ_offset,
+                              const mono_pool_part* parts, int n_parts, cudaStream_t s) {
+  const int D = mt->tables[k].dim;
+  if ((reinterpret_cast<uintptr_t>(rows_in) & 15) != 0) throw ArgError("gather_pool_parts: 16-byte aligned rows_in");
+  const int G = pick_group(D);
+  std::vector<GatherPart> by_kind[kGatherKinds];
+  int64_t work[kGatherKinds] = {0, 0, 0};
+  int order[kGatherKinds], n_kinds = 0;  // kinds in order of first use
+  int64_t occ = 0;
+  for (int i = 0; i < n_parts; ++i) {
+    const mono_pool_part& p = parts[i];
+    GatherPart g;
+    g.offs = occ_offset + occ;
+    g.row_offsets = p.row_offsets_dev;
+    g.n_rows = p.n_rows;
+    g.out = p.rows_dev;
+    g.out_stride = p.stride;
+    g.out_col = p.col;
+    // one occurrence per row: MEAN is x / 1, pooled as SUM (a copy), as launch_gather_pool does
+    g.pooling = p.row_offsets_dev ? p.pooling : MONO_POOL_SUM;
+    g.seq_len = p.pooling == MONO_POOL_FIRSTN ? p.max_seq_len : 0;
+    g.pad = 0;
+    occ += p.n_fids;
+    if (p.n_rows == 0) continue;
+    const bool rows = p.row_offsets_dev == nullptr && D <= 4 * G && (p.stride & 3) == 0 && (p.col & 3) == 0 &&
+                      (reinterpret_cast<uintptr_t>(p.rows_dev) & (4 * sizeof(T) - 1)) == 0;
+    const int kind = g.seq_len ? kGatherSeq : rows ? kGatherRows : kGatherPool;
+    if (by_kind[kind].empty()) order[n_kinds++] = kind;
+    by_kind[kind].push_back(g);
+    work[kind] = std::max(work[kind], kind == kGatherSeq ? p.n_rows * p.max_seq_len : p.n_rows);
+  }
+  if (n_kinds == 0) return;
+  const int rb = mt->ring.acquire();
+  static_assert(sizeof(GatherPart) * MONO_MAX_POOL_PARTS <= StageRing::kBlockBytes, "the parts fit one staged block");
+  size_t off = 0;
+  const GatherPart* d[kGatherKinds];
+  for (int q = 0; q < n_kinds; ++q) {
+    const auto& v = by_kind[order[q]];
+    std::memcpy(mt->ring.h(rb) + off, v.data(), sizeof(GatherPart) * v.size());
+    d[order[q]] = reinterpret_cast<const GatherPart*>(mt->ring.d(rb) + off);
+    off += sizeof(GatherPart) * v.size();
+  }
+  mt->ring.commit(rb, off, s);
+  by_group(G, [&](auto g) {
+    for (int q = 0; q < n_kinds; ++q) {
+      const int kind = order[q];
+      launch_gather_parts_kind<T, decltype(g)::value>(kind, work[kind], (unsigned)by_kind[kind].size(), rows_in, D,
+                                                      d[kind], s);
+    }
+  });
+}
+
+template void launch_gather_pool_parts<float>(mono_mtable*, int, const float*, const int32_t*, const mono_pool_part*,
+                                              int, cudaStream_t);
+template void launch_gather_pool_parts<__nv_bfloat16>(mono_mtable*, int, const float*, const int32_t*,
+                                                      const mono_pool_part*, int, cudaStream_t);
 template void launch_gather_pool<float>(const float*, const int32_t*, const int32_t*, int64_t, int, int, float*,
                                         int64_t, int, cudaStream_t);
 template void launch_gather_pool<__nv_bfloat16>(const float*, const int32_t*, const int32_t*, int64_t, int, int,

@@ -305,6 +305,7 @@ void xstep_destroy(mono_xstep* x) {
   cudaDeviceSynchronize();
   x->ws.release();
   x->miss_set.release();
+  x->fids_cat.release();
   for (int q = 0; q < 2; ++q) {
     x->uniq[q].release();
     x->offs[q].release();
@@ -315,11 +316,9 @@ void xstep_destroy(mono_xstep* x) {
   delete x;
 }
 
-// forward of one step: group, send FID buckets, serve the other ranks' buckets, pool.  Nothing returns to the host.
-void xstep_forward(mono_xstep* x, const int64_t* fids_dev, int64_t M, const int32_t* row_offsets, int64_t n_rows,
-                   int pooling, float* out, int64_t out_stride, int out_col, cudaStream_t s) {
-  MONO_CUDA(cudaSetDevice(x->mt->device));
-  if (M <= 0 || M > x->C) throw ArgError("xstep: batch larger than the window capacity (or empty)");
+// forward of one step up to the pooling: group, send FID buckets, serve the other ranks' buckets, wait for this rank's
+// rows.  Returns the occurrence offsets into the received rows (rows_in of the window).  Nothing returns to the host.
+static const int32_t* xstep_exchange_rows(mono_xstep* x, const int64_t* fids_dev, int64_t M, cudaStream_t s) {
   mono_mtable* mt = x->mt;
   upload_tables(mt, s);
   const XWin& w = x->w;
@@ -357,26 +356,46 @@ void xstep_forward(mono_xstep* x, const int64_t* fids_dev, int64_t M, const int3
   MONO_CHECK_LAUNCH();
   xwait_kernel<<<1, 32, 0, s>>>(w, kPhaseRows, seq, x->timeout_ns);
   MONO_CHECK_LAUNCH();
-  const float* rows_in = reinterpret_cast<const float*>(x->win->local + kPeerFlagBytes + w.off_rows);
-  launch_gather_pool(rows_in, offs, row_offsets, row_offsets ? n_rows : M, x->D, pooling, out, out_stride, out_col, s);
   x->last_m = M;
+  return offs;
+}
+
+static const float* xstep_rows_in(const mono_xstep* x) {
+  return reinterpret_cast<const float*>(x->win->local + kPeerFlagBytes + x->w.off_rows);
+}
+
+// forward of one step: the exchange, then the pooling of the received rows.  Nothing returns to the host.
+void xstep_forward(mono_xstep* x, const int64_t* fids_dev, int64_t M, const int32_t* row_offsets, int64_t n_rows,
+                   int pooling, float* out, int64_t out_stride, int out_col, cudaStream_t s) {
+  MONO_CUDA(cudaSetDevice(x->mt->device));
+  if (M <= 0 || M > x->C) throw ArgError("xstep: batch larger than the window capacity (or empty)");
+  const int32_t* offs = xstep_exchange_rows(x, fids_dev, M, s);
+  launch_gather_pool(xstep_rows_in(x), offs, row_offsets, row_offsets ? n_rows : M, x->D, pooling, out, out_stride,
+                     out_col, s);
   x->last_rows = row_offsets ? n_rows : M;
   x->fwd_done = true;
 }
 
-// backward of the step started by the last forward: per-FID gradient sums pushed to the owners, then this rank, as
-// an owner, resolves what it received and applies the sources in rank order.
-void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride, int grad_col,
-                    const int32_t* row_offsets, int pooling, const float* lr_host, int64_t update_time, cudaStream_t s,
-                    const float* grad_scale) {
+// forward over parts: the exchange of their concatenated FIDs (one part: its FIDs as they are), then the pooling of the
+// received rows part by part, one launch per distinct pooling kernel
+void xstep_forward_parts(mono_xstep* x, const mono_pool_part* parts, int n_parts, bool bf16, cudaStream_t s) {
+  const int64_t M = check_shard_parts("xstep_forward_parts", x->mt, x->k, parts, n_parts, false, bf16);
   MONO_CUDA(cudaSetDevice(x->mt->device));
-  if (!x->fwd_done) throw ArgError("xstep_backward without a forward");
-  // the owner's insert hands a new FID to the filter once per step (its leader), where the reference counts it once
-  // per requesting rank; until each source gets its own ordered filter pass, a filtered table trains at world 1 only.
-  // Thrown before anything is pushed, on every rank alike (the tables are configured alike).
-  if (x->N > 1 && x->mt->tables[x->k].dev.flt_cells)
-    throw ArgError("xstep_backward: a table with a hash filter needs world 1 (per-rank filter counts are not kept)");
-  x->fwd_done = false;
+  if (M <= 0 || M > x->C) throw ArgError("xstep: batch larger than the window capacity (or empty)");
+  const int64_t* fids = shard_parts_fids(x->mt, x->k, parts, n_parts, M, x->fids_cat, s);
+  const int32_t* offs = xstep_exchange_rows(x, fids, M, s);
+  if (bf16) launch_gather_pool_parts<__nv_bfloat16>(x->mt, x->k, xstep_rows_in(x), offs, parts, n_parts, s);
+  else launch_gather_pool_parts<float>(x->mt, x->k, xstep_rows_in(x), offs, parts, n_parts, s);
+  x->fwd_done = true;
+}
+
+// backward of the step started by the last forward: per-FID gradient sums pushed to the owners (reduce_push: the
+// requester's reduce into the owners' windows), then this rank, as an owner, resolves what it received and applies the
+// sources in rank order.
+template <class ReducePush>
+static void xstep_backward_impl(mono_xstep* x, const float* lr_host, int64_t update_time, cudaStream_t s,
+                                const ReducePush& reduce_push) {
+  MONO_CUDA(cudaSetDevice(x->mt->device));
   mono_mtable* mt = x->mt;
   mt->note_insert(s);
   HostTable& ht = mt->tables[x->k];
@@ -391,7 +410,7 @@ void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride
     po.base[r] = x->win->base[r] + kPeerFlagBytes + w.off_grads + (int64_t)x->me * x->C * x->D * 4;
   mono_grouping* g = x->grouping[par];
   po.cnt_dev = g->plan.ctr + kCtrOwners;
-  grouping_reduce_push(g, pooled_grad, grad_stride, grad_col, row_offsets, x->last_rows, pooling, po, s, grad_scale);
+  reduce_push(g, po);
   xsignal_kernel<<<1, 32, 0, s>>>(w, kPhaseGrads, seq, nullptr);
   MONO_CHECK_LAUNCH();
   // owner: resolve (+ insert) everything received, then apply source by source
@@ -451,6 +470,36 @@ void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride
   request_snapshot(mt, x->k, s);
   MONO_CUDA(cudaEventRecord(x->ev_bwd[par], s));  // grouping [par] is free again once this point is reached
   x->bwd_recorded[par] = true;
+}
+
+void xstep_backward(mono_xstep* x, const float* pooled_grad, int64_t grad_stride, int grad_col,
+                    const int32_t* row_offsets, int pooling, const float* lr_host, int64_t update_time, cudaStream_t s,
+                    const float* grad_scale) {
+  if (!x->fwd_done) throw ArgError("xstep_backward without a forward");
+  // the owner's insert hands a new FID to the filter once per step (its leader), where the reference counts it once
+  // per requesting rank; until each source gets its own ordered filter pass, a filtered table trains at world 1 only.
+  // Thrown before anything is pushed, on every rank alike (the tables are configured alike).
+  if (x->N > 1 && x->mt->tables[x->k].dev.flt_cells)
+    throw ArgError("xstep_backward: a table with a hash filter needs world 1 (per-rank filter counts are not kept)");
+  x->fwd_done = false;
+  xstep_backward_impl(x, lr_host, update_time, s, [&](mono_grouping* g, const PeerOut& po) {
+    grouping_reduce_push(g, pooled_grad, grad_stride, grad_col, row_offsets, x->last_rows, pooling, po, s, grad_scale);
+  });
+}
+
+// backward over parts: the parts must be the forward's (same FIDs and rows); their gradient rows reach the reduce
+// through the parts occurrence map, one launch more than xstep_backward
+void xstep_backward_parts(mono_xstep* x, const mono_pool_part* parts, int n_parts, bool bf16, const float* lr_host,
+                          int64_t update_time, cudaStream_t s, const float* grad_scale) {
+  const int64_t M = check_shard_parts("xstep_backward_parts", x->mt, x->k, parts, n_parts, true, bf16);
+  if (!x->fwd_done) throw ArgError("xstep_backward_parts without a forward");
+  if (x->N > 1 && x->mt->tables[x->k].dev.flt_cells)   // as xstep_backward
+    throw ArgError("xstep_backward: a table with a hash filter needs world 1 (per-rank filter counts are not kept)");
+  if (M != x->last_m) throw ArgError("xstep_backward_parts: the parts are not the forward's batch");
+  x->fwd_done = false;
+  xstep_backward_impl(x, lr_host, update_time, s, [&](mono_grouping* g, const PeerOut& po) {
+    grouping_reduce_parts(g, x->mt, x->k, parts, n_parts, bf16, nullptr, po, s, grad_scale);
+  });
 }
 
 // Build the grouping of the NEXT batch on stream s2 while the current step runs on its own stream: the grouping

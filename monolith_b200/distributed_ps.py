@@ -323,6 +323,71 @@ def exchange_plan(cnt, me: int):
           "rows_dst": row_pre[:N, me].copy(), "recv_at": col_pre[:N, me].copy()}
 
 
+class _FlatSource:
+  """What the peer and NCCL exchanges of ShardedStep.step() group, pool and reduce: one FID list, one pooling, one
+  output tensor and its gradient."""
+
+  def __init__(self, st, fids, pooled_grad, out, row_offsets, pooling, grad_scale):
+    self.st, self.fids, self.grad, self.out = st, fids, pooled_grad, out
+    self.row_offsets, self.pooling, self.grad_scale = row_offsets, pooling, grad_scale
+    self.n_fids, self.device = fids.numel(), fids.device
+
+  def build(self, N, D):
+    return self.st.grouping.build(self.fids, N, D)
+
+  def pool(self, rows, offs):
+    self.st.dops.gather_pool(rows, offs, self.st.dim, self.row_offsets, self.pooling, out=self.out)
+
+  def take_grads(self):
+    if callable(self.grad):
+      self.grad = self.grad()
+
+  def reduce(self, out_rows):
+    self.st.grouping.reduce(self.grad, out_rows, self.row_offsets, self.pooling, grad_scale=self.grad_scale)
+
+  def reduce_push(self, counts, window, region_off, dst_row_off):
+    self.st.grouping.reduce_push(self.grad, counts, window, region_off, dst_row_off, self.row_offsets, self.pooling,
+                                 grad_scale=self.grad_scale)
+
+
+class _PartsSource:
+  """What the peer and NCCL exchanges of ShardedStep.step_parts() group, pool and reduce: the parts of one table as
+  one batch (the mono_pool_part arrays of the forward rows and of the gradients)."""
+
+  def __init__(self, st, fwd, grads, grad_scale):
+    self.st, self.fwd, self.grads, self.grad_scale = st, fwd, grads, grad_scale
+    self.n_fids, self.device = fwd.n_fids, st.device
+    self.bwd = None
+
+  def build(self, N, D):
+    return self.st.grouping.build_parts(self.st.table, self.fwd.arr, self.fwd.n, self.n_fids, N, D)
+
+  def pool(self, rows, offs):
+    self.st.dops.gather_pool_parts(self.st.table, rows, offs, self.fwd.arr, self.fwd.n, self.fwd.bf16)
+
+  def take_grads(self):
+    self.bwd = self.st._grad_parts(self.fwd, self.grads() if callable(self.grads) else self.grads)
+
+  def reduce(self, out_rows):
+    self.st.grouping.reduce_parts(self.st.table, self.bwd.arr, self.bwd.n, self.bwd.bf16, out_rows,
+                                  grad_scale=self.grad_scale)
+
+  def reduce_push(self, counts, window, region_off, dst_row_off):
+    self.st.grouping.reduce_push_parts(self.st.table, self.bwd.arr, self.bwd.n, self.bwd.bf16, counts, window,
+                                       region_off, dst_row_off, grad_scale=self.grad_scale)
+
+
+class _PartsArr:
+  """A parts call's mono_pool_part array with the tensors it points at (alive until the kernels have run)."""
+
+  def __init__(self, table, parts, forward: bool):
+    self.parts = list(parts)
+    self.n = len(self.parts)
+    self.arr, self.keep, self.rows = table._parts_arr(self.parts, forward=forward)
+    self.bf16 = self.rows[0].dtype == torch.bfloat16
+    self.n_fids = sum(int(self.arr[i].n_fids) for i in range(self.n))
+
+
 class ShardedStep:
   """Sparse train step of ONE table on N GPUs, fast path: the batch is grouped once
   (distribution_ops.Grouping) and that grouping serves both the forward (dedup + bucket by owner + pooling
@@ -384,13 +449,14 @@ class ShardedStep:
     total = self.off_grads_out + al(self.cap_rows * D * 4)
     self.window = self.dops.PeerWindow(self.device, self.N, self.rank, total, self.group)
 
-  def _step_peer(self, fids, pooled_grad, out, req_time, row_offsets, pooling, grad_scale):
+  def _step_peer(self, src, req_time):
+    """src: what is pooled and reduced (_FlatSource for step(), _PartsSource for step_parts())."""
     import numpy as np
     N, D, me, ph = self.N, self.dim, self.rank, self.phases
     ph.mark("start")
-    uniq, offs, shard_sizes = self.grouping.build(fids, N, D)                         # 1
+    uniq, offs, shard_sizes = src.build(N, D)                                         # 1
     ph.mark("f1_group")
-    mat = self.hostx.exchange([fids.numel()] + list(shard_sizes))                     # 2 (host only)
+    mat = self.hostx.exchange([src.n_fids] + list(shard_sizes))                       # 2 (host only)
     max_m, cnt = int(mat[:, 0].max()), mat[:, 1:]                                     # cnt[r][o]
     need_recv = int(cnt.sum(axis=0).max())
     if self.window is None or max_m > self.cap_rows or need_recv > self.cap_recv:      # same decision on every rank
@@ -420,19 +486,17 @@ class ShardedStep:
       ph.fine("f5b_barrier")
       self.window.get(self.off_rows_out, my_seg * D * 4, rows_in, bucket_at * D * 4, cnt[me] * D * 4)  # 5 pull
       ph.mark("f5_lookup_pull")
-    self.dops.gather_pool(rows_in, offs, D, row_offsets, pooling, out=out)            # 6
+    src.pool(rows_in, offs)                                                           # 6
     ph.mark("f6_gather_pool")
-    if callable(pooled_grad):   # forward enqueued: the caller's dense tower / host round trip goes here
-      pooled_grad = pooled_grad()
+    src.take_grads()            # forward enqueued: the caller's dense tower / host round trip goes here
     if self.bulk == "push":
-      self.grouping.reduce_push(pooled_grad, cnt[me], self.window, self.off_grads, my_seg, row_offsets, pooling,  # 7+8
-                                grad_scale=grad_scale)
+      src.reduce_push(cnt[me], self.window, self.off_grads, my_seg)                   # 7+8
       ph.fine("b8a_reduce_push_kernels")
       self.window.barrier()
       ph.mark("b8_reduce_push")
     else:
       grads_out = self.window.view(self.off_grads_out, uniq.numel() * D, torch.float32)
-      self.grouping.reduce(pooled_grad, grads_out, row_offsets, pooling, grad_scale=grad_scale)  # 7 requester: bucketed by owner
+      src.reduce(grads_out)                                                           # 7 requester: bucketed by owner
       ph.fine("b8a_reduce")
       self.window.barrier()
       ph.fine("b8b_barrier")
@@ -532,6 +596,105 @@ class ShardedStep:
     self.direct_steps += 1
     return 0
 
+  # ---- several features of the table in one step (step_parts) ----------------------------------------------------
+  def _grad_parts(self, fwd, grads) -> _PartsArr:
+    """The gradient rows of step_parts, checked before any device work: one tensor per part, on the step's device with
+    unit column stride and at least the part's [n_rows, col + width] (width: dim, max_seq_len * dim for "firstn"), all
+    float32 or all bfloat16, with the rows the reduce reads (stride and col multiples of 4, 16-byte aligned float32 or
+    8-byte aligned bfloat16 rows).  The forward's array with the gradient rows in place of the output rows."""
+    import ctypes as C
+    if isinstance(grads, torch.Tensor) or len(grads) != fwd.n:
+      raise ValueError("step_parts: grads must be a list with one gradient tensor per part")
+    dtypes = {g.dtype for g in grads if isinstance(g, torch.Tensor)}
+    if len(dtypes) != 1 or not dtypes <= {torch.float32, torch.bfloat16}:
+      raise ValueError("step_parts: the gradients must be tensors, all float32 or all bfloat16")
+    gp = _PartsArr.__new__(_PartsArr)
+    gp.parts, gp.n, gp.n_fids, gp.rows, gp.keep = fwd.parts, fwd.n, fwd.n_fids, list(grads), fwd.keep
+    gp.bf16 = dtypes == {torch.bfloat16}
+    gp.arr = (type(fwd.arr[0]) * len(fwd.arr))()
+    C.memmove(gp.arr, fwd.arr, C.sizeof(fwd.arr))
+    esz = 2 if gp.bf16 else 4
+    for i, (p, g) in enumerate(zip(fwd.parts, grads)):
+      a = gp.arr[i]
+      width = self.dim * (p.max_seq_len if p.pooling == "firstn" else 1)
+      if g.dim() != 2 or g.device != self.table.device or g.stride(1) != 1 or g.shape[0] < a.n_rows or \
+          g.shape[1] < p.col + width:
+        raise ValueError("step_parts: a gradient must be a 2-D tensor on the step's device with unit column stride and "
+                         "at least the part's [n_rows, col + width]")
+      if g.stride(0) % 4 or p.col % 4 or g.data_ptr() % (4 * esz):
+        raise ValueError("step_parts: gradient rows need stride % 4 == 0, col % 4 == 0 and 16-byte (bfloat16: 8-byte) "
+                         "aligned rows")
+      a.rows_dev, a.stride = g.data_ptr(), g.stride(0)
+    return gp
+
+  def step_parts(self, parts, grads, req_time: int, grad_scale: Optional[torch.Tensor] = None):
+    """One sparse train step over several features of this table: the many-feature form of step(), with the semantics
+    of MultiHashTable.lookup_pool_parts / pool_backward_parts on the global table.
+
+    parts: PoolPart list, every one naming this step's table (ValueError otherwise).  Each part's rows are its forward
+    output ("sum", "mean" or "firstn" with max_seq_len, at any column and stride, so several parts may write disjoint
+    columns of one tower tensor; a part without rows gets a new tensor), all float32 or all bfloat16.
+    grads: one gradient tensor per part, with the part's shape and column, all float32 or all bfloat16 (independent of
+    the forward's dtype), or a callable returning that list: it is called once the forward has been enqueued.
+    grad_scale: as step()'s.
+
+    The occurrences of all parts are ONE batch, part order then occurrence order, so each distinct FID gets one upsert,
+    one timestamp bump, one admission-filter count and one optimizer step with the sum of its terms over all parts (a
+    "mean" term divided by its row's n; a "firstn" occurrence at j >= max_seq_len a +0.0 term).  bfloat16 outputs are
+    the float32 values rounded once; bfloat16 gradients are widened exactly first.  With one "sum" or "mean" part the
+    step is bit for bit step() on that part.  Bad inputs raise before any device work and leave the table unchanged (a
+    callable's list is checked when it returns, after the forward).  Returns each part's output rows, in part order."""
+    parts = list(parts)
+    if not parts:
+      raise ValueError("step_parts needs at least one part")
+    for p in parts:
+      if p.slot != self.name:
+        raise ValueError(f"step_parts: part of table {p.slot!r}, the step's table is {self.name!r}")
+    if grad_scale is not None:
+      from .clip_ops import scale_ptr
+      scale_ptr(grad_scale, self.device, "grad_scale")
+    from . import _lib
+    fwd = _PartsArr(self.table, parts, forward=True)
+    # the engine's own checks, here too: the direct exchange may re-create its window before its forward call
+    for i in range(fwd.n):
+      a = fwd.arr[i]
+      if a.pooling == _lib.POOL_FIRSTN and a.n_rows * a.max_seq_len > (1 << 31):
+        raise ValueError("step_parts: a 'firstn' part needs n_rows * max_seq_len <= 2^31")
+    if fwd.n_fids >= (1 << 29):
+      raise ValueError("step_parts: 2^29 occurrences or more in one step")
+    bwd = None if callable(grads) else self._grad_parts(fwd, grads)
+    if self.exchange == "direct":
+      self._step_parts_direct(fwd, bwd, grads, req_time, grad_scale)
+    else:
+      src = _PartsSource(self, fwd, grads, grad_scale)
+      if self.exchange == "peer":
+        self._step_peer(src, req_time)
+      else:
+        self._step_nccl(src, req_time)
+    return fwd.rows
+
+  def _step_parts_direct(self, fwd, bwd, grads, req_time, grad_scale):
+    import ctypes as C
+    from . import _lib
+    lib = _lib.load()
+    if self.xstep is None or fwd.n_fids > self.cap_pair:
+      # NOTE collective, as in _step_direct
+      self._make_xstep(fwd.n_fids)
+    stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+    fn = lib.mono_xstep_forward_parts_bf16 if fwd.bf16 else lib.mono_xstep_forward_parts
+    _lib.check(fn(self.xstep, fwd.arr, fwd.n, stream))
+    if bwd is None:   # forward enqueued: the caller's dense tower / host round trip goes here
+      bwd = self._grad_parts(fwd, grads())
+    lr = self.table.configs[self.name].call_learning_rate_fns()
+    lr_arr = (C.c_float * len(lr))(*lr)
+    stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+    name = "mono_xstep_backward_parts" + ("_bf16" if bwd.bf16 else "") + ("" if grad_scale is None else "_scaled")
+    args = (self.xstep, bwd.arr, bwd.n, lr_arr, int(req_time))
+    args += () if grad_scale is None else (C.c_void_p(grad_scale.data_ptr()),)
+    _lib.check(getattr(lib, name)(*args, stream))
+    self._keep = (fwd, bwd, grad_scale)   # alive until the kernels have consumed them
+    self.direct_steps += 1
+
   def _slot(self, per_shard):
     """per-(shard, table) sizes with only this table populated."""
     out = [0] * (self.N * self.K)
@@ -558,12 +721,16 @@ class ShardedStep:
       scale_ptr(grad_scale, self.device, "grad_scale")
     if self.exchange == "direct":
       return self._step_direct(fids, pooled_grad, out, req_time, row_offsets, pooling, grad_scale)
+    src = _FlatSource(self, fids, pooled_grad, out, row_offsets, pooling, grad_scale)
     if self.exchange == "peer":
-      return self._step_peer(fids, pooled_grad, out, req_time, row_offsets, pooling, grad_scale)
-    N, D, dev, ph = self.N, self.dim, fids.device, self.phases
+      return self._step_peer(src, req_time)
+    return self._step_nccl(src, req_time)
+
+  def _step_nccl(self, src, req_time):
+    N, D, dev, ph = self.N, self.dim, src.device, self.phases
     self.nccl_steps += 1
     ph.mark("start")
-    uniq, offs, shard_sizes = self.grouping.build(fids, N, D)                       # 1
+    uniq, offs, shard_sizes = src.build(N, D)                                       # 1
     ph.mark("f1_group")
     send_cnt = torch.tensor(shard_sizes, dtype=torch.int64, device=dev)               # 2
     recv_cnt = torch.empty_like(send_cnt)
@@ -578,12 +745,11 @@ class ShardedStep:
     recv_rows = torch.empty(uniq.numel() * D, dtype=torch.float32, device=dev)        # 5
     _a2a(recv_rows, rows, [s * D for s in shard_sizes], [s * D for s in recv_sizes], self.group)
     ph.mark("f5_a2a_rows")
-    self.dops.gather_pool(recv_rows, offs, D, row_offsets, pooling, out=out)          # 6
+    src.pool(recv_rows, offs)                                                         # 6
     ph.mark("f6_gather_pool")
-    if callable(pooled_grad):
-      pooled_grad = pooled_grad()
+    src.take_grads()
     grad_rows = torch.empty(uniq.numel() * D, dtype=torch.float32, device=dev)        # 7
-    self.grouping.reduce(pooled_grad, grad_rows, row_offsets, pooling, grad_scale=grad_scale)
+    src.reduce(grad_rows)
     ph.mark("b7_reduce_grads")
     owner_grads = torch.empty(sum(recv_sizes) * D, dtype=torch.float32, device=dev)   # 8
     _a2a(owner_grads, grad_rows, [s * D for s in recv_sizes], [s * D for s in shard_sizes], self.group)

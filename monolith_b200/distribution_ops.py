@@ -651,6 +651,46 @@ class Grouping:
     else:
       _lib.check(self._lib.mono_grouping_reduce_push_scaled(*args, sp, _stream(self.device)))
 
+  # ---- several features (mono_pool_part arrays) of ONE table as one batch: the sharded step over parts ----
+  def build_parts(self, table, parts_arr, n_parts: int, n_fids: int, num_shards: int, dim: int):
+    """build() over the concatenated FIDs of the parts (mono_grouping_build_parts; `table` is the MultiHashTable the
+    parts name, n_fids their total occurrence count)."""
+    uniq = torch.empty(max(n_fids, 1), dtype=torch.int64, device=self.device)
+    offs = torch.empty(max(n_fids, 1), dtype=torch.int32, device=self.device)
+    counts = (C.c_int32 * num_shards)()
+    n_u = C.c_int64(0)
+    _lib.check(self._lib.mono_grouping_build_parts(self._h, table._h, parts_arr, n_parts, num_shards, _ptr(uniq),
+                                                   _ptr(offs), counts, C.byref(n_u), _stream(self.device)))
+    self.dim = dim
+    return uniq[:n_u.value], offs[:n_fids], list(counts)
+
+  def reduce_parts(self, table, parts_arr, n_parts: int, bf16: bool, out_rows: torch.Tensor,
+                   grad_scale: Optional[torch.Tensor] = None):
+    """reduce() with the parts' rows as the gradients (mono_grouping_reduce_parts[_bf16][_scaled])."""
+    sp = _grad_scale_ptr(grad_scale, self.device)
+    name = "mono_grouping_reduce_parts" + ("_bf16" if bf16 else "") + ("" if sp is None else "_scaled")
+    args = (self._h, table._h, parts_arr, n_parts, _ptr(out_rows)) + (() if sp is None else (sp,))
+    _lib.check(getattr(self._lib, name)(*args, _stream(self.device)))
+    return out_rows
+
+  def reduce_push_parts(self, table, parts_arr, n_parts: int, bf16: bool, shard_sizes: Sequence[int],
+                        window: "PeerWindow", region_off: int, dst_row_off: Sequence[int],
+                        grad_scale: Optional[torch.Tensor] = None):
+    """reduce_push() with the parts' rows as the gradients (mono_grouping_reduce_push_parts[_bf16][_scaled])."""
+    sp = _grad_scale_ptr(grad_scale, self.device)
+    n = window.world
+    name = "mono_grouping_reduce_push_parts" + ("_bf16" if bf16 else "") + ("" if sp is None else "_scaled")
+    args = (self._h, table._h, parts_arr, n_parts, (C.c_int64 * n)(*[int(x) for x in shard_sizes]), window._h,
+            int(region_off), (C.c_int64 * n)(*[int(x) for x in dst_row_off])) + (() if sp is None else (sp,))
+    _lib.check(getattr(self._lib, name)(*args, _stream(self.device)))
+
+
+def gather_pool_parts(table, rows_in: torch.Tensor, occ_offsets: torch.Tensor, parts_arr, n_parts: int, bf16: bool):
+  """The pooling of looked-up rows into the rows of the parts (mono_gather_pool_parts[_bf16]): occ_offsets are a
+  parts grouping's row offsets (Grouping.build_parts), `table` the MultiHashTable the parts name."""
+  fn = table._lib.mono_gather_pool_parts_bf16 if bf16 else table._lib.mono_gather_pool_parts
+  _lib.check(fn(table._h, _ptr(rows_in), _ptr(occ_offsets), parts_arr, n_parts, _stream(rows_in.device)))
+
 
 class _RawCuda:
   """__cuda_array_interface__ carrier for a raw device pointer (torch.as_tensor makes a view of it)."""
