@@ -1,10 +1,13 @@
 """ctypes binding of libmono_emb.so (the C ABI in include/mono_emb.h).
 
 This is the same kind of stub a reference maintainer would write to call the engine from
-monolith/native_training (see INTEGRATION.md): plain pointers and sizes, no torch types.
+monolith/native_training (see INTEGRATION.md): plain pointers and sizes, no torch types.  The helpers at the
+end turn torch tensors and streams into those pointers and choose a call's _bf16 or _scaled twin.
 """
 import ctypes as C
 import os
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libmono_emb.so")
@@ -67,6 +70,21 @@ FLAG_IDS_UNIQUE, FLAG_DEDUP_SUM = 1, 2
 _p = C.c_void_p
 _i32, _i64, _u32 = C.c_int32, C.c_int64, C.c_uint32
 
+_BF16, _SCALED, _ALL = ("_bf16",), ("_scaled",), ("_bf16", "_scaled", "_bf16_scaled")
+
+
+def _twins(base, restype, argtypes, twins):
+  """`base` and its twins: a "_bf16" twin takes the base's arguments, a "_scaled" one adds the device pointer of the
+  gradient scale just before the stream."""
+  return {base + t: (restype, argtypes[:-1] + [_p] + argtypes[-1:] if t.endswith("_scaled") else argtypes)
+          for t in ("",) + twins}
+
+
+_LOOKUP = [_p, _p, _p, _p, _p]
+_FILL = [_i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _i64, _p, _p, _p]
+_FILL_GRAD = [_i32, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _p, _p]
+_LAYOUT = [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32, C.POINTER(SliceTask), _i32, _p, _p]
+
 # name -> (restype, argtypes); every symbol include/mono_emb.h declares
 SIGNATURES = {
     "mono_last_error": (C.c_char_p, []),
@@ -77,7 +95,7 @@ SIGNATURES = {
     "mono_xstep_destroy": (C.c_int, [_p]),
     "mono_xstep_prepare": (C.c_int, [_p, _p, _i64, _p]),
     "mono_xstep_forward": (C.c_int, [_p, _p, _i64, _p, _i64, _i32, _p, _i64, _i32, _p]),
-    "mono_xstep_backward": (C.c_int, [_p, _p, _i64, _i32, _p, _i32, _p, _i64, _p]),
+    **_twins("mono_xstep_backward", C.c_int, [_p, _p, _i64, _i32, _p, _i32, _p, _i64, _p], _SCALED),
     "mono_bench_tower_scratch_floats": (_i64, []),
     "mono_bench_tower_grad": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _p, _i64, _p]),
     "mono_set_option": (C.c_int, [C.c_char_p, _i64]),
@@ -93,18 +111,17 @@ SIGNATURES = {
     "mono_mtable_size": (C.c_int, [_p, _i32, C.POINTER(_i64), _p]),
     "mono_mtable_max_update_ts": (_i64, [_p, _i32]),
     "mono_mtable_counters": (C.c_int, [_p, _i32, _p, _i32, _p]),
-    "mono_mtable_lookup": (C.c_int, [_p, _p, _p, _p, _p]),
+    "mono_mtable_lookup": (C.c_int, _LOOKUP),
     "mono_mtable_fused_offsets": (C.c_int, [_p, _p, _i32, _p, _p, _p]),
     "mono_mtable_fused_lookup": (C.c_int, [_p, _p, _p, _i32, _i64, _p, _p]),
     "mono_mtable_set_hash_filter": (C.c_int, [_p, _i32, _i64, _u32, _p, _p, _i32, _p]),
     "mono_mtable_hash_filter_cells": (C.c_int, [_p, _i32, _p, _i64, _p]),
     "mono_mtable_contains": (C.c_int, [_p, _i32, _p, _i64, _p, _p]),
     "mono_mtable_lookup_pool": (C.c_int, [_p, _i32, _p, _p, _i64, _i32, _p, _i64, _i32, _p]),
-    "mono_mtable_pool_backward": (C.c_int, [_p, _i32, _p, _i64, _p, _i64, _i32, _p, _i64, _i32, _p, _i64, _i64, _p]),
-    "mono_mtable_lookup_pool_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p]),
-    "mono_mtable_pool_backward_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p]),
-    "mono_mtable_lookup_pool_parts_bf16": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p]),
-    "mono_mtable_pool_backward_parts_bf16": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p]),
+    **_twins("mono_mtable_pool_backward", C.c_int,
+             [_p, _i32, _p, _i64, _p, _i64, _i32, _p, _i64, _i32, _p, _i64, _i64, _p], _SCALED),
+    **_twins("mono_mtable_lookup_pool_parts", C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p], _BF16),
+    **_twins("mono_mtable_pool_backward_parts", C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p], _ALL),
     "mono_mtable_optimize": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i64, _u32, _p]),
     "mono_mtable_fused_optimize": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i32, _u32, _p]),
     "mono_mtable_assign": (C.c_int, [_p, _p, _p, _p, _i64, _u32, _p]),
@@ -120,23 +137,20 @@ SIGNATURES = {
                                             _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "mono_unique_key_with_value_and_offset": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _p]),
     "mono_ragged_split_by_indices": (C.c_int, [_i32, _p, _p, _i64, _p, _i32, _i32, _p, _p, _p, _p, _p, _p, _p]),
-    "mono_fill_with_offset_map": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _i64, _p, _p, _p]),
-    "mono_fill_with_offset_map_grad": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _p, _p]),
-    "mono_mtable_lookup_f16": (C.c_int, [_p, _p, _p, _p, _p]),
+    "mono_fill_with_offset_map": (C.c_int, _FILL),
+    "mono_fill_with_offset_map_grad": (C.c_int, _FILL_GRAD),
+    "mono_mtable_lookup_f16": (C.c_int, _LOOKUP),
     "mono_sharding_sparse_fids_v5": (C.c_int, [_i32, _p, _p, C.POINTER(ShardingFeature), _i32, _i32, _i32, _i32, _p,
                                                _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _p, _p, _p]),
     "mono_normalize_merged_split": (C.c_int, [_i32, _p, _i64, _p, _i64, _p, _p, _p]),
     "mono_round_to_f16": (C.c_int, [_i32, _p, _i64, _p, _p]),
-    "mono_embedding_to_layout_f16in": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
-                                                 C.POINTER(SliceTask), _i32, _p, _p]),
-    "mono_embedding_to_layout_f16in_bf16": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
-                                                      C.POINTER(SliceTask), _i32, _p, _p]),
-    "mono_fill_with_offset_map_f16": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _i64, _p, _p, _p]),
-    "mono_fill_with_offset_map_grad_f16": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _p, _p]),
+    **_twins("mono_embedding_to_layout_f16in", C.c_int, _LAYOUT, _BF16),
+    "mono_fill_with_offset_map_f16": (C.c_int, _FILL),
+    "mono_fill_with_offset_map_grad_f16": (C.c_int, _FILL_GRAD),
     "mono_grouping_create": (C.c_int, [_i32, C.POINTER(_p)]),
     "mono_grouping_destroy": (C.c_int, [_p]),
     "mono_grouping_build": (C.c_int, [_p, _p, _i64, _i32, _i32, _p, _p, _p, C.POINTER(_i64), _p]),
-    "mono_grouping_reduce": (C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p]),
+    **_twins("mono_grouping_reduce", C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p], _SCALED),
     "mono_peer_create": (C.c_int, [_i32, _i32, _i32, _i64, C.POINTER(_p)]),
     "mono_peer_destroy": (C.c_int, [_p]),
     "mono_peer_detach": (C.c_int, [_p]),
@@ -147,67 +161,26 @@ SIGNATURES = {
     "mono_peer_put": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p]),
     "mono_peer_get": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p]),
     "mono_mtable_lookup_push": (C.c_int, [_p, _i32, _p, _p, _p, _i64, _p, _p]),
-    "mono_grouping_reduce_push": (C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p, _i64, _p, _p]),
-    "mono_gather_pool": (C.c_int, [_i32, _p, _p, _p, _i64, _i32, _i32, _p, _i64, _i32, _p]),
-    "mono_gather_pool_grad": (C.c_int, [_i32, _p, _i64, _i32, _p, _p, _i64, _i32, _i32, _p, _p]),
-    "mono_scatter_grad_rows": (C.c_int, [_i32, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _i32, _p, _i64, _p]),
-    "mono_embedding_to_layout": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
-                                           C.POINTER(SliceTask), _i32, _p, _p]),
-    "mono_embedding_to_layout_grad": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
-                                                C.POINTER(SliceTask), _i32, _p, _p]),
-    "mono_gather_pool_bf16": (C.c_int, [_i32, _p, _p, _p, _i64, _i32, _i32, _p, _i64, _i32, _p]),
-    "mono_gather_pool_grad_bf16": (C.c_int, [_i32, _p, _i64, _i32, _p, _p, _i64, _i32, _i32, _p, _p]),
-    "mono_scatter_grad_rows_bf16": (C.c_int, [_i32, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _i32, _p, _i64, _p]),
-    "mono_embedding_to_layout_bf16": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
-                                                C.POINTER(SliceTask), _i32, _p, _p]),
-    "mono_embedding_to_layout_grad_bf16": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
-                                                     C.POINTER(SliceTask), _i32, _p, _p]),
-    "mono_reduce_and_split": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
-    "mono_reduce_and_split_grad": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
-    "mono_reduce_and_split_bf16": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
-    "mono_reduce_and_split_grad_bf16": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p]),
+    **_twins("mono_grouping_reduce_push", C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p, _i64, _p, _p],
+             _SCALED),
+    **_twins("mono_gather_pool", C.c_int, [_i32, _p, _p, _p, _i64, _i32, _i32, _p, _i64, _i32, _p], _BF16),
+    **_twins("mono_gather_pool_grad", C.c_int, [_i32, _p, _i64, _i32, _p, _p, _i64, _i32, _i32, _p, _p], _ALL),
+    **_twins("mono_scatter_grad_rows", C.c_int, [_i32, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _i32, _p, _i64, _p],
+             _ALL),
+    **_twins("mono_embedding_to_layout", C.c_int, _LAYOUT, _BF16),
+    **_twins("mono_embedding_to_layout_grad", C.c_int, _LAYOUT, _ALL),
+    **_twins("mono_reduce_and_split", C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p], _BF16),
+    **_twins("mono_reduce_and_split_grad", C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p], _ALL),
     "mono_mtable_note_update_ts": (C.c_int, [_p, _i32, _i64]),
     "mono_global_norm": (C.c_int, [_i32, C.POINTER(NormTensor), _i32, C.c_float, _p, _p, _p]),
-    "mono_mtable_pool_backward_parts_scaled": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p, _p]),
-    "mono_mtable_pool_backward_parts_bf16_scaled": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _i64, _p,
-                                                              _p]),
-    "mono_embedding_to_layout_grad_scaled": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
-                                                       C.POINTER(SliceTask), _i32, _p, _p, _p]),
-    "mono_embedding_to_layout_grad_bf16_scaled": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _i32, _p, _i32, _i32,
-                                                            C.POINTER(SliceTask), _i32, _p, _p, _p]),
-    "mono_gather_pool_grad_scaled": (C.c_int, [_i32, _p, _i64, _i32, _p, _p, _i64, _i32, _i32, _p, _p, _p]),
-    "mono_gather_pool_grad_bf16_scaled": (C.c_int, [_i32, _p, _i64, _i32, _p, _p, _i64, _i32, _i32, _p, _p, _p]),
-    "mono_scatter_grad_rows_scaled": (C.c_int, [_i32, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _i32, _p, _i64, _p,
-                                                _p]),
-    "mono_scatter_grad_rows_bf16_scaled": (C.c_int, [_i32, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _i32, _p, _i64,
-                                                     _p, _p]),
-    "mono_mtable_pool_backward_scaled": (C.c_int, [_p, _i32, _p, _i64, _p, _i64, _i32, _p, _i64, _i32, _p, _i64, _i64,
-                                                   _p, _p]),
-    "mono_reduce_and_split_grad_scaled": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p, _p]),
-    "mono_reduce_and_split_grad_bf16_scaled": (C.c_int, [_i32, C.POINTER(ReduceFeature), _i32, _p, _p, _p]),
-    "mono_grouping_reduce_scaled": (C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p, _p]),
-    "mono_grouping_reduce_push_scaled": (C.c_int, [_p, _p, _i64, _i32, _p, _i64, _i32, _p, _p, _i64, _p, _p, _p]),
-    "mono_xstep_backward_scaled": (C.c_int, [_p, _p, _i64, _i32, _p, _i32, _p, _i64, _p, _p]),
-    "mono_xstep_forward_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p]),
-    "mono_xstep_forward_parts_bf16": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p]),
-    "mono_xstep_backward_parts": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _p]),
-    "mono_xstep_backward_parts_bf16": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _p]),
-    "mono_xstep_backward_parts_scaled": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _p, _p]),
-    "mono_xstep_backward_parts_bf16_scaled": (C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _p, _p]),
+    **_twins("mono_xstep_forward_parts", C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p], _BF16),
+    **_twins("mono_xstep_backward_parts", C.c_int, [_p, C.POINTER(PoolPartC), _i32, _p, _i64, _p], _ALL),
     "mono_grouping_build_parts": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _i32, _p, _p, _p, C.POINTER(_i64),
                                             _p]),
-    "mono_gather_pool_parts": (C.c_int, [_p, _p, _p, C.POINTER(PoolPartC), _i32, _p]),
-    "mono_gather_pool_parts_bf16": (C.c_int, [_p, _p, _p, C.POINTER(PoolPartC), _i32, _p]),
-    "mono_grouping_reduce_parts": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p]),
-    "mono_grouping_reduce_parts_bf16": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p]),
-    "mono_grouping_reduce_parts_scaled": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _p]),
-    "mono_grouping_reduce_parts_bf16_scaled": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _p]),
-    "mono_grouping_reduce_push_parts": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _i64, _p, _p]),
-    "mono_grouping_reduce_push_parts_bf16": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _i64, _p, _p]),
-    "mono_grouping_reduce_push_parts_scaled": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _i64, _p, _p,
-                                                         _p]),
-    "mono_grouping_reduce_push_parts_bf16_scaled": (C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _i64, _p,
-                                                              _p, _p]),
+    **_twins("mono_gather_pool_parts", C.c_int, [_p, _p, _p, C.POINTER(PoolPartC), _i32, _p], _BF16),
+    **_twins("mono_grouping_reduce_parts", C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p], _ALL),
+    **_twins("mono_grouping_reduce_push_parts", C.c_int, [_p, _p, C.POINTER(PoolPartC), _i32, _p, _p, _i64, _p, _p],
+             _ALL),
     "mono_ckpt_last_error": (C.c_char_p, []),
     "mono_ckpt_writer_open": (C.c_int, [C.c_char_p, C.c_char_p, _i32, C.POINTER(_p)]),
     "mono_ckpt_writer_begin_table": (C.c_int, [_p, C.c_char_p, C.POINTER(SegmentCfg), _i32]),
@@ -254,8 +227,47 @@ def load():
   return lib
 
 
-def check(status):
+def check(status, value_error: bool = False):
+  """Raises MonoError for a failed call's status; with value_error, an invalid argument (-1) raises ValueError with
+  the engine's message alone."""
   if status != 0:
     msg = load().mono_last_error()
+    msg = msg.decode() if msg else ''
+    if status == -1 and value_error:
+      raise ValueError(msg)
     kinds = {-1: "InvalidArgument", -2: "ResourceExhausted", -3: "CudaError", -4: "Internal"}
-    raise MonoError(f"{kinds.get(status, status)}: {msg.decode() if msg else ''}")
+    raise MonoError(f"{kinds.get(status, status)}: {msg}")
+
+
+def call(base: str, *args, bf16: bool = False, scale=None, stream, value_error: bool = False):
+  """Calls `base`, or its twin: `base`_bf16 for bf16=True, `base`[_bf16]_scaled for a scale pointer, which goes just
+  before the stream.  The symbol is looked up on the loaded library at every call; a twin SIGNATURES does not
+  declare raises KeyError.  The status goes to check()."""
+  name = base + ("_bf16" if bf16 else "") + ("" if scale is None else "_scaled")
+  if name not in SIGNATURES:
+    raise KeyError(f"{name} is not a C entry point")
+  check(getattr(load(), name)(*args, *(() if scale is None else (scale,)), stream), value_error)
+
+
+def ptr(t):
+  """A tensor's device pointer (None for None)."""
+  return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def stream(device):
+  """The current CUDA stream of `device`."""
+  return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+# pooling name -> mono pooling code: the calls that pool one flat feature take SUM and MEAN, PoolPart FIRSTN too
+POOLINGS = {"sum": POOL_SUM, "mean": POOL_MEAN}
+PART_POOLINGS = dict(POOLINGS, firstn=POOL_FIRSTN)
+
+
+def row_offsets(offsets, n_rows: int, device=None):
+  """-> (offsets as contiguous int32 on `device` (None: where they are), their row count), or (None, n_rows) without
+  offsets (one FID per row)."""
+  if offsets is None:
+    return None, n_rows
+  offsets = offsets.to(device=device, dtype=torch.int32).contiguous()
+  return offsets, offsets.numel() - 1

@@ -63,9 +63,8 @@ def _norm_call(t_list: Sequence[torch.Tensor], clip_norm: float) -> Tuple[Option
   arr = (_lib.NormTensor * max(len(t_list), 1))()
   for i, t in enumerate(t_list):
     arr[i] = _lib.NormTensor(C.c_void_p(t.data_ptr()), t.numel(), _DTYPES[t.dtype])
-  _lib.check(lib.mono_global_norm(dev.index, arr, len(t_list), clip_norm, C.c_void_p(norm.data_ptr()),
-                                  None if scale is None else C.c_void_p(scale.data_ptr()),
-                                  C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+  _lib.check(lib.mono_global_norm(dev.index, arr, len(t_list), clip_norm, _lib.ptr(norm), _lib.ptr(scale),
+                                  _lib.stream(dev)))
   return scale, norm
 
 

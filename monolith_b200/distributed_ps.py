@@ -28,6 +28,9 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 import torch.distributed as dist
 
+from . import _lib
+from .clip_ops import scale_ptr
+
 
 class CudaBackend:
   """The engine's kernels behind the five compute steps of the exchange."""
@@ -62,23 +65,8 @@ class CudaBackend:
     kernels, no extra pass)."""
     if self.vec_ok and dim <= 128:
       self.dops.scatter_grad_rows(pooled_grad, offs, dim, grad_buf, row_offsets, pooling, scale=scale)
-      return
-    import ctypes as C
-    from . import _lib
-    lib = _lib.load()
-    n_rows = offs.numel() if row_offsets is None else row_offsets.numel() - 1
-    pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-    ro = None if row_offsets is None else C.c_void_p(row_offsets.data_ptr())
-    args = (pooled_grad.device.index, C.c_void_p(pooled_grad.data_ptr()), pooled_grad.stride(0), 0,
-            C.c_void_p(offs.data_ptr()), ro, n_rows, dim, pool, C.c_void_p(grad_buf.data_ptr()))
-    stream = C.c_void_p(torch.cuda.current_stream(pooled_grad.device).cuda_stream)
-    bf16 = pooled_grad.dtype == torch.bfloat16
-    if scale is None:
-      fn = lib.mono_gather_pool_grad_bf16 if bf16 else lib.mono_gather_pool_grad
-      _lib.check(fn(*args, stream))
     else:
-      fn = lib.mono_gather_pool_grad_bf16_scaled if bf16 else lib.mono_gather_pool_grad_scaled
-      _lib.check(fn(*args, C.c_void_p(scale.data_ptr()), stream))
+      self.dops._gather_pool_grad_into(grad_buf, pooled_grad, offs, dim, row_offsets, pooling, 0, scale)
 
   def zeros(self, n, like):
     return torch.zeros(n, dtype=torch.float32, device=like.device)
@@ -226,9 +214,7 @@ class PartitionedHashTable:
     multiplied by it in float32 inside the scatter of step 7; the backend receives it only when it is given."""
     be, N = self.backend, self.N
     some = next(iter(pooled_grads.values()))
-    if grad_scale is not None:
-      from .clip_ops import scale_ptr
-      scale_ptr(grad_scale, some.device, "grad_scale")
+    scale_ptr(grad_scale, some.device, "grad_scale")
     extra = {} if grad_scale is None else {"scale": grad_scale}
     ph = self.phases
     ph.mark("bwd_start")
@@ -514,7 +500,6 @@ class ShardedStep:
     """(Re)create the fixed-capacity window and the step object; collective: the capacity is the largest batch of
     any rank (+ 25 % headroom), so every rank decides the same."""
     import ctypes as C
-    from . import _lib
     lib = _lib.load()
     self.close_direct()
     cap = int(m)
@@ -535,7 +520,6 @@ class ShardedStep:
     """exchange == "direct": build the grouping of the NEXT batch on a side stream while the step in flight runs
     (no table dependency).  Pass the SAME tensor to the next step()."""
     import ctypes as C
-    from . import _lib
     if self.exchange != "direct" or self.xstep is None:
       return
     f = fids_next.reshape(-1)
@@ -549,7 +533,6 @@ class ShardedStep:
     self._keep_prep = f
 
   def close_direct(self):
-    from . import _lib
     if self.xstep is not None:
       torch.cuda.synchronize(self.device)
       _lib.check(_lib.load().mono_xstep_destroy(self.xstep))
@@ -561,7 +544,6 @@ class ShardedStep:
 
   def _step_direct(self, fids, pooled_grad, out, req_time, row_offsets, pooling, grad_scale):
     import ctypes as C
-    from . import _lib
     lib = _lib.load()
     fids = fids.reshape(-1)
     if fids.dtype != torch.int64 or not fids.is_contiguous():
@@ -570,28 +552,20 @@ class ShardedStep:
     if self.xstep is None or m > self.cap_pair:
       # NOTE collective: every rank must come here in the same step (constant batch sizes never do after step 1)
       self._make_xstep(m)
-    pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-    ro = None
-    n_rows = m
-    if row_offsets is not None:
-      row_offsets = row_offsets.to(device=self.device, dtype=torch.int32).contiguous()
-      ro, n_rows = C.c_void_p(row_offsets.data_ptr()), row_offsets.numel() - 1
-    stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-    _lib.check(lib.mono_xstep_forward(self.xstep, C.c_void_p(fids.data_ptr()), m, ro, n_rows, pool,
-                                      C.c_void_p(out.data_ptr()), out.stride(0) if out.dim() == 2 else self.dim, 0, stream))
+    pool = _lib.POOLINGS[pooling]
+    row_offsets, n_rows = _lib.row_offsets(row_offsets, m, self.device)
+    ro = _lib.ptr(row_offsets)
+    _lib.check(lib.mono_xstep_forward(self.xstep, _lib.ptr(fids), m, ro, n_rows, pool, _lib.ptr(out),
+                                      out.stride(0) if out.dim() == 2 else self.dim, 0, _lib.stream(self.device)))
     if callable(pooled_grad):   # forward enqueued: the caller's dense tower / host round trip goes here
       pooled_grad = pooled_grad()
     if pooled_grad.dtype != torch.float32 or pooled_grad.stride(-1) != 1:
       pooled_grad = pooled_grad.to(torch.float32).contiguous()
     lr = self.table.configs[self.name].call_learning_rate_fns()
     lr_arr = (C.c_float * len(lr))(*lr)
-    stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-    args = (self.xstep, C.c_void_p(pooled_grad.data_ptr()), pooled_grad.stride(0) if pooled_grad.dim() == 2 else self.dim,
-            0, ro, pool, lr_arr, int(req_time))
-    if grad_scale is None:
-      _lib.check(lib.mono_xstep_backward(*args, stream))
-    else:
-      _lib.check(lib.mono_xstep_backward_scaled(*args, C.c_void_p(grad_scale.data_ptr()), stream))
+    _lib.call("mono_xstep_backward", self.xstep, _lib.ptr(pooled_grad),
+              pooled_grad.stride(0) if pooled_grad.dim() == 2 else self.dim, 0, ro, pool, lr_arr, int(req_time),
+              scale=_lib.ptr(grad_scale), stream=_lib.stream(self.device))
     self._keep = (fids, pooled_grad, row_offsets, grad_scale)   # alive until the kernels have consumed them
     self.direct_steps += 1
     return 0
@@ -650,10 +624,7 @@ class ShardedStep:
     for p in parts:
       if p.slot != self.name:
         raise ValueError(f"step_parts: part of table {p.slot!r}, the step's table is {self.name!r}")
-    if grad_scale is not None:
-      from .clip_ops import scale_ptr
-      scale_ptr(grad_scale, self.device, "grad_scale")
-    from . import _lib
+    scale_ptr(grad_scale, self.device, "grad_scale")
     fwd = _PartsArr(self.table, parts, forward=True)
     # the engine's own checks, here too: the direct exchange may re-create its window before its forward call
     for i in range(fwd.n):
@@ -675,23 +646,16 @@ class ShardedStep:
 
   def _step_parts_direct(self, fwd, bwd, grads, req_time, grad_scale):
     import ctypes as C
-    from . import _lib
-    lib = _lib.load()
     if self.xstep is None or fwd.n_fids > self.cap_pair:
       # NOTE collective, as in _step_direct
       self._make_xstep(fwd.n_fids)
-    stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-    fn = lib.mono_xstep_forward_parts_bf16 if fwd.bf16 else lib.mono_xstep_forward_parts
-    _lib.check(fn(self.xstep, fwd.arr, fwd.n, stream))
+    _lib.call("mono_xstep_forward_parts", self.xstep, fwd.arr, fwd.n, bf16=fwd.bf16, stream=_lib.stream(self.device))
     if bwd is None:   # forward enqueued: the caller's dense tower / host round trip goes here
       bwd = self._grad_parts(fwd, grads())
     lr = self.table.configs[self.name].call_learning_rate_fns()
     lr_arr = (C.c_float * len(lr))(*lr)
-    stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-    name = "mono_xstep_backward_parts" + ("_bf16" if bwd.bf16 else "") + ("" if grad_scale is None else "_scaled")
-    args = (self.xstep, bwd.arr, bwd.n, lr_arr, int(req_time))
-    args += () if grad_scale is None else (C.c_void_p(grad_scale.data_ptr()),)
-    _lib.check(getattr(lib, name)(*args, stream))
+    _lib.call("mono_xstep_backward_parts", self.xstep, bwd.arr, bwd.n, lr_arr, int(req_time), bf16=bwd.bf16,
+              scale=_lib.ptr(grad_scale), stream=_lib.stream(self.device))
     self._keep = (fwd, bwd, grad_scale)   # alive until the kernels have consumed them
     self.direct_steps += 1
 
@@ -716,9 +680,7 @@ class ShardedStep:
     The value is read on the device when that reduce runs, not when step() is entered: a callable `pooled_grad`
     may fill the tensor on the current stream, e.g.
     `scale_buf.copy_(clip_ops.global_norm_scale(dense_grads + [g], clip_norm)[0])` before it returns g."""
-    if grad_scale is not None:
-      from .clip_ops import scale_ptr
-      scale_ptr(grad_scale, self.device, "grad_scale")
+    scale_ptr(grad_scale, self.device, "grad_scale")
     if self.exchange == "direct":
       return self._step_direct(fids, pooled_grad, out, req_time, row_offsets, pooling, grad_scale)
     src = _FlatSource(self, fids, pooled_grad, out, row_offsets, pooling, grad_scale)

@@ -11,14 +11,8 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 
 from . import _lib
-
-
-def _ptr(t):
-  return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _stream(device):
-  return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+from ._lib import ptr, stream
+from .clip_ops import scale_ptr
 
 
 _TOWER_DTYPES = (torch.float32, torch.bfloat16)
@@ -57,9 +51,9 @@ def fused_reorder_by_indices(inputs: Sequence[torch.Tensor], num_of_shards: int,
   shard_sizes = (C.c_int32 * num_of_shards)()
   slot_sizes = (C.c_int32 * (num_of_shards * K))()
   n_unique = C.c_int64(0)
-  _lib.check(lib.mono_reorder_by_indices(device.index, _ptr(ids), c_split, K, num_of_shards, c_dims,
-                                         1 if rank0_empty_shard else 0, _ptr(out), None, _ptr(offs), shard_sizes,
-                                         slot_sizes, C.byref(n_unique), _stream(device)))
+  _lib.check(lib.mono_reorder_by_indices(device.index, ptr(ids), c_split, K, num_of_shards, c_dims,
+                                         1 if rank0_empty_shard else 0, ptr(out), None, ptr(offs), shard_sizes,
+                                         slot_sizes, C.byref(n_unique), stream(device)))
   emb_offset_sz = [t.numel() for t in inputs]
   return out[:n_unique.value], list(shard_sizes), list(slot_sizes), emb_offset_sz, offs[:M]
 
@@ -73,8 +67,8 @@ def unique_with_inverse(ids: torch.Tensor, sync: bool = True):
   inv = torch.empty(max(n, 1), dtype=torch.int32, device=ids.device)
   n_dev = torch.zeros(1, dtype=torch.int32, device=ids.device)
   n_host = C.c_int64(0)
-  _lib.check(lib.mono_dedup(ids.device.index, _ptr(ids), n, _ptr(uniq), _ptr(inv), _ptr(n_dev),
-                            C.byref(n_host) if sync else None, _stream(ids.device)))
+  _lib.check(lib.mono_dedup(ids.device.index, ptr(ids), n, ptr(uniq), ptr(inv), ptr(n_dev),
+                            C.byref(n_host) if sync else None, stream(ids.device)))
   if sync:
     return uniq[:n_host.value], inv[:n]
   return uniq, inv[:n], n_dev
@@ -225,15 +219,15 @@ def _sharding_sparse_fids_device(features, feature_table, feature_dims_sum, N, s
   row_splits = torch.empty(N * (F + K), dtype=torch.int64, device=device)
   table_len, shard_len, emb_len = torch.empty(N * K, **i32), torch.empty(N, **i32), torch.empty(N * K, **i32)
   host_len = (C.c_int32 * (N * K))() if sync else None
-  args = (device.index, _ptr(fids), _ptr(splits), recs, F, K, N, 1 if unique else 0, _ptr(fused), _ptr(fid_offset),
-          _ptr(feature_offset), _ptr(nfl_offset), _ptr(row_splits), _ptr(table_len), _ptr(shard_len), _ptr(emb_len),
+  args = (device.index, ptr(fids), ptr(splits), recs, F, K, N, 1 if unique else 0, ptr(fused), ptr(fid_offset),
+          ptr(feature_offset), ptr(nfl_offset), ptr(row_splits), ptr(table_len), ptr(shard_len), ptr(emb_len),
           None, host_len)
   if v5_batch_size is None:
-    _lib.check(lib.mono_sharding_sparse_fids(*args, _stream(device)))
+    _lib.check(lib.mono_sharding_sparse_fids(*args, stream(device)))
   else:
     rs_size, emb_size, sizes = torch.empty(K * N, **i32), torch.empty(K * N, **i32), torch.empty(4, **i32)
-    _lib.check(lib.mono_sharding_sparse_fids_v5(*args, v5_batch_size, _ptr(rs_size), _ptr(emb_size), _ptr(sizes),
-                                                _stream(device)))
+    _lib.check(lib.mono_sharding_sparse_fids_v5(*args, v5_batch_size, ptr(rs_size), ptr(emb_size), ptr(sizes),
+                                                stream(device)))
   # lists of table k: features first[k] .. first[k + 1] - 1 in table-major order; row splits block of (n, k) at
   # n * (F + K) + first[k] + k
   per_table = [sum(1 for n in names if t_idx[feature_table[n]] == k) for k in range(K)]
@@ -279,7 +273,7 @@ def normalize_merged_split(row_split: torch.Tensor, row_split_size: torch.Tensor
     raise ValueError(f"normalize_merged_split: {m} merged splits for {n} entries")
   out = torch.empty(n + 1 - m if m else 0, dtype=torch.int64, device=dev)
   bad = torch.zeros(1, dtype=torch.int32, device=dev)
-  _lib.check(lib.mono_normalize_merged_split(dev.index, _ptr(rs), n, _ptr(sz), m, _ptr(out), _ptr(bad), _stream(dev)))
+  _lib.check(lib.mono_normalize_merged_split(dev.index, ptr(rs), n, ptr(sz), m, ptr(out), ptr(bad), stream(dev)))
   if sync and int(bad.item()):
     raise ValueError("normalize_merged_split: every row_split_size must be >= 1 and they must add up to row_split's "
                      "length")
@@ -292,7 +286,7 @@ def round_to_f16(x: torch.Tensor) -> torch.Tensor:
     raise ValueError(f"round_to_f16 takes a CUDA float32 tensor, not {x.dtype} on {x.device}")
   x = x.contiguous()
   out = torch.empty(x.shape, dtype=torch.float16, device=x.device)
-  _lib.check(_lib.load().mono_round_to_f16(x.device.index, _ptr(x), x.numel(), _ptr(out), _stream(x.device)))
+  _lib.check(_lib.load().mono_round_to_f16(x.device.index, ptr(x), x.numel(), ptr(out), stream(x.device)))
   return out
 
 
@@ -304,18 +298,13 @@ def gather_pool(fused_embeddings: torch.Tensor, fused_embedding_offsets: torch.T
   The pooled rows are float32 or bfloat16: out's dtype when out is given, else `dtype`.  bfloat16 rows are the
   float32 results rounded once to nearest even; the fused buffer stays float32."""
   dtype = _tower_dtype(out.dtype if out is not None else dtype, "gather_pool's output")
-  lib = _lib.load()
   dev = fused_embeddings.device
   offs = fused_embedding_offsets.to(torch.int32).contiguous()
-  n_rows = offs.numel() if row_offsets is None else row_offsets.numel() - 1
-  if row_offsets is not None:
-    row_offsets = row_offsets.to(torch.int32).contiguous()
+  row_offsets, n_rows = _lib.row_offsets(row_offsets, offs.numel())
   if out is None:
     out = torch.empty(n_rows, dim, dtype=dtype, device=dev)
-  pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-  fn = lib.mono_gather_pool_bf16 if dtype == torch.bfloat16 else lib.mono_gather_pool
-  _lib.check(fn(dev.index, _ptr(fused_embeddings), _ptr(offs), _ptr(row_offsets), n_rows, dim,
-                                  pool, _ptr(out), out.stride(0), out_col, _stream(dev)))
+  _lib.call("mono_gather_pool", dev.index, ptr(fused_embeddings), ptr(offs), ptr(row_offsets), n_rows, dim,
+            _lib.POOLINGS[pooling], ptr(out), out.stride(0), out_col, bf16=dtype == torch.bfloat16, stream=stream(dev))
   return out
 
 
@@ -327,26 +316,21 @@ def gather_pool_grad(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.T
   exactly); the returned buffer is float32.  scale: a one-element float32 tensor on pooled_grad's device (the
   reference kernel's `input * scale`): each gradient element is multiplied by it in float32 before the MEAN
   division (mono_gather_pool_grad[_bf16]_scaled)."""
-  from .clip_ops import scale_ptr
-  bf16 = _tower_dtype(pooled_grad.dtype, "pooled_grad") == torch.bfloat16
-  lib = _lib.load()
-  dev = pooled_grad.device
-  sp = scale_ptr(scale, dev, "scale")
-  offs = fused_embedding_offsets.to(torch.int32).contiguous()
-  n_rows = offs.numel() if row_offsets is None else row_offsets.numel() - 1
-  if row_offsets is not None:
-    row_offsets = row_offsets.to(torch.int32).contiguous()
-  grad = torch.zeros(total_floats, dtype=torch.float32, device=dev)
-  pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-  args = (dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs), _ptr(row_offsets), n_rows, dim,
-          pool, _ptr(grad))
-  if sp is None:
-    fn = lib.mono_gather_pool_grad_bf16 if bf16 else lib.mono_gather_pool_grad
-    _lib.check(fn(*args, _stream(dev)))
-  else:
-    fn = lib.mono_gather_pool_grad_bf16_scaled if bf16 else lib.mono_gather_pool_grad_scaled
-    _lib.check(fn(*args, sp, _stream(dev)))
+  _tower_dtype(pooled_grad.dtype, "pooled_grad")
+  scale_ptr(scale, pooled_grad.device, "scale")
+  grad = torch.zeros(total_floats, dtype=torch.float32, device=pooled_grad.device)
+  _gather_pool_grad_into(grad, pooled_grad, fused_embedding_offsets, dim, row_offsets, pooling, grad_col, scale)
   return grad
+
+
+def _gather_pool_grad_into(grad, pooled_grad, fused_embedding_offsets, dim, row_offsets, pooling, grad_col, scale):
+  """gather_pool_grad's launch: scatter-adds into the float32 buffer `grad`; scale is checked by the caller."""
+  dev = pooled_grad.device
+  offs = fused_embedding_offsets.to(torch.int32).contiguous()
+  row_offsets, n_rows = _lib.row_offsets(row_offsets, offs.numel())
+  _lib.call("mono_gather_pool_grad", dev.index, ptr(pooled_grad), pooled_grad.stride(0), grad_col, ptr(offs),
+            ptr(row_offsets), n_rows, dim, _lib.POOLINGS[pooling], ptr(grad), bf16=pooled_grad.dtype == torch.bfloat16,
+            scale=ptr(scale), stream=stream(dev))
 
 
 def scatter_grad_rows(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.Tensor, dim: int,
@@ -356,26 +340,16 @@ def scatter_grad_rows(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.
   `grad_fused` (written in place; rows nobody refers to are left as they are).  pooled_grad is float32 or
   bfloat16 (widened exactly); grad_fused must be float32.  scale: as gather_pool_grad's; the result is bit for bit
   this call on pooled_grad multiplied by it in float32 (mono_scatter_grad_rows[_bf16]_scaled)."""
-  from .clip_ops import scale_ptr
   bf16 = _tower_dtype(pooled_grad.dtype, "pooled_grad") == torch.bfloat16
   if grad_fused.dtype != torch.float32:
     raise ValueError(f"grad_fused must be torch.float32, not {grad_fused.dtype}")
-  lib = _lib.load()
   dev = pooled_grad.device
   sp = scale_ptr(scale, dev, "scale")
   offs = fused_embedding_offsets.to(torch.int32).contiguous()
-  n_rows = offs.numel() if row_offsets is None else row_offsets.numel() - 1
-  if row_offsets is not None:
-    row_offsets = row_offsets.to(torch.int32).contiguous()
-  pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-  args = (dev.index, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(offs), offs.numel(), _ptr(row_offsets),
-          n_rows, dim, pool, _ptr(grad_fused), grad_fused.numel())
-  if sp is None:
-    fn = lib.mono_scatter_grad_rows_bf16 if bf16 else lib.mono_scatter_grad_rows
-    _lib.check(fn(*args, _stream(dev)))
-  else:
-    fn = lib.mono_scatter_grad_rows_bf16_scaled if bf16 else lib.mono_scatter_grad_rows_scaled
-    _lib.check(fn(*args, sp, _stream(dev)))
+  row_offsets, n_rows = _lib.row_offsets(row_offsets, offs.numel())
+  _lib.call("mono_scatter_grad_rows", dev.index, ptr(pooled_grad), pooled_grad.stride(0), grad_col, ptr(offs),
+            offs.numel(), ptr(row_offsets), n_rows, dim, _lib.POOLINGS[pooling], ptr(grad_fused), grad_fused.numel(),
+            bf16=bf16, scale=sp, stream=stream(dev))
   return grad_fused
 
 
@@ -383,12 +357,9 @@ def scatter_grad_rows(pooled_grad: torch.Tensor, fused_embedding_offsets: torch.
 # ref: distribution_ops.py:689-884 and RT/ops/reduce_op.{cc,cu.cc}.  Every function below is one call of
 # mono_reduce_and_split[_grad][_bf16]: see include/mono_emb.h for the arithmetic.
 
-_POOLINGS = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}
-
-
 def _poolings(pooling, n):
   ps = [pooling] * n if isinstance(pooling, str) else list(pooling)
-  if len(ps) != n or any(p not in _POOLINGS for p in ps):
+  if len(ps) != n or any(p not in _lib.POOLINGS for p in ps):
     raise ValueError(f"pooling must be 'sum', 'mean' or one of them per feature, not {pooling!r}")
   return ps
 
@@ -403,7 +374,6 @@ def _reduce_split_call(backward, splits, rows, slices, poolings, bad_splits, sca
   """splits[f]: int32 [B + 1]; rows[f]: [n_f, D_f] float32 (read forward, written backward); slices[f]: the 2-D
   tensors of feature f's slices (written forward, read backward), all float32 or all bfloat16.  scale (backward
   only): the clip_ops.scale_ptr of the gradient scale, or None for the unscaled call."""
-  lib = _lib.load()
   F = len(splits)
   flat = [t for s in slices for t in s]
   dtype = _tower_dtype(flat[0].dtype if flat else torch.float32, "the slice tensors")
@@ -420,16 +390,10 @@ def _reduce_split_call(backward, splits, rows, slices, poolings, bad_splits, sca
     r = rows[f]
     recs[f].splits_dev, recs[f].batch_size = splits[f].data_ptr(), splits[f].numel() - 1
     recs[f].rows_dev, recs[f].n_rows, recs[f].row_stride = r.data_ptr(), r.size(0), r.stride(0) if r.size(0) > 1 else r.size(1)
-    recs[f].dim, recs[f].pooling = r.size(1), _POOLINGS[poolings[f]]
+    recs[f].dim, recs[f].pooling = r.size(1), _lib.POOLINGS[poolings[f]]
     recs[f].slices, recs[f].n_slices = sl, len(slices[f])
-  bf16 = dtype == torch.bfloat16
-  if scale is not None:
-    fn = lib.mono_reduce_and_split_grad_bf16_scaled if bf16 else lib.mono_reduce_and_split_grad_scaled
-    _lib.check(fn(dev.index, recs, F, _ptr(bad_splits), scale, _stream(dev)))
-    return
-  fn = {(False, False): lib.mono_reduce_and_split, (True, False): lib.mono_reduce_and_split_grad,
-        (False, True): lib.mono_reduce_and_split_bf16, (True, True): lib.mono_reduce_and_split_grad_bf16}[backward, bf16]
-  _lib.check(fn(dev.index, recs, F, _ptr(bad_splits), _stream(dev)))
+  _lib.call("mono_reduce_and_split_grad" if backward else "mono_reduce_and_split", dev.index, recs, F,
+            ptr(bad_splits), bf16=dtype == torch.bfloat16, scale=scale, stream=stream(dev))
 
 
 def _splits32(splits):
@@ -471,7 +435,8 @@ def fused_reduce_and_split_gpu_grad(splits: Sequence[torch.Tensor], embeddings: 
   grad_scale: a one-element float32 tensor on the splits' device (clip_ops.global_norm_scale's scale), read on the
   device: the result is bit for bit this call on every slice gradient multiplied by it in float32 first (a bfloat16
   gradient is widened before the multiply; MEAN's factor comes after it).  mono_reduce_and_split_grad[_bf16]_scaled."""
-  sc = _grad_scale_ptr(grad_scale, splits[0].device if len(splits) else None)
+  sc = None if grad_scale is None else scale_ptr(
+      grad_scale, splits[0].device if len(splits) else torch.device("cuda", torch.cuda.current_device()))
   F = len(splits)
   sp = [_splits32(s) for s in splits]
   shapes = [(e.size(0), e.size(1)) for e in embeddings]
@@ -516,16 +481,8 @@ def _reduce(id_indices, id_values, B, split_dims, pooling, dtype, sync):
   return fused_reduce_and_split_gpu([splits], [id_values], [split_dims], pooling=pooling, dtype=dtype)
 
 
-def _grad_scale_ptr(grad_scale, dev):
-  """grad_scale checked before any device work (clip_ops.scale_ptr; dev None: the current CUDA device)."""
-  if grad_scale is None:
-    return None
-  from .clip_ops import scale_ptr
-  return scale_ptr(grad_scale, dev if dev is not None else torch.device("cuda", torch.cuda.current_device()))
-
-
 def _reduce_grad(id_indices, grads, split_dims, pooling, sync, B=None, grad_scale=None):
-  _grad_scale_ptr(grad_scale, id_indices.device)
+  scale_ptr(grad_scale, id_indices.device)
   B = grads[0].size(0) if B is None else B
   splits = _splits_from_indices(id_indices, B, sync)
   out = torch.empty(id_indices.size(0), sum(split_dims), dtype=torch.float32, device=splits.device)
@@ -610,8 +567,8 @@ class Grouping:
     offs = torch.empty(max(M, 1), dtype=torch.int32, device=self.device)
     counts = (C.c_int32 * num_shards)()
     n_u = C.c_int64(0)
-    _lib.check(self._lib.mono_grouping_build(self._h, _ptr(fids), M, num_shards, dim, _ptr(uniq), _ptr(offs), counts,
-                                             C.byref(n_u), _stream(self.device)))
+    _lib.check(self._lib.mono_grouping_build(self._h, ptr(fids), M, num_shards, dim, ptr(uniq), ptr(offs), counts,
+                                             C.byref(n_u), stream(self.device)))
     self.dim = dim
     self._keep = fids  # the grouping refers to positions of this tensor until the next build
     return uniq[:n_u.value], offs[:M], list(counts)
@@ -620,16 +577,10 @@ class Grouping:
              pooling: str = "sum", grad_col: int = 0, grad_scale: Optional[torch.Tensor] = None):
     """grad_scale: a one-element float32 tensor on the grouping's device, read on the device when the reduce runs:
     the rows are bit for bit this call's on pooled_grad multiplied by it in float32 (mono_grouping_reduce_scaled)."""
-    sp = _grad_scale_ptr(grad_scale, self.device)
-    n_rows = self._keep.numel() if row_offsets is None else row_offsets.numel() - 1
-    if row_offsets is not None:
-      row_offsets = row_offsets.to(torch.int32).contiguous()
-    pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-    args = (self._h, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(row_offsets), n_rows, pool, _ptr(out_rows))
-    if sp is None:
-      _lib.check(self._lib.mono_grouping_reduce(*args, _stream(self.device)))
-    else:
-      _lib.check(self._lib.mono_grouping_reduce_scaled(*args, sp, _stream(self.device)))
+    sp = scale_ptr(grad_scale, self.device)
+    row_offsets, n_rows = _lib.row_offsets(row_offsets, self._keep.numel())
+    _lib.call("mono_grouping_reduce", self._h, ptr(pooled_grad), pooled_grad.stride(0), grad_col, ptr(row_offsets),
+              n_rows, _lib.POOLINGS[pooling], ptr(out_rows), scale=sp, stream=stream(self.device))
     return out_rows
 
   def reduce_push(self, pooled_grad: torch.Tensor, shard_sizes: Sequence[int], window: "PeerWindow", region_off: int,
@@ -637,19 +588,13 @@ class Grouping:
                   grad_col: int = 0, grad_scale: Optional[torch.Tensor] = None):
     """reduce() whose output rows are stored into the owners' windows (fused gradient exchange).  grad_scale: as
     reduce()'s (mono_grouping_reduce_push_scaled)."""
-    sp = _grad_scale_ptr(grad_scale, self.device)
-    n_rows = self._keep.numel() if row_offsets is None else row_offsets.numel() - 1
-    if row_offsets is not None:
-      row_offsets = row_offsets.to(torch.int32).contiguous()
-    pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
+    sp = scale_ptr(grad_scale, self.device)
+    row_offsets, n_rows = _lib.row_offsets(row_offsets, self._keep.numel())
     n = window.world
-    args = (self._h, _ptr(pooled_grad), pooled_grad.stride(0), grad_col, _ptr(row_offsets), n_rows, pool,
-            (C.c_int64 * n)(*[int(x) for x in shard_sizes]), window._h, int(region_off),
-            (C.c_int64 * n)(*[int(x) for x in dst_row_off]))
-    if sp is None:
-      _lib.check(self._lib.mono_grouping_reduce_push(*args, _stream(self.device)))
-    else:
-      _lib.check(self._lib.mono_grouping_reduce_push_scaled(*args, sp, _stream(self.device)))
+    _lib.call("mono_grouping_reduce_push", self._h, ptr(pooled_grad), pooled_grad.stride(0), grad_col,
+              ptr(row_offsets), n_rows, _lib.POOLINGS[pooling], (C.c_int64 * n)(*[int(x) for x in shard_sizes]),
+              window._h, int(region_off), (C.c_int64 * n)(*[int(x) for x in dst_row_off]), scale=sp,
+              stream=stream(self.device))
 
   # ---- several features (mono_pool_part arrays) of ONE table as one batch: the sharded step over parts ----
   def build_parts(self, table, parts_arr, n_parts: int, n_fids: int, num_shards: int, dim: int):
@@ -659,37 +604,35 @@ class Grouping:
     offs = torch.empty(max(n_fids, 1), dtype=torch.int32, device=self.device)
     counts = (C.c_int32 * num_shards)()
     n_u = C.c_int64(0)
-    _lib.check(self._lib.mono_grouping_build_parts(self._h, table._h, parts_arr, n_parts, num_shards, _ptr(uniq),
-                                                   _ptr(offs), counts, C.byref(n_u), _stream(self.device)))
+    _lib.check(self._lib.mono_grouping_build_parts(self._h, table._h, parts_arr, n_parts, num_shards, ptr(uniq),
+                                                   ptr(offs), counts, C.byref(n_u), stream(self.device)))
     self.dim = dim
     return uniq[:n_u.value], offs[:n_fids], list(counts)
 
   def reduce_parts(self, table, parts_arr, n_parts: int, bf16: bool, out_rows: torch.Tensor,
                    grad_scale: Optional[torch.Tensor] = None):
     """reduce() with the parts' rows as the gradients (mono_grouping_reduce_parts[_bf16][_scaled])."""
-    sp = _grad_scale_ptr(grad_scale, self.device)
-    name = "mono_grouping_reduce_parts" + ("_bf16" if bf16 else "") + ("" if sp is None else "_scaled")
-    args = (self._h, table._h, parts_arr, n_parts, _ptr(out_rows)) + (() if sp is None else (sp,))
-    _lib.check(getattr(self._lib, name)(*args, _stream(self.device)))
+    sp = scale_ptr(grad_scale, self.device)
+    _lib.call("mono_grouping_reduce_parts", self._h, table._h, parts_arr, n_parts, ptr(out_rows), bf16=bf16, scale=sp,
+              stream=stream(self.device))
     return out_rows
 
   def reduce_push_parts(self, table, parts_arr, n_parts: int, bf16: bool, shard_sizes: Sequence[int],
                         window: "PeerWindow", region_off: int, dst_row_off: Sequence[int],
                         grad_scale: Optional[torch.Tensor] = None):
     """reduce_push() with the parts' rows as the gradients (mono_grouping_reduce_push_parts[_bf16][_scaled])."""
-    sp = _grad_scale_ptr(grad_scale, self.device)
+    sp = scale_ptr(grad_scale, self.device)
     n = window.world
-    name = "mono_grouping_reduce_push_parts" + ("_bf16" if bf16 else "") + ("" if sp is None else "_scaled")
-    args = (self._h, table._h, parts_arr, n_parts, (C.c_int64 * n)(*[int(x) for x in shard_sizes]), window._h,
-            int(region_off), (C.c_int64 * n)(*[int(x) for x in dst_row_off])) + (() if sp is None else (sp,))
-    _lib.check(getattr(self._lib, name)(*args, _stream(self.device)))
+    _lib.call("mono_grouping_reduce_push_parts", self._h, table._h, parts_arr, n_parts,
+              (C.c_int64 * n)(*[int(x) for x in shard_sizes]), window._h, int(region_off),
+              (C.c_int64 * n)(*[int(x) for x in dst_row_off]), bf16=bf16, scale=sp, stream=stream(self.device))
 
 
 def gather_pool_parts(table, rows_in: torch.Tensor, occ_offsets: torch.Tensor, parts_arr, n_parts: int, bf16: bool):
   """The pooling of looked-up rows into the rows of the parts (mono_gather_pool_parts[_bf16]): occ_offsets are a
   parts grouping's row offsets (Grouping.build_parts), `table` the MultiHashTable the parts name."""
-  fn = table._lib.mono_gather_pool_parts_bf16 if bf16 else table._lib.mono_gather_pool_parts
-  _lib.check(fn(table._h, _ptr(rows_in), _ptr(occ_offsets), parts_arr, n_parts, _stream(rows_in.device)))
+  _lib.call("mono_gather_pool_parts", table._h, ptr(rows_in), ptr(occ_offsets), parts_arr, n_parts, bf16=bf16,
+            stream=stream(rows_in.device))
 
 
 class _RawCuda:
@@ -742,15 +685,15 @@ class PeerWindow:
     return self._local[offset:offset + nb].view(dtype)
 
   def barrier(self):
-    _lib.check(self._lib.mono_peer_barrier(self._h, _stream(self.device)))
+    _lib.check(self._lib.mono_peer_barrier(self._h, stream(self.device)))
 
   def put(self, region_off: int, dst_off: Sequence[int], src: torch.Tensor, src_off: Sequence[int],
           nbytes: Sequence[int]):
     """nbytes[r] bytes of src (+ src_off[r]) -> rank r's window at region_off + dst_off[r]."""
     n = self.world
     arr = lambda xs: (C.c_int64 * n)(*[int(x) for x in xs])
-    _lib.check(self._lib.mono_peer_put(self._h, int(region_off), arr(dst_off), _ptr(src), arr(src_off), arr(nbytes),
-                                       _stream(self.device)))
+    _lib.check(self._lib.mono_peer_put(self._h, int(region_off), arr(dst_off), ptr(src), arr(src_off), arr(nbytes),
+                                       stream(self.device)))
 
 
   def get(self, region_off: int, src_off: Sequence[int], dst: torch.Tensor, dst_off: Sequence[int],
@@ -758,8 +701,8 @@ class PeerWindow:
     """nbytes[r] bytes of rank r's window at region_off + src_off[r] -> dst (+ dst_off[r], bytes)."""
     n = self.world
     arr = lambda xs: (C.c_int64 * n)(*[int(x) for x in xs])
-    _lib.check(self._lib.mono_peer_get(self._h, int(region_off), arr(src_off), _ptr(dst), arr(dst_off), arr(nbytes),
-                                       _stream(self.device)))
+    _lib.check(self._lib.mono_peer_get(self._h, int(region_off), arr(src_off), ptr(dst), arr(dst_off), arr(nbytes),
+                                       stream(self.device)))
 
 
 # ---- generic fused layout op ------------------------------------------------------------------
@@ -827,18 +770,14 @@ def fused_embedding_to_layout(embeddings_list: Sequence[torch.Tensor], emb_strid
   f16_in = len(embeddings_list) > 0 and embeddings_list[0].dtype == torch.float16
   dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, embeddings_list, "embeddings_list",
                              torch.float16 if f16_in else torch.float32)
-  lib = _lib.load()
   outs = [torch.zeros(*s, dtype=dtype, device=dev) for s in out_shapes]
   embs = [e.contiguous() for e in embeddings_list]
   ep, op = _ptr_table(embs, dev), _ptr_table(outs, dev)
   st = torch.tensor(list(emb_strides), dtype=torch.int32, device=dev)
-  if f16_in:
-    fn = lib.mono_embedding_to_layout_f16in_bf16 if bf16 else lib.mono_embedding_to_layout_f16in
-  else:
-    fn = lib.mono_embedding_to_layout_bf16 if bf16 else lib.mono_embedding_to_layout
-  _lib.check(fn(dev.index, _ptr(ep), _ptr(st), len(embs), _ptr(fid_offset), fid_offset.numel(), _ptr(feature_offset),
-                feature_offset.numel(), _ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks), len(tasks),
-                _ptr(op), _stream(dev)))
+  _lib.call("mono_embedding_to_layout_f16in" if f16_in else "mono_embedding_to_layout", dev.index, ptr(ep), ptr(st),
+            len(embs), ptr(fid_offset), fid_offset.numel(), ptr(feature_offset), feature_offset.numel(),
+            ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks), len(tasks), ptr(op), bf16=bf16,
+            stream=stream(dev))
   return outs
 
 
@@ -854,13 +793,11 @@ def fused_embedding_to_layout_grad(emb_sizes: Sequence[int], emb_strides: Sequen
   multiplied by it in float32 before the MEAN division (mono_embedding_to_layout_grad[_bf16]_scaled).
   out: zero-filled contiguous float32 tensors of emb_sizes elements on that device (e.g. views of one buffer) that
   receive the gradients and are returned, in place of fresh ones."""
-  from .clip_ops import scale_ptr
   dtype = _tower_dtype(out_grads[0].dtype if len(out_grads) else torch.float32, "out_grads")
   if any(g.dtype != dtype for g in out_grads):
     raise ValueError(f"out_grads must be all torch.float32 or all torch.bfloat16, not {[g.dtype for g in out_grads]}")
   dev = _check_layout_inputs(fid_offset, feature_offset, nfl_offset, out_grads, "out_grads", dtype)
   sp = scale_ptr(layout_tensors_grad_scale, dev, "layout_tensors_grad_scale")
-  lib = _lib.load()
   if out is None:
     grads = [torch.zeros(n, dtype=torch.float32, device=dev) for n in emb_sizes]
   else:
@@ -871,16 +808,10 @@ def fused_embedding_to_layout_grad(emb_sizes: Sequence[int], emb_strides: Sequen
   og = [g.contiguous() for g in out_grads]
   gp, op = _ptr_table(grads, dev), _ptr_table(og, dev)
   st = torch.tensor(list(emb_strides), dtype=torch.int32, device=dev)
-  args = (dev.index, _ptr(gp), _ptr(st), len(grads), _ptr(fid_offset), fid_offset.numel(), _ptr(feature_offset),
-          feature_offset.numel(), _ptr(nfl_offset), nfl_offset.numel(), batch_size, _tasks_arr(tasks), len(tasks),
-          _ptr(op))
-  if sp is None:
-    fn = lib.mono_embedding_to_layout_grad_bf16 if dtype == torch.bfloat16 else lib.mono_embedding_to_layout_grad
-    _lib.check(fn(*args, _stream(dev)))
-  else:
-    fn = (lib.mono_embedding_to_layout_grad_bf16_scaled if dtype == torch.bfloat16 else
-          lib.mono_embedding_to_layout_grad_scaled)
-    _lib.check(fn(*args, sp, _stream(dev)))
+  _lib.call("mono_embedding_to_layout_grad", dev.index, ptr(gp), ptr(st), len(grads), ptr(fid_offset),
+            fid_offset.numel(), ptr(feature_offset), feature_offset.numel(), ptr(nfl_offset), nfl_offset.numel(),
+            batch_size, _tasks_arr(tasks), len(tasks), ptr(op), bf16=dtype == torch.bfloat16, scale=sp,
+            stream=stream(dev))
   return grads
 
 
@@ -930,8 +861,8 @@ def unique_key_with_value_and_offset(ids: torch.Tensor, key_split: Sequence[int]
   value_len = C.c_int64(0)
   host = (C.c_int64 * (K + 1))() if sync else None
   _lib.check(lib.mono_unique_key_with_value_and_offset(
-      dev.index, _ptr(ids), (C.c_int64 * (K + 1))(*splits), K, (C.c_int32 * K)(*[int(d) for d in dims]), _ptr(uniq),
-      _ptr(uniq_split), _ptr(off), _ptr(off_split), C.byref(value_len), host, _stream(dev)))
+      dev.index, ptr(ids), (C.c_int64 * (K + 1))(*splits), K, (C.c_int32 * K)(*[int(d) for d in dims]), ptr(uniq),
+      ptr(uniq_split), ptr(off), ptr(off_split), C.byref(value_len), host, stream(dev)))
   buf = torch.empty(value_len.value, dtype=torch.float32, device=dev) if generate_buffer else None
   U = host[K] if sync else None
   if sync:
@@ -979,12 +910,9 @@ def ragged_split_by_indices(indices: torch.Tensor, values: torch.Tensor, row_spl
   rs_out, offs = torch.empty(max(S, 0) * max(K + 1, 0), **i64), torch.empty(max(S, 0) + 1, **i64)
   bad = torch.zeros(1, dtype=torch.int32, device=dev)
   host = (C.c_int64 * (S * (K + 1)))() if sync and S > 0 and K > 0 else None
-  status = lib.mono_ragged_split_by_indices(dev.index, _ptr(indices), _ptr(values), cap, _ptr(row_splits), K, S,
-                                            _ptr(v_out), _ptr(p_out), _ptr(rs_out), _ptr(offs), _ptr(bad), host,
-                                            _stream(dev))
-  if status == -1:
-    raise ValueError(_lib.load().mono_last_error().decode())
-  _lib.check(status)
+  _lib.check(lib.mono_ragged_split_by_indices(dev.index, ptr(indices), ptr(values), cap, ptr(row_splits), K, S,
+                                              ptr(v_out), ptr(p_out), ptr(rs_out), ptr(offs), ptr(bad), host,
+                                              stream(dev)), value_error=True)
   rs2 = rs_out.view(S, K + 1)
   out = RaggedSplit(None, None, None, v_out[:cap], p_out[:cap], rs2, offs, bad)
   if sync:
@@ -1009,7 +937,6 @@ def split_by_indices(indices: torch.Tensor, tensor: torch.Tensor, num_splits: in
 
 
 def _fill_call(grad, pos, pos_split, src, value_offset, dims, num_unique, dst, sync):
-  lib = _lib.load()
   splits = _host_splits(pos_split, "pos_split")
   K = len(splits) - 1
   if len(dims) != K:
@@ -1026,16 +953,13 @@ def _fill_call(grad, pos, pos_split, src, value_offset, dims, num_unique, dst, s
   bad = torch.zeros(1, dtype=torch.int32, device=dev)
   c_split, c_dims = (C.c_int64 * (K + 1))(*splits), (C.c_int32 * K)(*[int(d) for d in dims])
   if grad:
-    fn = lib.mono_fill_with_offset_map_grad_f16 if dst.dtype == torch.float16 else lib.mono_fill_with_offset_map_grad
-    status = fn(dev.index, _ptr(pos), c_split, K, c_dims, _ptr(src), _ptr(offs), _ptr(offs_split), U, _ptr(dst),
-                _ptr(bad), _stream(dev))
+    _lib.call("mono_fill_with_offset_map_grad_f16" if dst.dtype == torch.float16 else "mono_fill_with_offset_map_grad",
+              dev.index, ptr(pos), c_split, K, c_dims, ptr(src), ptr(offs), ptr(offs_split), U, ptr(dst), ptr(bad),
+              stream=stream(dev), value_error=True)
   else:
-    fn = lib.mono_fill_with_offset_map_f16 if f16_src else lib.mono_fill_with_offset_map
-    status = fn(dev.index, _ptr(pos), c_split, K, c_dims, _ptr(src), src.numel(), _ptr(offs), _ptr(offs_split), U,
-                _ptr(dst), _ptr(bad), _stream(dev))
-  if status == -1:
-    raise ValueError(lib.mono_last_error().decode())
-  _lib.check(status)
+    _lib.call("mono_fill_with_offset_map_f16" if f16_src else "mono_fill_with_offset_map", dev.index, ptr(pos),
+              c_split, K, c_dims, ptr(src), src.numel(), ptr(offs), ptr(offs_split), U, ptr(dst), ptr(bad),
+              stream=stream(dev), value_error=True)
   if sync and int(bad.item()):
     raise ValueError(f"pos is bigger than offset size: a pos outside [0, {U})")
   return dst

@@ -16,15 +16,9 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 
 from . import _lib
+from ._lib import ptr, stream
+from .clip_ops import scale_ptr
 from .entry import HashTableConfigInstance, to_c_table_cfgs
-
-
-def _ptr(t: Optional[torch.Tensor]):
-  return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _stream(device) -> C.c_void_p:
-  return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 def _ids(t, device) -> torch.Tensor:
@@ -153,7 +147,7 @@ class MultiHashTable:
     for n in names:
       v = C.c_int64()
       _lib.check(self._lib.mono_mtable_size(self._h, self._table_names.index(n), C.byref(v),
-                                            _stream(self._device)))
+                                            stream(self._device)))
       res[n] = v.value
     return res[name] if name else res
 
@@ -166,7 +160,7 @@ class MultiHashTable:
     raises on nothing (size() raises on the error bits)."""
     words = (C.c_uint32 * 16)()
     _lib.check(self._lib.mono_mtable_counters(self._h, self._table_names.index(slot), words, 16,
-                                              _stream(self._device)))
+                                              stream(self._device)))
     return {n: int(words[i]) for n, i in MultiHashTable.COUNTER_WORDS.items()}
 
   # ---- ragged packing (ref: get_ragged_id / get_flat_value / get_embeddings :528-548) -------
@@ -224,9 +218,9 @@ class MultiHashTable:
     values, splits = self.get_ragged_id({k: v[0] for k, v in slot_to_id_and_value.items()})
     flat = self.get_flat_value({k: v[1] for k, v in slot_to_id_and_value.items()})
     self._check_values(values, splits, flat)
-    _lib.check(self._lib.mono_mtable_assign_add(self._h, _ptr(values), self._split_arr(splits), _ptr(flat),
+    _lib.check(self._lib.mono_mtable_assign_add(self._h, ptr(values), self._split_arr(splits), ptr(flat),
                                                 int(req_time), _lib.FLAG_IDS_UNIQUE if ids_unique else 0,
-                                                _stream(self._device)))
+                                                stream(self._device)))
     return self
 
   def reinitialize(self, slot: str, ids: torch.Tensor):
@@ -234,8 +228,8 @@ class MultiHashTable:
     ids = _ids(ids, self._device)
     status = torch.empty(ids.numel(), dtype=torch.int32, device=self._device)
     k = self._table_names.index(slot) if slot in self._table_names else -1
-    _lib.check(self._lib.mono_mtable_reinitialize(self._h, k, _ptr(ids), ids.numel(), _ptr(status),
-                                                  int(time.time()), _stream(self._device)))
+    _lib.check(self._lib.mono_mtable_reinitialize(self._h, k, ptr(ids), ids.numel(), ptr(status),
+                                                  int(time.time()), stream(self._device)))
     return self, status
 
   def apply_gradients(self, slot_to_id_and_grad: Dict[str, Tuple[torch.Tensor, torch.Tensor]],
@@ -261,8 +255,8 @@ class MultiHashTable:
     out = torch.empty(total, dtype=dtype, device=self._device)
     if id_split[-1] != ids.numel():
       raise ValueError("id_split does not cover ids")
-    fn = self._lib.mono_mtable_lookup_f16 if dtype == torch.float16 else self._lib.mono_mtable_lookup
-    _lib.check(fn(self._h, _ptr(ids), self._split_arr(id_split), _ptr(out), _stream(self._device)))
+    _lib.call("mono_mtable_lookup_f16" if dtype == torch.float16 else "mono_mtable_lookup", self._h, ptr(ids),
+              self._split_arr(id_split), ptr(out), stream=stream(self._device))
     return out
 
   def _check_values(self, ids, id_split, flat):
@@ -280,18 +274,18 @@ class MultiHashTable:
     lr = self.learning_rates()
     lr_arr = (C.c_float * len(lr))(*lr)
     flags = (_lib.FLAG_IDS_UNIQUE if ids_unique else 0) | (_lib.FLAG_DEDUP_SUM if enable_dedup else 0)
-    _lib.check(self._lib.mono_mtable_optimize(self._h, _ptr(ids), self._split_arr(id_split), _ptr(flat_grad),
+    _lib.check(self._lib.mono_mtable_optimize(self._h, ptr(ids), self._split_arr(id_split), ptr(flat_grad),
                                               lr_arr, int(req_time), int(global_step), flags,
-                                              _stream(self._device)))
+                                              stream(self._device)))
     return self
 
   def raw_assign(self, ids: torch.Tensor, id_split: Sequence[int], flat_value: torch.Tensor, req_time: int = 0,
                  ids_unique: bool = False):
     ids, flat_value = _ids(ids, self._device), _f32(flat_value, self._device).reshape(-1)
     self._check_values(ids, id_split, flat_value)
-    _lib.check(self._lib.mono_mtable_assign(self._h, _ptr(ids), self._split_arr(id_split), _ptr(flat_value),
+    _lib.check(self._lib.mono_mtable_assign(self._h, ptr(ids), self._split_arr(id_split), ptr(flat_value),
                                             int(req_time), _lib.FLAG_IDS_UNIQUE if ids_unique else 0,
-                                            _stream(self._device)))
+                                            stream(self._device)))
     return self
 
   # ---- fused ops for sync training (ref: multi_hash_table_ops.py:438-483) ----------------------
@@ -318,8 +312,8 @@ class MultiHashTable:
       out = torch.empty(emb_off[-1], dtype=torch.float32, device=self._device)
     elif out.numel() < emb_off[-1] or out.dtype != torch.float32 or not out.is_contiguous():
       raise ValueError("fused_lookup: out must be a contiguous float32 buffer of at least emb_offsets[-1] floats")
-    _lib.check(self._lib.mono_mtable_fused_lookup(self._h, _ptr(ids), ss, num_of_shards, int(req_time), _ptr(out),
-                                                  _stream(self._device)))
+    _lib.check(self._lib.mono_mtable_fused_lookup(self._h, ptr(ids), ss, num_of_shards, int(req_time), ptr(out),
+                                                  stream(self._device)))
     return out, emb_splits, id_off, emb_off, ids
 
   def fused_apply_gradient(self, ids: torch.Tensor, indices: torch.Tensor, fused_slot_size: Sequence[int],
@@ -337,9 +331,9 @@ class MultiHashTable:
     lr_arr = (C.c_float * len(lr))(*lr)
     flags = (_lib.FLAG_IDS_UNIQUE if (ids_unique and not enable_grad_accumulation) else 0) | \
             (_lib.FLAG_DEDUP_SUM if enable_grad_accumulation else 0)
-    _lib.check(self._lib.mono_mtable_fused_optimize(self._h, _ptr(ids), ss, _ptr(id_grads), io, go, lr_arr,
+    _lib.check(self._lib.mono_mtable_fused_optimize(self._h, ptr(ids), ss, ptr(id_grads), io, go, lr_arr,
                                                     int(req_time), int(global_step), num_of_shards, flags,
-                                                    _stream(self._device)))
+                                                    stream(self._device)))
     return self
 
   # ---- engine extensions -------------------------------------------------------------------
@@ -350,8 +344,8 @@ class MultiHashTable:
     k = self._table_names.index(slot)
     n = window.world
     _lib.check(self._lib.mono_mtable_lookup_push(
-        self._h, k, _ptr(ids), (C.c_int64 * n)(*[int(x) for x in counts]), window._h, int(region_off),
-        (C.c_int64 * n)(*[int(x) for x in dst_row_off]), _stream(self._device)))
+        self._h, k, ptr(ids), (C.c_int64 * n)(*[int(x) for x in counts]), window._h, int(region_off),
+        (C.c_int64 * n)(*[int(x) for x in dst_row_off]), stream(self._device)))
 
   def lookup_pool(self, slot: str, fids: torch.Tensor, row_offsets: Optional[torch.Tensor] = None,
                   pooling: str = "sum", out: Optional[torch.Tensor] = None, out_col: int = 0) -> torch.Tensor:
@@ -362,17 +356,13 @@ class MultiHashTable:
     lookup() give ReduceSum's and ReduceMean's bits."""
     k = self._table_names.index(slot)
     fids = _ids(fids, self._device)
-    if row_offsets is not None:
-      row_offsets = row_offsets.to(device=self._device, dtype=torch.int32).contiguous()
-      n_rows = row_offsets.numel() - 1
-    else:
-      n_rows = fids.numel()
+    row_offsets, n_rows = _lib.row_offsets(row_offsets, fids.numel(), self._device)
     if out is None:
       out = torch.empty(n_rows, self._dims[k], dtype=torch.float32, device=self._device)
     stride = out.stride(0) if out.dim() == 2 else self._dims[k]
-    pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-    _lib.check(self._lib.mono_mtable_lookup_pool(self._h, k, _ptr(fids), _ptr(row_offsets), n_rows, pool,
-                                                 _ptr(out), stride, out_col, _stream(self._device)))
+    _lib.check(self._lib.mono_mtable_lookup_pool(self._h, k, ptr(fids), ptr(row_offsets), n_rows,
+                                                 _lib.POOLINGS[pooling], ptr(out), stride, out_col,
+                                                 stream(self._device)))
     return out
 
   def pool_backward(self, slot: str, fids: torch.Tensor, pooled_grad: torch.Tensor,
@@ -385,31 +375,17 @@ class MultiHashTable:
 
     grad_scale: as pool_backward_parts' (mono_mtable_pool_backward_scaled): the call is bit for bit this call on
     pooled_grad multiplied by it in float32 first."""
-    sp = None
-    if grad_scale is not None:
-      from .clip_ops import scale_ptr
-      sp = scale_ptr(grad_scale, self._device, "grad_scale")
+    sp = scale_ptr(grad_scale, self._device, "grad_scale")
     k = self._table_names.index(slot)
     fids = _ids(fids, self._device)
     pooled_grad = _f32(pooled_grad, self._device)
-    if row_offsets is not None:
-      row_offsets = row_offsets.to(device=self._device, dtype=torch.int32).contiguous()
-      n_rows = row_offsets.numel() - 1
-    else:
-      n_rows = fids.numel()
+    row_offsets, n_rows = _lib.row_offsets(row_offsets, fids.numel(), self._device)
     stride = pooled_grad.stride(0) if pooled_grad.dim() == 2 else self._dims[k]
     lr = self._configs[slot].call_learning_rate_fns()
     lr_arr = (C.c_float * len(lr))(*lr)
-    pool = {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN}[pooling]
-    if sp is None:
-      _lib.check(self._lib.mono_mtable_pool_backward(self._h, k, _ptr(fids), fids.numel(), _ptr(row_offsets), n_rows,
-                                                     pool, _ptr(pooled_grad), stride, grad_col, lr_arr, int(req_time),
-                                                     int(global_step), _stream(self._device)))
-    else:
-      _lib.check(self._lib.mono_mtable_pool_backward_scaled(self._h, k, _ptr(fids), fids.numel(), _ptr(row_offsets),
-                                                            n_rows, pool, _ptr(pooled_grad), stride, grad_col, lr_arr,
-                                                            int(req_time), int(global_step), sp,
-                                                            _stream(self._device)))
+    _lib.call("mono_mtable_pool_backward", self._h, k, ptr(fids), fids.numel(), ptr(row_offsets), n_rows,
+              _lib.POOLINGS[pooling], ptr(pooled_grad), stride, grad_col, lr_arr, int(req_time), int(global_step),
+              scale=sp, stream=stream(self._device))
     return self
 
   @staticmethod
@@ -437,12 +413,7 @@ class MultiHashTable:
         raise KeyError(f"unknown table {p.slot}")
       k = self._table_names.index(p.slot)
       fids = _ids(p.fids, self._device)
-      ro = None
-      if p.row_offsets is not None:
-        ro = p.row_offsets.to(device=self._device, dtype=torch.int32).contiguous()
-        n_rows = ro.numel() - 1
-      else:
-        n_rows = fids.numel()
+      ro, n_rows = _lib.row_offsets(p.row_offsets, fids.numel(), self._device)
       width = self._dims[k] * (p.max_seq_len if p.pooling == "firstn" else 1)
       rows = p.rows
       if rows is None:
@@ -459,8 +430,7 @@ class MultiHashTable:
       keep += [fids, ro]
       outs.append(rows)
       arr[i] = _lib.PoolPartC(k, fids.data_ptr(), fids.numel(), None if ro is None else ro.data_ptr(), n_rows,
-                              {"sum": _lib.POOL_SUM, "mean": _lib.POOL_MEAN, "firstn": _lib.POOL_FIRSTN}[p.pooling],
-                              rows.data_ptr(), rows.stride(0), p.col, p.max_seq_len)
+                              _lib.PART_POOLINGS[p.pooling], rows.data_ptr(), rows.stride(0), p.col, p.max_seq_len)
     return arr, keep, outs
 
   def lookup_pool_parts(self, parts: Sequence[PoolPart], dtype: Optional[torch.dtype] = None) -> List[torch.Tensor]:
@@ -474,9 +444,8 @@ class MultiHashTable:
     torch.bfloat16 (mono_mtable_lookup_pool_parts_bf16) every row is the float32 result rounded once to bfloat16."""
     dtype = self._parts_dtype(parts, dtype)
     arr, keep, outs = self._parts_arr(parts, forward=True, dtype=dtype)
-    fn = (self._lib.mono_mtable_lookup_pool_parts_bf16 if dtype == torch.bfloat16 else
-          self._lib.mono_mtable_lookup_pool_parts)
-    _lib.check(fn(self._h, arr, len(parts), _stream(self._device)))
+    _lib.call("mono_mtable_lookup_pool_parts", self._h, arr, len(parts), bf16=dtype == torch.bfloat16,
+              stream=stream(self._device))
     del keep
     return outs
 
@@ -494,20 +463,13 @@ class MultiHashTable:
     grad_scale: a one-element float32 tensor on the table's device (clip_ops.global_norm_scale's scale), read on the
     device: the call is then bit for bit this call on every gradient row multiplied by it in float32 first
     (mono_mtable_pool_backward_parts[_bf16]_scaled; a bfloat16 row is widened before the multiply)."""
-    from .clip_ops import scale_ptr
     dtype = self._parts_dtype(parts)
     sp = scale_ptr(grad_scale, self._device, "grad_scale")
     arr, keep, _ = self._parts_arr(parts, forward=False, dtype=dtype)
     lr = self.learning_rates()
     lr_arr = (C.c_float * max(len(lr), 1))(*lr)
-    if sp is None:
-      fn = (self._lib.mono_mtable_pool_backward_parts_bf16 if dtype == torch.bfloat16 else
-            self._lib.mono_mtable_pool_backward_parts)
-      _lib.check(fn(self._h, arr, len(parts), lr_arr, int(req_time), int(global_step), _stream(self._device)))
-    else:
-      fn = (self._lib.mono_mtable_pool_backward_parts_bf16_scaled if dtype == torch.bfloat16 else
-            self._lib.mono_mtable_pool_backward_parts_scaled)
-      _lib.check(fn(self._h, arr, len(parts), lr_arr, int(req_time), int(global_step), sp, _stream(self._device)))
+    _lib.call("mono_mtable_pool_backward_parts", self._h, arr, len(parts), lr_arr, int(req_time), int(global_step),
+              bf16=dtype == torch.bfloat16, scale=sp, stream=stream(self._device))
     del keep
     return self
 
@@ -520,7 +482,7 @@ class MultiHashTable:
     ks = (C.c_uint32 * max(len(st), 1))(*[int(x) for x in st.keys()])
     vs = (C.c_uint32 * max(len(st), 1))(*[int(x) for x in st.values()])
     _lib.check(self._lib.mono_mtable_set_hash_filter(self._h, k, int(capacity), int(default_threshold), ks, vs, len(st),
-                                                     _stream(self._device)))
+                                                     stream(self._device)))
     self._filter_cells[slot] = max(int(int(capacity) * 1.5), 1) + 64
     return self
 
@@ -534,20 +496,20 @@ class MultiHashTable:
       raise ValueError(f"table '{slot}' has no hash filter")
     out = np.zeros(n, np.uint16)
     _lib.check(self._lib.mono_mtable_hash_filter_cells(self._h, k, out.ctypes.data_as(C.c_void_p), n,
-                                                       _stream(self._device)))
+                                                       stream(self._device)))
     return out
 
   def contains(self, slot: str, ids: torch.Tensor) -> torch.Tensor:
     ids = _ids(ids, self._device)
     out = torch.empty(ids.numel(), dtype=torch.uint8, device=self._device)
-    _lib.check(self._lib.mono_mtable_contains(self._h, self._table_names.index(slot), _ptr(ids), ids.numel(),
-                                              _ptr(out), _stream(self._device)))
+    _lib.check(self._lib.mono_mtable_contains(self._h, self._table_names.index(slot), ptr(ids), ids.numel(),
+                                              ptr(out), stream(self._device)))
     return out.bool()
 
   def evict(self, slot: str, max_update_time: int):
     """ref: CuckooEmbeddingHashTable::Evict; the reference runs it from a background thread."""
     _lib.check(self._lib.mono_mtable_evict(self._h, self._table_names.index(slot), int(max_update_time),
-                                           _stream(self._device)))
+                                           stream(self._device)))
     return self
 
   def lookup_entry(self, slot: str, ids: torch.Tensor) -> Dict[str, torch.Tensor]:
@@ -556,8 +518,8 @@ class MultiHashTable:
     ids = _ids(ids, self._device)
     D, S = self._dims[k], self._lib.mono_mtable_state_floats(self._h, k)
     raw = torch.empty(ids.numel(), D + S + 2, dtype=torch.float32, device=self._device)
-    _lib.check(self._lib.mono_mtable_lookup_entry(self._h, k, _ptr(ids), ids.numel(), _ptr(raw),
-                                                  _stream(self._device)))
+    _lib.check(self._lib.mono_mtable_lookup_entry(self._h, k, ptr(ids), ids.numel(), ptr(raw),
+                                                  stream(self._device)))
     meta = raw[:, D + S:].contiguous().view(torch.int32)
     return {"num": raw[:, :D], "opt": raw[:, D:D + S], "found": meta[:, 0].bool(),
             "last_update_ts_sec": meta[:, 1].to(torch.int64) & 0xFFFFFFFF, "raw": raw}
@@ -570,8 +532,8 @@ class MultiHashTable:
     while cursor.value >= 0:
       ids = torch.empty(chunk, dtype=torch.int64, device=self._device)
       rows = torch.empty(chunk, D + S + 2, dtype=torch.float32, device=self._device)
-      _lib.check(self._lib.mono_mtable_export(self._h, k, C.byref(cursor), chunk, _ptr(ids), _ptr(rows),
-                                              C.byref(n), _stream(self._device)))
+      _lib.check(self._lib.mono_mtable_export(self._h, k, C.byref(cursor), chunk, ptr(ids), ptr(rows),
+                                              C.byref(n), stream(self._device)))
       if n.value:
         yield ids[:n.value], rows[:n.value]
 
@@ -609,6 +571,6 @@ class MultiHashTable:
   def restore_rows(self, slot: str, ids: torch.Tensor, raw_rows: torch.Tensor):
     k = self._table_names.index(slot)
     ids, raw_rows = _ids(ids, self._device), _f32(raw_rows, self._device)
-    _lib.check(self._lib.mono_mtable_restore_rows(self._h, k, _ptr(ids), ids.numel(), _ptr(raw_rows),
-                                                  _stream(self._device)))
+    _lib.check(self._lib.mono_mtable_restore_rows(self._h, k, ptr(ids), ids.numel(), ptr(raw_rows),
+                                                  stream(self._device)))
     return self
